@@ -1,13 +1,13 @@
 #!/usr/bin/env python
 """bench.py - pileup positions/sec through the consensus-inference hot path (BASELINE.json metric).
 
-    python bench.py --gpus N --steps K --warmup W            # this repo's B200 engine
+    python bench.py --gpus N --steps K --warmup W            # this repo's H100 engine
     python bench.py --impl reference --gpus N --steps K --warmup W   # the reference's CPU path
 
 Workload (config.workload): BASELINE.json configs[1] - r1041_e82_400bps_sup_v5 consensus on a
 synthetic 10 Mb draft: 1111 windows x 10000 pileup columns x 10 features (chunk_len 10000,
-overlap 1000; the reference's six 200-window batches coalesced into ONE device batch - the
-engine takes any batch size and a B200 holds the whole draft).  One step = one pass of the
+overlap 1000; the reference's six 200-window batches coalesced into 1056-window device groups -
+one wave of an H100; the engine takes any batch size).  One step = one pass of the
 hot path over that batch (features in -> probabilities + labels out).  Weights are seeded
 synthetic (random-init, the archives in the reference are Git-LFS stubs).
 
@@ -20,6 +20,8 @@ synthetic (random-init, the archives in the reference are Git-LFS stubs).
             launch / its mean launch duration (CUDA events per stage, recorded every step).
 N > 1: one process per GPU (torchrun), weights broadcast once over NCCL from rank 0, each rank
 runs the same per-GPU workload on its own windows (weak scaling, no data-path collective).
+--dump-outputs DIR: after the timed steps, the last device-resident step's probabilities and labels of a fixed, seeded
+sample of windows go to DIR/probs.npy, DIR/labels.npy (float32) and DIR/windows.npy (the sampled window indices).
 """
 import argparse
 import concurrent.futures
@@ -44,6 +46,23 @@ FLOP_INPROJ0 = 2 * (2 * 384 * 10)                 # 15 360
 FLOP_GRU_TOTAL = 2 * FLOP_REC_PER_LAYER + FLOP_INPROJ1 + FLOP_INPROJ0   # 801 792
 
 
+DUMP_WINDOWS = 48        # 48 x 10000 positions: 9.6 MB of probabilities, well under 64 MB
+
+
+def dump_outputs(out_dir, lib, ffi, lm, dev, d_probs, d_labels, B, T):
+    """Probabilities and labels of a fixed, seeded sample of windows (the whole output is > 64 MB) as float32 .npy."""
+    os.makedirs(out_dir, exist_ok=True)
+    wins = np.sort(np.random.RandomState(1234).choice(B, min(B, DUMP_WINDOWS), replace=False))
+    probs = np.empty((len(wins), T, 5), dtype=np.float32)
+    labels = np.empty((len(wins), T), dtype=np.uint8)
+    for i, w in enumerate(wins):
+        lm.check(lib.mdk_memcpy_d2h(dev, ffi.from_buffer(probs[i]), ffi.cast("float *", d_probs) + int(w) * T * 5, T * 5 * 4))
+        lm.check(lib.mdk_memcpy_d2h(dev, ffi.from_buffer(labels[i]), ffi.cast("uint8_t *", d_labels) + int(w) * T, T))
+    np.save(os.path.join(out_dir, "probs.npy"), probs)
+    np.save(os.path.join(out_dir, "labels.npy"), labels.astype(np.float32))
+    np.save(os.path.join(out_dir, "windows.npy"), wins.astype(np.float64))
+
+
 def measured_peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
@@ -51,11 +70,12 @@ def measured_peaks():
             d = json.load(fh)
         return {"hbm_gbs": d["hbm_gbs"], "tflops_burst": d["bf16_tflops"],
                 "tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "tflops_burst": 1590.0, "tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W card): HBM3 bandwidth, dense BF16 - an upper bound, not a measurement
+    return {"hbm_gbs": 3350.0, "tflops_burst": 989.0, "tflops_sustained": 989.0, "source": "fallback"}
 
 
 class ClockSampler(object):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -350,6 +370,8 @@ def main():
                     help="columns per window in the CPU sample (0 = the full window length for the cpu_baseline of the "
                          "default run, ~15 s; sized for ~12 s per step for --impl reference)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs (probabilities, labels) of a seeded window sample as .npy")
     args = ap.parse_args()
 
     capture_stdout()
@@ -482,6 +504,9 @@ def main():
     n_fwd = min(args.steps * len(chunks), 32)
     lm.check(lib.mdk_engine_mean_timings(eng, n_fwd, tm))
     stage = {k: float(getattr(tm, k)) for k in ("inproj0_ms", "rec0_ms", "inproj1_ms", "rec1_ms", "head_ms")}
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, lib, ffi, lm, dev, d_probs_set[(step_no[0] - 1) & 1],
+                     d_labels_set[(step_no[0] - 1) & 1], B, T)
 
     # sanity: the timed path produced real outputs (labels consistent with probabilities)
     chk = np.empty((min(B, 4), T, 5), dtype=np.float32)
@@ -497,13 +522,13 @@ def main():
     lm.check(lib.mdk_engine_mean_timings(eng, 1, tm))
     solo = {k: float(getattr(tm, k)) for k in ("inproj0_ms", "rec0_ms", "inproj1_ms", "rec1_ms", "head_ms")}
 
-    # the recurrent kernel with one CTA on every SM, alone on the GPU: a full wave of windows (2368 for the two-tile
+    # the recurrent kernel with one CTA on every SM, alone on the GPU: a full wave of windows (16 per SM for the two-tile
     # kernel) over as many columns as the reserved workspace holds - the per-step cost of the persistent kernel does
     # not depend on the window length
     full_wave = None
     if args.precision == "tc" and args.config != 5:
         tiles_b0 = (b0 + 15) // 16
-        pp_sel = args.rec_mode == "pp" or (args.rec_mode == "auto" and tiles_b0 * 2 > sm_count // 2)
+        pp_sel = args.rec_mode == "pp" or (args.rec_mode == "auto" and tiles_b0 * 2 > sm_count)
         fw_windows = 16 * sm_count if pp_sel else 8 * sm_count
         fw_cols = (b0 * T) // fw_windows
         if fw_cols >= 256:
@@ -520,7 +545,8 @@ def main():
             full_wave = {"windows": fw_windows, "cols": fw_cols, "ctas": sm_count, "rec0_ms": float(tm.rec0_ms),
                          "rec1_ms": float(tm.rec1_ms), "inproj1_ms": float(tm.inproj1_ms), "achieved": fw_tf,
                          "peak": pk["tflops_burst"], "frac": fw_tf / pk["tflops_burst"],
-                         "peak_source": "MEASURED_PEAKS.json bf16 burst (kernel timed alone)"}
+                         "peak_source": "MEASURED_PEAKS.json bf16 burst (kernel timed alone)" if pk["source"] == "measured"
+                         else "H100 SXM data sheet, dense bf16 (kernel timed alone)"}
 
     # ---- host-buffer leg ("e2e"): the reference-facing call with HOST buffers, the way run_prediction drives it -
     # batches of --batch-windows windows (the reference's --batch_size) submitted with a look-ahead
@@ -564,20 +590,19 @@ def main():
     e2e = total_positions / (e2e_ms * 1e-3)
 
     # ---- roofline of the dominant kernel (tensor bound) ----
-    # The recurrent kernel of a config-2 group runs on a PART of the GPU (ping-pong kernel: one CTA per window tile =
-    # 70 of 148 SMs for 1111 windows; the other lane's kernels use the rest), so its roofline is the tensor peak of the
-    # SMs it holds: peak = sustained bf16 peak x CTAs / SMs.  achieved = algorithmic FLOPs per launch / mean launch
+    # The recurrent kernel of a group may run on a PART of the GPU (one CTA per window tile and direction; a 1056-window
+    # group fills the 132 SMs of an H100), so its roofline is the tensor peak of the SMs it holds: peak = sustained bf16 peak x CTAs / SMs.  achieved = algorithmic FLOPs per launch / mean launch
     # duration in the TIMED REGION (event to event on the launching stream; includes any wait for SMs, so it is a lower
     # bound).  full_wave_solo is the same kernel launched alone with one CTA on every SM.
     peaks = measured_peaks()
     p0 = b0 * T
     tiles0 = (b0 + 15) // 16
-    use_pp = args.precision == "tc" and (args.rec_mode == "pp" or (args.rec_mode == "auto" and tiles0 * 2 > sm_count // 2))
-    rec_ctas = tiles0 if use_pp else min(2 * tiles0, sm_count)
+    use_pp = args.precision == "tc" and (args.rec_mode == "pp" or (args.rec_mode == "auto" and tiles0 * 2 > sm_count))
+    rec_ctas = 2 * ((tiles0 + 1) // 2) if use_pp else 2 * tiles0
     sm_share = min(1.0, rec_ctas / float(sm_count))
     rec_ms_region = 0.5 * (stage["rec0_ms"] + stage["rec1_ms"])
     kernels = {
-        "recurrent kernel (%s: GRU recurrence, layer-0 and layer-1 launches)" % ("rec_pp_kernel" if use_pp else "rec_tc_kernel"):
+        "recurrent kernel (rec_tc_kernel, %s: GRU recurrence, layer-0 and layer-1 launches)" % ("two tiles per CTA" if use_pp else "one tile per CTA"):
             (rec_ms_region, p0 * FLOP_REC_PER_LAYER, solo["rec0_ms"] + solo["rec1_ms"], sm_share),
         "gemm_tc_kernel (layer-1 input projection)": (stage["inproj1_ms"], p0 * FLOP_INPROJ1, solo["inproj1_ms"], 1.0),
     }
@@ -585,18 +610,12 @@ def main():
     k_ms, k_flop, k_share_ms, k_sms = kernels[dom]
     achieved = k_flop / (k_ms * 1e-3) / 1e12
     peak = peaks["tflops_sustained"] * k_sms
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if args.config == 2 and args.precision == "tc" and os.path.exists(tpath):
-        with open(tpath) as fh:
-            tj = json.load(fh)
-        traffic = tj.get(("rec_pp_kernel" if use_pp else "rec_tc_kernel") if dom.startswith("recurrent") else "gemm_tc_kernel")
     flop_gru = 2 * FLOP_REC_PER_LAYER + FLOP_INPROJ1 + 2 * (2 * 384 * F)
     roofline = {
         "bound": "tensor", "kernel": dom, "achieved": achieved, "peak": peak,
-        "unit": "TFLOP/s", "frac": achieved / peak, "traffic": traffic,
+        "unit": "TFLOP/s", "frac": achieved / peak,
         "peak_source": ("MEASURED_PEAKS.json bf16 sustained (kernel timed inside a long step) x %d/%d SMs the launch occupies"
-                        % (round(k_sms * sm_count), sm_count)) if peaks["source"] == "measured" else "fallback (B200_PROFILING.md)",
+                        % (round(k_sms * sm_count), sm_count)) if peaks["source"] == "measured" else "H100 SXM data sheet, dense bf16",
         "launch": {"windows": b0, "cols": T, "ctas": rec_ctas if dom.startswith("recurrent") else None,
                    "flop_per_launch": k_flop, "mean_ms_in_timed_region": k_ms},
         "note": "algorithmic FLOPs; operands are fp16 hi/lo pairs so the kernel issues 3 MMAs per product "

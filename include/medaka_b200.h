@@ -1,5 +1,5 @@
 /*
- * medaka_b200.h - C ABI of libmedaka_b200.so, the sm_100a engine behind medaka's
+ * medaka_b200.h - C ABI of libmedaka_b200.so, the sm_90a engine behind medaka's
  * inference hot path (medaka/prediction.py:44-52).
  *
  * Plain C: opaque handles, pointers + sizes, int return codes (0 = MDK_OK).  No torch
@@ -41,7 +41,7 @@ extern "C" {
 #define MDK_ERR_NOMEM -5
 
 /* precision modes of the GRU gate matmuls */
-#define MDK_PREC_TC 0    /* tcgen05 tensor cores, fp16 hi/lo split operands (3 MMAs), fp32 accumulate */
+#define MDK_PREC_TC 0    /* wgmma tensor cores, fp16 hi/lo split operands (3 MMAs), fp32 accumulate */
 #define MDK_PREC_FP32 1  /* CUDA-core fp32 FFMA path: validation / --full_precision */
 
 /* which recurrent kernel the tensor-core path runs (mdk_engine_set_rec_mode) */
@@ -133,11 +133,11 @@ int mdk_engine_forward(mdk_engine *e, const float *feats_host, int64_t B, int64_
  * page-locked) until mdk_engine_wait(ticket) returns.
  * Batches are COALESCED: consecutive submits with the same T collect in a group (their features are copied to the
  * device as they arrive, behind the previous group's compute) and the group runs as ONE forward over all of its
- * windows - the reference's default batches (medaka/prediction.py:14, 100-200 windows) are a fraction of what fills a
- * B200.  A group is launched when it is full (one wave of windows, mdk_engine_preferred_windows, or as far as the
+ * windows - the reference's default batches (medaka/prediction.py:14, 100-200 windows) are a fraction of what fills an
+ * H100.  A group is launched when it is full (one wave of windows, mdk_engine_preferred_windows, or as far as the
  * buffers sized by mdk_engine_reserve reach), when a batch with another T arrives, or when somebody waits for one of
- * its tickets.  Groups alternate between two compute lanes (own stream, own workspace), so the layer-1 pass of one
- * group shares the GPU with the layer-0 pass of the next; small forwards (<= 2^18 positions: the B = 1 remainder
+ * its tickets.  Groups rotate over the staging lanes and compute on one workspace (a one-wave group fills every SM),
+ * so the copies of the neighbouring groups run under the compute; small forwards (<= 2^18 positions: the B = 1 remainder
  * regions of prediction.py:196-209) rotate over 14 more lanes and run concurrently.  Results are identical to
  * uncoalesced forwards: windows never interact. */
 int mdk_engine_submit(mdk_engine *e, const float *feats_host, int64_t B, int64_t T,
@@ -167,8 +167,8 @@ int mdk_engine_keep_activations(mdk_engine *e, int keep);
 /* number of kernels launched by this engine since creation (bench.py "gpu_launches") */
 int64_t mdk_engine_launch_count(mdk_engine *e);
 /* Number of windows per predict_on_batch call that fills the device exactly once: the recurrent kernel runs one CTA per
- * (16-window tile, direction), so 16 * (SMs / 2) windows = 1184 on a B200 is one full wave (the reference's --batch_size
- * default, medaka/prediction.py:14 / medaka.py, is sized for its own GPUs' memory; a 200-window batch uses 26 of 148 SMs).
+ * (16-window tile, direction), so 16 * (SMs / 2) windows = 1056 on an H100 is one full wave (the reference's --batch_size
+ * default, medaka/prediction.py:14 / medaka.py, is sized for its own GPUs' memory; a 200-window batch uses 26 of 132 SMs).
  * Callers that own the batching (run_prediction) should coalesce to this size. */
 int64_t mdk_engine_preferred_windows(mdk_engine *e);
 
@@ -263,7 +263,7 @@ int mdk_rl_create(int device, int32_t lstm_size, int32_t cnn_size, int32_t use_d
                   mdk_rl_engine **out);
 int mdk_rl_destroy(mdk_rl_engine *e);
 int mdk_rl_load(mdk_rl_engine *e, const char *name, const float *data, int64_t n);
-/* which parts run on tcgen05 with fp16 hi/lo operand pairs (bit set) or on the fp32 CUDA cores (validation twins):
+/* which parts run on wgmma with fp16 hi/lo operand pairs (bit set) or on the fp32 CUDA cores (validation twins):
  * bit 0 = the k = 17 convolution (99 % of the network's FLOPs), bit 1 = the LSTM recurrences.  Default 3. */
 int mdk_rl_set_conv(mdk_rl_engine *e, int tensor_cores);
 int mdk_rl_forward(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P, int64_t D, int64_t F,
@@ -351,24 +351,15 @@ int mdk_decode_variants(int device, const float *probs, const int64_t *minor, co
                         int64_t *run_start, int64_t *run_len, float *run_pred_q, float *run_ref_q,
                         int64_t *n_runs_out);
 
-/* ---- self test of the tcgen05 building block (one 128xN tile GEMM), used by tests ----------
+/* ---- self test of the wgmma building block (one 128xN tile GEMM), used by tests ------------
  * Computes D[128][N] = A[128][K] * B[N][K]^T with the same smem layouts, descriptors and
- * fp16 hi/lo split the GRU kernels use.  A, B, D are host fp32.  variant selects descriptor
- * hypotheses (0 = production encoding). */
+ * fp16 hi/lo split the GRU kernels use.  A, B, D are host fp32.  variant must be 0 (the
+ * production descriptor encoding). */
 int mdk_selftest_umma(int device, const float *A, const float *B, float *D, int N, int K,
                       int variant);
 
-/* ---- diagnostics: cycle stamps of the recurrent kernel's hand-off points ------------------
- * enable != 0 switches the (slower, instrumented) recurrent kernels on for subsequent forwards on `device` at batch
- * sizes that run one tile per CTA; enable == 0 switches back.  If out is not NULL it first receives the stamps of
- * the last traced forward: uint64 [2 layers][16 time steps (512..527)][32 slots] of %clock64 on CTA (0,0); the slot
- * meanings are listed in tools/diag.py.  Not part of the hot path. */
-int mdk_debug_rec_trace(int device, int enable, uint64_t *out);
-/* diagnostics of the TRACED ping-pong recurrent kernels: a bit set that switches parts of a time step off (1: h-tile
- * stores, 2: proxy fence, 4: gate arithmetic, 8: x staging, 16: gi staging, 32: tile copy-out) so that the cycle trace
- * shows what each costs; results are wrong while any bit is set.  0 restores normal operation. */
-int mdk_debug_pp_flags(int flags);
-/* completion times (ms after mdk_engine_timer_start's event) of the eight stage events of the last n_last forwards,
+/* ---- diagnostics -------------------------------------------------------------------------
+ * completion times (ms after mdk_engine_timer_start's event) of the eight stage events of the last n_last forwards,
  * oldest first: out is float[n_last][8] = start, features in, inproj0, rec0, inproj1, rec1, head, end.  Shows how the
  * lanes' kernels actually interleaved. */
 int mdk_debug_timeline(mdk_engine *e, int n_last, float *out);

@@ -1,6 +1,6 @@
 // C ABI of libmedaka_b200 (include/medaka_b200.h): engine life-cycle, weight loading, the forward
 // pipeline, and the featuriser / decode entry points.  Host orchestration only - kernels live in
-// misc.cu, gru_fp32.cu and gru_tc.cu.
+// misc.cu, gru_fp32.cu and gru_wg.cu.
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -78,7 +78,7 @@ static int prepare_weights(mdk_engine *e) {
     }
     {
         int rc;
-        if (!e->lin_w_tc && (rc = dev_alloc(&e->lin_w_tc, (size_t)NDIR * 2 * 16 * 64 * 8 + (size_t)NDIR * H * H))) return rc;
+        if (!e->lin_w_tc && (rc = dev_alloc(&e->lin_w_tc, (size_t)NDIR * 2 * 16 * 64 * 8))) return rc;
         MDK_CUDA(launch_pack_linear(e->lin_w, e->lin_w_tc, e->stream));
         e->launches++;
     }
@@ -103,7 +103,6 @@ static int ensure_workspace(mdk_engine *e, mdk_ws &ws, int64_t B, int64_t T) {
     if ((rc = dev_alloc(&ws.gi, (size_t)need * GI_COLS))) return rc;
     MDK_CUDA(cudaMalloc(&ws.h0, (size_t)need * H2 * sizeof(float)));
     if ((rc = dev_alloc(&ws.plog, (size_t)NDIR * (need / WT) * PLOG_TS_FLOATS))) return rc;
-    if (!ws.gemm_ctr) MDK_CUDA(cudaMalloc(&ws.gemm_ctr, 8 * sizeof(int)));
     ws.cap_pos = need;
     return MDK_OK;
 }
@@ -138,14 +137,14 @@ static int ensure_io(mdk_engine *e, mdk_lane &ln, int64_t B, int64_t T) {
     return MDK_OK;
 }
 
-// Which recurrent kernel runs a batch of B windows (tensor-core path).  One tile per CTA (rec_tc_kernel, NT = 1) is a
-// single dependent chain per SM; two tiles per CTA (rec_pp_kernel) interleave two chains on one SM and need half as many
-// CTAs, so two groups on two lanes share the GPU.  AUTO: ping-pong from half a wave of tiles up.
+// Which recurrent kernel runs a batch of B windows (tensor-core path).  One tile per CTA (NT = 1) is a single dependent
+// chain per SM; two tiles per CTA (NT = 2, one N = 32 MMA chain) need half as many CTAs.  AUTO: two tiles per CTA only
+// once the tiles of both directions outnumber the SMs.
 static bool use_pingpong(const mdk_engine *e, int64_t B) {
     const int64_t tiles = (B + WT - 1) / WT;
     if (e->rec_mode == MDK_REC_PINGPONG) return true;
     if (e->rec_mode == MDK_REC_ONE_TILE) return false;
-    return tiles * NDIR > (int64_t)e->sm_count / 2;
+    return tiles * NDIR > (int64_t)e->sm_count;
 }
 
 // The forward pipeline on the workspace's stream.  ev[1..6] bracket the stages for mdk_timings.
@@ -184,7 +183,7 @@ static int run_forward(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int64_
     launches++;
     MDK_CUDA(cudaEventRecord(e->ev[3], s));
     if (tc) MDK_CUDA(launch_gemm_tc(ws.h0, e->layer[1].w_in_tc, e->layer[1].bias_gi_tc, ws.gi, tiled_rows(B, T), e->sm_count, s,
-                                    e->prod_mask, ws.gemm_ctr));
+                                    e->prod_mask));
     else MDK_CUDA(launch_gemm_fp32((const float *)ws.h0, e->layer[1].w_in_packed, e->layer[1].bias_gi, ws.gi, P, s));
     launches++;
     MDK_CUDA(cudaEventRecord(e->ev[4], s));
@@ -289,7 +288,7 @@ size_t mdk_featlen(void) { return 10; }
 size_t mdk_fwd_del(void) { return 9; }
 size_t mdk_rev_del(void) { return 8; }
 const char *mdk_last_error(void) { return g_last_error.c_str(); }
-const char *mdk_version(void) { return "medaka_b200 0.1.0 (sm_100a)"; }
+const char *mdk_version(void) { return "medaka_b200 0.1.0 (sm_90a)"; }
 
 int mdk_device_count(int *count) {
     MDK_REQUIRE(count, MDK_ERR_ARG, "count is NULL");
@@ -359,8 +358,8 @@ int mdk_engine_create(int device, const mdk_model_desc *desc, mdk_engine **out) 
     MDK_REQUIRE(device >= 0 && device < ndev, MDK_ERR_ARG, "engine_create: no such CUDA device");
     cudaDeviceProp prop;
     MDK_CUDA(cudaGetDeviceProperties(&prop, device));
-    MDK_REQUIRE(prop.major == 10, MDK_ERR_UNSUPPORTED,
-                "engine_create: this library is built for sm_100a (Blackwell B200) only");
+    MDK_REQUIRE(prop.major == 9 && prop.minor == 0, MDK_ERR_UNSUPPORTED,
+                "engine_create: this library is built for sm_90a (Hopper H100) only");
     MDK_CUDA(cudaSetDevice(device));
     mdk_engine *e = new (std::nothrow) mdk_engine();
     MDK_REQUIRE(e, MDK_ERR_NOMEM, "engine_create: out of host memory");
@@ -413,7 +412,6 @@ int mdk_engine_destroy(mdk_engine *e) {
     dev_free(e->lin_w); dev_free(e->lin_b); dev_free(e->lin_w_tc);
     for (auto &ws : e->ws) {
         dev_free(ws.gi); dev_free(ws.h1); dev_free(ws.plog);
-        if (ws.gemm_ctr) { cudaFree(ws.gemm_ctr); ws.gemm_ctr = nullptr; }
         if (ws.h0) cudaFree(ws.h0);
         if (ws.stream) cudaStreamDestroy(ws.stream);
     }
@@ -762,10 +760,6 @@ int mdk_engine_read_activation(mdk_engine *e, int which, float *out_host, int64_
     return MDK_OK;
 }
 
-int mdk_debug_pp_flags(int flags) {
-    pp_set_debug((uint32_t)flags);
-    return MDK_OK;
-}
 
 int mdk_debug_read_plog(mdk_engine *e, float *out_host, int64_t n_floats) {
     MDK_REQUIRE(e && out_host, MDK_ERR_ARG, "NULL argument");
@@ -788,7 +782,7 @@ int mdk_engine_keep_activations(mdk_engine *e, int keep) {
 }
 
 int64_t mdk_engine_preferred_windows(mdk_engine *e) {
-    const int sms = e ? e->sm_count : 148;
+    const int sms = e ? e->sm_count : 132;
     return (int64_t)mdk::WT * (sms / mdk::NDIR);
 }
 
@@ -1024,11 +1018,5 @@ int mdk_selftest_umma(int device, const float *A, const float *B, float *D, int 
     return selftest_umma(device, A, B, D, N, K, variant);
 }
 
-int mdk_debug_rec_trace(int device, int enable, uint64_t *out) {
-    MDK_CUDA(cudaSetDevice(device));
-    MDK_CUDA(cudaDeviceSynchronize());
-    MDK_CUDA(rec_trace_control(enable, reinterpret_cast<unsigned long long *>(out)));
-    return MDK_OK;
-}
 
 }  // extern "C"

@@ -36,7 +36,7 @@ int cuda_fail(cudaError_t err, const char *what, const char *file, int line);
         }                             \
     } while (0)
 
-// Geometry of the fp16 hi/lo operand tiles the tcgen05 kernels consume (K-major, no swizzle:
+// Geometry of the fp16 hi/lo operand tiles the wgmma kernels consume (K-major, no swizzle:
 // [k-group][row][8 halfs]; see ptx.cuh make_smem_desc).
 constexpr int XT_ROWS = 128;                       // positions per activation tile
 constexpr int XT_K = H2;                           // 256
@@ -87,21 +87,21 @@ struct LayerWeights {
     float *bias_gi_tc = nullptr;    // [768] = bias_gi * gate_scale
     float *b_hn_tc = nullptr;       // [2][128] = b_hn * gate_scale(n)
     float *w_hh_t = nullptr;        // [2][128(k)][384] fp32 (transposed) for the FFMA path
-    __half *w_hh_tm = nullptr;      // [2][hi/lo][gate][row128][k128] fp16 row-major: source of the TMEM-resident A operand
+    __half *w_hh_tm = nullptr;      // [2][hi/lo][gate][row128][k128] fp16 row-major: source of the recurrent kernel's A operand
     __half *w_x_tm = nullptr;       // layer 0, F <= 16: [2][hi/lo][gate][row128][16] fp16 (K zero-padded): fused input projection
     __half *w_in_tc = nullptr;      // layer 1 only: [6 blocks][hi/lo][row128][k256] fp16 row-major: source of the
-                                    // gemm_tc TMEM-resident A operand
+                                    // gemm_tc shared-memory A operand
 };
 
 }  // namespace mdk
 
 // The engine runs GROUPS of windows.  A workspace (mdk_ws) is a compute stream plus the intermediates of one forward; a
 // lane (mdk_lane) is the device-side staging of one group of submitted batches (features in, probabilities / labels
-// out) and is bound to one workspace.  There are more big lanes than big workspaces: while two groups compute, a third
-// is receiving its features and a fourth is draining its results, so the copies never hold a workspace (48 GB for a
-// 1184 x 10 000 group) idle.  Groups on the two big workspaces run concurrently: the ping-pong recurrent kernels
-// (gru_pp.cu) need half of the SMs for a 1184-window group.  Small forwards (the B = 1 remainder regions of
-// medaka/prediction.py:196-209) spread over the small lanes, each with a workspace of its own.
+// out) and is bound to one workspace.  There are more big lanes than big workspaces: while one group computes, others
+// are receiving their features or draining their results, so the copies never hold the workspace (43 GB for a
+// 1056 x 10 000 group, 4 KiB per position) idle.  One big workspace: a one-wave group (one 16-window tile per CTA and
+// direction) already fills every SM, and a second 43 GB workspace would not fit beside it in 80 GB.  Small forwards (the
+// B = 1 remainder regions of medaka/prediction.py:196-209) spread over the small lanes, each with a workspace of its own.
 struct mdk_ws {
     cudaStream_t stream = nullptr;
     int64_t cap_pos = 0;       // capacity in positions (rounded up to XT_ROWS)
@@ -110,7 +110,6 @@ struct mdk_ws {
     float *h1 = nullptr;       // [cap_pos][256], allocated on first use (unfused head only)
     int64_t cap_h1 = 0;
     float *plog = nullptr;     // fused head: per-direction partial logits [dir][tile-step][class 5][16 windows]
-    int *gemm_ctr = nullptr;   // the GEMM's six tile counters (zeroed in front of each launch)
     // geometry of the last forward run here (mdk_engine_read_activation)
     int64_t last_B = 0, last_T = 0;
     int last_precision = -1;
@@ -143,11 +142,11 @@ struct mdk_engine {
     int device = 0;
     mdk_model_desc desc{};
     int precision = MDK_PREC_TC;
-    int sm_count = 148;
+    int sm_count = 132;
     bool fuse_x = true;           // layer-0 input projection fused into the recurrence (F <= 16); MDK_NO_FUSE_X=1 disables
     int rec_mode = MDK_REC_AUTO;  // which recurrent kernel the tensor-core path runs (MDK_REC_*)
     uint32_t prod_mask = 7u;      // fp16 products per contraction (mdk_engine_set_products)
-    static constexpr int BIG_WS = 2, BIG_LANES = 4, SMALL_LANES = 14;
+    static constexpr int BIG_WS = 1, BIG_LANES = 4, SMALL_LANES = 14;
     static constexpr int N_LANES = BIG_LANES + SMALL_LANES, N_WS = BIG_WS + SMALL_LANES;
     static constexpr int64_t SMALL_POS = 1 << 18;   // forwards up to this many positions run on the small lanes
     mdk_ws ws[N_WS];              // [0, BIG_WS): big groups; then one per small lane
@@ -204,34 +203,32 @@ cudaError_t launch_rec_fp32(const float *gi, const float *w_hh_t, const float *b
                             int64_t T, cudaStream_t s);
 cudaError_t launch_gemm_fp32(const float *A, const float *W, const float *bias, float *C, int64_t P,
                              cudaStream_t s);
-// gru_tc.cu
+// gru_wg.cu
 struct RecXArgs {            // fused layer-0 input projection (rec_tc FUSE_X)
     const float *feats;      // [B][T][F]
     const __half *w_x;       // LayerWeights::w_x_tm
     const float *bias;       // LayerWeights::bias_gi
     int F;
 };
-cudaError_t rec_trace_control(int enable, unsigned long long *host_out);
 // lin_w_tc != nullptr (layer 1, one tile per CTA): the 5-class linear head runs inside the recurrence as extra MMAs and
 // the kernel writes partial logits to plog instead of h_out; *fused_logits tells the caller whether it did
 bool rec_tc_can_fuse_logits(int64_t B, int sm_count);
 cudaError_t launch_rec_tc(const float *gi, const RecXArgs *fuse, const __half *w_hh_tm, const float *b_hn,
                           void *h_out, int out_tiles, int64_t B, int64_t T, int sm_count, cudaStream_t s,
                           const __half *lin_w_tc = nullptr, float *plog = nullptr, uint32_t prod_mask = 7u);
-// gru_pp.cu: two tiles per CTA (ping-pong).  layer 0: fused projection when `fuse` is given (F <= 16), else gi in; operand
+// two tiles per CTA.  layer 0: fused projection when `fuse` is given (F <= 16), else gi in; operand
 // tiles out.  layer 1: gi in, partial logits out (lin_w_tc, plog required).  prod_mask: fp16 products per contraction
 // (bit 0 W_hi.h_hi, bit 1 W_hi.h_lo, bit 2 W_lo.h_hi; 7 = fp32-faithful)
 cudaError_t launch_rec_pp(int layer, const float *gi, const RecXArgs *fuse, const __half *w_hh_tm, const float *b_hn,
                           void *h_out, int64_t B, int64_t T, cudaStream_t s, const __half *lin_w_tc, float *plog,
                           uint32_t prod_mask);
-void pp_set_debug(uint32_t flags);   // diagnostics of the traced ping-pong kernels (gru_pp.cu PPArgs::debug)
 // head on the partial logits of the fused path: sum of the two directions + bias -> softmax / argmax
 cudaError_t launch_head_plog(const float *plog, const float *lin_b, int64_t B, int64_t T, float *probs, float *logits,
                              uint8_t *labels, cudaStream_t s);
 cudaError_t launch_pack_linear(const float *lin_w, __half *lin_w_tc, cudaStream_t s);
 constexpr int PLOG_TS_FLOATS = NCLS * WT;     // 80 floats per (tile-step, direction)
 cudaError_t launch_gemm_tc(const void *x_tiles, const __half *w_in_tm, const float *bias, float *gi, int64_t P,
-                           int sm_count, cudaStream_t s, uint32_t prod_mask, int *tile_ctr);
+                           int sm_count, cudaStream_t s, uint32_t prod_mask);
 int selftest_umma(int device, const float *A, const float *B, float *D, int N, int K, int variant);
 // pileup.cu
 cudaError_t plp_scratch(size_t bytes, uint8_t **out, int slot);   // per-host-thread cached device buffers (slot 0 / 1)

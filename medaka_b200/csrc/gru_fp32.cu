@@ -1,5 +1,5 @@
 // fp32 CUDA-core (FFMA) implementation of the GRU layer: the --full_precision / validation path
-// (MDK_PREC_FP32).  Same data flow as the tensor-core path (gru_tc.cu) with fp32 operands:
+// (MDK_PREC_FP32).  Same data flow as the tensor-core path (gru_wg.cu) with fp32 operands:
 //   gi  = X . W_ih^T + folded bias           (time-parallel GEMM, gemm_fp32)
 //   h_t = GRU cell(gi_t, h_{t-1} . W_hh^T)   (persistent recurrent kernel, rec_fp32)
 // Reference arithmetic: torch.nn.GRU as used by medaka/architectures/gru.py:46-52,66.

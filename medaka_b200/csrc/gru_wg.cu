@@ -1,0 +1,564 @@
+// Tensor-core (wgmma) implementation of the GRU gate matmuls for sm_90a  (MDK_PREC_TC).
+//
+// Reference arithmetic: torch.nn.GRU as used by medaka/architectures/gru.py:46-52,66; parity target is
+// the fp32 CPU path (medaka/prediction.py:146-148).  To stay inside 1e-3 (scale-aware) of fp32 through a
+// 10 000-step recurrence, every operand is carried as an fp16 pair (hi + lo, ~22 significant bits) and each
+// product is three fp16 MMAs, hi*hi + hi*lo + lo*hi, accumulated in fp32.
+//
+// Both kernels use the TRANSPOSED formulation  G^T[gate rows, N] = W[gate rows, K] . X^T[K, N]:
+//   A operand = weights (M = 64 gate rows per warpgroup, K-major = torch's native [out][in] layout)
+//   B operand = activations (N windows or positions, K-major = row-major [n][k])
+//   D (registers) = hidden unit j x window / position n
+// so the thread that holds r_j of a window also holds z_j and n_j of it: the gate math needs no exchange.
+//
+// Shared-memory operand layout (K-major, no swizzle): [k-group = k/8][row][8 halfs]; a core matrix is 8 rows
+// x 16 B = 128 contiguous bytes, LBO = k-group stride, SBO = 128 B (next 8 rows).
+#include "common.cuh"
+#include "ptx.cuh"
+#include "rec_common.cuh"
+
+namespace mdk {
+
+// =====================================================================================================
+// Recurrent kernel.  One CTA = NT tiles of 16 windows (N = 16 NT) of one direction, for the whole sequence.
+// Two warpgroups; warpgroup g owns hidden units [64g, 64g + 64) of all three gates, so the h tile of a step is
+// complete only when both have written their half: one __syncthreads per step, with the tile double buffered
+// (step t reads buffer t & 1 and writes the other).
+// W_hh hi stays in REGISTERS for the whole sequence (the A operand of the register form of wgmma: 96 registers per
+// thread), W_hh lo is a shared-memory A operand, so per step shared memory feeds only one of the three weight planes.
+// The pre-activations of the next step are loaded straight into the accumulators (r, z) while the step ends; the
+// n gate needs W_in.x and W_hn.h apart, so its input part sits in registers of its own.
+// FUSE_X (layer 0, F <= 16): the input projection W_ih . x_t is three more products per gate on a 16-column x tile,
+// so layer 0 needs no gi buffer.  OUT: fp16 hi/lo operand tiles of the projection GEMM (layer 0), fp32 rows, or
+// (layer 1) partial logits: the 5-row linear head as three more products on the h tile, one step behind (the tile it
+// reads is the previous step's h); both warpgroups issue them (a warpgroup-dependent branch around a wgmma makes ptxas
+// serialise them all), warpgroup 0 stores rows 0..4.
+// =====================================================================================================
+constexpr int RW_THREADS = 256;
+constexpr int RW_ABLK = (H / 8) * 64 * 16;          // W_hh lo of one (gate, warpgroup): [kg 16][row 64][8] = 16 KiB
+constexpr int RW_XBLK = 2 * 64 * 16;                // W_ih lo (K = 16) of one (gate, warpgroup): 2 KiB
+constexpr int RW_WL_PLANE = 16 * 64 * 16;           // one plane of W_lin: [kg 16][row 64][8] = 16 KiB
+enum { OUT_TILES = 0, OUT_ROWS = 1, OUT_LOGITS = 2 };
+
+template <int NT, bool FUSE_X, int OUT>
+struct RwCfg {
+    static constexpr int N = NT * RT_N;
+    static constexpr int KG = N * 16 + 16;          // k-group stride of an activation tile (+16 B spreads the 2-byte
+                                                    // stores of one k-group over the banks)
+    static constexpr int HPLANE = (H / 8) * KG;
+    static constexpr int XPLANE = 2 * KG;
+    static constexpr int wlo_off = 0;                                            // [gate 3][wg 2] RW_ABLK
+    static constexpr int wxlo_off = wlo_off + 6 * RW_ABLK;                       // [gate 3][wg 2] RW_XBLK
+    static constexpr int wl_off = wxlo_off + (FUSE_X ? 6 * RW_XBLK : 0);         // [plane 2] RW_WL_PLANE
+    static constexpr int h_off = wl_off + (OUT == OUT_LOGITS ? 2 * RW_WL_PLANE : 0);   // [buf 2][plane 2] HPLANE
+    static constexpr int x_off = h_off + 4 * HPLANE;                             // [buf 2][plane 2] XPLANE
+    static constexpr int total = x_off + (FUSE_X ? 4 * XPLANE : 0);
+    static_assert(total <= 227 * 1024, "smem budget");
+};
+
+__device__ __forceinline__ uint32_t ld_u32(const __half *p) { return *reinterpret_cast<const uint32_t *>(p); }
+
+// ALL3: the product set is the full one (the production path) and known at compile time.  A run-time product set puts a
+// branch between the wgmmas of one accumulator chain, and ptxas then inserts a warpgroup.arrive in front of each of them
+// (warning C7519); the run-time form is kept for the precision experiments of mdk_engine_set_products.
+template <int NT, bool FUSE_X, int OUT, bool ALL3>
+__global__ void __launch_bounds__(RW_THREADS, 1)
+rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__ w_hh, const float *__restrict__ b_hn,
+              void *__restrict__ h_out, int64_t B, int64_t T, const __half *__restrict__ lin_w_tc,
+              float *__restrict__ plog, uint32_t prod_mask_rt) {
+    const uint32_t prod_mask = ALL3 ? 7u : prod_mask_rt;
+    using L = RwCfg<NT, FUSE_X, OUT>;
+    constexpr int N = L::N, NA = N / 2;             // accumulator values per thread and gate
+    using MMA = Wgmma<N>;
+    constexpr bool LOGITS = OUT == OUT_LOGITS;
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
+    const int gq = lane >> 2, cq = lane & 3;
+    const int dir = blockIdx.y;
+    const int64_t ntiles = (B + RT_N - 1) / RT_N;
+    const int64_t wtile0 = (int64_t)blockIdx.x * NT;
+    const int j0 = wg * 64 + warp * 16 + gq;        // this thread's hidden units: j0 and j0 + 8
+    const uint32_t sbase = smem_u32(smem);
+
+    // ---- prologue: zero the activation tiles, weights into shared memory and registers ----
+    for (int i = tid; i < (L::total - L::h_off) / 16; i += RW_THREADS)
+        reinterpret_cast<int4 *>(smem + L::h_off)[i] = make_int4(0, 0, 0, 0);
+    for (int i = tid; i < 3 * H * (H / 8); i += RW_THREADS) {
+        const int kg = i & 15, r = (i >> 4) & (H - 1), gate = i >> 11;
+        const uint4 v = *reinterpret_cast<const uint4 *>(w_hh + ((((size_t)dir * 2 + 1) * 3 + gate) * H + r) * H + kg * 8);
+        *reinterpret_cast<uint4 *>(smem + L::wlo_off + (gate * 2 + (r >> 6)) * RW_ABLK + kg * 1024 + (r & 63) * 16) = v;
+    }
+    if (FUSE_X) {
+        for (int i = tid; i < 3 * H * 2; i += RW_THREADS) {
+            const int kg = i & 1, r = (i >> 1) & (H - 1), gate = i >> 8;
+            const uint4 v = *reinterpret_cast<const uint4 *>(xin.w_x + ((((size_t)dir * 2 + 1) * 3 + gate) * H + r) * 16 + kg * 8);
+            *reinterpret_cast<uint4 *>(smem + L::wxlo_off + (gate * 2 + (r >> 6)) * RW_XBLK + kg * 1024 + (r & 63) * 16) = v;
+        }
+    }
+    if (LOGITS) {   // this direction's half of W_lin, already in operand layout [plane][kg][row 64][8]
+        const int4 *src = reinterpret_cast<const int4 *>(lin_w_tc + (size_t)dir * 2 * (RW_WL_PLANE / 2));
+        for (int i = tid; i < 2 * RW_WL_PLANE / 16; i += RW_THREADS) reinterpret_cast<int4 *>(smem + L::wl_off)[i] = src[i];
+    }
+    uint32_t whi[3][H / 16][4];
+#pragma unroll
+    for (int gate = 0; gate < 3; ++gate)
+#pragma unroll
+        for (int ks = 0; ks < H / 16; ++ks) {
+            const __half *w = w_hh + ((((size_t)dir * 2) * 3 + gate) * H + j0) * H + ks * 16 + 2 * cq;
+            whi[gate][ks][0] = ld_u32(w);
+            whi[gate][ks][1] = ld_u32(w + 8 * H);
+            whi[gate][ks][2] = ld_u32(w + 8);
+            whi[gate][ks][3] = ld_u32(w + 8 * H + 8);
+        }
+    uint32_t wxhi[3][4];
+    float bx[3][2] = {};                            // FUSE_X: folded biases of r, z and the input part of n
+    if (FUSE_X) {
+#pragma unroll
+        for (int gate = 0; gate < 3; ++gate) {
+            const __half *w = xin.w_x + ((((size_t)dir * 2) * 3 + gate) * H + j0) * 16 + 2 * cq;
+            wxhi[gate][0] = ld_u32(w);
+            wxhi[gate][1] = ld_u32(w + 8 * 16);
+            wxhi[gate][2] = ld_u32(w + 8);
+            wxhi[gate][3] = ld_u32(w + 8 * 16 + 8);
+            bx[gate][0] = xin.bias[dir * G3 + gate * H + j0];
+            bx[gate][1] = xin.bias[dir * G3 + gate * H + j0 + 8];
+        }
+    }
+    const float bhn[2] = {b_hn[dir * H + j0], b_hn[dir * H + j0 + 8]};
+
+    // Accumulator element k = 4i + 2hb + e: hidden unit j0 + 8hb, window n = 8i + 2cq + e of tile wtile0 + i/2.
+    float ar[NA], az[NA], an[NA], axn[NA], hp[NA], alg[NA];
+#pragma unroll
+    for (int k = 0; k < NA; ++k) hp[k] = 0.f;
+    // pre-activations of time t into the accumulators (gi in quad layout, common.cuh: the pair e = 0, 1 is contiguous)
+    auto load_pre = [&](int64_t t) {
+#pragma unroll
+        for (int i = 0; i < N / 8; ++i)
+#pragma unroll
+            for (int hb = 0; hb < 2; ++hb) {
+                float2 v[3] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
+                if (FUSE_X) {
+#pragma unroll
+                    for (int gate = 0; gate < 3; ++gate) v[gate] = make_float2(bx[gate][hb], bx[gate][hb]);
+                } else if (wtile0 + (i >> 1) < ntiles) {
+                    const float *p = gi + ((wtile0 + (i >> 1)) * T + t) * GI_TS_FLOATS +
+                                     (((dir * 3) * 4 + 2 * (i & 1) + (cq >> 1)) * H + j0 + 8 * hb) * 4 + 2 * (cq & 1);
+#pragma unroll
+                    for (int gate = 0; gate < 3; ++gate) v[gate] = __ldcs(reinterpret_cast<const float2 *>(p + gate * 16 * H));
+                }
+                const int k = 4 * i + 2 * hb;
+                ar[k] = v[0].x; ar[k + 1] = v[0].y;
+                az[k] = v[1].x; az[k + 1] = v[1].y;
+                axn[k] = v[2].x; axn[k + 1] = v[2].y;
+                an[k] = bhn[hb]; an[k + 1] = bhn[hb];
+            }
+    };
+    // FUSE_X: x_t staged as the B tile [plane][kg 2][n][8]; thread entry q = tid + 256 m covers (window q / F, feature q % F)
+    const int xF = FUSE_X ? xin.F : 1;
+    const float *xsrc[NT];
+    int xoff[NT];
+    float xreg[NT];
+#pragma unroll
+    for (int m = 0; m < NT; ++m) {
+        const int q = tid + RW_THREADS * m, xn = q / xF, xf = q - xn * xF;
+        const bool own = FUSE_X && q < N * xF;
+        xoff[m] = own ? (xf >> 3) * L::KG + xn * 16 + (xf & 7) * 2 : -1;
+        xsrc[m] = (own && wtile0 * RT_N + xn < B) ? xin.feats + ((wtile0 * RT_N + xn) * T) * xF + xf : nullptr;
+        xreg[m] = 0.f;
+    }
+    auto stage_x = [&](int buf, int m, float v) {
+        __half hi, lo;
+        split_f16(v, hi, lo);
+        *reinterpret_cast<__half *>(smem + L::x_off + buf * 2 * L::XPLANE + xoff[m]) = hi;
+        *reinterpret_cast<__half *>(smem + L::x_off + buf * 2 * L::XPLANE + L::XPLANE + xoff[m]) = lo;
+    };
+    const int64_t t_first = dir ? T - 1 : 0;
+    if (FUSE_X) {
+#pragma unroll
+        for (int m = 0; m < NT; ++m) {
+            if (xoff[m] < 0) continue;
+            stage_x(0, m, xsrc[m] ? xsrc[m][t_first * xF] : 0.f);
+            if (xsrc[m] && T > 1) xreg[m] = xsrc[m][(dir ? T - 2 : 1) * xF];
+        }
+    }
+    load_pre(t_first);
+    fence_proxy_async_smem();   // generic-proxy writes above (weights, zeroed tiles, x_0) -> visible to wgmma reads
+    __syncthreads();            // h_{-1} = 0, x_0 and the weights are in shared memory
+
+    // logits of h in buffer `buf` (warpgroup 0): class c = row gq of warp 0, c < 5
+    auto issue_logits = [&](int buf) {
+        const uint32_t hb_addr = sbase + L::h_off + buf * 2 * L::HPLANE;
+#pragma unroll
+        for (int ks = 0; ks < H / 16; ++ks) {
+            const uint64_t bh = make_smem_desc(hb_addr + ks * 2 * L::KG, L::KG, 128);
+            const uint64_t bl = make_smem_desc(hb_addr + L::HPLANE + ks * 2 * L::KG, L::KG, 128);
+            const uint64_t wh = make_smem_desc(sbase + L::wl_off + ks * 2 * 1024, 1024, 128);
+            const uint64_t wl = make_smem_desc(sbase + L::wl_off + RW_WL_PLANE + ks * 2 * 1024, 1024, 128);
+            MMA::ss(alg, wh, bh, ks ? 1u : 0u);
+            if (prod_mask & 2u) MMA::ss(alg, wh, bl, 1u);
+            if (prod_mask & 4u) MMA::ss(alg, wl, bh, 1u);
+        }
+    };
+    auto store_logits = [&](int64_t t) {
+        if (warp != 0 || gq >= NCLS) return;
+#pragma unroll
+        for (int k = 0; k < NA; ++k) {
+            if ((k >> 1) & 1) continue;             // rows 8..15 are padding
+            const int i = k >> 2, n = 8 * i + 2 * cq + (k & 1);
+            const int64_t wt = wtile0 + (i >> 1);
+            if (wt < ntiles) plog[((dir * ntiles + wt) * T + t) * PLOG_TS_FLOATS + gq * RT_N + (n & 15)] = alg[k];
+        }
+    };
+
+#pragma unroll 1
+    for (int64_t step = 0; step < T; ++step) {
+        const int64_t t = dir ? T - 1 - step : step;
+        const int buf = (int)(step & 1);
+        const uint32_t hb_addr = sbase + L::h_off + buf * 2 * L::HPLANE;
+        wg_fence();
+#pragma unroll
+        for (int gate = 0; gate < 3; ++gate) {
+            float(&acc)[NA] = gate == 0 ? ar : (gate == 1 ? az : an);
+#pragma unroll
+            for (int ks = 0; ks < H / 16; ++ks) {
+                const uint64_t bh = make_smem_desc(hb_addr + ks * 2 * L::KG, L::KG, 128);
+                MMA::rs(acc, whi[gate][ks], bh, 1u);
+                if (prod_mask & 2u) MMA::rs(acc, whi[gate][ks], make_smem_desc(hb_addr + L::HPLANE + ks * 2 * L::KG, L::KG, 128), 1u);
+                if (prod_mask & 4u)
+                    MMA::ss(acc, make_smem_desc(sbase + L::wlo_off + (gate * 2 + wg) * RW_ABLK + ks * 2 * 1024, 1024, 128), bh, 1u);
+            }
+        }
+        if (FUSE_X) {
+            const uint32_t xa = sbase + L::x_off + buf * 2 * L::XPLANE;
+            const uint64_t bh = make_smem_desc(xa, L::KG, 128), bl = make_smem_desc(xa + L::XPLANE, L::KG, 128);
+#pragma unroll
+            for (int gate = 0; gate < 3; ++gate) {
+                float(&acc)[NA] = gate == 0 ? ar : (gate == 1 ? az : axn);
+                MMA::rs(acc, wxhi[gate], bh, 1u);
+                if (prod_mask & 2u) MMA::rs(acc, wxhi[gate], bl, 1u);
+                if (prod_mask & 4u) MMA::ss(acc, make_smem_desc(sbase + L::wxlo_off + (gate * 2 + wg) * RW_XBLK, 1024, 128), bh, 1u);
+            }
+        }
+        // the tile holds h of the previous step (zeros at step 0: not stored).  Both warpgroups issue the same chain and
+        // only warpgroup 0 stores: issued under a warpgroup-dependent branch, ptxas serialises every wgmma of the kernel
+        if (LOGITS) issue_logits(buf);
+        wg_commit();
+        // the next step's L2 prefetch and feature loads run under the MMAs
+        if (!FUSE_X && tid == 0 && step + GI_PREFETCH_STEPS < T) {
+            const int64_t tp = dir ? t - GI_PREFETCH_STEPS : t + GI_PREFETCH_STEPS;
+#pragma unroll
+            for (int m = 0; m < NT; ++m) {
+                if (wtile0 + m >= ntiles) break;
+                const float *blk = gi + ((wtile0 + m) * T + tp) * GI_TS_FLOATS + (int64_t)dir * (GI_TS_FLOATS / 2);
+#pragma unroll
+                for (int i = 0; i < 12; ++i) bulk_prefetch_l2(blk + i * 512, 2048);
+            }
+        }
+        wg_wait_all();
+        wg_hold(ar); wg_hold(az); wg_hold(an); wg_hold(axn);
+        if (LOGITS) wg_hold(alg);
+
+        // ---- gate math (weights and biases carry the exp2 scale factors, common.cuh gate_scale) ----
+        uint8_t *hw = smem + L::h_off + (buf ^ 1) * 2 * L::HPLANE;
+#pragma unroll
+        for (int k = 0; k < NA; ++k) {
+            const float r = rcp_approx(1.f + ex2_approx(fminf(ar[k], EXP_CLAMP)));
+            const float z = rcp_approx(1.f + ex2_approx(fminf(az[k], EXP_CLAMP)));
+            const float en = ex2_approx(fminf(fmaf(r, an[k], axn[k]), EXP_CLAMP));
+            const float n = (en - 1.f) * rcp_approx(en + 1.f);
+            hp[k] = fmaf(z, hp[k] - n, n);
+            const int j = j0 + 8 * ((k >> 1) & 1), col = 8 * (k >> 2) + 2 * cq + (k & 1);
+            __half hi, lo;
+            split_f16(hp[k], hi, lo);
+            *reinterpret_cast<__half *>(hw + (j >> 3) * L::KG + col * 16 + (j & 7) * 2) = hi;
+            *reinterpret_cast<__half *>(hw + L::HPLANE + (j >> 3) * L::KG + col * 16 + (j & 7) * 2) = lo;
+        }
+        if (FUSE_X && step + 1 < T) {
+#pragma unroll
+            for (int m = 0; m < NT; ++m) {
+                if (xoff[m] < 0) continue;
+                stage_x(buf ^ 1, m, xreg[m]);
+                if (xsrc[m] && step + 2 < T) xreg[m] = xsrc[m][(dir ? t - 2 : t + 2) * xF];
+            }
+        }
+        // ---- outputs of this step ----
+        if (LOGITS) {
+            if (wg == 0 && step > 0) store_logits(dir ? t + 1 : t - 1);
+        } else {
+#pragma unroll
+            for (int k = 0; k < NA; ++k) {
+                const int i = k >> 2, n = 8 * i + 2 * cq + (k & 1);
+                const int64_t wt = wtile0 + (i >> 1);
+                if (wt >= ntiles) continue;
+                const int64_t orow = (wt * T + t) * RT_N + (n & 15);
+                const int kcol = dir * H + j0 + 8 * ((k >> 1) & 1);
+                if (OUT == OUT_TILES) {
+                    __half hi, lo;
+                    split_f16(hp[k], hi, lo);
+                    __half *o = reinterpret_cast<__half *>(reinterpret_cast<uint8_t *>(h_out) + (orow >> 7) * (int64_t)XT_TILE_BYTES +
+                                                           (kcol >> 3) * (XT_ROWS * 16) + (orow & (XT_ROWS - 1)) * 16) + (kcol & 7);
+                    o[0] = hi;
+                    o[XT_PLANE_BYTES / 2] = lo;
+                } else {
+                    reinterpret_cast<float *>(h_out)[orow * H2 + kcol] = hp[k];
+                }
+            }
+        }
+        if (step + 1 < T) load_pre(dir ? t - 1 : t + 1);
+        fence_proxy_async_smem();     // h / x tile writes -> visible to the next step's wgmma operand reads
+        __syncthreads();
+    }
+    if (LOGITS) {                     // h of the last step (made visible by the last barrier)
+        wg_fence();
+        issue_logits((int)(T & 1));
+        wg_commit();
+        wg_wait_all();
+        wg_hold(alg);
+        if (wg == 0) store_logits(dir ? 0 : T - 1);
+    }
+}
+
+bool rec_tc_can_fuse_logits(int64_t B, int sm_count) {
+    const int64_t tiles = (B + RT_N - 1) / RT_N;
+    return tiles > 0 && tiles * NDIR <= (int64_t)sm_count;      // one tile per CTA (NT == 1)
+}
+
+template <int NT, bool FX, int OUT>
+static cudaError_t launch_rec(const float *gi, const RecX &xin, const __half *w_hh_tm, const float *b_hn, void *h_out,
+                              int64_t B, int64_t T, cudaStream_t s, const __half *lin_w_tc, float *plog, uint32_t prod_mask) {
+    prod_mask = (prod_mask & 7u) | 1u;
+    auto kern = prod_mask == 7u ? rec_tc_kernel<NT, FX, OUT, true> : rec_tc_kernel<NT, FX, OUT, false>;
+    constexpr int smem_bytes = RwCfg<NT, FX, OUT>::total;
+    // (the attribute is per device: set it on every launch, a process may drive several GPUs)
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
+    if (e != cudaSuccess) return e;
+    const int64_t tiles = (B + RT_N - 1) / RT_N;
+    dim3 grid((unsigned)((tiles + NT - 1) / NT), NDIR);
+    kern<<<grid, RW_THREADS, smem_bytes, s>>>(gi, xin, w_hh_tm, b_hn, h_out, B, T, lin_w_tc, plog, prod_mask);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_rec_tc(const float *gi, const RecXArgs *fuse, const __half *w_hh_tm, const float *b_hn,
+                          void *h_out, int out_tiles, int64_t B, int64_t T, int sm_count, cudaStream_t s,
+                          const __half *lin_w_tc, float *plog, uint32_t prod_mask) {
+    if (B == 0 || T == 0) return cudaSuccess;
+    const int64_t tiles = (B + RT_N - 1) / RT_N;
+    // two tiles per CTA only once there are more tiles than SMs to run them one per CTA
+    const bool two = tiles * NDIR > (int64_t)sm_count;
+    RecX xin{nullptr, nullptr, nullptr, 0};
+    if (fuse) xin = RecX{fuse->feats, fuse->w_x, fuse->bias, fuse->F};
+    if (lin_w_tc) {
+        // layer 1 with the linear head fused in (partial logits instead of h1)
+        if (fuse || out_tiles || two || !plog) return cudaErrorInvalidValue;
+        return launch_rec<1, false, OUT_LOGITS>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, lin_w_tc, plog, prod_mask);
+    }
+    if (fuse) {
+        if (!out_tiles) return cudaErrorInvalidValue;   // the fused projection is layer 0, which feeds the GEMM
+        return two ? launch_rec<2, true, OUT_TILES>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, nullptr, nullptr, prod_mask)
+                   : launch_rec<1, true, OUT_TILES>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, nullptr, nullptr, prod_mask);
+    }
+    if (two)
+        return out_tiles ? launch_rec<2, false, OUT_TILES>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, nullptr, nullptr, prod_mask)
+                         : launch_rec<2, false, OUT_ROWS>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, nullptr, nullptr, prod_mask);
+    return out_tiles ? launch_rec<1, false, OUT_TILES>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, nullptr, nullptr, prod_mask)
+                     : launch_rec<1, false, OUT_ROWS>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, nullptr, nullptr, prod_mask);
+}
+
+cudaError_t launch_rec_pp(int layer, const float *gi, const RecXArgs *fuse, const __half *w_hh_tm, const float *b_hn,
+                          void *h_out, int64_t B, int64_t T, cudaStream_t s, const __half *lin_w_tc, float *plog,
+                          uint32_t prod_mask) {
+    if (B == 0 || T == 0) return cudaSuccess;
+    RecX xin{nullptr, nullptr, nullptr, 0};
+    if (fuse) xin = RecX{fuse->feats, fuse->w_x, fuse->bias, fuse->F};
+    if (layer == 0)
+        return fuse ? launch_rec<2, true, OUT_TILES>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, nullptr, nullptr, prod_mask)
+                    : launch_rec<2, false, OUT_TILES>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, nullptr, nullptr, prod_mask);
+    if (fuse || !lin_w_tc || !plog) return cudaErrorInvalidValue;
+    return launch_rec<2, false, OUT_LOGITS>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, lin_w_tc, plog, prod_mask);
+}
+
+// =====================================================================================================
+// Layer-1 input projection on tensor cores:  gi[p][blk*128 + j] = sum_k W_ih[blk*128 + j][k] * x[p][k] + bias
+// Persistent: grid = 6 weight blocks x CT CTAs; each CTA keeps its 128x256 weight block (hi+lo, 128 KiB) resident in
+// shared memory and streams 128-position activation tiles (written by the layer-0 recurrent kernel directly in operand
+// layout) through a 2-stage ring of 64-wide K slices, filled by bulk async copies (TMA engine) behind an mbarrier.
+// Each warpgroup computes 64 gate rows x 128 positions with M64 N128 K16 wgmmas.
+// =====================================================================================================
+constexpr int GW_THREADS = 256;
+constexpr int GW_QK = 8;                                        // k-groups per stage (K = 64)
+constexpr int GW_STAGE_PLANE = GW_QK * XT_ROWS * 16;            // 16 KiB
+constexpr int GW_STAGE = 2 * GW_STAGE_PLANE;                    // hi + lo
+constexpr int GW_NQ = XT_K / 8 / GW_QK;                         // stages per tile
+constexpr int GW_X_OFF = XT_TILE_BYTES;                         // behind the weight block
+constexpr int GW_BAR_OFF = GW_X_OFF + 2 * GW_STAGE;
+constexpr int GW_SMEM = GW_BAR_OFF + 16;
+
+template <bool ALL3>   // as in rec_tc_kernel: the full product set known at compile time
+__global__ void __launch_bounds__(GW_THREADS, 1)
+gemm_tc_kernel(const uint8_t *__restrict__ x_tiles, const __half *__restrict__ w_in_tm, const float *__restrict__ bias,
+               float *__restrict__ gi, int64_t P, int64_t ntiles, uint32_t prod_mask_rt) {
+    const uint32_t prod_mask = ALL3 ? 7u : prod_mask_rt;
+    extern __shared__ __align__(128) uint8_t smem[];
+    uint64_t *full = reinterpret_cast<uint64_t *>(smem + GW_BAR_OFF);
+    const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
+    const int gq = lane >> 2, cq = lane & 3;
+    const int blk = blockIdx.x;                 // weight block: dir*3 + gate
+    const uint32_t sbase = smem_u32(smem);
+    // weights (row-major fp16 [blk][plane][row j][k 256]) -> [plane][kg 32][row 128][8]
+    for (int i = tid; i < 2 * H * (H2 / 8); i += GW_THREADS) {
+        const int kg = i & 31, r = (i >> 5) & (H - 1), p = i >> 12;
+        const uint4 v = reinterpret_cast<const uint4 *>(w_in_tm + (((size_t)blk * 2 + p) * H + r) * H2)[kg];
+        *reinterpret_cast<uint4 *>(smem + p * XT_PLANE_BYTES + kg * (XT_ROWS * 16) + r * 16) = v;
+    }
+    if (tid == 0) {
+        mbar_init(&full[0], 1);
+        mbar_init(&full[1], 1);
+        fence_mbar_init();
+    }
+    fence_proxy_async_smem();   // the weight block's generic-proxy stores -> visible to wgmma reads
+    __syncthreads();
+    const int64_t my_tiles = blockIdx.y < ntiles ? (ntiles - 1 - blockIdx.y) / gridDim.y + 1 : 0;
+    const int64_t nst = my_tiles * GW_NQ;
+    auto issue = [&](int64_t it) {
+        const int64_t tile = blockIdx.y + (it / GW_NQ) * gridDim.y;
+        const int q = (int)(it % GW_NQ), s = (int)(it & 1);
+        const uint8_t *src = x_tiles + tile * (int64_t)XT_TILE_BYTES + q * GW_STAGE_PLANE;
+        mbar_arrive_expect_tx(&full[s], GW_STAGE);
+        bulk_g2s(smem + GW_X_OFF + s * GW_STAGE, src, GW_STAGE_PLANE, &full[s]);
+        bulk_g2s(smem + GW_X_OFF + s * GW_STAGE + GW_STAGE_PLANE, src + XT_PLANE_BYTES, GW_STAGE_PLANE, &full[s]);
+    };
+    if (tid == 0) {
+        if (nst > 0) issue(0);
+        if (nst > 1) issue(1);
+    }
+    const float bj[2] = {bias[blk * H + wg * 64 + warp * 16 + gq], bias[blk * H + wg * 64 + warp * 16 + gq + 8]};
+    float acc[64];
+#pragma unroll 1
+    for (int64_t it = 0; it < nst; ++it) {
+        const int q = (int)(it % GW_NQ), s = (int)(it & 1);
+        mbar_wait(&full[s], (uint32_t)((it >> 1) & 1));
+        wg_fence();
+#pragma unroll
+        for (int prod = 0; prod < 3; ++prod) {
+            if (prod && !(prod_mask & (1u << prod))) continue;
+            const int pa = prod == 2, pb = prod == 1;   // W part hi, hi, lo ; x part hi, lo, hi
+#pragma unroll
+            for (int kk = 0; kk < GW_QK / 2; ++kk) {
+                const uint64_t a = make_smem_desc(sbase + pa * XT_PLANE_BYTES + (q * GW_QK + 2 * kk) * (XT_ROWS * 16) + wg * 64 * 16,
+                                                  XT_ROWS * 16, 128);
+                const uint64_t b = make_smem_desc(sbase + GW_X_OFF + s * GW_STAGE + pb * GW_STAGE_PLANE + 2 * kk * (XT_ROWS * 16),
+                                                  XT_ROWS * 16, 128);
+                Wgmma<128>::ss(acc, a, b, (q | prod | kk) ? 1u : 0u);
+            }
+        }
+        wg_commit();
+        wg_wait_all();
+        wg_hold(acc);
+        __syncthreads();                          // both warpgroups have read stage s
+        if (tid == 0 && it + 2 < nst) issue(it + 2);
+        if (q == GW_NQ - 1) {
+            // quad layout (common.cuh): position c of this tile = tile-step tile*8 + c/16, window c%16
+            const int64_t tile = blockIdx.y + (it / GW_NQ) * gridDim.y;
+            const int64_t prem = P - tile * XT_ROWS;   // rows of this tile that exist (a multiple of 16)
+#pragma unroll
+            for (int k = 0; k < 64; k += 2) {
+                const int c = 8 * (k >> 2) + 2 * cq, hb = (k >> 1) & 1;
+                if (c >= prem) continue;
+                const int j = wg * 64 + warp * 16 + gq + 8 * hb;
+                float *o = gi + ((((tile * (XT_ROWS / WT) + (c >> 4)) * 6 + blk) * 4 + ((c & 15) >> 2)) * H + j) * 4 + (c & 3);
+                __stcs(reinterpret_cast<float2 *>(o), make_float2(acc[k] + bj[hb], acc[k + 1] + bj[hb]));
+            }
+        }
+    }
+}
+
+cudaError_t launch_gemm_tc(const void *x_tiles, const __half *w_in_tm, const float *bias, float *gi, int64_t P,
+                           int sm_count, cudaStream_t s, uint32_t prod_mask) {
+    if (P == 0) return cudaSuccess;
+    const int64_t ntiles = (P + XT_ROWS - 1) / XT_ROWS;
+    prod_mask = (prod_mask & 7u) | 1u;
+    auto kern = prod_mask == 7u ? gemm_tc_kernel<true> : gemm_tc_kernel<false>;
+    cudaError_t ea = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GW_SMEM);
+    if (ea != cudaSuccess) return ea;
+    int64_t ct = sm_count / 6;
+    if (ct < 1) ct = 1;
+    if (ct > ntiles) ct = ntiles;
+    dim3 grid(6, (unsigned)ct);
+    kern<<<grid, GW_THREADS, GW_SMEM, s>>>(reinterpret_cast<const uint8_t *>(x_tiles), w_in_tm, bias, gi, P, ntiles,
+                                           prod_mask);
+    return cudaGetLastError();
+}
+
+// =====================================================================================================
+// Self test of the wgmma building block: D[128][N] = A[128][K] . B[N][K]^T, fp16 hi/lo split, one CTA of two
+// warpgroups (64 rows each), N in 16-column slices, both operands from shared memory in the production layout.
+// =====================================================================================================
+__global__ void __launch_bounds__(256, 1)
+selftest_kernel(const float *__restrict__ A, const float *__restrict__ Bm, float *__restrict__ D, int N, int K) {
+    extern __shared__ __align__(128) uint8_t smem[];
+    const int a_plane = 128 * K * 2, b_plane = N * K * 2;
+    uint8_t *sa = smem, *sb = smem + 2 * a_plane;
+    const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
+    for (int i = tid; i < 128 * K; i += 256) {
+        const int r = i / K, k = i % K;
+        __half hi, lo;
+        split_f16(A[i], hi, lo);
+        const int off = (k / 8) * (128 * 16) + r * 16 + (k % 8) * 2;
+        *reinterpret_cast<__half *>(sa + off) = hi;
+        *reinterpret_cast<__half *>(sa + a_plane + off) = lo;
+    }
+    for (int i = tid; i < N * K; i += 256) {
+        const int r = i / K, k = i % K;
+        __half hi, lo;
+        split_f16(Bm[i], hi, lo);
+        const int off = (k / 8) * (N * 16) + r * 16 + (k % 8) * 2;
+        *reinterpret_cast<__half *>(sb + off) = hi;
+        *reinterpret_cast<__half *>(sb + b_plane + off) = lo;
+    }
+    fence_proxy_async_smem();
+    __syncthreads();
+    for (int n0 = 0; n0 < N; n0 += 16) {
+        float d[8];
+        wg_fence();
+        uint32_t acc = 0;
+        for (int prod = 0; prod < 3; ++prod) {
+            const int pa = (prod == 2), pb = (prod == 1);
+            for (int ks = 0; ks < K / 16; ++ks) {
+                const uint64_t ad = make_smem_desc(smem_u32(sa + pa * a_plane) + ks * 2 * 128 * 16 + wg * 64 * 16, 128 * 16, 128);
+                const uint64_t bd = make_smem_desc(smem_u32(sb + pb * b_plane) + ks * 2 * N * 16 + n0 * 16, N * 16, 128);
+                Wgmma<16>::ss(d, ad, bd, acc);
+                acc = 1;
+            }
+        }
+        wg_commit();
+        wg_wait_all();
+        wg_hold(d);
+        const int row = wg * 64 + warp * 16 + (lane >> 2);
+        for (int k = 0; k < 8; ++k)
+            D[(row + 8 * ((k >> 1) & 1)) * N + n0 + 8 * (k >> 2) + 2 * (lane & 3) + (k & 1)] = d[k];
+    }
+}
+
+int selftest_umma(int device, const float *A, const float *B, float *D, int N, int K, int variant) {
+    MDK_REQUIRE(N >= 16 && N <= 128 && N % 16 == 0, MDK_ERR_ARG, "selftest_umma: N must be a multiple of 16 in [16,128]");
+    MDK_REQUIRE(K >= 16 && K <= 256 && K % 16 == 0, MDK_ERR_ARG, "selftest_umma: K must be a multiple of 16 in [16,256]");
+    MDK_REQUIRE(variant == 0, MDK_ERR_ARG, "selftest_umma: variant must be 0");
+    MDK_CUDA(cudaSetDevice(device));
+    float *dA = nullptr, *dB = nullptr, *dD = nullptr;
+    MDK_CUDA(cudaMalloc(&dA, sizeof(float) * 128 * K));
+    MDK_CUDA(cudaMalloc(&dB, sizeof(float) * N * K));
+    MDK_CUDA(cudaMalloc(&dD, sizeof(float) * 128 * N));
+    MDK_CUDA(cudaMemcpy(dA, A, sizeof(float) * 128 * K, cudaMemcpyHostToDevice));
+    MDK_CUDA(cudaMemcpy(dB, B, sizeof(float) * N * K, cudaMemcpyHostToDevice));
+    const int smem = 2 * 128 * K * 2 + 2 * N * K * 2;
+    MDK_REQUIRE(smem <= 227 * 1024, MDK_ERR_ARG, "selftest_umma: N*K too large for shared memory");
+    MDK_CUDA(cudaFuncSetAttribute(selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    selftest_kernel<<<1, 256, smem>>>(dA, dB, dD, N, K);
+    MDK_CUDA(cudaGetLastError());
+    MDK_CUDA(cudaDeviceSynchronize());
+    MDK_CUDA(cudaMemcpy(D, dD, sizeof(float) * 128 * N, cudaMemcpyDeviceToHost));
+    cudaFree(dA); cudaFree(dB); cudaFree(dD);
+    return MDK_OK;
+}
+
+}  // namespace mdk

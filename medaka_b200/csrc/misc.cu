@@ -453,7 +453,7 @@ cudaError_t launch_head(const float *h1, const float *lin_w, const float *lin_b,
     const int64_t P = B * T;
     if (P == 0) return cudaSuccess;
     int64_t blocks = (P + 31) / 32;            // 8 warps per block, 4 positions per warp per iteration
-    if (blocks > 148 * 8) blocks = 148 * 8;    // persistent-ish grid: multiple of the SM count
+    if (blocks > 132 * 8) blocks = 132 * 8;    // persistent-ish grid: multiple of the SM count
     head_kernel<<<(unsigned)blocks, 256, 0, s>>>(h1, lin_w, lin_b, P, B, T, tiled, probs, logits, labels);
     return cudaGetLastError();
 }
@@ -546,12 +546,6 @@ __global__ void pack_linear_kernel(const float *__restrict__ lin_w, __half *__re
     const int plane = 16 * 64 * 8;
     out[(d * 2 + 0) * plane + (i & (plane - 1))] = hi;
     out[(d * 2 + 1) * plane + (i & (plane - 1))] = lo;
-    // second part of the buffer: the hi plane once more, row-major [dir][row 128][k 128] (rows >= 5 zero): source of the
-    // TMEM-resident A operand of the hi x hi and hi x lo products (M = 128, like W_hh)
-    __half *rm = out + NDIR * 2 * plane;
-    const int k = kg * 8 + k8;
-    rm[(d * H + row) * H + k] = hi;
-    rm[(d * H + row + 64) * H + k] = __float2half_rn(0.f);
 }
 
 cudaError_t launch_pack_linear(const float *lin_w, __half *lin_w_tc, cudaStream_t s) {

@@ -1,6 +1,5 @@
-// Inline-PTX wrappers for sm_100a: mbarrier, tcgen05 (MMA / TMEM / commit), bulk async copies.
-// Hand-written; field layouts follow the PTX ISA "tcgen05" chapter (cross-checked against the
-// CUTLASS headers vendored in this image, cute/arch/mma_sm100_desc.hpp).
+// Inline-PTX wrappers for sm_90a: mbarrier, wgmma (warpgroup MMA), bulk async copies.
+// Hand-written; field layouts follow the PTX ISA "wgmma" chapter (matrix descriptor format).
 #pragma once
 #include <cstdint>
 #include <cuda_fp16.h>
@@ -15,12 +14,9 @@ __device__ __forceinline__ uint32_t smem_u32(const void *p) {
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }
-// make mbarrier.init visible to the async proxy (TMA / tcgen05.commit)
+// make mbarrier.init visible to the async proxy (bulk copies)
 __device__ __forceinline__ void fence_mbar_init() {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t *bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
@@ -38,63 +34,17 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t *bar, uint32_t parity) {
     return ok != 0;
 }
 // Bounded wait: a protocol bug must surface as a trapped kernel (an error code on the host),
-// never as a hung GPU.  ~4e9 SM cycles is > 2 s, far beyond any legitimate wait here.
+// never as a hung GPU.  ~4e9 SM cycles is > 2 s, far beyond any legitimate wait here.  No printf: a function call
+// inside a loop that issues wgmma makes ptxas serialise the MMAs (warning C7510).
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
     if (mbar_try_wait(bar, parity)) return;
     const long long t0 = clock64();
     while (!mbar_try_wait(bar, parity)) {
-        if (clock64() - t0 > 4000000000LL) {
-            printf("mdk: mbarrier wait timed out (block %d thread %d parity %u)\n", blockIdx.x, threadIdx.x,
-                   parity);
-            __trap();
-        }
+        if (clock64() - t0 > 4000000000LL) __trap();
     }
 }
 
-// Named hardware barriers (ids 1..15; 0 is __syncthreads).  `count` = number of THREADS that take part (multiple of 32);
-// executed by whole warps.  bar.arrive + bar.sync is the PTX producer/consumer pattern: the arriving threads' earlier
-// shared-memory writes are visible to the threads that complete the barrier with bar.sync.  A warp-level arrival is one
-// instruction on the barrier unit, where an mbarrier arrival / try_wait is one SYNCS lane-op per thread.
-template <int ID, int COUNT>
-__device__ __forceinline__ void named_bar_sync() {
-    asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(COUNT) : "memory");
-}
-template <int ID, int COUNT>
-__device__ __forceinline__ void named_bar_arrive() {
-    asm volatile("bar.arrive %0, %1;" ::"n"(ID), "n"(COUNT) : "memory");
-}
-
-// same with the barrier id in a register (the two tiles of rec_pp_kernel run ONE copy of the code: template-per-tile
-// copies doubled the hot instruction footprint of the kernel)
-template <int COUNT>
-__device__ __forceinline__ void named_bar_sync_id(int id) {
-    asm volatile("bar.sync %0, %1;" ::"r"(id), "n"(COUNT) : "memory");
-}
-template <int COUNT>
-__device__ __forceinline__ void named_bar_arrive_id(int id) {
-    asm volatile("bar.arrive %0, %1;" ::"r"(id), "n"(COUNT) : "memory");
-}
-
-// one lane of the (converged) warp; the compiler keeps operands of code under this predicate in uniform registers
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "elect.sync _|p, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(pred));
-    return pred != 0;
-}
-
-// Whole-warp wait with ONE polling lane: mbarrier.try_wait is one lane-op per thread on the barrier unit, so 16 warps of
-// 32 pollers are released one after the other when the phase flips; one lane per warp + __syncwarp keeps the unit's
-// queue 32x shorter.  (The other lanes get their acquire through the __syncwarp.)
-__device__ __forceinline__ void mbar_wait_warp(uint64_t *bar, uint32_t parity) {
-    if (elect_one()) mbar_wait(bar, parity);
-    __syncwarp();
-}
-
-// generic-proxy smem writes -> visible to the async proxy (tcgen05.mma operand reads, bulk copies)
+// generic-proxy smem writes -> visible to the async proxy (wgmma operand reads, bulk copies)
 __device__ __forceinline__ void fence_proxy_async_smem() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -114,164 +64,86 @@ __device__ __forceinline__ void bulk_g2s(void *smem_dst, const void *gmem_src, u
         : "memory");
 }
 
-// shared -> global (bulk-group completion).  16-B aligned, size % 16 == 0.  The source must have been made visible to
-// the async proxy (fence.proxy.async by the writers + a barrier) before the issuing thread gets here.
-__device__ __forceinline__ void bulk_s2g(void *gmem_dst, const void *smem_src, uint32_t bytes) {
-    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gmem_dst), "r"(smem_u32(smem_src)),
-                 "r"(bytes)
-                 : "memory");
-}
-__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// all bulk groups of this thread have finished READING their shared-memory source (it may be overwritten)
-__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-// ... and have completed entirely
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
-// ---------------------------------------------------------------- tcgen05: TMEM management
-__device__ __forceinline__ void tmem_alloc(uint32_t *smem_result, uint32_t ncols) {  // whole warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {  // whole warp
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before_sync() {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after_sync() {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---------------------------------------------------------------- tcgen05: descriptors
+// ---------------------------------------------------------------- wgmma (warpgroup MMA, sm_90a)
 // Shared-memory matrix descriptor, K-major operand, no swizzle ("interleaved" core matrices):
 //   core matrix = 8 rows x 16 bytes, stored as 128 contiguous bytes (row r at +16*r);
 //   LBO = byte distance between core matrices adjacent along K,
 //   SBO = byte distance between core matrices adjacent along M/N (next 8 rows).
-// bits [0,14) addr>>4, [16,30) LBO>>4, [32,46) SBO>>4, [46,48) version=1, [61,64) layout type 0.
+// bits [0,14) addr>>4, [16,30) LBO>>4, [32,46) SBO>>4, [49,52) base offset 0, [62,64) layout type 0.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
     d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
     return d;
 }
-// Instruction descriptor for kind::f16, A/B = fp16 (format 0), D = fp32, both operands K-major.
-// bits [4,6) D fmt (1 = f32), [7,10) A fmt, [10,13) B fmt, [15] A major, [16] B major,
-// [17,23) N>>3, [24,29) M>>4.
-__host__ __device__ constexpr uint32_t make_idesc_f16(uint32_t M, uint32_t N) {
-    return (1u << 4) | (0u << 7) | (0u << 10) | (0u << 15) | (0u << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
+// ordering of register / shared-memory writes before the warpgroup's next wgmma (whole warpgroup)
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from touching an accumulator between the asynchronous MMA and wg_wait_all
+template <int R>
+__device__ __forceinline__ void wg_hold(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread.
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                         uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// Same with the A operand read from TENSOR MEMORY: a_tmem addresses 128 lanes (row m = lane m) x (K/2) 32-bit
-// columns, each cell holding the fp16 pair (k = 2c, 2c+1), low half = even k.  Removes the per-MMA 4 KiB
-// shared-memory read of a 128x16 A tile, which is what bounds small-N MMAs in SS mode.
-__device__ __forceinline__ void umma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// The same two instructions with the shared-memory descriptor passed as its two 32-bit halves.  Stepping through an
-// operand (next k-slice, other plane, other buffer) only changes the address field in the LOW word, so the issuing warp
-// does 32-bit adds - which the compiler keeps on the uniform datapath - instead of 64-bit vector arithmetic followed by
-// register-to-uniform moves for every MMA.
-__device__ __forceinline__ uint32_t smem_desc_lo(uint32_t smem_addr, uint32_t lbo_bytes) {
-    return ((smem_addr & 0x3FFFF) >> 4) | (((lbo_bytes >> 4) & 0x3FFF) << 16);
-}
-__device__ __forceinline__ uint32_t smem_desc_hi(uint32_t sbo_bytes) { return ((sbo_bytes >> 4) & 0x3FFF) | (1u << 14); }
-__device__ __forceinline__ void umma_f16_ts2(uint32_t d_tmem, uint32_t a_tmem, uint32_t b_lo, uint32_t b_hi, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 bd;\n\t"
-        "mov.b64 bd, {%2, %3};\n\t"
-        "setp.ne.b32 p, %5, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], bd, %4, p;\n\t}" ::"r"(d_tmem),
-        "r"(a_tmem), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_f16_ss2(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                             uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 ad, bd;\n\t"
-        "mov.b64 ad, {%1, %2};\n\t"
-        "mov.b64 bd, {%3, %4};\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], ad, bd, %5, p;\n\t}" ::"r"(d_tmem),
-        "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// registers -> TMEM, 32x32b: lane i of the warp writes 8 consecutive 32-bit columns of TMEM lane 32*(warp%4)+i
-__device__ __forceinline__ void tmem_st_x8(uint32_t taddr, const uint32_t (&r)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(r[0]),
-                 "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// arrive (count 1) on an mbarrier once all previously issued MMAs of this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                     smem_u32(bar))
-                 : "memory");
-}
-
-// ---------------------------------------------------------------- tcgen05: TMEM -> registers
-// 32x32b: lane i of the warp reads TMEM lane (32*(warp%4) + i), N consecutive 32-bit columns.
-// taddr = (lane << 16) | column.
-__device__ __forceinline__ void tmem_ld_x4(uint32_t taddr, uint32_t (&r)[4]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-                 : "r"(taddr)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld_x8(uint32_t taddr, uint32_t (&r)[8]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]),
-          "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]),
-          "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
+// D[64 x N] (+)= A[64 x 16] . B[N x 16]^T, fp16 in, fp32 accumulate; issued by all 128 threads of a warpgroup.
+// Accumulator fragment: warp w of the warpgroup, lane l holds rows 16w + l/4 (+8) and columns 8i + 2(l%4) (+1):
+// d[4i] = (row, col), d[4i+1] = (row, col+1), d[4i+2] = (row+8, col), d[4i+3] = (row+8, col+1).
+// SS: A from shared memory (descriptor).  RS: A from registers, the mma.m16n8k16 A fragment of the warp's 16 rows:
+// a[0] = (row, k 2(l%4) +0/1), a[1] = (row+8, same k), a[2] = (row, k+8), a[3] = (row+8, k+8).
+template <int N> struct Wgmma;
+template <> struct Wgmma<16> {
+    __device__ __forceinline__ static void ss(float (&d)[8], uint64_t a, uint64_t b, uint32_t accumulate) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+            : "l"(a), "l"(b), "r"(accumulate));
+    }
+    __device__ __forceinline__ static void rs(float (&d)[8], const uint32_t (&a)[4], uint64_t b, uint32_t accumulate) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, {%8,%9,%10,%11}, %12, p, 1, 1, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(accumulate));
+    }
+};
+template <> struct Wgmma<32> {
+    __device__ __forceinline__ static void ss(float (&d)[16], uint64_t a, uint64_t b, uint32_t accumulate) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(a), "l"(b), "r"(accumulate));
+    }
+    __device__ __forceinline__ static void rs(float (&d)[16], const uint32_t (&a)[4], uint64_t b, uint32_t accumulate) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(accumulate));
+    }
+};
+template <> struct Wgmma<128> {
+    __device__ __forceinline__ static void ss(float (&d)[64], uint64_t a, uint64_t b, uint32_t accumulate) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+              "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+              "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+              "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+              "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+            : "l"(a), "l"(b), "r"(accumulate));
+    }
+};
 
 // ---------------------------------------------------------------- fp16 hi/lo split
 // v ~= hi + lo with hi = fp16(v), lo = fp16(v - hi): ~22 significant bits for |v| in [2^-14, 65504],
@@ -280,34 +152,6 @@ __device__ __forceinline__ void tmem_ld_x32(uint32_t taddr, uint32_t (&r)[32]) {
 __device__ __forceinline__ void split_f16(float v, __half &hi, __half &lo) {
     hi = __float2half_rn(v);
     lo = __float2half_rn(v - __half2float(hi));
-}
-
-// ---------------------------------------------------------------- packed fp32 pairs (FADD2 / FMUL2 / FFMA2)
-// Blackwell issues two fp32 operations per instruction on a 64-bit register pair; the gate phase of the recurrent
-// kernel is instruction-issue bound, so its arithmetic runs on pairs of (independent) windows.
-struct F2 { unsigned long long v; };
-__device__ __forceinline__ F2 f2_make(float lo, float hi) {
-    F2 r;
-    asm("mov.b64 %0, {%1,%2};" : "=l"(r.v) : "f"(lo), "f"(hi));
-    return r;
-}
-__device__ __forceinline__ void f2_get(F2 a, float &lo, float &hi) {
-    asm("mov.b64 {%0,%1}, %2;" : "=f"(lo), "=f"(hi) : "l"(a.v));
-}
-__device__ __forceinline__ F2 f2_add(F2 a, F2 b) {
-    F2 r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v));
-    return r;
-}
-__device__ __forceinline__ F2 f2_mul(F2 a, F2 b) {
-    F2 r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r.v) : "l"(a.v), "l"(b.v));
-    return r;
-}
-__device__ __forceinline__ F2 f2_fma(F2 a, F2 b, F2 c) {
-    F2 r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r.v) : "l"(a.v), "l"(b.v), "l"(c.v));
-    return r;
 }
 
 // ---------------------------------------------------------------- streaming global access
@@ -323,12 +167,6 @@ __device__ __forceinline__ float4 ld_stream4(const float *p) {
                  : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
                  : "l"(p));
     return v;
-}
-
-// 16-byte store of data that is written once and read much later (gi: 34 GB per launch): evict-first in L2 so that it
-// does not push out the activation tiles the other weight-block CTAs of the GEMM are about to re-read
-__device__ __forceinline__ void st_stream4(float4 *p, float4 v) {
-    asm volatile("st.global.cs.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
 
 }  // namespace mdk

@@ -25,7 +25,7 @@
 //                         per thread of the second half); c and h stay on chip for all P steps
 //   head_kernel (misc.cu) Linear(2H -> 5) + softmax, shared with the counts models
 // All of it is CUDA-core fp32: parity first (tests/test_read_level.py against the reference's own class); the convolution
-// is 99 % of the FLOPs (557 kFLOP per read and position) and belongs on tcgen05 next.
+// is 99 % of the FLOPs (557 kFLOP per read and position); the tensor-core kernels below take it and the recurrence.
 #include <cstdlib>
 #include <string>
 #include <unordered_map>
@@ -206,205 +206,148 @@ __global__ void __launch_bounds__(256) rl_conv17_pool_kernel(const float *__rest
     }
 }
 
-// ---------------------------------------------------------------------------------------------- conv k=17 on tcgen05
+// ---------------------------------------------------------------------------------------------- conv k=17 on wgmma
 // The same convolution as an implicit GEMM on the tensor cores:  D[co][p] = sum_t sum_ci W[co][ci][t] . y1[p + t - 8][ci].
 //   A = one tap's weights [128 co][128 ci]  (K-major fp16 hi | lo planes, pre-tiled in HBM, streamed through a two-stage
-//       shared-memory ring with bulk copies; SS mode: 17 x 64 KiB of weights fit neither tensor memory nor shared memory)
+//       shared-memory ring with bulk copies: 17 x 64 KiB of weights do not fit shared memory)
 //   B = ONE staged activation tile [144 positions][128 ci] (hi | lo) serves all 17 taps: tap t is the same buffer with the
-//       descriptor's start address moved down t rows (K-major SWIZZLE_NONE: a row is 16 bytes inside its k-group block)
-//   D = 128 columns of tensor memory (lane = output channel, column = position), three fp16 products per contraction like
-//       the GRU kernels (fp32-faithful)
-// A CTA owns (window b, 128 positions, a group of reads): for TWO reads at a time it builds the activation tiles in shared
-// memory straight from the int8 features (embedding + k = 1 convolution + ReLU + BN1, never written to HBM), runs
-// 17 x 24 MMAs per read against one pass of the weights, drains the two accumulators through ReLU + BN2 into per-thread
-// sums (one output channel x 128 positions per thread), and writes the group's sum once.  Warp 0: weight producer; warp 1: MMA issuer, TMEM owner; warps 4-7: epilogue; all eight
-// warps build the activation tile.
+//       descriptor's start address moved down t rows (K-major, no swizzle: a row is 16 bytes inside its k-group block)
+//   D = registers, M64 N128 per warpgroup (warpgroup g: output channels 64g .. 64g + 63); three fp16 products per
+//       contraction like the GRU kernels (fp32-faithful)
+// A CTA owns (window b, 128 positions, a group of reads): for each read it builds the activation tile in shared memory
+// straight from the int8 features (embedding + k = 1 convolution + ReLU + BN1, never written to HBM), runs 17 x 24 MMAs
+// against one pass of the weights, folds the accumulators through ReLU + BN2 into per-thread sums, and writes the
+// group's sum once.
 constexpr int CT_NPOS = 128;
 constexpr int CT_ROWS = CT_NPOS + 2 * RL_PAD;            // 144 staged positions
 constexpr int CT_BPLANE = (RL_C / 8) * CT_ROWS * 16;     // 36 864 B
 constexpr int CT_BTILE = 2 * CT_BPLANE;                  // hi + lo of one read's activation tile
-constexpr int CT_PAIR = 2;                               // reads that share one pass over the weights
 constexpr int CT_WPLANE = (RL_C / 8) * RL_C * 16;        // 32 768 B: one plane of one tap = one ring stage
 constexpr int CT_STAGES = 2;
-constexpr int CT_OFF_W = CT_PAIR * CT_BTILE;
+constexpr int CT_OFF_W = CT_BTILE;
 constexpr int CT_OFF_IN = CT_OFF_W + CT_STAGES * CT_WPLANE;
-constexpr int CT_OFF_BAR = CT_OFF_IN + CT_PAIR * CT_ROWS * 8 * 4;
-constexpr int CT_SMEM = CT_OFF_BAR + 128;
+constexpr int CT_OFF_BAR = CT_OFF_IN + CT_ROWS * 8 * 4;
+constexpr int CT_SMEM = CT_OFF_BAR + 64;
 
 __global__ void __launch_bounds__(256, 1) rl_conv17_tc_kernel(const int8_t *__restrict__ x, const uint8_t *__restrict__ mask,
                                                               RlConv1 c1, RlConv17 c17, const uint8_t *__restrict__ w_tc,
                                                               int64_t P, int D, int F, int use_dwells, int dgroup,
                                                               float *__restrict__ partial) {
     extern __shared__ __align__(128) uint8_t smem_ct[];
-    uint8_t *sb = smem_ct;                                             // [pair][hi | lo][k-group][144][8 halfs]
+    uint8_t *sb = smem_ct;                                             // [hi | lo][k-group][144][8 halfs]
     uint8_t *sw = smem_ct + CT_OFF_W;                                  // [stage][k-group][128][8 halfs]
-    float *sin = reinterpret_cast<float *>(smem_ct + CT_OFF_IN);       // [pair][144][8]
+    float *sin = reinterpret_cast<float *>(smem_ct + CT_OFF_IN);       // [144][8]
     uint64_t *full = reinterpret_cast<uint64_t *>(smem_ct + CT_OFF_BAR);
-    uint64_t *empty = full + CT_STAGES;
-    uint64_t *acc_full = empty + CT_STAGES;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(acc_full + 1);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
+    const int gq = lane >> 2, cq = lane & 3;
     const int64_t b = blockIdx.z;
     const int g = blockIdx.y;
     const int64_t p0 = (int64_t)blockIdx.x * CT_NPOS;
     const int nin = RL_EMB + 1 + (use_dwells ? 1 : 0);
 
     if (tid == 0) {
-        for (int i = 0; i < CT_STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-        mbar_init(acc_full, 1);
+        for (int i = 0; i < CT_STAGES; ++i) mbar_init(&full[i], 1);
         fence_mbar_init();
     }
-    if (warp == 1) { tmem_alloc(tmem_slot, 256); tmem_relinquish(); }
-    tc_fence_before_sync();
     __syncthreads();
-    tc_fence_after_sync();
-    const uint32_t tmem_base = *tmem_slot;
 
     // builder constants: this thread's k = 1 convolution channel
     const int bc = tid & 127;
     float w1[RL_EMB + 2];
     for (int i = 0; i < nin; ++i) w1[i] = c1.w[bc * nin + i];
     const float b1 = c1.b[bc], m1 = c1.bn_mean[bc], s1 = c1.bn_invstd[bc], g1 = c1.bn_w[bc], o1 = c1.bn_b[bc];
-    // epilogue constants: this thread's output channel (TMEM lane)
-    const int co = (warp & 3) * 32 + lane;
-    const float b2 = c17.b[co], m2 = c17.bn_mean[co], s2 = c17.bn_invstd[co], g2 = c17.bn_w[co], o2 = c17.bn_b[co];
-    float pooled[CT_NPOS];
-    if (warp >= 4) {
-#pragma unroll
-        for (int i = 0; i < CT_NPOS; ++i) pooled[i] = 0.f;
+    // epilogue constants: this thread's output channels co0 and co0 + 8 (accumulator rows)
+    const int co0 = wg * 64 + warp * 16 + gq;
+    float b2[2], m2[2], s2[2], g2[2], o2[2];
+    for (int hb = 0; hb < 2; ++hb) {
+        const int co = co0 + 8 * hb;
+        b2[hb] = c17.b[co]; m2[hb] = c17.bn_mean[co]; s2[hb] = c17.bn_invstd[co]; g2[hb] = c17.bn_w[co]; o2[hb] = c17.bn_b[co];
     }
-    const uint32_t idesc = make_idesc_f16(128, CT_NPOS);
+    float pooled[64], acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) pooled[i] = 0.f;
     const int d0 = g * dgroup, d1 = min(D, d0 + dgroup);
-    uint32_t it = 0;             // weight-plane stages handed over so far (producer and issuer count alike)
-    uint32_t n_done = 0;         // passes over the weights
-    int d = d0;
-    while (true) {
-        // ---- the next one or two non-empty reads of the group share one pass over the 17 taps' weights (the weights
-        //      come from L2 each time: with one read per pass all SMs together ask for more than L2 delivers)
-        int dq[CT_PAIR], n_pair = 0;
-        while (d < d1 && n_pair < CT_PAIR) {
-            if (mask[b * D + d]) dq[n_pair++] = d;
-            ++d;
-        }
-        if (n_pair == 0) break;                                    // uniform over the CTA
-        // ---- build the activation tiles (the previous pass's MMAs are complete: everybody waited on acc_full below)
-        for (int q = 0; q < n_pair; ++q) {
-            if (tid < CT_ROWS) {
-                const int64_t p = p0 - RL_PAD + tid;
-                float *row = sin + (q * CT_ROWS + tid) * 8;
-                if (p >= 0 && p < P) {
-                    const int8_t *v = x + ((b * P + p) * D + dq[q]) * F;
-                    const int base = min(max((int)v[0], 0), 5), strand = min(max((int)v[2] + 1, 0), 2);
-                    for (int i = 0; i < RL_EMB; ++i) row[i] = c1.emb_base[base * RL_EMB + i] + c1.emb_strand[strand * RL_EMB + i];
-                    row[RL_EMB] = (float)v[1] / 25.0f - 1.0f;
-                    row[RL_EMB + 1] = use_dwells ? (float)v[4] : 0.f;
-                } else {
-                    row[0] = __int_as_float(0x7fc00000);          // marker: outside the window -> zero row (conv padding)
-                }
+    uint32_t it = 0;             // weight-plane stages consumed so far
+    auto issue = [&](uint32_t k) {   // stage k of the running sequence = plane (k % 34) of the taps
+        const uint32_t st = k % CT_STAGES;
+        const uint8_t *src = w_tc + (size_t)(k % (2 * RL_TAPS)) * CT_WPLANE;     // [tap][hi | lo] back to back
+        mbar_arrive_expect_tx(&full[st], CT_WPLANE);
+        bulk_g2s(sw + st * CT_WPLANE, src, CT_WPLANE, &full[st]);
+    };
+    for (int d = d0; d < d1; ++d) {
+        if (!mask[b * D + d]) continue;                            // uniform over the CTA
+        // ---- build the activation tile (the previous read's MMAs are complete)
+        if (tid < CT_ROWS) {
+            const int64_t p = p0 - RL_PAD + tid;
+            float *row = sin + tid * 8;
+            if (p >= 0 && p < P) {
+                const int8_t *v = x + ((b * P + p) * D + d) * F;
+                const int base = min(max((int)v[0], 0), 5), strand = min(max((int)v[2] + 1, 0), 2);
+                for (int i = 0; i < RL_EMB; ++i) row[i] = c1.emb_base[base * RL_EMB + i] + c1.emb_strand[strand * RL_EMB + i];
+                row[RL_EMB] = (float)v[1] / 25.0f - 1.0f;
+                row[RL_EMB + 1] = use_dwells ? (float)v[4] : 0.f;
+            } else {
+                row[0] = __int_as_float(0x7fc00000);              // marker: outside the window -> zero row (conv padding)
             }
+        }
+        if (tid == 0) {                                            // the first two weight planes of this read
+            issue(it);
+            issue(it + 1);
         }
         __syncthreads();
-        for (int q = 0; q < n_pair; ++q) {
-            uint8_t *tile = sb + q * CT_BTILE;
-            for (int r = tid >> 7; r < CT_ROWS; r += 2) {
-                const float *row = sin + (q * CT_ROWS + r) * 8;
-                float y = 0.f;
-                if (!(row[0] != row[0])) {
-                    float acc = b1;
-                    for (int k = 0; k < nin; ++k) acc = fmaf(w1[k], row[k], acc);
-                    acc = fmaxf(acc, 0.f);
-                    y = (acc - m1) * s1 * g1 + o1;
-                }
-                __half hi, lo;
-                split_f16(y, hi, lo);
-                const int off = (bc >> 3) * (CT_ROWS * 16) + r * 16 + (bc & 7) * 2;
-                *reinterpret_cast<__half *>(tile + off) = hi;
-                *reinterpret_cast<__half *>(tile + CT_BPLANE + off) = lo;
+        for (int r = tid >> 7; r < CT_ROWS; r += 2) {
+            const float *row = sin + r * 8;
+            float y = 0.f;
+            if (!(row[0] != row[0])) {
+                float a = b1;
+                for (int k = 0; k < nin; ++k) a = fmaf(w1[k], row[k], a);
+                a = fmaxf(a, 0.f);
+                y = (a - m1) * s1 * g1 + o1;
             }
+            __half hi, lo;
+            split_f16(y, hi, lo);
+            const int off = (bc >> 3) * (CT_ROWS * 16) + r * 16 + (bc & 7) * 2;
+            *reinterpret_cast<__half *>(sb + off) = hi;
+            *reinterpret_cast<__half *>(sb + CT_BPLANE + off) = lo;
         }
         fence_proxy_async_smem();
-        tc_fence_before_sync();
         __syncthreads();
-        tc_fence_after_sync();
-        // ---- 17 taps x (hi plane, lo plane)
-        if (warp == 0) {
-            if (lane == 0) {
-                for (int ps = 0; ps < 2 * RL_TAPS; ++ps, ++it) {
-                    const uint32_t st = it % CT_STAGES;
-                    mbar_wait(&empty[st], ((it / CT_STAGES) & 1) ^ 1);
-                    mbar_arrive_expect_tx(&full[st], CT_WPLANE);
-                    const uint8_t *src = w_tc + (size_t)ps * CT_WPLANE;           // [tap][hi | lo] back to back
+        // ---- 17 taps x (hi plane, lo plane) of the weights
+        for (int ps = 0; ps < 2 * RL_TAPS; ++ps, ++it) {
+            const uint32_t st = it % CT_STAGES;
+            const int t = ps >> 1, lo_plane = ps & 1;
+            mbar_wait(&full[st], (it / CT_STAGES) & 1);
+            wg_fence();
+            const uint32_t a0 = smem_u32(sw + st * CT_WPLANE) + wg * 64 * 16;
+            const uint32_t bb0 = smem_u32(sb) + (uint32_t)t * 16u;
+            // hi plane of the weights: x activation hi, then x activation lo;  lo plane: x activation hi
 #pragma unroll
-                    for (int c = 0; c < 2; ++c) bulk_g2s(sw + st * CT_WPLANE + c * (CT_WPLANE / 2), src + c * (CT_WPLANE / 2), CT_WPLANE / 2, &full[st]);
-                }
-            } else {
-                it += 2 * RL_TAPS;
+            for (int ks = 0; ks < RL_C / 16; ++ks) {
+                const uint64_t ad = make_smem_desc(a0 + ks * 2 * (RL_C * 16), RL_C * 16, 128);
+                const uint64_t bh = make_smem_desc(bb0 + ks * 2 * (CT_ROWS * 16), CT_ROWS * 16, 128);
+                Wgmma<128>::ss(acc, ad, bh, (ps | ks) ? 1u : 0u);
+                if (!lo_plane) Wgmma<128>::ss(acc, ad, make_smem_desc(bb0 + CT_BPLANE + ks * 2 * (CT_ROWS * 16), CT_ROWS * 16, 128), 1u);
             }
-        } else if (warp == 1) {
-            for (int ps = 0; ps < 2 * RL_TAPS; ++ps, ++it) {
-                const uint32_t st = it % CT_STAGES;
-                const int t = ps >> 1, lo_plane = ps & 1;
-                mbar_wait(&full[st], (it / CT_STAGES) & 1);
-                tc_fence_after_sync();
-                if (elect_one()) {
-                    const uint32_t a0 = smem_u32(sw + st * CT_WPLANE);
-                    for (int q = 0; q < n_pair; ++q) {
-                        const uint32_t dcol = tmem_base + (uint32_t)(q * CT_NPOS);
-                        const uint32_t bb0 = smem_u32(sb + q * CT_BTILE) + (uint32_t)t * 16u;
-                        // hi plane of the weights: x activation hi, then x activation lo;  lo plane: x activation hi
-                        const int n_prod = lo_plane ? 1 : 2;
-                        for (int prod = 0; prod < n_prod; ++prod) {
-                            const int pb = lo_plane ? 0 : prod;
-#pragma unroll
-                            for (int ks = 0; ks < RL_C / 16; ++ks) {
-                                const uint64_t ad = make_smem_desc(a0 + ks * 2 * (RL_C * 16), RL_C * 16, 128);
-                                const uint64_t bdsc = make_smem_desc(bb0 + pb * CT_BPLANE + ks * 2 * (CT_ROWS * 16), CT_ROWS * 16, 128);
-                                umma_f16(dcol, ad, bdsc, idesc, (ps | prod | ks) ? 1u : 0u);
-                            }
-                        }
-                    }
-                    umma_commit(&empty[st]);
-                    if (ps == 2 * RL_TAPS - 1) umma_commit(acc_full);
-                }
-                __syncwarp();
-            }
-        } else {
-            it += 2 * RL_TAPS;
+            wg_commit();
+            wg_wait_all();
+            wg_hold(acc);
+            __syncthreads();                                       // both warpgroups have read stage st
+            if (tid == 0 && ps + 2 < 2 * RL_TAPS) issue(it + 2);
         }
-        // ---- everybody waits for the pass's accumulators (the activation tiles may then be rebuilt)
-        mbar_wait(acc_full, n_done & 1);
-        tc_fence_after_sync();
-        if (warp >= 4) {
-            for (int q = 0; q < n_pair; ++q) {
-                const uint32_t t_lane = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(q * CT_NPOS);
 #pragma unroll
-                for (int c32 = 0; c32 < CT_NPOS; c32 += 32) {
-                    uint32_t v[32];
-                    tmem_ld_x32(t_lane + c32, v);
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) {
-                        const float av = fmaxf(__uint_as_float(v[i]) + b2, 0.f);
-                        pooled[c32 + i] += (av - m2) * s2 * g2 + o2;
-                    }
-                }
-            }
+        for (int k = 0; k < 64; ++k) {
+            const int hb = (k >> 1) & 1;
+            const float av = fmaxf(acc[k] + b2[hb], 0.f);
+            pooled[k] += (av - m2[hb]) * s2[hb] * g2[hb] + o2[hb];
         }
-        tc_fence_before_sync();
-        __syncthreads();                                           // accumulators drained, tiles free
-        tc_fence_after_sync();
-        ++n_done;
     }
-    if (warp >= 4) {
-        const int n_groups = gridDim.y;
-        float *dst = partial + ((b * n_groups + g) * P + p0) * RL_C + co;
+    const int n_groups = gridDim.y;
+    float *dst = partial + ((b * n_groups + g) * P + p0) * RL_C + co0;
 #pragma unroll
-        for (int i = 0; i < CT_NPOS; ++i)
-            if (p0 + i < P) dst[(int64_t)i * RL_C] = pooled[i];
+    for (int k = 0; k < 64; ++k) {
+        const int n = 8 * (k >> 2) + 2 * cq + (k & 1);
+        if (p0 + n < P) dst[(int64_t)n * RL_C + 8 * ((k >> 1) & 1)] = pooled[k];
     }
-    tc_fence_before_sync();
-    __syncthreads();
-    if (warp == 1) { tc_fence_after_sync(); tmem_dealloc(tmem_base, 256); }
 }
 
 // ---------------------------------------------------------------------------------------------- mean + Linear(C -> H)
@@ -630,188 +573,117 @@ __global__ void __launch_bounds__(256, 1) rl_lstm_kernel(const float *__restrict
     }
 }
 
-// ---------------------------------------------------------------------------------------------- LSTM on tcgen05
+// ---------------------------------------------------------------------------------------------- LSTM on wgmma
 // The recurrence with the matvec on the tensor cores:  G^T[4H][16 windows] = W_hh[4H][H] . h^T[H][16]  per time step.
-//   A = W_hh: the fp16 hi plane of all four gates lives in TENSOR MEMORY (4 x 64 columns, TS mode) and so does the lo
-//       plane of gates i and f (2 x 64 columns behind the accumulators); the lo plane of gates g and o comes from shared
-//       memory as K-major operand tiles (SS mode) - hi + lo of all four gates would fill all 512 columns
-//   B = the h tile [16 windows][128] the gate warps publish every step (fp16 hi | lo, K-major)
-//   D = four 16-column accumulators (lane = hidden unit, column = window); three products per contraction:
-//       W_hi.h_hi and W_hi.h_lo from tensor memory, W_lo.h_hi from shared memory
-// One CTA = 16 windows of one direction; warps 0-7: gate warps (thread = hidden unit x 8 windows: c and h stay in
-// registers, the input pre-activations are fetched one step ahead), warp 8: MMA issuer.  A step is the dependent chain
-// publish h -> 96 MMAs -> gate arithmetic, like the one-tile GRU kernel.
+//   A = W_hh: the fp16 hi plane of all four gates stays in REGISTERS (the register form of wgmma; warpgroup g holds
+//       hidden units 64g .. 64g + 63 of every gate), the lo plane is a shared-memory operand (pre-tiled per direction)
+//   B = the h tile [16 windows][128] (fp16 hi | lo, K-major, double buffered: step t reads buffer t & 1)
+//   D = four M64 N16 accumulators per warpgroup, preloaded with the input pre-activations; three products per
+//       contraction: W_hi.h_hi, W_hi.h_lo, W_lo.h_hi
+// One CTA = 16 windows of one direction, two warpgroups; c and h stay in registers.
 constexpr int LT_N = 16;
 constexpr int LT_WLO_GATE = (RL_H / 8) * RL_H * 16;          // 32 768 B: one gate's lo plane as A operand tiles
-constexpr int LT_HPLANE = (RL_H / 8) * LT_N * 16;            // 4 096 B
+constexpr int LT_KG = LT_N * 16 + 16;                        // k-group stride of the h tile (+16 B spreads the stores)
+constexpr int LT_HPLANE = (RL_H / 8) * LT_KG;
 constexpr int LT_OFF_H = 4 * LT_WLO_GATE;
-constexpr int LT_OFF_BAR = LT_OFF_H + 2 * LT_HPLANE;
-constexpr int LT_SMEM = LT_OFF_BAR + 64;
-constexpr uint32_t LT_ACC_COL = 256;                         // accumulators behind the four 64-column weight blocks
-constexpr uint32_t LT_LO_COL = 320;                          // lo plane of the first LT_LO_TMEM_GATES gates
-constexpr int LT_LO_TMEM_GATES = 2;
-constexpr int LT_W = LT_N / 2;                               // windows per gate thread
-constexpr int LT_ISSUER = 8;                                 // warps 0-7 gate warps, warp 8 issues
-constexpr int LT_THREADS = 32 * (LT_ISSUER + 1);
-// MUFU-based gate functions (ex2.approx / rcp.approx, ~2 ulp): the gate phase is instruction bound
+constexpr int LT_SMEM = LT_OFF_H + 4 * LT_HPLANE;
+constexpr int LT_THREADS = 256;
+// MUFU-based gate functions (ex2.approx / rcp.approx, ~2 ulp)
 __device__ __forceinline__ float lt_ex2(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float lt_rcp(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float lt_sigmoid(float x) { return lt_rcp(1.0f + lt_ex2(-1.4426950408889634f * x)); }
 __device__ __forceinline__ float lt_tanh(float x) { return fmaf(-2.0f, lt_rcp(1.0f + lt_ex2(2.8853900817779268f * x)), 1.0f); }
 
 __global__ void __launch_bounds__(LT_THREADS, 1) rl_lstm_tc_kernel(const float *__restrict__ gi, const __half *__restrict__ w_hi,
-                                                            const __half *__restrict__ w_lo_rm,
                                                             const uint8_t *__restrict__ w_lo_tiles, float *__restrict__ out,
                                                             int64_t B, int64_t P) {
     extern __shared__ __align__(128) uint8_t smem_lt[];
     uint8_t *swlo = smem_lt;
-    uint8_t *sh = smem_lt + LT_OFF_H;
-    uint64_t *acc_full = reinterpret_cast<uint64_t *>(smem_lt + LT_OFF_BAR);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(acc_full + 1);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    uint8_t *sh = smem_lt + LT_OFF_H;                            // [buf 2][hi | lo] LT_HPLANE
+    const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
+    const int gq = lane >> 2, cq = lane & 3;
     const int dir = blockIdx.y;
     const int64_t b0 = (int64_t)blockIdx.x * LT_N;
     const int nb = (int)min((int64_t)LT_N, B - b0);
-    if (tid == 0) { mbar_init(acc_full, 1); fence_mbar_init(); }
-    if (warp == LT_ISSUER) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
-    // lo plane of W_hh -> shared memory (pre-tiled per direction: [gate][k-group][row][8 halfs]); h tile = 0
+    const int j0 = wg * 64 + warp * 16 + gq;                   // hidden units j0 and j0 + 8
     {
         const uint4 *src = reinterpret_cast<const uint4 *>(w_lo_tiles + (size_t)dir * 4 * LT_WLO_GATE);
         for (int i = tid; i < 4 * LT_WLO_GATE / 16; i += LT_THREADS) reinterpret_cast<uint4 *>(swlo)[i] = src[i];
-        for (int i = tid; i < 2 * LT_HPLANE / 16; i += LT_THREADS) reinterpret_cast<uint4 *>(sh)[i] = make_uint4(0u, 0u, 0u, 0u);
+        for (int i = tid; i < 4 * LT_HPLANE / 16; i += LT_THREADS) reinterpret_cast<uint4 *>(sh)[i] = make_uint4(0u, 0u, 0u, 0u);
     }
-    tc_fence_before_sync();
-    __syncthreads();
-    tc_fence_after_sync();
-    const uint32_t tmem_base = *tmem_slot;
-    const int j = tid & 127;                                 // hidden unit of a gate thread
-    if (warp < 4) {
-        // (one warp per lane quarter) hi plane of W_hh (row-major fp16 [dir][4H][H]) -> tensor memory: gate g, k-step ks at column g*64 + ks*8
-        const uint32_t t_w = tmem_base + ((uint32_t)(warp * 32) << 16);
-        for (int g = 0; g < 4; ++g) {
-            const uint4 *src = reinterpret_cast<const uint4 *>(w_hi + (((size_t)dir * 4 + g) * RL_H + j) * RL_H);
+    uint32_t whi[4][RL_H / 16][4];
 #pragma unroll
-            for (int ks = 0; ks < RL_H / 16; ++ks) {
-                const uint4 lo4 = src[2 * ks], hi4 = src[2 * ks + 1];
-                const uint32_t v[8] = {lo4.x, lo4.y, lo4.z, lo4.w, hi4.x, hi4.y, hi4.z, hi4.w};
-                tmem_st_x8(t_w + (uint32_t)(g * 64 + ks * 8), v);
-            }
-        }
-        // the lo plane of gates i and f fits behind the accumulators (columns 320..447): their third product runs in
-        // TS mode too (10 instead of 40 cycles per MMA); gates g and o take theirs from shared memory
-        for (int g = 0; g < LT_LO_TMEM_GATES; ++g) {
-            const uint4 *src = reinterpret_cast<const uint4 *>(w_lo_rm + (((size_t)dir * 4 + g) * RL_H + j) * RL_H);
+    for (int g = 0; g < 4; ++g)
 #pragma unroll
-            for (int ks = 0; ks < RL_H / 16; ++ks) {
-                const uint4 lo4 = src[2 * ks], hi4 = src[2 * ks + 1];
-                const uint32_t v[8] = {lo4.x, lo4.y, lo4.z, lo4.w, hi4.x, hi4.y, hi4.z, hi4.w};
-                tmem_st_x8(t_w + LT_LO_COL + (uint32_t)(g * 64 + ks * 8), v);
-            }
+        for (int ks = 0; ks < RL_H / 16; ++ks) {
+            const __half *w = w_hi + (((size_t)dir * 4 + g) * RL_H + j0) * RL_H + ks * 16 + 2 * cq;
+            whi[g][ks][0] = *reinterpret_cast<const uint32_t *>(w);
+            whi[g][ks][1] = *reinterpret_cast<const uint32_t *>(w + 8 * RL_H);
+            whi[g][ks][2] = *reinterpret_cast<const uint32_t *>(w + 8);
+            whi[g][ks][3] = *reinterpret_cast<const uint32_t *>(w + 8 * RL_H + 8);
         }
-        tmem_st_wait();
-    }
+    // accumulator element k = 4i + 2hb + e: hidden unit j0 + 8hb, window 8i + 2cq + e
+    float acc[4][8], c_state[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) c_state[k] = 0.f;
+    auto fetch = [&](int64_t t) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const int wdw = 8 * (k >> 2) + 2 * cq + (k & 1);
+            const bool ok = wdw < nb;
+            const float *row = gi + (((b0 + (ok ? wdw : 0)) * P + t) * 2 + dir) * RL_G4 + j0 + 8 * ((k >> 1) & 1);
+#pragma unroll
+            for (int g = 0; g < 4; ++g) acc[g][k] = ok ? __ldg(row + g * RL_H) : 0.f;
+        }
+    };
+    fetch(dir ? (P - 1) : 0);
     fence_proxy_async_smem();
-    tc_fence_before_sync();
     __syncthreads();
-    tc_fence_after_sync();
-
-    if (warp == LT_ISSUER) {
-        const uint32_t idesc = make_idesc_f16(128, LT_N);
-        const uint32_t h_hi = smem_u32(sh), h_lo = smem_u32(sh + LT_HPLANE), wl = smem_u32(swlo);
-        for (int64_t step = 0; step < P; ++step) {
-            if (elect_one()) {
+    const uint32_t wl = smem_u32(swlo) + wg * 64 * 16;
+    for (int64_t step = 0; step < P; ++step) {
+        const int64_t t = dir ? (P - 1 - step) : step;
+        const int buf = (int)(step & 1);
+        const uint32_t h_hi = smem_u32(sh + buf * 2 * LT_HPLANE), h_lo = h_hi + LT_HPLANE;
+        wg_fence();
 #pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    const uint32_t d = tmem_base + LT_ACC_COL + (uint32_t)(g * LT_N);
+        for (int g = 0; g < 4; ++g)
 #pragma unroll
-                    for (int ks = 0; ks < RL_H / 16; ++ks) {
-                        const uint64_t bh = make_smem_desc(h_hi + ks * 2 * (LT_N * 16), LT_N * 16, 128);
-                        umma_f16_ts(d, tmem_base + (uint32_t)(g * 64 + ks * 8), bh, idesc, ks ? 1u : 0u);
-                    }
-#pragma unroll
-                    for (int ks = 0; ks < RL_H / 16; ++ks) {
-                        const uint64_t bl = make_smem_desc(h_lo + ks * 2 * (LT_N * 16), LT_N * 16, 128);
-                        umma_f16_ts(d, tmem_base + (uint32_t)(g * 64 + ks * 8), bl, idesc, 1u);
-                    }
-#pragma unroll
-                    for (int ks = 0; ks < RL_H / 16; ++ks) {
-                        const uint64_t bh = make_smem_desc(h_hi + ks * 2 * (LT_N * 16), LT_N * 16, 128);
-                        if (g < LT_LO_TMEM_GATES) {
-                            umma_f16_ts(d, tmem_base + LT_LO_COL + (uint32_t)(g * 64 + ks * 8), bh, idesc, 1u);
-                        } else {
-                            const uint64_t ad = make_smem_desc(wl + g * LT_WLO_GATE + ks * 2 * (RL_H * 16), RL_H * 16, 128);
-                            umma_f16(d, ad, bh, idesc, 1u);
-                        }
-                    }
-                }
-                umma_commit(acc_full);
+            for (int ks = 0; ks < RL_H / 16; ++ks) {
+                const uint64_t bh = make_smem_desc(h_hi + ks * 2 * LT_KG, LT_KG, 128);
+                Wgmma<16>::rs(acc[g], whi[g][ks], bh, 1u);
+                Wgmma<16>::rs(acc[g], whi[g][ks], make_smem_desc(h_lo + ks * 2 * LT_KG, LT_KG, 128), 1u);
+                Wgmma<16>::ss(acc[g], make_smem_desc(wl + g * LT_WLO_GATE + ks * 2 * (RL_H * 16), RL_H * 16, 128), bh, 1u);
             }
-            __syncwarp();
-            tc_fence_before_sync();
-            __syncthreads();                                   // the gate warps have published the next h tile
-            tc_fence_after_sync();
+        wg_commit();
+        wg_wait_all();
+#pragma unroll
+        for (int g = 0; g < 4; ++g) wg_hold(acc[g]);
+        uint8_t *hw = sh + (buf ^ 1) * 2 * LT_HPLANE;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const float ig = lt_sigmoid(acc[0][k]);
+            const float fg = lt_sigmoid(acc[1][k]);
+            const float gg = lt_tanh(acc[2][k]);
+            const float og = lt_sigmoid(acc[3][k]);
+            const float c = fmaf(fg, c_state[k], ig * gg);
+            c_state[k] = c;
+            const float h = og * lt_tanh(c);
+            const int wdw = 8 * (k >> 2) + 2 * cq + (k & 1), j = j0 + 8 * ((k >> 1) & 1);
+            if (wdw < nb) out[((b0 + wdw) * P + t) * (2 * RL_H) + dir * RL_H + j] = h;
+            __half hi, lo;
+            split_f16(h, hi, lo);
+            *reinterpret_cast<__half *>(hw + (j >> 3) * LT_KG + wdw * 16 + (j & 7) * 2) = hi;
+            *reinterpret_cast<__half *>(hw + LT_HPLANE + (j >> 3) * LT_KG + wdw * 16 + (j & 7) * 2) = lo;
         }
-    } else {
-        // warps w and w + 4 share TMEM lane quarter w (hidden units 32 w .. 32 w + 31) and split the 16 windows.
-        // the input pre-activations of the NEXT step are loaded right after this step's arithmetic has consumed the
-        // current ones: the loads fly under the publish and the next step's MMAs (one register set, not two)
-        const int half = warp >> 2;
-        float c_state[LT_W], gcur[4][LT_W];
-#pragma unroll
-        for (int n = 0; n < LT_W; ++n) c_state[n] = 0.f;
-        auto fetch = [&](int64_t t) {
-#pragma unroll
-            for (int n = 0; n < LT_W; ++n) {
-                const int wdw = half * LT_W + n;
-                const bool ok = wdw < nb;
-                const float *row = gi + (((b0 + (ok ? wdw : 0)) * P + t) * 2 + dir) * RL_G4 + j;
-#pragma unroll
-                for (int g = 0; g < 4; ++g) gcur[g][n] = ok ? __ldg(row + g * RL_H) : 0.f;
-            }
-        };
-        fetch(dir ? (P - 1) : 0);
-        const uint32_t t_lane = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + LT_ACC_COL + (uint32_t)(half * LT_W);
-        const int hoff = (j >> 3) * (LT_N * 16) + (j & 7) * 2 + half * LT_W * 16;
-        for (int64_t step = 0; step < P; ++step) {
-            const int64_t t = dir ? (P - 1 - step) : step;
-            mbar_wait(acc_full, (uint32_t)(step & 1));
-            tc_fence_after_sync();
-            uint32_t a[4][LT_W];
-#pragma unroll
-            for (int g = 0; g < 4; ++g) tmem_ld_x8(t_lane + (uint32_t)(g * LT_N), a[g]);
-            tmem_ld_wait();
-#pragma unroll
-            for (int n = 0; n < LT_W; ++n) {
-                const float ig = lt_sigmoid(gcur[0][n] + __uint_as_float(a[0][n]));
-                const float fg = lt_sigmoid(gcur[1][n] + __uint_as_float(a[1][n]));
-                const float gg = lt_tanh(gcur[2][n] + __uint_as_float(a[2][n]));
-                const float og = lt_sigmoid(gcur[3][n] + __uint_as_float(a[3][n]));
-                const float c = fmaf(fg, c_state[n], ig * gg);
-                c_state[n] = c;
-                const float h = og * lt_tanh(c);
-                const int wdw = half * LT_W + n;
-                if (wdw < nb) out[((b0 + wdw) * P + t) * (2 * RL_H) + dir * RL_H + j] = h;
-                __half hi, lo;
-                split_f16(h, hi, lo);
-                *reinterpret_cast<__half *>(sh + hoff + n * 16) = hi;
-                *reinterpret_cast<__half *>(sh + LT_HPLANE + hoff + n * 16) = lo;
-            }
-            if (step + 1 < P) fetch(dir ? (t - 1) : (t + 1));
-            fence_proxy_async_smem();
-            tc_fence_before_sync();
-            __syncthreads();
-            tc_fence_after_sync();
-        }
+        if (step + 1 < P) fetch(dir ? (t - 1) : (t + 1));
+        fence_proxy_async_smem();
+        __syncthreads();
     }
-    tc_fence_before_sync();
-    __syncthreads();
-    if (warp == LT_ISSUER) { tc_fence_after_sync(); tmem_dealloc(tmem_base, 512); }
 }
 
 // ---------------------------------------------------------------------------------------------- engine
 struct RlLstmLayer {
-    __half *w_hi = nullptr;     // [2][4H][H] fp16 hi plane of W_hh (tensor-core kernel: -> tensor memory)
-    __half *w_lo_rm = nullptr;  // [2][4H][H] fp16 lo plane, row-major (gates i, f: -> tensor memory)
+    __half *w_hi = nullptr;     // [2][4H][H] fp16 hi plane of W_hh (tensor-core kernel: -> registers)
     uint8_t *w_lo = nullptr;    // [2][4 gates][k-group 16][row 128][8 halfs] lo plane as shared-memory A operand tiles
     float *w_ih = nullptr;      // [2 dirs * 4H][in]   (both directions stacked: one GEMM)
     float *bias = nullptr;      // [2 * 4H]  b_ih + b_hh
@@ -833,8 +705,8 @@ struct mdk_rl_engine {
     float *c1_w = nullptr, *c1_b = nullptr, *bn1[4] = {nullptr, nullptr, nullptr, nullptr};
     float *c17_wt = nullptr, *c17_b = nullptr, *bn2[4] = {nullptr, nullptr, nullptr, nullptr};
     uint8_t *c17_tc = nullptr;     // [17 taps][hi | lo][k-group 16][co 128][8 halfs]: the tensor-core kernel's A operand tiles
-    int conv_tc = 1;               // 1: k = 17 convolution on tcgen05 (default), 0: fp32 CUDA cores
-    int lstm_tc = 1;               // 1: LSTM recurrence on tcgen05 (default), 0: fp32 CUDA cores
+    int conv_tc = 1;               // 1: k = 17 convolution on wgmma (default), 0: fp32 CUDA cores
+    int lstm_tc = 1;               // 1: LSTM recurrence on wgmma (default), 0: fp32 CUDA cores
     float *pool_w = nullptr, *pool_b = nullptr;
     RlLstmLayer lstm[2];
     float *lin_w = nullptr, *lin_b = nullptr;
@@ -953,7 +825,7 @@ int rl_prepare(mdk_rl_engine *e) {
             (rc = rl_upload(e, w3t, &e->lstm[l].w3t)) || (rc = rl_upload(e, wo, &e->lstm[l].wo)))
             return rc;
         // tensor-core operands: hi plane row-major (torch's [4H][H] as it is), lo plane as K-major tiles per gate
-        std::vector<__half> hi((size_t)2 * RL_G4 * RL_H), lo_t((size_t)2 * RL_G4 * RL_H), lo_rm((size_t)2 * RL_G4 * RL_H);
+        std::vector<__half> hi((size_t)2 * RL_G4 * RL_H), lo_t((size_t)2 * RL_G4 * RL_H);
         for (int d = 0; d < 2; ++d) {
             const std::string sfx = "_l" + std::to_string(l) + (d ? "_reverse" : "");
             const std::vector<float> &whh = e->host["lstm.weight_hh" + sfx];
@@ -965,14 +837,9 @@ int rl_prepare(mdk_rl_engine *e) {
                     const int g = r / RL_H, jj = r % RL_H;
                     const __half l16 = __float2half_rn(v - __half2float(h16));
                     lo_t[(size_t)d * RL_G4 * RL_H + (((size_t)g * (RL_H / 8) + k / 8) * RL_H + jj) * 8 + (k % 8)] = l16;
-                    lo_rm[((size_t)d * RL_G4 + r) * RL_H + k] = l16;
                 }
         }
-        void *p1 = nullptr, *p2 = nullptr, *p3 = nullptr;
-        MDK_CUDA(cudaMalloc(&p3, lo_rm.size() * sizeof(__half)));
-        e->allocs.push_back(p3);
-        MDK_CUDA(cudaMemcpy(p3, lo_rm.data(), lo_rm.size() * sizeof(__half), cudaMemcpyHostToDevice));
-        e->lstm[l].w_lo_rm = static_cast<__half *>(p3);
+        void *p1 = nullptr, *p2 = nullptr;
         MDK_CUDA(cudaMalloc(&p1, hi.size() * sizeof(__half)));
         e->allocs.push_back(p1);
         MDK_CUDA(cudaMalloc(&p2, lo_t.size() * sizeof(__half)));
@@ -1095,8 +962,8 @@ int mdk_rl_forward(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P,
                                                                                        d_gi, BP, in, 2 * RL_G4);
         if (e->lstm_tc) {
             MDK_CUDA(cudaFuncSetAttribute(rl_lstm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LT_SMEM));
-            rl_lstm_tc_kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N), 2), LT_THREADS, LT_SMEM, s>>>(d_gi, e->lstm[l].w_hi, e->lstm[l].w_lo_rm,
-                                                                                            e->lstm[l].w_lo, layer_out[l], B, P);
+            rl_lstm_tc_kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N), 2), LT_THREADS, LT_SMEM, s>>>(d_gi, e->lstm[l].w_hi, e->lstm[l].w_lo,
+                                                                                            layer_out[l], B, P);
         } else {
             rl_lstm_kernel<<<dim3((unsigned)((B + RL_NB - 1) / RL_NB), 2), 256, RL_LSTM_SMEM, s>>>(d_gi, e->lstm[l].w3t, e->lstm[l].wo,
                                                                                                 layer_out[l], B, P);

@@ -1,12 +1,11 @@
-// Device helpers shared by the recurrent tensor-core kernels (gru_tc.cu: one tile per CTA; gru_pp.cu: two tiles per
-// CTA, ping-pong): approximate activations on the MUFU / FMA pipes, the phase fence, tile geometry.
+// Device helpers of the recurrent tensor-core kernel (gru_wg.cu): approximate activations, tile geometry.
 #pragma once
 #include "common.cuh"
 #include "ptx.cuh"
 
 namespace mdk {
 
-// ---- activations: ex2.approx / rcp.approx only (MUFU is the gate phase's binding pipe: 5 ops per element) ----
+// ---- activations: ex2.approx / rcp.approx only ----
 __device__ __forceinline__ float ex2_approx(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -17,45 +16,9 @@ __device__ __forceinline__ float rcp_approx(float x) {
     asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
-// 1 / d for d = -nd >= 1 on the FMA pipe (packed pairs): integer seed (5 % error), one cubic step, one Newton step
-// -> 1.7e-8 relative.  The gate phase is bound by the MUFU (XU) pipe - ncu: mio_throttle is its top stall, XU 33 % of
-// the whole step while the FMA pipe sits at 13 % (profiles/r01e_*) - so the reciprocals that are on the critical path
-// are moved off it.  Takes -d because the callers get the negation for free from an FMA.
-__device__ __forceinline__ F2 rcp_neg_fma2(F2 nd, F2 one2) {
-    float a, b;
-    f2_get(nd, a, b);
-    F2 y = f2_make(__uint_as_float(0xFEF311C7u - __float_as_uint(a)), __uint_as_float(0xFEF311C7u - __float_as_uint(b)));
-    F2 e = f2_fma(nd, y, one2);          // 1 - d*y
-    y = f2_fma(y, f2_fma(e, e, e), y);   // y * (1 + e + e^2)
-    e = f2_fma(nd, y, one2);
-    return f2_fma(y, e, y);
-}
-
-// Phase fence for the gate warps.  ptxas is free to move register-only arithmetic across bar.sync, and it does: it
-// hoisted the z and n barriers above the sigmoid(r) math, so the warp sat in the z / n barrier with that math still
-// to do (ncu source view: 130 + 164 cycles of barrier stall per step inside the r phase).  A trap predicated on the
-// phase's results (never taken: the bit pattern is a NaN the arithmetic cannot produce) makes the barrier that follows
-// control-dependent on them.
-__device__ __forceinline__ void phase_fence(F2 a, F2 b) {
-    float a0, a1, b0, b1;
-    f2_get(a, a0, a1);
-    f2_get(b, b0, b1);
-    const uint32_t u = __float_as_uint(a0) & __float_as_uint(a1) & __float_as_uint(b0) & __float_as_uint(b1);
-    if (u == 0xFFFFFFFFu) __trap();
-}
-
-
 // ---- geometry of the recurrent kernels' shared-memory operand tiles (K-major, SWIZZLE_NONE: [k-group][row][8 halfs]) ----
-constexpr int RT_N = 16;                                 // windows per tile (UMMA N)
-constexpr int RT_KG = RT_N * 16 + 16;                    // k-group stride of the h tile: 256 B of rows + 16 B pad, so the
-                                                         // 2-byte stores of 8-lane groups land in different banks
-constexpr int RT_HPLANE = (H / 8) * RT_KG;               // one h plane (hi or lo) of a tile: 4352 B
-constexpr int RT_XPLANE = 2 * RT_KG;                     // one x plane (K = 16): 544 B
-constexpr int RT_XBUF = 2 * RT_XPLANE;                   // hi + lo
-constexpr int RT_WT_COLS = 2 * 3 * (H / 2);              // W_hh hi+lo as TMEM A operand: 384 columns
-constexpr int RT_WX_COLS = 2 * 3 * 8;                    // W_ih (K = 16) hi+lo as TMEM A operand: 48 columns
+constexpr int RT_N = 16;                                 // windows per tile
 constexpr int GI_PREFETCH_STEPS = 3;
-constexpr int X_PREFETCH_EVERY = 8, X_PREFETCH_AHEAD = 16;   // feature rows: 8 steps at a time, 16..23 steps ahead
 constexpr float EXP_CLAMP = 60.0f;
 
 // arguments of the fused input projection (layer 0)

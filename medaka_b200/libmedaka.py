@@ -85,7 +85,7 @@ def device_count():
 
 
 def require_gpu(device=0):
-    """Raise unless a Blackwell (sm_100) device is present - the hot path has no other backend."""
+    """Raise unless a Hopper (sm_90) device is present - the hot path has no other backend."""
     load()
     n = device_count()
     if n <= device:
@@ -94,6 +94,6 @@ def require_gpu(device=0):
     sms = ffi.new("int *")
     mem = ffi.new("size_t *")
     check(lib.mdk_device_info(device, arch, sms, mem))
-    if arch[0] // 10 != 10:
-        raise MedakaB200Error(-102, "device {} is sm_{}; libmedaka_b200 is sm_100a only".format(device, arch[0]))
+    if arch[0] != 90:
+        raise MedakaB200Error(-102, "device {} is sm_{}; libmedaka_b200 is sm_90a only".format(device, arch[0]))
     return {"sm_arch": int(arch[0]), "sm_count": int(sms[0]), "total_mem": int(mem[0])}

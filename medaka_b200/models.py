@@ -56,7 +56,7 @@ class PinnedArray(object):
 
 
 class GRUModel(object):
-    """Bidirectional GRU consensus model (gru.py:10-72) executing on a B200.
+    """Bidirectional GRU consensus model (gru.py:10-72) executing on an H100.
 
     The constructor signature is the reference's, so ``model_from_dict``-style
     configs (medaka/models.py:392-400) instantiate it directly.
@@ -116,7 +116,7 @@ class GRUModel(object):
         return self
 
     def set_precision(self, mode):
-        """'tc' (tcgen05, default) or 'fp32' (CUDA-core FFMA, the --full_precision path)."""
+        """'tc' (wgmma, default) or 'fp32' (CUDA-core FFMA, the --full_precision path)."""
         _lm.check(_lm.lib.mdk_engine_set_precision(self._engine, _PRECISIONS[mode]))
 
     def parameters(self):
@@ -245,7 +245,7 @@ class GRUModel(object):
         Up to ``slots`` calls may be in flight (each owns one set of page-locked staging arrays).  The engine
         packs consecutive batches of the same window length into one-wave groups window by window (mdk_engine_submit;
         a batch may straddle two groups), so ``run_prediction`` keeps about three groups of batches queued: the
-        reference's default 200-window batches then run as 1184-window groups, two computing at a time, with the
+        reference's default 200-window batches then run as 1056-window groups, one computing at a time, with the
         PCIe copies of the neighbouring groups under the compute.
         """
         import torch
@@ -339,7 +339,7 @@ class GRUModel(object):
         _lm.check(_lm.lib.mdk_engine_keep_activations(self._engine, 1 if keep else 0))
 
     def preferred_batch_size(self):
-        """Windows per batch that fill the device in one wave (1184 on a B200); ``batch_size="auto"`` in
+        """Windows per batch that fill the device in one wave (1056 on an H100); ``batch_size="auto"`` in
         ``prediction.run_prediction`` / ``predict_regions`` resolves to this."""
         return int(_lm.lib.mdk_engine_preferred_windows(self._engine))
 

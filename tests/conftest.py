@@ -10,7 +10,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run by `pytest -m gpu` on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with `pytest -m gpu`)")
 
 
 @pytest.fixture(scope="session")

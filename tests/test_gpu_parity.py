@@ -1,4 +1,4 @@
-"""GPU parity tests (run with `pytest -m gpu` on a B200): the CUDA path, called through the C ABI
+"""GPU parity tests (run with `pytest -m gpu` on an H100): the CUDA path, called through the C ABI
 (medaka_b200.libmedaka -> libmedaka_b200.so), against the CPU oracle and the committed golden
 vectors produced by the real reference classes.
 
@@ -56,7 +56,7 @@ def _make_model(sd, F=10, precision="tc"):
     return m
 
 
-# ------------------------------------------------------------------ tcgen05 building block
+# ------------------------------------------------------------------ wgmma building block
 @pytest.mark.parametrize("N,K", [(16, 128), (128, 128), (64, 256), (32, 16)])
 def test_umma_tile_selftest(lm, N, K):
     rs = np.random.RandomState(N * 1000 + K)

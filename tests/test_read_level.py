@@ -40,7 +40,7 @@ def _check(got, want):
 @pytest.mark.parametrize("conv", ["tc", "fp32"])
 @pytest.mark.parametrize("name", ["small", "deep", "dwells", "hot"])
 def test_device_matches_reference_class(name, conv):
-    """Both implementations of the k = 17 convolution: tcgen05 implicit GEMM (default) and fp32 CUDA cores."""
+    """Both implementations of the k = 17 convolution: wgmma implicit GEMM (default) and fp32 CUDA cores."""
     from medaka_b200 import read_level
     g = np.load(GOLD)
     sd, x, dw, want = _case(g, name)

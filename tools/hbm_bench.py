@@ -1,8 +1,7 @@
 #!/usr/bin/env python
-"""Drives every HBM-bound kernel of the path at a realistic size through the C ABI, so that
-    ncu --set full -k regex:"normalise|decode_kernel|head_plog|stitch_|plp_|vd_" python tools/hbm_bench.py
-captures them (tools/hbm_summary.py turns the report into profiles/r02_hbm_kernels.md), and prints wall-clock figures
-of the host-pointer calls (copies included) plus the pileup rate next to the CPU restatement (oracle/pileup_oracle.py).
+"""Drives every HBM-bound kernel of the path at a realistic size through the C ABI (a workload for a kernel profiler),
+and prints wall-clock figures of the host-pointer calls (copies included) plus the pileup rate next to the CPU
+restatement (oracle/pileup_oracle.py).
 
     python tools/hbm_bench.py [--n 4000000] [--reads 20000] [--cpu-pileup]
 """
