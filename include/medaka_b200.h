@@ -250,8 +250,10 @@ int mdk_read_matrix(int device, int64_t n_rec, const int32_t *pos, const uint16_
 /* ---- read-level model seam: LatentSpaceLSTM (medaka/architectures/latent_space_lstm.py:34-207, the model class of the
  * `rl_` consensus models) behind TorchModel.predict_on_batch (medaka/models.py:303-313) with
  * ReadLevelFeaturesModel.get_model_input_features = batch.read_level_features (base_classes.py:29-36).
- *   mdk_rl_create   lstm_size = cnn_size = 128 (the class defaults), 5 classes, kernel sizes [1, 17], mean pooling,
- *                   bidirectional; anything else -> MDK_ERR_UNSUPPORTED
+ *   mdk_rl_create   lstm_size 128 (the class default) or 384 (every released `rl_lstm384_` model) with cnn_size = 128,
+ *                   5 classes, kernel sizes [1, 17], mean pooling, bidirectional; anything else -> MDK_ERR_UNSUPPORTED.
+ *                   At 384 the recurrence runs on 8-CTA thread-block clusters: the first forward fails with
+ *                   MDK_ERR_UNSUPPORTED if no such cluster fits the device
  *   mdk_rl_load     one state-dict tensor by its torch name ("base_embedder.weight", "read_level_conv.convs.0.weight",
  *                   "read_level_conv.convs.2.running_mean", "lstm.weight_ih_l0_reverse", "linear.bias", ...), host float32,
  *                   torch's own layouts; tensors the forward does not use (num_batches_tracked,
@@ -264,10 +266,16 @@ int mdk_rl_create(int device, int32_t lstm_size, int32_t cnn_size, int32_t use_d
 int mdk_rl_destroy(mdk_rl_engine *e);
 int mdk_rl_load(mdk_rl_engine *e, const char *name, const float *data, int64_t n);
 /* which parts run on wgmma with fp16 hi/lo operand pairs (bit set) or on the fp32 CUDA cores (validation twins):
- * bit 0 = the k = 17 convolution (99 % of the network's FLOPs), bit 1 = the LSTM recurrences.  Default 3. */
+ * bit 0 = the k = 17 convolution (99 % of the network's FLOPs at lstm_size 128), bit 1 = the LSTM recurrences (at
+ * lstm_size 384 also the LSTM input projections).  Default 3. */
 int mdk_rl_set_conv(mdk_rl_engine *e, int tensor_cores);
 int mdk_rl_forward(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P, int64_t D, int64_t F,
                    float *probs_host);
+/* per-stage device times of the forwards that follow mdk_rl_set_timing(e, 1) (CUDA events on the engine's stream);
+ * mdk_rl_stage_ms writes the last forward's 6 times in ms: convolution (mask, k = 1 and k = 17 convolutions, pooling
+ * Linear), layer-0 projection, layer-0 recurrence, layer-1 projection, layer-1 recurrence, head */
+int mdk_rl_set_timing(mdk_rl_engine *e, int on);
+int mdk_rl_stage_ms(mdk_rl_engine *e, float *ms);
 
 /* ---- alignment access: what calculate_pileup gets from htslib (create_bam_fset src/medaka_bamiter.c:52-63,
  * bam_itr_querys src/medaka_counts.c:233, the flag / mapQ part of read_bam src/medaka_bamiter.c:19-21).  Native BGZF

@@ -49,6 +49,60 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
+// ---------------------------------------------------------------- thread-block clusters (distributed shared memory)
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+// shared::cta address of this CTA -> shared::cluster address of the same variable in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t mapa_shared(uint32_t smem_addr, uint32_t rank) {
+    uint32_t r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
+    return r;
+}
+__device__ __forceinline__ void st_cluster_u32(uint32_t cluster_addr, uint32_t v) {
+    asm volatile("st.shared::cluster.u32 [%0], %1;" ::"r"(cluster_addr), "r"(v) : "memory");
+}
+// generic-proxy writes to shared memory anywhere in the cluster (st.shared::cluster) -> visible to the async proxy of
+// the CTA that owns the memory, once a release / acquire at cluster scope orders them before its wgmma
+__device__ __forceinline__ void fence_proxy_async_cluster() {
+    asm volatile("fence.proxy.async.shared::cluster;" ::: "memory");
+}
+// arrive on an mbarrier of another CTA of the cluster (address from mapa_shared); release at cluster scope: the
+// arriving thread's prior writes, and those ordered before it by a CTA barrier, are visible to an acquiring waiter
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
+}
+__device__ __forceinline__ bool mbar_try_wait_cluster(uint64_t *bar, uint32_t parity) {
+    uint32_t ok;
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(ok)
+        : "r"(smem_u32(bar)), "r"(parity)
+        : "memory");
+    return ok != 0;
+}
+// bounded like mbar_wait; acquire at cluster scope pairs with mbar_arrive_cluster
+__device__ __forceinline__ void mbar_wait_cluster(uint64_t *bar, uint32_t parity) {
+    if (mbar_try_wait_cluster(bar, parity)) return;
+    const long long t0 = clock64();
+    while (!mbar_try_wait_cluster(bar, parity)) {
+        if (clock64() - t0 > 4000000000LL) __trap();
+    }
+}
+// whole-cluster barrier (all threads of every CTA), release / acquire at cluster scope.  Used once, after the mbarrier
+// initialisation: the CTAs of a cluster are co-scheduled, so it cannot wait on a CTA that has not started.
+__device__ __forceinline__ void cluster_sync_all() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// named barrier over `count` threads (a warpgroup: 128)
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
 // L2 prefetch of a contiguous range (16-B aligned, size % 16 == 0); no destination, no completion tracking
 __device__ __forceinline__ void bulk_prefetch_l2(const void *gmem_src, uint32_t bytes) {
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gmem_src), "r"(bytes) : "memory");

@@ -8,7 +8,8 @@
 //   y2 = BN2(ReLU(Conv1d k=17, zero padding 8 (C -> C)))
 //   z  = mean over the non-empty reads of Linear(C -> H)(y2)                                        :192-197, MeanPooler
 //   two bidirectional LSTM layers (H), Linear(2H -> 5), softmax                                    :198-205
-// Sizes: C = cnn_size = H = lstm_size = 128 (the class defaults); other sizes are refused.  BatchNorm runs in inference
+// Sizes: C = cnn_size = 128 with H = lstm_size = 128 (the class defaults) or 384 (every released read-level model; its
+// LSTM kernels are in the "lstm_size = 384" section below); other sizes are refused.  BatchNorm runs in inference
 // mode (running statistics), in torch's operation order ((x - mean) * invstd * weight + bias).
 //
 // Kernels:
@@ -352,10 +353,12 @@ __global__ void __launch_bounds__(256, 1) rl_conv17_tc_kernel(const int8_t *__re
 
 // ---------------------------------------------------------------------------------------------- mean + Linear(C -> H)
 constexpr int RL_PLT = 16;        // positions per CTA of the pooling kernel
-__global__ void __launch_bounds__(RL_H) rl_pool_linear_kernel(const float *__restrict__ partial, const uint8_t *__restrict__ mask,
+template <int HO>                 // output width H: 128 threads, each owns HO / 128 output units
+__global__ void __launch_bounds__(RL_C) rl_pool_linear_kernel(const float *__restrict__ partial, const uint8_t *__restrict__ mask,
                                                               const float *__restrict__ w_t, const float *__restrict__ bias,
                                                               int64_t P, int D, int n_groups, float *__restrict__ out) {
-    // grid: (position tiles of 16, B); thread = channel while summing, output unit afterwards.  w_t [C k][H] (transposed)
+    // grid: (position tiles of 16, B); thread = channel while summing, output unit(s) afterwards.  w_t [C k][HO] (transposed)
+    constexpr int U = HO / RL_C;
     const int64_t b = blockIdx.y, p0 = (int64_t)blockIdx.x * RL_PLT;
     __shared__ float v[RL_PLT][RL_C];
     __shared__ int n_reads;
@@ -374,17 +377,24 @@ __global__ void __launch_bounds__(RL_H) rl_pool_linear_kernel(const float *__res
     }
     __syncthreads();
     const int h = threadIdx.x;
-    float acc[RL_PLT];
+    float acc[U][RL_PLT];
 #pragma unroll
-    for (int i = 0; i < RL_PLT; ++i) acc[i] = bias[h];
+    for (int u = 0; u < U; ++u)
+#pragma unroll
+        for (int i = 0; i < RL_PLT; ++i) acc[u][i] = bias[h + u * RL_C];
     for (int k = 0; k < RL_C; ++k) {
-        const float w = w_t[k * RL_H + h];
 #pragma unroll
-        for (int i = 0; i < RL_PLT; ++i) acc[i] = fmaf(w, v[i][k], acc[i]);
+        for (int u = 0; u < U; ++u) {
+            const float w = w_t[k * HO + h + u * RL_C];
+#pragma unroll
+            for (int i = 0; i < RL_PLT; ++i) acc[u][i] = fmaf(w, v[i][k], acc[u][i]);
+        }
     }
 #pragma unroll
-    for (int i = 0; i < RL_PLT; ++i)
-        if (p0 + i < P) out[(b * P + p0 + i) * RL_H + h] = acc[i];
+    for (int u = 0; u < U; ++u)
+#pragma unroll
+        for (int i = 0; i < RL_PLT; ++i)
+            if (p0 + i < P) out[(b * P + p0 + i) * HO + h + u * RL_C] = acc[u][i];
 }
 
 // ---------------------------------------------------------------------------------------------- generic fp32 GEMM
@@ -681,14 +691,362 @@ __global__ void __launch_bounds__(LT_THREADS, 1) rl_lstm_tc_kernel(const float *
     }
 }
 
+// ============================================================================================== lstm_size = 384
+// Every released read-level model is `..._rl_lstm384_...`: H = 384 with C = 128.  The convolution and the mask are the
+// kernels above; the pooling Linear is rl_pool_linear_kernel<384>.  What changes is the LSTM: W_hh is 4H x H per
+// direction (2.25 MiB as fp16 hi + lo, more than one SM holds) and the input projections grow nine-fold (7.1 MFLOP per
+// position for both layers and directions), so both get kernels of their own.
+constexpr int RL_H3 = 384;
+constexpr int RL_G43 = 4 * RL_H3;                  // 1536 gate rows per direction
+
+// ---------------------------------------------------------------------------------------------- projections on wgmma
+// gi[M][N] = X[M][K] . W[N][K]^T + bias[N]  (N = 2 dirs x 4H = 3072: both directions in one launch, K = 384 or 768)
+// in the transposed formulation: D[128 gate rows][128 positions] per CTA, warpgroup g owns gate rows 64g .. 64g + 63.
+//   A = W, pre-tiled per (128-row block, 64-wide K chunk) as [hi | lo][k-group 8][row 128][8 halfs] (32 KiB, one bulk copy)
+//   B = X, read as fp32 and split into fp16 hi / lo while it is staged ([hi | lo][k-group 8][position 128][8 halfs])
+// K runs in 64-wide chunks through two stages: while the 12 MMAs of chunk c run, the threads stage the activations of
+// chunk c + 1 and the bulk copy brings its weights.  Three products per contraction (DESIGN §3).
+constexpr int PJ_M = 128;
+constexpr int PJ_N = 128;
+constexpr int PJ_KC = 64;
+constexpr int PJ_WPLANE = (PJ_KC / 8) * PJ_M * 16;          // 16 KiB
+constexpr int PJ_XPLANE = (PJ_KC / 8) * PJ_N * 16;          // 16 KiB
+constexpr int PJ_WCHUNK = 2 * PJ_WPLANE;                    // hi + lo of one weight chunk (the pre-tiled unit in HBM)
+constexpr int PJ_STAGE = PJ_WCHUNK + 2 * PJ_XPLANE;         // 64 KiB
+constexpr int PJ_OFF_BAR = 2 * PJ_STAGE;
+constexpr int PJ_SMEM = PJ_OFF_BAR + 64;
+
+__global__ void __launch_bounds__(256, 1) rl_proj_tc_kernel(const float *__restrict__ X, const uint8_t *__restrict__ w_tc,
+                                                            const float *__restrict__ bias, float *__restrict__ C, int64_t M,
+                                                            int K, int N) {
+    extern __shared__ __align__(128) uint8_t smem_pj[];
+    uint64_t *full = reinterpret_cast<uint64_t *>(smem_pj + PJ_OFF_BAR);
+    const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
+    const int gq = lane >> 2, cq = lane & 3;
+    const int64_t m0 = (int64_t)blockIdx.x * PJ_N;
+    const int rb = blockIdx.y;
+    const int nchunks = K / PJ_KC;
+    if (tid == 0) {
+        mbar_init(&full[0], 1);
+        mbar_init(&full[1], 1);
+        fence_mbar_init();
+    }
+    __syncthreads();
+    auto issue_w = [&](int c) {
+        const int st = c & 1;
+        mbar_arrive_expect_tx(&full[st], PJ_WCHUNK);
+        bulk_g2s(smem_pj + st * PJ_STAGE, w_tc + ((size_t)rb * nchunks + c) * PJ_WCHUNK, PJ_WCHUNK, &full[st]);
+    };
+    auto stage_x = [&](int c) {
+        uint8_t *xs = smem_pj + (c & 1) * PJ_STAGE + PJ_WCHUNK;
+        // 128 positions x 64 k: a lane pair reads one 32-byte sector (8 k of one position) and writes one 16-byte row
+#pragma unroll 2
+        for (int i = tid; i < PJ_N * PJ_KC / 4; i += 256) {
+            const int q2 = i & 1, n = (i >> 1) & (PJ_N - 1), kg = i >> 8;
+            const int64_t p = m0 + n;
+            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (p < M) v = *reinterpret_cast<const float4 *>(X + p * K + c * PJ_KC + kg * 8 + q2 * 4);
+            __half h0, h1, h2, h3, l0, l1, l2, l3;
+            split_f16(v.x, h0, l0); split_f16(v.y, h1, l1); split_f16(v.z, h2, l2); split_f16(v.w, h3, l3);
+            const int off = kg * (PJ_N * 16) + n * 16 + q2 * 8;
+            __half2 hv[2] = {__halves2half2(h0, h1), __halves2half2(h2, h3)};
+            __half2 lv[2] = {__halves2half2(l0, l1), __halves2half2(l2, l3)};
+            *reinterpret_cast<uint2 *>(xs + off) = *reinterpret_cast<uint2 *>(hv);
+            *reinterpret_cast<uint2 *>(xs + PJ_XPLANE + off) = *reinterpret_cast<uint2 *>(lv);
+        }
+    };
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    if (tid == 0) issue_w(0);
+    stage_x(0);
+    fence_proxy_async_smem();
+    for (int c = 0; c < nchunks; ++c) {
+        const int st = c & 1;
+        __syncthreads();             // activations of chunk c staged and fenced; stage st ^ 1 no longer read (chunk c - 1)
+        if (tid == 0 && c + 1 < nchunks) issue_w(c + 1);
+        mbar_wait(&full[st], (uint32_t)(c >> 1) & 1u);
+        wg_fence();
+        const uint32_t wbase = smem_u32(smem_pj + st * PJ_STAGE) + wg * 64 * 16;
+        const uint32_t xbase = smem_u32(smem_pj + st * PJ_STAGE + PJ_WCHUNK);
+#pragma unroll
+        for (int ks = 0; ks < PJ_KC / 16; ++ks) {
+            const uint64_t ah = make_smem_desc(wbase + ks * 2 * (PJ_M * 16), PJ_M * 16, 128);
+            const uint64_t al = make_smem_desc(wbase + PJ_WPLANE + ks * 2 * (PJ_M * 16), PJ_M * 16, 128);
+            const uint64_t bh = make_smem_desc(xbase + ks * 2 * (PJ_N * 16), PJ_N * 16, 128);
+            const uint64_t bl = make_smem_desc(xbase + PJ_XPLANE + ks * 2 * (PJ_N * 16), PJ_N * 16, 128);
+            Wgmma<128>::ss(acc, ah, bh, (c | ks) ? 1u : 0u);
+            Wgmma<128>::ss(acc, ah, bl, 1u);
+            Wgmma<128>::ss(acc, al, bh, 1u);
+        }
+        wg_commit();
+        if (c + 1 < nchunks) {
+            stage_x(c + 1);
+            fence_proxy_async_smem();
+        }
+        wg_wait_all();
+        wg_hold(acc);
+    }
+    // accumulator element k = 4i + 2hb + e: gate row 64wg + 16warp + gq + 8hb, position 8i + 2cq + e
+    const int r0 = rb * PJ_M + wg * 64 + warp * 16 + gq;
+    const float bias0 = bias[r0], bias1 = bias[r0 + 8];
+#pragma unroll
+    for (int k = 0; k < 64; ++k) {
+        const int64_t p = m0 + 8 * (k >> 2) + 2 * cq + (k & 1);
+        const int hb = (k >> 1) & 1;
+        if (p < M) C[p * N + r0 + 8 * hb] = acc[k] + (hb ? bias1 : bias0);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------- recurrence on a cluster
+// Per time step G^T[4H = 1536][16 windows] = W_hh . h^T with h the 16 windows' previous output, split over a cluster of
+// 8 CTAs: CTA rank r owns hidden units 48r .. 48r + 47, i.e. 192 gate rows (4 gates x 48 units), in three warpgroups of
+// 64 rows (16 units x 4 gates, warp w = gate w).
+//   A = W_hh rows: the fp16 hi plane in registers (24 k-steps x 4 = 96 per thread), the lo plane as shared-memory operand
+//       tiles (144 KiB per CTA, pre-tiled per (direction, rank, warpgroup))
+//   B = the full h tile [16 windows][384] (fp16 hi | lo, K-major, double buffered): every CTA holds all 384 units
+//   D = one M64 N16 accumulator per warpgroup, preloaded with the input pre-activations; 24 k-steps x 3 products
+// The four gates of a unit come from four warps: they meet in a 5 KiB exchange buffer per warpgroup (named barrier),
+// where each thread takes two (unit, window) pairs; c stays in its registers.  Each thread writes its two new h values
+// (hi / lo) into the next h buffer of all 8 CTAs with st.shared::cluster, then fences them to the async proxy at cluster
+// scope.  After a CTA barrier, threads 0..7 arrive (release, cluster scope) on the step barrier of CTA 0..7; every
+// thread waits (acquire, cluster scope, bounded) on its own CTA's barrier for all 8 arrivals before the next step's MMAs
+// read the buffer.  That wait after the last step is also the exit barrier: once a CTA has seen its 8 arrivals, no peer
+// writes into its shared memory any more.  The buffer a step writes was last read by the MMAs of the step before, which
+// every CTA completed (wgmma.wait_group) before it arrived.
+constexpr int L3_CL = 8;                                     // CTAs per cluster
+constexpr int L3_UNITS = RL_H3 / L3_CL;                      // 48 hidden units per CTA
+constexpr int L3_THREADS = 384;                              // 3 warpgroups
+constexpr int L3_KS = RL_H3 / 16;                            // 24 k-steps
+constexpr int L3_WLO_WG = (RL_H3 / 8) * 64 * 16;             // 48 KiB: one warpgroup's lo plane as A operand tiles
+constexpr int L3_KG = LT_N * 16 + 16;                        // k-group stride of the h tile (272 B)
+constexpr int L3_HPLANE = (RL_H3 / 8) * L3_KG;               // 13 056 B
+constexpr int L3_XS = 20;                                    // window stride of the gate exchange (floats): no bank conflicts
+constexpr int L3_XCH_WG = 4 * LT_N * L3_XS * 4;              // 5 KiB
+constexpr int L3_OFF_H = 3 * L3_WLO_WG;
+constexpr int L3_OFF_X = L3_OFF_H + 4 * L3_HPLANE;
+constexpr int L3_OFF_BAR = L3_OFF_X + 3 * L3_XCH_WG;
+constexpr int L3_SMEM = L3_OFF_BAR + 16;                     // 210 KiB
+
+__global__ void __cluster_dims__(L3_CL, 1, 1) __launch_bounds__(L3_THREADS, 1)
+    rl_lstm384_tc_kernel(const float *__restrict__ gi, const __half *__restrict__ w_hi, const uint8_t *__restrict__ w_lo_tiles,
+                         float *__restrict__ out, int64_t B, int64_t P) {
+    extern __shared__ __align__(128) uint8_t smem_l3[];
+    uint8_t *swlo = smem_l3;
+    uint8_t *sh = smem_l3 + L3_OFF_H;                            // [buf 2][hi | lo] L3_HPLANE
+    uint64_t *hbar = reinterpret_cast<uint64_t *>(smem_l3 + L3_OFF_BAR);
+    const int tid = threadIdx.x, wg = tid >> 7, wt = tid & 127, warp = (tid >> 5) & 3, lane = tid & 31;
+    const int gq = lane >> 2, cq = lane & 3;
+    const uint32_t rank = cluster_ctarank();
+    const int dir = blockIdx.y;
+    const int64_t b0 = (int64_t)(blockIdx.x / L3_CL) * LT_N;
+    const int nb = (int)min((int64_t)LT_N, B - b0);
+    const int u0 = (int)rank * L3_UNITS + wg * 16;                 // first hidden unit of this warpgroup
+    float *xw = reinterpret_cast<float *>(smem_l3 + L3_OFF_X + wg * L3_XCH_WG);     // [gate 4][window 16][L3_XS]
+    {
+        const uint4 *src = reinterpret_cast<const uint4 *>(w_lo_tiles + ((size_t)dir * L3_CL + rank) * 3 * L3_WLO_WG);
+        for (int i = tid; i < 3 * L3_WLO_WG / 16; i += L3_THREADS) reinterpret_cast<uint4 *>(swlo)[i] = src[i];
+        for (int i = tid; i < 4 * L3_HPLANE / 16; i += L3_THREADS) reinterpret_cast<uint4 *>(sh)[i] = make_uint4(0u, 0u, 0u, 0u);
+    }
+    if (tid == 0) {
+        mbar_init(&hbar[0], L3_CL);
+        mbar_init(&hbar[1], L3_CL);
+        fence_mbar_init();
+    }
+    // hi plane: gate `warp`, units u0 + gq (+8)
+    uint32_t whi[L3_KS][4];
+#pragma unroll
+    for (int ks = 0; ks < L3_KS; ++ks) {
+        const __half *w = w_hi + (((size_t)dir * 4 + warp) * RL_H3 + u0 + gq) * RL_H3 + ks * 16 + 2 * cq;
+        whi[ks][0] = *reinterpret_cast<const uint32_t *>(w);
+        whi[ks][1] = *reinterpret_cast<const uint32_t *>(w + 8 * RL_H3);
+        whi[ks][2] = *reinterpret_cast<const uint32_t *>(w + 8);
+        whi[ks][3] = *reinterpret_cast<const uint32_t *>(w + 8 * RL_H3 + 8);
+    }
+    // accumulator element k = 4i + 2hb + e: unit u0 + gq + 8hb of gate `warp`, window 8i + 2cq + e
+    float acc[8];
+    auto fetch = [&](int64_t t) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const int wdw = 8 * (k >> 2) + 2 * cq + (k & 1);
+            const bool ok = wdw < nb;
+            const float *row = gi + (((b0 + (ok ? wdw : 0)) * P + t) * 2 + dir) * RL_G43 + warp * RL_H3 + u0 + gq + 8 * ((k >> 1) & 1);
+            acc[k] = ok ? __ldg(row) : 0.f;
+        }
+    };
+    // gate math: this thread's pairs are units u0 + ue, u0 + ue + 1 of window we
+    const int ue = 2 * (wt & 7), we = wt >> 3;
+    float c_state[2] = {0.f, 0.f};
+    const int jg = u0 + ue;                                         // even: the two units share one 32-bit h word
+    const uint32_t h_off = (uint32_t)((jg >> 3) * L3_KG + we * 16 + (jg & 7) * 2);
+    uint32_t peer_h[L3_CL];
+#pragma unroll
+    for (int q = 0; q < L3_CL; ++q) peer_h[q] = mapa_shared(smem_u32(sh), (uint32_t)q);
+    const uint32_t bar_peer = tid < L3_CL ? mapa_shared(smem_u32(&hbar[0]), (uint32_t)tid) : 0u;
+    fetch(dir ? (P - 1) : 0);
+    fence_proxy_async_smem();                                     // zeroed h tiles and lo planes -> wgmma
+    cluster_sync_all();                                           // every CTA's barriers initialised, h zeroed
+    const uint32_t wl = smem_u32(swlo) + wg * L3_WLO_WG;
+    for (int64_t step = 0; step < P; ++step) {
+        const int64_t t = dir ? (P - 1 - step) : step;
+        const int buf = (int)(step & 1);
+        const uint32_t h_hi = smem_u32(sh + buf * 2 * L3_HPLANE), h_lo = h_hi + L3_HPLANE;
+        wg_fence();
+#pragma unroll
+        for (int ks = 0; ks < L3_KS; ++ks) {
+            const uint64_t bh = make_smem_desc(h_hi + ks * 2 * L3_KG, L3_KG, 128);
+            Wgmma<16>::rs(acc, whi[ks], bh, 1u);
+            Wgmma<16>::rs(acc, whi[ks], make_smem_desc(h_lo + ks * 2 * L3_KG, L3_KG, 128), 1u);
+            Wgmma<16>::ss(acc, make_smem_desc(wl + ks * 2 * (64 * 16), 64 * 16, 128), bh, 1u);
+        }
+        wg_commit();
+        wg_wait_all();
+        wg_hold(acc);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const int wdw = 8 * (k >> 2) + 2 * cq + (k & 1);
+            xw[(warp * LT_N + wdw) * L3_XS + gq + 8 * ((k >> 1) & 1)] = acc[k];
+        }
+        if (step + 1 < P) fetch(dir ? (t - 1) : (t + 1));           // the next pre-activations load under the gate math
+        named_bar_sync(1 + wg, 128);
+        float hv[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const float *x = xw + we * L3_XS + ue + e;
+            const float ig = lt_sigmoid(x[0]);
+            const float fg = lt_sigmoid(x[1 * LT_N * L3_XS]);
+            const float gg = lt_tanh(x[2 * LT_N * L3_XS]);
+            const float og = lt_sigmoid(x[3 * LT_N * L3_XS]);
+            const float c = fmaf(fg, c_state[e], ig * gg);
+            c_state[e] = c;
+            hv[e] = og * lt_tanh(c);
+        }
+        if (we < nb)
+            *reinterpret_cast<float2 *>(out + ((b0 + we) * P + t) * (2 * RL_H3) + dir * RL_H3 + jg) = make_float2(hv[0], hv[1]);
+        __half hi0, lo0, hi1, lo1;
+        split_f16(hv[0], hi0, lo0);
+        split_f16(hv[1], hi1, lo1);
+        __half2 hp = __halves2half2(hi0, hi1), lp = __halves2half2(lo0, lo1);
+        const uint32_t hw = *reinterpret_cast<uint32_t *>(&hp), lw = *reinterpret_cast<uint32_t *>(&lp);
+        const uint32_t nxt = (uint32_t)((buf ^ 1) * 2 * L3_HPLANE) + h_off;
+#pragma unroll
+        for (int q = 0; q < L3_CL; ++q) {
+            st_cluster_u32(peer_h[q] + nxt, hw);
+            st_cluster_u32(peer_h[q] + nxt + L3_HPLANE, lw);
+        }
+        fence_proxy_async_cluster();
+        __syncthreads();
+        if (tid < L3_CL) mbar_arrive_cluster(bar_peer + (uint32_t)((buf ^ 1) * 8));
+        mbar_wait_cluster(&hbar[buf ^ 1], (uint32_t)(step >> 1) & 1u);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------- fp32 twins at 384
+// The recurrence on the CUDA cores (validation path): one CTA = 8 windows of one direction, thread = hidden unit j with
+// all four gates, W_hh^T [k][4H] read from global memory (2.36 MB per direction, L2-resident), h in shared memory.
+constexpr int R3_NB = 8;
+__global__ void __launch_bounds__(RL_H3) rl_lstm384_kernel(const float *__restrict__ gi, const float *__restrict__ wt,
+                                                           float *__restrict__ out, int64_t B, int64_t P) {
+    __shared__ __align__(16) float hs[R3_NB][RL_H3];
+    const int j = threadIdx.x;
+    const int dir = blockIdx.y;
+    const int64_t b0 = (int64_t)blockIdx.x * R3_NB;
+    const int nb = (int)min((int64_t)R3_NB, B - b0);
+    const float *w = wt + (size_t)dir * RL_H3 * RL_G43 + j;
+#pragma unroll
+    for (int n = 0; n < R3_NB; ++n) hs[n][j] = 0.f;
+    float c_state[R3_NB];
+#pragma unroll
+    for (int n = 0; n < R3_NB; ++n) c_state[n] = 0.f;
+    __syncthreads();
+    for (int64_t step = 0; step < P; ++step) {
+        const int64_t t = dir ? (P - 1 - step) : step;
+        float a[4][R3_NB];
+#pragma unroll
+        for (int n = 0; n < R3_NB; ++n) {
+            const bool ok = n < nb;
+            const float *row = gi + (((b0 + (ok ? n : 0)) * P + t) * 2 + dir) * RL_G43 + j;
+#pragma unroll
+            for (int g = 0; g < 4; ++g) a[g][n] = ok ? __ldg(row + g * RL_H3) : 0.f;
+        }
+#pragma unroll 4
+        for (int k = 0; k < RL_H3; ++k) {
+            float wv[4];
+#pragma unroll
+            for (int g = 0; g < 4; ++g) wv[g] = __ldg(w + (size_t)k * RL_G43 + g * RL_H3);
+#pragma unroll
+            for (int n = 0; n < R3_NB; ++n) {
+                const float hk = hs[n][k];
+#pragma unroll
+                for (int g = 0; g < 4; ++g) a[g][n] = fmaf(wv[g], hk, a[g][n]);
+            }
+        }
+        __syncthreads();                                     // every thread has read h of the previous step
+#pragma unroll
+        for (int n = 0; n < R3_NB; ++n) {
+            const float ig = rl_sigmoid(a[0][n]), fg = rl_sigmoid(a[1][n]), gg = tanhf(a[2][n]), og = rl_sigmoid(a[3][n]);
+            const float c = fg * c_state[n] + ig * gg;
+            c_state[n] = c;
+            const float h = og * tanhf(c);
+            hs[n][j] = h;
+            if (n < nb) out[((b0 + n) * P + t) * (2 * RL_H3) + dir * RL_H3 + j] = h;
+        }
+        __syncthreads();
+    }
+}
+
+// Linear(2H = 768 -> 5) + softmax: one warp per position, 24 inputs per lane, the weights in shared memory
+__global__ void __launch_bounds__(256) rl_head768_kernel(const float *__restrict__ h1, const float *__restrict__ lin_w,
+                                                         const float *__restrict__ lin_b, int64_t n_pos,
+                                                         float *__restrict__ probs) {
+    constexpr int W2 = 2 * RL_H3;
+    __shared__ __align__(16) float ws[NCLS * W2];
+    for (int i = threadIdx.x; i < NCLS * W2; i += blockDim.x) ws[i] = lin_w[i];
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t p = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; p < n_pos; p += nwarps) {
+        float s[NCLS];
+#pragma unroll
+        for (int c = 0; c < NCLS; ++c) s[c] = 0.f;
+#pragma unroll
+        for (int q = 0; q < W2 / 128; ++q) {
+            const int k = q * 128 + lane * 4;
+            const float4 x = ld_stream4(h1 + p * W2 + k);
+#pragma unroll
+            for (int c = 0; c < NCLS; ++c) {
+                const float4 wv = *reinterpret_cast<const float4 *>(ws + c * W2 + k);
+                s[c] = fmaf(x.x, wv.x, fmaf(x.y, wv.y, fmaf(x.z, wv.z, fmaf(x.w, wv.w, s[c]))));
+            }
+        }
+#pragma unroll
+        for (int c = 0; c < NCLS; ++c)
+#pragma unroll
+            for (int m = 16; m >= 1; m >>= 1) s[c] += __shfl_xor_sync(0xffffffffu, s[c], m);
+        float mx = -INFINITY;
+#pragma unroll
+        for (int c = 0; c < NCLS; ++c) { s[c] += lin_b[c]; mx = fmaxf(mx, s[c]); }
+        float sum = 0.f;
+#pragma unroll
+        for (int c = 0; c < NCLS; ++c) { s[c] = expf(s[c] - mx); sum += s[c]; }
+        if (lane < NCLS) {
+            float v = s[0];
+#pragma unroll
+            for (int c = 1; c < NCLS; ++c) if (lane == c) v = s[c];
+            probs[p * NCLS + lane] = v / sum;
+        }
+    }
+}
+
 // ---------------------------------------------------------------------------------------------- engine
 struct RlLstmLayer {
     __half *w_hi = nullptr;     // [2][4H][H] fp16 hi plane of W_hh (tensor-core kernel: -> registers)
     uint8_t *w_lo = nullptr;    // [2][4 gates][k-group 16][row 128][8 halfs] lo plane as shared-memory A operand tiles
     float *w_ih = nullptr;      // [2 dirs * 4H][in]   (both directions stacked: one GEMM)
     float *bias = nullptr;      // [2 * 4H]  b_ih + b_hh
-    float *w3t = nullptr;       // [2][H][3H]
-    float *wo = nullptr;        // [2][H][H]
+    float *w3t = nullptr;       // H = 128: [2][H][3H];   H = 384: W_hh^T [2][H k][4H] (fp32 recurrence)
+    float *wo = nullptr;        // [2][H][H]  (H = 128)
+    uint8_t *w_ih_tc = nullptr; // H = 384: W_ih as rl_proj_tc_kernel's A tiles [row block 24][K chunk][hi | lo][8][128][8]
 };
 
 }  // namespace mdk
@@ -698,6 +1056,10 @@ using namespace mdk;
 struct mdk_rl_engine {
     int device = 0;
     int use_dwells = 0;
+    int H = RL_H;                  // lstm_size: 128 or 384
+    int timing = 0;                // record per-stage CUDA events in mdk_rl_forward
+    cudaEvent_t ev[7] = {};
+    float stage_ms[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     std::unordered_map<std::string, std::vector<float>> host;     // state-dict tensors as loaded
     bool prepared = false;
     // device parameters
@@ -738,10 +1100,91 @@ const std::vector<float> *rl_get(mdk_rl_engine *e, const std::string &name, size
     return &it->second;
 }
 
+template <class T>
+int rl_upload_raw(mdk_rl_engine *e, const std::vector<T> &v, T **out) {
+    void *p = nullptr;
+    MDK_CUDA(cudaMalloc(&p, v.size() * sizeof(T)));
+    e->allocs.push_back(p);
+    MDK_CUDA(cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+    *out = static_cast<T *>(p);
+    return MDK_OK;
+}
+
+// LSTM weights at H = 384: fp32 copies for the CUDA-core twins, fp16 hi / lo operand tiles for the tensor-core kernels
+int rl_prepare_lstm384(mdk_rl_engine *e) {
+    constexpr int H3 = RL_H3, G4 = RL_G43;
+    int rc;
+    for (int l = 0; l < 2; ++l) {
+        const int in = l == 0 ? H3 : 2 * H3;
+        const int nchunks = in / PJ_KC;
+        std::vector<float> w_ih((size_t)2 * G4 * in), bias((size_t)2 * G4), wt((size_t)2 * H3 * G4);
+        std::vector<__half> hi((size_t)2 * G4 * H3), lo_t((size_t)2 * G4 * H3), ih_t((size_t)2 * G4 * in * 2);
+        for (int d = 0; d < 2; ++d) {
+            const std::string sfx = "_l" + std::to_string(l) + (d ? "_reverse" : "");
+            const std::vector<float> *wih = rl_get(e, "lstm.weight_ih" + sfx, (size_t)G4 * in);
+            const std::vector<float> *whh = rl_get(e, "lstm.weight_hh" + sfx, (size_t)G4 * H3);
+            const std::vector<float> *bih = rl_get(e, "lstm.bias_ih" + sfx, G4);
+            const std::vector<float> *bhh = rl_get(e, "lstm.bias_hh" + sfx, G4);
+            if (!wih || !whh || !bih || !bhh) return MDK_ERR_STATE;
+            std::copy(wih->begin(), wih->end(), w_ih.begin() + (size_t)d * G4 * in);
+            for (int r = 0; r < G4; ++r) bias[(size_t)d * G4 + r] = (*bih)[r] + (*bhh)[r];
+            for (int r = 0; r < G4; ++r)
+                for (int k = 0; k < H3; ++k) {
+                    const float v = (*whh)[(size_t)r * H3 + k];
+                    wt[((size_t)d * H3 + k) * G4 + r] = v;
+                    const __half h16 = __float2half_rn(v), l16 = __float2half_rn(v - __half2float(h16));
+                    hi[((size_t)d * G4 + r) * H3 + k] = h16;
+                    // lo tiles per (direction, cluster rank, warpgroup): row m = 16 gate + unit within the warpgroup
+                    const int gate = r / H3, j = r % H3, rank = j / L3_UNITS, wg = (j % L3_UNITS) / 16, m = gate * 16 + j % 16;
+                    lo_t[(((size_t)(d * L3_CL + rank) * 3 + wg) * (H3 / 8) + k / 8) * (64 * 8) + m * 8 + k % 8] = l16;
+                }
+        }
+        // W_ih of both directions as one [3072][in] matrix, tiled per (128-row block, 64-wide K chunk)
+        for (int r = 0; r < 2 * G4; ++r)
+            for (int k = 0; k < in; ++k) {
+                const float v = w_ih[(size_t)r * in + k];
+                const __half h16 = __float2half_rn(v), l16 = __float2half_rn(v - __half2float(h16));
+                const size_t chunk = ((size_t)(r / PJ_M) * nchunks + k / PJ_KC) * (PJ_WCHUNK / 2);
+                const size_t off = (size_t)((k % PJ_KC) / 8) * (PJ_M * 8) + (r % PJ_M) * 8 + k % 8;
+                ih_t[chunk + off] = h16;
+                ih_t[chunk + PJ_WPLANE / 2 + off] = l16;
+            }
+        if ((rc = rl_upload(e, w_ih, &e->lstm[l].w_ih)) || (rc = rl_upload(e, bias, &e->lstm[l].bias)) ||
+            (rc = rl_upload(e, wt, &e->lstm[l].w3t)) || (rc = rl_upload_raw(e, hi, &e->lstm[l].w_hi)))
+            return rc;
+        __half *p = nullptr;
+        if ((rc = rl_upload_raw(e, lo_t, &p))) return rc;
+        e->lstm[l].w_lo = reinterpret_cast<uint8_t *>(p);
+        if ((rc = rl_upload_raw(e, ih_t, &p))) return rc;
+        e->lstm[l].w_ih_tc = reinterpret_cast<uint8_t *>(p);
+    }
+    return MDK_OK;
+}
+
 int rl_prepare(mdk_rl_engine *e) {
     if (e->prepared) return MDK_OK;
     const int nin = RL_EMB + 1 + (e->use_dwells ? 1 : 0);
+    const int HH = e->H;
     int rc;
+    if (HH == RL_H3) {   // one 8-CTA cluster of the recurrence must fit the device
+        MDK_CUDA(cudaFuncSetAttribute(rl_lstm384_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L3_SMEM));
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3(L3_CL, 2);
+        cfg.blockDim = dim3(L3_THREADS);
+        cfg.dynamicSmemBytes = L3_SMEM;
+        cudaLaunchAttribute attr;
+        attr.id = cudaLaunchAttributeClusterDimension;
+        attr.val.clusterDim.x = L3_CL;
+        attr.val.clusterDim.y = 1;
+        attr.val.clusterDim.z = 1;
+        cfg.attrs = &attr;
+        cfg.numAttrs = 1;
+        int clusters = 0;
+        MDK_CUDA(cudaOccupancyMaxActiveClusters(&clusters, (void *)rl_lstm384_tc_kernel, &cfg));
+        MDK_REQUIRE(clusters >= 1, MDK_ERR_UNSUPPORTED,
+                    "read-level model: lstm_size = 384 needs a cluster of 8 CTAs with 210 KiB of shared memory each; "
+                    "none fits this device");
+    }
 #define RL_NEED(var, name, n) const std::vector<float> *var = rl_get(e, name, (size_t)(n)); if (!var) return MDK_ERR_STATE;
     RL_NEED(eb, "base_embedder.weight", 6 * RL_EMB)
     RL_NEED(es, "strand_embedder.weight", 3 * RL_EMB)
@@ -749,18 +1192,18 @@ int rl_prepare(mdk_rl_engine *e) {
     RL_NEED(c1b, "read_level_conv.convs.0.bias", RL_C)
     RL_NEED(c17w, "read_level_conv.convs.3.weight", RL_C * RL_C * RL_TAPS)
     RL_NEED(c17b, "read_level_conv.convs.3.bias", RL_C)
-    RL_NEED(pw, "pre_pool_expansion_layer.weight", RL_H * RL_C)
-    RL_NEED(pb, "pre_pool_expansion_layer.bias", RL_H)
-    RL_NEED(lw, "linear.weight", NCLS * 2 * RL_H)
+    RL_NEED(pw, "pre_pool_expansion_layer.weight", HH * RL_C)
+    RL_NEED(pb, "pre_pool_expansion_layer.bias", HH)
+    RL_NEED(lw, "linear.weight", NCLS * 2 * HH)
     RL_NEED(lb, "linear.bias", NCLS)
     if ((rc = rl_upload(e, *eb, &e->emb_base)) || (rc = rl_upload(e, *es, &e->emb_strand)) || (rc = rl_upload(e, *c1w, &e->c1_w)) ||
         (rc = rl_upload(e, *c1b, &e->c1_b)) || (rc = rl_upload(e, *c17b, &e->c17_b)) ||
         (rc = rl_upload(e, *pb, &e->pool_b)) || (rc = rl_upload(e, *lw, &e->lin_w)) || (rc = rl_upload(e, *lb, &e->lin_b)))
         return rc;
     {   // Linear(C -> H) weights transposed to [k][h]: coalesced across the output units
-        std::vector<float> wt((size_t)RL_C * RL_H);
-        for (int h = 0; h < RL_H; ++h)
-            for (int k = 0; k < RL_C; ++k) wt[(size_t)k * RL_H + h] = (*pw)[(size_t)h * RL_C + k];
+        std::vector<float> wt((size_t)RL_C * HH);
+        for (int h = 0; h < HH; ++h)
+            for (int k = 0; k < RL_C; ++k) wt[(size_t)k * HH + h] = (*pw)[(size_t)h * RL_C + k];
         if ((rc = rl_upload(e, wt, &e->pool_w))) return rc;
     }
     // conv k = 17 weights: torch [out][in][tap] -> [tap][in][out]
@@ -801,6 +1244,11 @@ int rl_prepare(mdk_rl_engine *e) {
         if ((rc = rl_upload(e, *mean, &dst[0])) || (rc = rl_upload(e, invstd, &dst[1])) || (rc = rl_upload(e, *w, &dst[2])) ||
             (rc = rl_upload(e, *b, &dst[3])))
             return rc;
+    }
+    if (HH == RL_H3) {
+        if ((rc = rl_prepare_lstm384(e))) return rc;
+        e->prepared = true;
+        return MDK_OK;
     }
     for (int l = 0; l < 2; ++l) {
         const int in = l == 0 ? RL_H : 2 * RL_H;
@@ -862,13 +1310,15 @@ int mdk_rl_create(int device, int32_t lstm_size, int32_t cnn_size, int32_t use_d
                   mdk_rl_engine **out) {
     MDK_REQUIRE(out, MDK_ERR_ARG, "rl_create: out is NULL");
     *out = nullptr;
-    MDK_REQUIRE(lstm_size == RL_H && cnn_size == RL_C, MDK_ERR_UNSUPPORTED, "rl_create: lstm_size = cnn_size = 128 only");
+    MDK_REQUIRE((lstm_size == RL_H || lstm_size == RL_H3) && cnn_size == RL_C, MDK_ERR_UNSUPPORTED,
+                "rl_create: supported sizes are lstm_size 128 or 384 with cnn_size 128");
     MDK_REQUIRE(num_classes == NCLS, MDK_ERR_UNSUPPORTED, "rl_create: 5 classes only");
     MDK_CUDA(cudaSetDevice(device));
     mdk_rl_engine *e = new (std::nothrow) mdk_rl_engine();
     MDK_REQUIRE(e, MDK_ERR_NOMEM, "rl_create: out of host memory");
     e->device = device;
     e->use_dwells = use_dwells ? 1 : 0;
+    e->H = lstm_size;
     {
         const char *v = getenv("MDK_RL_CONV");      // "fp32": CUDA-core convolution (validation)
         if (v && v[0] == 'f') { e->conv_tc = 0; e->lstm_tc = 0; }
@@ -883,6 +1333,8 @@ int mdk_rl_destroy(mdk_rl_engine *e) {
     if (!e) return MDK_OK;
     cudaSetDevice(e->device);
     if (e->stream) { cudaStreamSynchronize(e->stream); cudaStreamDestroy(e->stream); }
+    for (cudaEvent_t ev : e->ev)
+        if (ev) cudaEventDestroy(ev);
     for (void *p : e->allocs) cudaFree(p);
     if (e->scratch) cudaFree(e->scratch);
     delete e;
@@ -904,6 +1356,22 @@ int mdk_rl_set_conv(mdk_rl_engine *e, int tensor_cores) {
     return MDK_OK;
 }
 
+int mdk_rl_set_timing(mdk_rl_engine *e, int on) {
+    MDK_REQUIRE(e, MDK_ERR_ARG, "rl_set_timing: engine is NULL");
+    if (on && !e->ev[0]) {
+        MDK_CUDA(cudaSetDevice(e->device));
+        for (cudaEvent_t &ev : e->ev) MDK_CUDA(cudaEventCreate(&ev));
+    }
+    e->timing = on ? 1 : 0;
+    return MDK_OK;
+}
+
+int mdk_rl_stage_ms(mdk_rl_engine *e, float *ms) {
+    MDK_REQUIRE(e && ms, MDK_ERR_ARG, "rl_stage_ms: NULL argument");
+    for (int i = 0; i < 6; ++i) ms[i] = e->stage_ms[i];
+    return MDK_OK;
+}
+
 int mdk_rl_forward(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P, int64_t D, int64_t F, float *probs_host) {
     MDK_REQUIRE(e && x_host && probs_host, MDK_ERR_ARG, "rl_forward: NULL argument");
     MDK_REQUIRE(B >= 1 && P >= 1 && D >= 1, MDK_ERR_ARG, "rl_forward: need B, P, D >= 1");
@@ -917,12 +1385,13 @@ int mdk_rl_forward(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P,
     const int dgroup = 4;
     const int n_groups = (int)((D + dgroup - 1) / dgroup);
     const int64_t BP = B * P;
+    const int HH = e->H;
     size_t off = 0;
     auto take = [&off](size_t bytes) { size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
     const size_t o_x = take((size_t)BP * D * F), o_mask = take((size_t)B * D), o_y1 = take(e->conv_tc ? 256 : (size_t)B * D * P * RL_C * 4),
-                 o_part = take((size_t)B * n_groups * P * RL_C * 4), o_z = take((size_t)BP * RL_H * 4),
-                 o_gi = take((size_t)BP * 2 * RL_G4 * 4), o_h0 = take((size_t)BP * 2 * RL_H * 4),
-                 o_h1 = take((size_t)BP * 2 * RL_H * 4), o_probs = take((size_t)BP * NCLS * 4);
+                 o_part = take((size_t)B * n_groups * P * RL_C * 4), o_z = take((size_t)BP * HH * 4),
+                 o_gi = take((size_t)BP * 2 * 4 * HH * 4), o_h0 = take((size_t)BP * 2 * HH * 4),
+                 o_h1 = take((size_t)BP * 2 * HH * 4), o_probs = take((size_t)BP * NCLS * 4);
     if (off > e->scratch_bytes) {
         if (e->scratch) cudaFree(e->scratch);
         e->scratch = nullptr;
@@ -937,6 +1406,8 @@ int mdk_rl_forward(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P,
           *d_gi = (float *)(buf + o_gi), *d_h0 = (float *)(buf + o_h0), *d_h1 = (float *)(buf + o_h1),
           *d_probs = (float *)(buf + o_probs);
     MDK_CUDA(cudaMemcpyAsync(d_x, x_host, (size_t)BP * D * F, cudaMemcpyHostToDevice, s));
+    auto mark = [e, s](int i) { if (e->timing) cudaEventRecord(e->ev[i], s); };
+    mark(0);
     rl_mask_kernel<<<(unsigned)(B * D), 256, 0, s>>>(d_x, P, (int)D, (int)F, d_mask);
     RlConv1 c1{e->emb_base, e->emb_strand, e->c1_w, e->c1_b, e->bn1[0], e->bn1[1], e->bn1[2], e->bn1[3]};
     RlConv17 c17{e->c17_wt, e->c17_b, e->bn2[0], e->bn2[1], e->bn2[2], e->bn2[3]};
@@ -951,29 +1422,65 @@ int mdk_rl_forward(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P,
         rl_conv17_pool_kernel<<<dim3((unsigned)((P + RL_PT - 1) / RL_PT), (unsigned)n_groups, (unsigned)B), 256, RL_CONV_SMEM, s>>>(
             d_y1, d_mask, c17, P, (int)D, dgroup, d_part);
     }
-    rl_pool_linear_kernel<<<dim3((unsigned)((P + RL_PLT - 1) / RL_PLT), (unsigned)B), RL_H, 0, s>>>(d_part, d_mask, e->pool_w, e->pool_b, P, (int)D,
-                                                                          n_groups, d_z);
-    MDK_CUDA(cudaFuncSetAttribute(rl_lstm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RL_LSTM_SMEM));
     const float *layer_in = d_z;
     float *layer_out[2] = {d_h0, d_h1};
-    for (int l = 0; l < 2; ++l) {
-        const int in = l == 0 ? RL_H : 2 * RL_H;
-        rl_gemm_kernel<<<dim3((unsigned)((BP + 127) / 128), 2 * RL_G4 / 128), 256, 0, s>>>(layer_in, e->lstm[l].w_ih, e->lstm[l].bias,
-                                                                                       d_gi, BP, in, 2 * RL_G4);
-        if (e->lstm_tc) {
-            MDK_CUDA(cudaFuncSetAttribute(rl_lstm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LT_SMEM));
-            rl_lstm_tc_kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N), 2), LT_THREADS, LT_SMEM, s>>>(d_gi, e->lstm[l].w_hi, e->lstm[l].w_lo,
-                                                                                            layer_out[l], B, P);
-        } else {
-            rl_lstm_kernel<<<dim3((unsigned)((B + RL_NB - 1) / RL_NB), 2), 256, RL_LSTM_SMEM, s>>>(d_gi, e->lstm[l].w3t, e->lstm[l].wo,
-                                                                                                layer_out[l], B, P);
+    if (HH == RL_H3) {
+        rl_pool_linear_kernel<RL_H3><<<dim3((unsigned)((P + RL_PLT - 1) / RL_PLT), (unsigned)B), RL_C, 0, s>>>(
+            d_part, d_mask, e->pool_w, e->pool_b, P, (int)D, n_groups, d_z);
+        mark(1);
+        for (int l = 0; l < 2; ++l) {
+            const int in = l == 0 ? RL_H3 : 2 * RL_H3;
+            if (e->lstm_tc) {
+                MDK_CUDA(cudaFuncSetAttribute(rl_proj_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PJ_SMEM));
+                rl_proj_tc_kernel<<<dim3((unsigned)((BP + PJ_N - 1) / PJ_N), 2 * RL_G43 / PJ_M), 256, PJ_SMEM, s>>>(
+                    layer_in, e->lstm[l].w_ih_tc, e->lstm[l].bias, d_gi, BP, in, 2 * RL_G43);
+                mark(2 + 2 * l);
+                rl_lstm384_tc_kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N * L3_CL), 2), L3_THREADS, L3_SMEM, s>>>(
+                    d_gi, e->lstm[l].w_hi, e->lstm[l].w_lo, layer_out[l], B, P);
+            } else {
+                rl_gemm_kernel<<<dim3((unsigned)((BP + 127) / 128), 2 * RL_G43 / 128), 256, 0, s>>>(
+                    layer_in, e->lstm[l].w_ih, e->lstm[l].bias, d_gi, BP, in, 2 * RL_G43);
+                mark(2 + 2 * l);
+                rl_lstm384_kernel<<<dim3((unsigned)((B + R3_NB - 1) / R3_NB), 2), RL_H3, 0, s>>>(d_gi, e->lstm[l].w3t,
+                                                                                               layer_out[l], B, P);
+            }
+            mark(3 + 2 * l);
+            layer_in = layer_out[l];
         }
-        layer_in = layer_out[l];
+        MDK_CUDA(cudaGetLastError());
+        int64_t blocks = (BP + 7) / 8;
+        if (blocks > 132 * 8) blocks = 132 * 8;
+        rl_head768_kernel<<<(unsigned)blocks, 256, 0, s>>>(d_h1, e->lin_w, e->lin_b, BP, d_probs);
+        MDK_CUDA(cudaGetLastError());
+    } else {
+        rl_pool_linear_kernel<RL_H><<<dim3((unsigned)((P + RL_PLT - 1) / RL_PLT), (unsigned)B), RL_H, 0, s>>>(d_part, d_mask, e->pool_w, e->pool_b, P,
+                                                                                                     (int)D, n_groups, d_z);
+        mark(1);
+        MDK_CUDA(cudaFuncSetAttribute(rl_lstm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RL_LSTM_SMEM));
+        for (int l = 0; l < 2; ++l) {
+            const int in = l == 0 ? RL_H : 2 * RL_H;
+            rl_gemm_kernel<<<dim3((unsigned)((BP + 127) / 128), 2 * RL_G4 / 128), 256, 0, s>>>(layer_in, e->lstm[l].w_ih, e->lstm[l].bias,
+                                                                                           d_gi, BP, in, 2 * RL_G4);
+            mark(2 + 2 * l);
+            if (e->lstm_tc) {
+                MDK_CUDA(cudaFuncSetAttribute(rl_lstm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LT_SMEM));
+                rl_lstm_tc_kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N), 2), LT_THREADS, LT_SMEM, s>>>(d_gi, e->lstm[l].w_hi, e->lstm[l].w_lo,
+                                                                                                layer_out[l], B, P);
+            } else {
+                rl_lstm_kernel<<<dim3((unsigned)((B + RL_NB - 1) / RL_NB), 2), 256, RL_LSTM_SMEM, s>>>(d_gi, e->lstm[l].w3t, e->lstm[l].wo,
+                                                                                                    layer_out[l], B, P);
+            }
+            mark(3 + 2 * l);
+            layer_in = layer_out[l];
+        }
+        MDK_CUDA(cudaGetLastError());
+        MDK_CUDA(launch_head(d_h1, e->lin_w, e->lin_b, B, P, 0, d_probs, nullptr, nullptr, s));
     }
-    MDK_CUDA(cudaGetLastError());
-    MDK_CUDA(launch_head(d_h1, e->lin_w, e->lin_b, B, P, 0, d_probs, nullptr, nullptr, s));
+    mark(6);
     MDK_CUDA(cudaMemcpyAsync(probs_host, d_probs, (size_t)BP * NCLS * 4, cudaMemcpyDeviceToHost, s));
     MDK_CUDA(cudaStreamSynchronize(s));
+    if (e->timing)   // convolution (mask + conv + pooling Linear), projection / recurrence of each layer, head
+        for (int i = 0; i < 6; ++i) MDK_CUDA(cudaEventElapsedTime(&e->stage_ms[i], e->ev[i], e->ev[i + 1]));
     return MDK_OK;
 }
 

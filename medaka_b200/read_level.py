@@ -35,7 +35,9 @@ class LatentSpaceLSTM(object):
         pe = ffi.new("mdk_rl_engine **")
         _lm.check(lib.mdk_rl_create(device, lstm_size, cnn_size, 1 if use_dwells else 0, num_classes, pe))
         self._engine = pe[0]
-        self.max_cells = 1 << 26            # positions x reads per device call (bounds the per-call device scratch)
+        self.max_cells = 1 << 26            # positions x reads per device call
+        self.max_bytes = 8 << 30            # device scratch per call (mdk_rl_forward's intermediates), bytes
+        self._fp32_conv = False
 
     # ---- TorchModel interface (medaka/models.py:233-313) ----
     def load_state_dict(self, state_dict, strict=True):
@@ -52,6 +54,25 @@ class LatentSpaceLSTM(object):
         if lstm_tensor_cores is None:
             lstm_tensor_cores = tensor_cores
         _lm.check(_lm.lib.mdk_rl_set_conv(self._engine, (1 if tensor_cores else 0) | (2 if lstm_tensor_cores else 0)))
+        self._fp32_conv = not tensor_cores
+
+    STAGES = ("convolution", "projection_0", "recurrence_0", "projection_1", "recurrence_1", "head")
+
+    def set_timing(self, on=True):
+        """Record per-stage device times (CUDA events) in the forwards that follow; read them with stage_ms()."""
+        _lm.check(_lm.lib.mdk_rl_set_timing(self._engine, 1 if on else 0))
+
+    def stage_ms(self):
+        """Device time of each stage of the last device call, in ms, keyed by the names in STAGES."""
+        ms = _lm.ffi.new("float[6]")
+        _lm.check(_lm.lib.mdk_rl_stage_ms(self._engine, ms))
+        return dict(zip(self.STAGES, (float(v) for v in ms)))
+
+    def scratch_bytes_per_window(self, P, D, F):
+        """Device scratch one window of P positions and D reads takes in mdk_rl_forward (its intermediates)."""
+        H, groups = self.lstm_size, -(-D // 4)
+        per_pos = D * F + groups * 512 + 4 * H + 32 * H + 16 * H + 20 + (D * 512 if self._fp32_conv else 0)
+        return P * per_pos + D
 
     def eval(self):
         return self
@@ -85,7 +106,9 @@ class LatentSpaceLSTM(object):
         B, P, D, F = x.shape
         lib, ffi = _lm.lib, _lm.ffi
         probs = np.empty((B, P, 5), dtype=np.float32)
-        step = max(1, int(self.max_cells // max(P * D, 1)))
+        # windows per device call: bounded in cells and in scratch bytes (at lstm_size 384, gi alone takes 12 KiB per
+        # position); the windows are independent, so the split does not change the outputs
+        step = max(1, min(int(self.max_cells // max(P * D, 1)), int(self.max_bytes // self.scratch_bytes_per_window(P, D, F))))
         for b0 in range(0, B, step):
             xb = np.ascontiguousarray(x[b0:b0 + step])
             pb = probs[b0:b0 + step]
