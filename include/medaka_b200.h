@@ -147,13 +147,22 @@ int mdk_engine_wait(mdk_engine *e, int64_t ticket);
 int mdk_engine_flush(mdk_engine *e);
 /* most windows coalesced into one group; 0 (default) = one wave, 1 = never coalesce */
 int mdk_engine_set_group_windows(mdk_engine *e, int64_t windows);
-/* same forward with DEVICE buffers (inputs resident in HBM); asynchronous on the next compute lane (consecutive calls
- * alternate lanes and may overlap: give them distinct output buffers), complete after mdk_engine_sync(). */
+/* same forward with DEVICE buffers (inputs resident in HBM); asynchronous, complete after mdk_engine_sync().  Calls are
+ * packed into groups exactly like submitted batches: the features are copied into the open group's staging when the
+ * call is made, a call that does not fit what is left of the group is split, and the group is launched when full, when
+ * T changes, or on flush / sync; results are copied from the staging into the call's own buffers (each output buffer is
+ * written only by the pieces of its call).  So the tail of one call (say 55 windows) runs together with the head of
+ * the next instead of as a forward that fills a few SMs for as long as a full one.  A call of more windows than a
+ * group holds runs as one forward of its own.  feats_dev and the outputs must stay untouched until the sync; give
+ * calls that may be in flight together distinct output buffers. */
 int mdk_engine_forward_dev(mdk_engine *e, const float *feats_dev, int64_t B, int64_t T,
                            float *probs_dev, float *logits_dev, uint8_t *labels_dev);
 int mdk_engine_sync(mdk_engine *e);
+/* mdk_engine_mean_timings(e, 1, out) */
 int mdk_engine_last_timings(mdk_engine *e, mdk_timings *out);
-/* mean per-stage device times over the last n_last (<= 32) forward calls */
+/* mean per-stage device times over the last min(n_last, groups launched) forwards, n_last <= 32.  A "forward" here is
+ * one launched group (one pass of the kernels over all of its windows), not one call: there can be fewer groups than
+ * calls.  A group that is still open is launched first, as mdk_engine_sync does. */
 int mdk_engine_mean_timings(mdk_engine *e, int n_last, mdk_timings *out);
 /* bracket a timed region on the engine stream with CUDA events (bench.py) */
 int mdk_engine_timer_start(mdk_engine *e);
@@ -367,9 +376,9 @@ int mdk_selftest_umma(int device, const float *A, const float *B, float *D, int 
                       int variant);
 
 /* ---- diagnostics -------------------------------------------------------------------------
- * completion times (ms after mdk_engine_timer_start's event) of the eight stage events of the last n_last forwards,
- * oldest first: out is float[n_last][8] = start, features in, inproj0, rec0, inproj1, rec1, head, end.  Shows how the
- * lanes' kernels actually interleaved. */
+ * completion times (ms after mdk_engine_timer_start's event) of the eight stage events of the last n_last launched
+ * groups, oldest first: out is float[n_last][8] = start, features in, inproj0, rec0, inproj1, rec1, head, end.  Shows
+ * how the lanes' kernels actually interleaved.  An open group is launched first. */
 int mdk_debug_timeline(mdk_engine *e, int n_last, float *out);
 /* partial logits of the last forward on the fused-head path: float32 [2 directions][tiles][T][5 classes][16 windows]
  * (what the layer-1 recurrence writes instead of h1); per-direction parity checks of the fused linear head */

@@ -229,7 +229,8 @@ static int acquire_lane(mdk_engine *e, int64_t P, int *out) {
     return MDK_OK;
 }
 
-// Seal the open group: one forward over all of its windows, then the results back to each batch's host buffers.
+// Seal the open group: one forward over all of its windows, then the results back to each call's buffers (host or
+// device: cudaMemcpyDefault).
 static int launch_group(mdk_engine *e) {
     if (e->open_lane < 0) return MDK_OK;
     mdk_lane &ln = e->lane[e->open_lane];
@@ -252,14 +253,77 @@ static int launch_group(mdk_engine *e) {
     int64_t w0 = 0;
     for (const mdk_lane::Item &it : ln.items) {
         const size_t P = (size_t)it.B * ln.gT, off = (size_t)w0 * ln.gT;
-        MDK_CUDA(cudaMemcpyAsync(it.probs, ln.d_probs + off * NCLS, P * NCLS * sizeof(float), cudaMemcpyDeviceToHost, e->copy_out));
+        MDK_CUDA(cudaMemcpyAsync(it.probs, ln.d_probs + off * NCLS, P * NCLS * sizeof(float), cudaMemcpyDefault, e->copy_out));
         if (it.logits)
-            MDK_CUDA(cudaMemcpyAsync(it.logits, ln.d_logits + off * NCLS, P * NCLS * sizeof(float), cudaMemcpyDeviceToHost, e->copy_out));
-        if (it.labels) MDK_CUDA(cudaMemcpyAsync(it.labels, ln.d_labels + off, P, cudaMemcpyDeviceToHost, e->copy_out));
+            MDK_CUDA(cudaMemcpyAsync(it.logits, ln.d_logits + off * NCLS, P * NCLS * sizeof(float), cudaMemcpyDefault, e->copy_out));
+        if (it.labels) MDK_CUDA(cudaMemcpyAsync(it.labels, ln.d_labels + off, P, cudaMemcpyDefault, e->copy_out));
         w0 += it.B;
     }
     MDK_CUDA(cudaEventRecord(ln.ev_out, e->copy_out));
     ln.busy = true;
+    return MDK_OK;
+}
+
+// Most windows one group collects: one wave unless mdk_engine_set_group_windows says otherwise.
+static int64_t group_limit(mdk_engine *e) {
+    return e->group_windows > 0 ? e->group_windows : mdk_engine_preferred_windows(e);
+}
+
+// One call's windows into the open group, window by window: a call that does not fit what is left of the group is split
+// (windows are independent, medaka/prediction.py:40-52 treats every row of a batch separately), so every group of a long
+// run holds gmax windows however the caller sized its calls.  Features are copied into the group's staging as they
+// arrive; results go back to each piece's own range of the call's buffers when the group completes.  Host and device
+// buffers take the same path (cudaMemcpyDefault).  ticket (may be NULL) follows the call's last piece.
+static int enqueue(mdk_engine *e, const float *feats, int64_t B, int64_t T, float *probs, float *logits,
+                   uint8_t *labels, int64_t gmax, int64_t *ticket) {
+    int rc;
+    const int64_t F = e->desc.num_features;
+    if (e->open_lane >= 0 && e->lane[e->open_lane].gT != T && (rc = launch_group(e))) return rc;
+    int64_t done = 0;
+    while (done < B) {
+        if (e->open_lane < 0) {
+            int li;
+            if ((rc = acquire_lane(e, B * T, &li))) return rc;      // size class of the CALL: the tail piece of a split
+                                                                    // call stays with the big lanes
+            mdk_lane &ln = e->lane[li];
+            // the staging grows to this call (at most one group of it); a reserved lane is already larger and keeps
+            // collecting further calls up to its size
+            if ((rc = ensure_io(e, ln, std::min<int64_t>(B - done, gmax), T))) return rc;
+            ln.items.clear();
+            ln.gB = 0; ln.gT = T;
+            ln.want_logits = false; ln.want_labels = false;
+            ln.open = true;
+            ln.group++;
+            e->open_lane = li;
+        }
+        mdk_lane &ln = e->lane[e->open_lane];
+        // windows the open group can still take: gmax, and what the lane's staging reaches
+        int64_t room = std::min(gmax, std::min(ln.cap_io / T, ln.cap_feats / (T * F))) - ln.gB;
+        if (ln.gB == 0 && room < 1) room = 1;        // (ensure_io above sized the staging for at least one window)
+        if (room < 1) {
+            if ((rc = launch_group(e))) return rc;
+            continue;
+        }
+        const int64_t n = std::min(room, B - done);
+        // copy-in stream: features into the staging (asynchronous for device and page-locked host memory), behind the
+        // group's earlier pieces
+        MDK_CUDA(cudaMemcpyAsync(ln.d_feats + (size_t)ln.gB * T * F, feats + (size_t)done * T * F,
+                                 (size_t)n * T * F * sizeof(float), cudaMemcpyDefault, e->copy_in));
+        ln.items.push_back(mdk_lane::Item{feats + (size_t)done * T * F, probs + (size_t)done * T * NCLS,
+                                          logits ? logits + (size_t)done * T * NCLS : nullptr,
+                                          labels ? labels + (size_t)done * T : nullptr, n});
+        ln.gB += n;
+        ln.want_logits = ln.want_logits || logits != nullptr;
+        ln.want_labels = ln.want_labels || labels != nullptr;
+        done += n;
+        if (done == B && ticket) {
+            const int64_t tk = e->submit_count++;
+            e->ticket_lane[tk % mdk_engine::TICKET_RING] = (int16_t)e->open_lane;
+            e->ticket_group[tk % mdk_engine::TICKET_RING] = ln.group;
+            *ticket = tk;
+        }
+        if (n == room && (rc = launch_group(e))) return rc;      // full: launch right away
+    }
     return MDK_OK;
 }
 
@@ -505,7 +569,7 @@ int mdk_engine_set_group_windows(mdk_engine *e, int64_t windows) {
 }
 
 // Reserve = size the big workspaces and the big lanes' staging for groups of up to B windows of T columns.  This is also
-// what switches coalescing on: a group collects submitted batches only as far as its lane's staging buffers reach.
+// what switches coalescing on: a group collects calls only as far as its lane's staging buffers reach.
 int mdk_engine_reserve(mdk_engine *e, int64_t B, int64_t T) {
     MDK_REQUIRE(e && B >= 1 && T >= 1, MDK_ERR_ARG, "reserve: bad arguments");
     MDK_CUDA(cudaSetDevice(e->device));
@@ -527,83 +591,27 @@ int mdk_engine_forward_dev(mdk_engine *e, const float *feats_dev, int64_t B, int
     int rc;
     if ((rc = check_shapes(e, feats_dev, B, T, probs_dev))) return rc;
     MDK_CUDA(cudaSetDevice(e->device));
-    if ((rc = launch_group(e))) return rc;
-    // device buffers need no staging: take the next workspace of the size class (stream order keeps it safe)
-    int wi;
-    if (B * T > mdk_engine::SMALL_POS) {
-        wi = e->next_big_ws;
-        e->next_big_ws = (e->next_big_ws + 1) % mdk_engine::BIG_WS;
-    } else {
-        wi = mdk_engine::BIG_WS + e->next_small;
-        e->next_small = (e->next_small + 1) % mdk_engine::SMALL_LANES;
+    int64_t gmax = group_limit(e);
+    // A call of more than one group's windows was sized by its caller (one full wave of the two-tile kernel is 2112
+    // windows on an H100): it runs as one forward of its own instead of being cut into groups that each fill part of
+    // the device.
+    if (B > gmax) {
+        if ((rc = launch_group(e))) return rc;
+        gmax = B;
     }
-    mdk_ws &ws = e->ws[wi];
-    e->ev = e->evr[e->fwd_count % mdk_engine::EV_RING];
-    e->fwd_count++;
-    MDK_CUDA(cudaEventRecord(e->ev[0], ws.stream));
-    if ((rc = run_forward(e, ws, feats_dev, B, T, probs_dev, logits_dev, labels_dev))) return rc;
-    MDK_CUDA(cudaEventRecord(e->ev[7], ws.stream));
-    return MDK_OK;
+    return enqueue(e, feats_dev, B, T, probs_dev, logits_dev, labels_dev, gmax, nullptr);
 }
 
-// Submitted batches are packed into groups window by window: a batch that does not fit what is left of the open group
-// is split (windows are independent, medaka/prediction.py:40-52 treats every row of a batch separately), so every
-// group of a long run is exactly one wave however the caller sized its batches.  The ticket follows the batch's last
-// piece; groups complete in submission order per lane and the pieces of one batch sit in consecutive groups.
+// Submitted batches are packed into groups window by window (enqueue), so every group of a long run is exactly one wave
+// however the caller sized its batches.  The ticket follows the batch's last piece; groups complete in submission order
+// per lane and the pieces of one batch sit in consecutive groups.
 int mdk_engine_submit(mdk_engine *e, const float *feats_host, int64_t B, int64_t T, float *probs_host,
                       float *logits_host, uint8_t *labels_host, int64_t *ticket) {
     int rc;
     if ((rc = check_shapes(e, feats_host, B, T, probs_host))) return rc;
     MDK_REQUIRE(ticket, MDK_ERR_ARG, "submit: ticket is NULL");
     MDK_CUDA(cudaSetDevice(e->device));
-    const int64_t gmax = e->group_windows > 0 ? e->group_windows : mdk_engine_preferred_windows(e);
-    const int64_t F = e->desc.num_features;
-    if (e->open_lane >= 0 && e->lane[e->open_lane].gT != T && (rc = launch_group(e))) return rc;
-    int64_t done = 0;
-    while (done < B) {
-        if (e->open_lane < 0) {
-            int li;
-            if ((rc = acquire_lane(e, B * T, &li))) return rc;      // size class of the BATCH: the tail piece of a split
-                                                                    // batch stays with the big lanes
-            mdk_lane &ln = e->lane[li];
-            // the staging grows to this batch (at most one wave of it); a reserved lane is already larger and keeps
-            // collecting further batches up to its size
-            if ((rc = ensure_io(e, ln, std::min<int64_t>(B - done, gmax), T))) return rc;
-            ln.items.clear();
-            ln.gB = 0; ln.gT = T;
-            ln.want_logits = false; ln.want_labels = false;
-            ln.open = true;
-            ln.group++;
-            e->open_lane = li;
-        }
-        mdk_lane &ln = e->lane[e->open_lane];
-        // windows the open group can still take: one wave, and what the lane's staging reaches
-        int64_t room = std::min(gmax, std::min(ln.cap_io / T, ln.cap_feats / (T * F))) - ln.gB;
-        if (ln.gB == 0 && room < 1) room = 1;        // (ensure_io above sized the staging for at least one window)
-        if (room < 1) {
-            if ((rc = launch_group(e))) return rc;
-            continue;
-        }
-        const int64_t n = std::min(room, B - done);
-        // copy-in stream: features H2D (asynchronous when feats_host is page-locked), behind the group's earlier pieces
-        MDK_CUDA(cudaMemcpyAsync(ln.d_feats + (size_t)ln.gB * T * F, feats_host + (size_t)done * T * F,
-                                 (size_t)n * T * F * sizeof(float), cudaMemcpyHostToDevice, e->copy_in));
-        ln.items.push_back(mdk_lane::Item{feats_host + (size_t)done * T * F, probs_host + (size_t)done * T * NCLS,
-                                          logits_host ? logits_host + (size_t)done * T * NCLS : nullptr,
-                                          labels_host ? labels_host + (size_t)done * T : nullptr, n});
-        ln.gB += n;
-        ln.want_logits = ln.want_logits || logits_host != nullptr;
-        ln.want_labels = ln.want_labels || labels_host != nullptr;
-        done += n;
-        if (done == B) {
-            const int64_t tk = e->submit_count++;
-            e->ticket_lane[tk % mdk_engine::TICKET_RING] = (int16_t)e->open_lane;
-            e->ticket_group[tk % mdk_engine::TICKET_RING] = ln.group;
-            *ticket = tk;
-        }
-        if (n == room && (rc = launch_group(e))) return rc;      // full: launch right away
-    }
-    return MDK_OK;
+    return enqueue(e, feats_host, B, T, probs_host, logits_host, labels_host, group_limit(e), ticket);
 }
 
 int mdk_engine_flush(mdk_engine *e) {
@@ -665,11 +673,16 @@ static void stage_times(cudaEvent_t *ev, mdk_timings *t) {
 
 int mdk_engine_last_timings(mdk_engine *e, mdk_timings *out) { return mdk_engine_mean_timings(e, 1, out); }
 
+// Calls are packed into groups, so there may be fewer groups than calls: the mean is over the last
+// min(n_last, groups launched) groups.  The open group is launched first so that its events are not read stale.
 int mdk_engine_mean_timings(mdk_engine *e, int n_last, mdk_timings *out) {
     MDK_REQUIRE(e && out, MDK_ERR_ARG, "NULL argument");
     MDK_REQUIRE(n_last >= 1 && n_last <= mdk_engine::EV_RING, MDK_ERR_ARG, "mean_timings: n_last out of range");
-    MDK_REQUIRE(e->fwd_count >= n_last, MDK_ERR_STATE, "mean_timings: fewer forwards recorded than requested");
     MDK_CUDA(cudaSetDevice(e->device));
+    int rc = launch_group(e);
+    if (rc) return rc;
+    MDK_REQUIRE(e->fwd_count >= 1, MDK_ERR_STATE, "mean_timings: no forward recorded");
+    n_last = (int)std::min<int64_t>(n_last, e->fwd_count);
     for (auto &ws : e->ws) MDK_CUDA(cudaStreamSynchronize(ws.stream));
     mdk_timings acc{};
     for (int i = 0; i < n_last; ++i) {
@@ -687,12 +700,14 @@ int mdk_engine_mean_timings(mdk_engine *e, int n_last, mdk_timings *out) {
     return MDK_OK;
 }
 
-// Diagnostics: completion times (ms after the timer's start event) of the eight stage events of the last n forwards,
-// oldest first - the schedule the lanes actually ran (tools/diag.py --check timeline).
+// Diagnostics: completion times (ms after the timer's start event) of the eight stage events of the last n launched
+// groups, oldest first - the schedule the lanes actually ran.  The open group is launched first, as in mean_timings.
 int mdk_debug_timeline(mdk_engine *e, int n_last, float *out) {
     MDK_REQUIRE(e && out, MDK_ERR_ARG, "NULL argument");
-    MDK_REQUIRE(n_last >= 1 && n_last <= mdk_engine::EV_RING && e->fwd_count >= n_last, MDK_ERR_ARG, "timeline: bad n_last");
     MDK_CUDA(cudaSetDevice(e->device));
+    int rc = launch_group(e);
+    if (rc) return rc;
+    MDK_REQUIRE(n_last >= 1 && n_last <= mdk_engine::EV_RING && e->fwd_count >= n_last, MDK_ERR_ARG, "timeline: bad n_last");
     for (auto &ws : e->ws) MDK_CUDA(cudaStreamSynchronize(ws.stream));
     for (int i = 0; i < n_last; ++i) {
         cudaEvent_t *ev = e->evr[(e->fwd_count - n_last + i) % mdk_engine::EV_RING];

@@ -96,10 +96,10 @@ struct LayerWeights {
 }  // namespace mdk
 
 // The engine runs GROUPS of windows.  A workspace (mdk_ws) is a compute stream plus the intermediates of one forward; a
-// lane (mdk_lane) is the device-side staging of one group of submitted batches (features in, probabilities / labels
-// out) and is bound to one workspace.  There are more big lanes than big workspaces: while one group computes, others
-// are receiving their features or draining their results, so the copies never hold the workspace (43 GB for a
-// 1056 x 10 000 group, 4 KiB per position) idle.  One big workspace: a one-wave group (one 16-window tile per CTA and
+// lane (mdk_lane) is the device-side staging of one group of calls - submitted host batches and device-resident
+// forward_dev calls alike (features in, probabilities / labels out) - and is bound to one workspace.  There are more
+// big lanes than big workspaces: while one group computes, others are receiving their features or draining their
+// results, so the copies never hold the workspace (43 GB for a 1056 x 10 000 group, 4 KiB per position) idle.  One big workspace: a one-wave group (one 16-window tile per CTA and
 // direction) already fills every SM, and a second 43 GB workspace would not fit beside it in 80 GB.  Small forwards (the
 // B = 1 remainder regions of medaka/prediction.py:196-209) spread over the small lanes, each with a workspace of its own.
 struct mdk_ws {
@@ -118,7 +118,7 @@ struct mdk_ws {
 
 struct mdk_lane {
     mdk_ws *ws = nullptr;      // where the lane's groups compute (fixed at engine creation)
-    // device staging of the group's host buffers
+    // device staging of the group's calls (their buffers may be host or device memory)
     int64_t cap_io = 0;        // positions
     int64_t cap_feats = 0;     // floats
     float *d_feats = nullptr, *d_probs = nullptr, *d_logits = nullptr;
@@ -151,15 +151,15 @@ struct mdk_engine {
     static constexpr int64_t SMALL_POS = 1 << 18;   // forwards up to this many positions run on the small lanes
     mdk_ws ws[N_WS];              // [0, BIG_WS): big groups; then one per small lane
     mdk_lane lane[N_LANES];       // big lane j computes on ws[j % BIG_WS], small lane i on ws[BIG_WS + i]
-    int next_big = 0, next_small = 0, next_big_ws = 0;
+    int next_big = 0, next_small = 0;
     int open_lane = -1;           // lane whose group is still collecting batches (at most one), -1 = none
     int last_ws = 0;              // workspace of the most recent forward
     int64_t group_windows = 0;    // most windows coalesced into one group (0 = one wave, mdk_engine_preferred_windows)
     cudaStream_t stream = nullptr;       // == ws[0].stream: weight preparation, timers
-    static constexpr int EV_RING = 32;   // per-forward event sets kept for mdk_engine_mean_timings
+    static constexpr int EV_RING = 32;   // per-group event sets kept for mdk_engine_mean_timings
     cudaEvent_t evr[EV_RING][8] = {};
-    cudaEvent_t *ev = evr[0];            // event set of the forward being queued
-    int64_t fwd_count = 0;
+    cudaEvent_t *ev = evr[0];            // event set of the group being launched
+    int64_t fwd_count = 0;               // groups launched
     cudaEvent_t ev_timer[2] = {};
     cudaEvent_t ev_join = nullptr;
     mdk::LayerWeights layer[2];
