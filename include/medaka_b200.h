@@ -117,8 +117,8 @@ int mdk_engine_load_linear(mdk_engine *e, const float *w, const float *b);
 int mdk_engine_set_precision(mdk_engine *e, int mode);
 int mdk_engine_get_precision(mdk_engine *e, int *mode);
 /* fp16 products per tensor-core contraction, a bit set: 1 = W_hi.x_hi (required), 2 = W_hi.x_lo, 4 = W_lo.x_hi.
- * 7 (default) reproduces fp32 to ~2e-6; the 2- and 1-product sets trade parity for tensor time - measured in
- * profiles/precision_r02.md; they do NOT meet the labels-bit-exact bar and are never selected automatically. */
+ * 7 (default) reproduces fp32 to ~2e-6; the 2- and 1-product sets trade parity for tensor time - tabulated by
+ * tools/precision_table.py; they do NOT meet the labels-bit-exact bar and are never selected automatically. */
 int mdk_engine_set_products(mdk_engine *e, int mask);
 /* MDK_REC_*: recurrent-kernel selection (A/B measurements; AUTO is the default) */
 int mdk_engine_set_rec_mode(mdk_engine *e, int mode);
@@ -383,6 +383,11 @@ int mdk_debug_timeline(mdk_engine *e, int n_last, float *out);
 /* partial logits of the last forward on the fused-head path: float32 [2 directions][tiles][T][5 classes][16 windows]
  * (what the layer-1 recurrence writes instead of h1); per-direction parity checks of the fused linear head */
 int mdk_debug_read_plog(mdk_engine *e, float *out_host, int64_t n_floats);
+/* layer-wise parity of the read-level network: copy one intermediate of the LAST mdk_rl_forward call (B, P of that call)
+ * from the engine's scratch to host.  which: 0 = z [B][P][H] (the pooled pre_pool_expansion_layer output, the LSTM
+ * input), 1 = h0 [B][P][2H] (layer-0 output, columns direction * H + unit), 2 = h1 [B][P][2H] (layer-1 output).
+ * MDK_ERR_STATE before the first completed forward, MDK_ERR_ARG when n_floats is not the stage's size. */
+int mdk_rl_debug_read(mdk_rl_engine *e, int which, float *out_host, int64_t n_floats);
 
 #ifdef __cplusplus
 }

@@ -313,7 +313,12 @@ __global__ void __launch_bounds__(256, 1) rl_conv17_tc_kernel(const int8_t *__re
         }
         fence_proxy_async_smem();
         __syncthreads();
-        // ---- 17 taps x (hi plane, lo plane) of the weights
+        // ---- 17 taps x (hi plane, lo plane) of the weights.  Each plane starts a fresh wgmma accumulator (16 or 8 MMAs
+        // deep) that is added into the fp32 sum on the CUDA cores: one accumulator chained over all 34 planes (400 MMAs,
+        // K = 17 x 128 x 3) lost ~10x the fp32 path's accuracy on the pooled output in the tensor core's accumulation.
+        float sum[64];
+#pragma unroll
+        for (int k = 0; k < 64; ++k) sum[k] = 0.f;
         for (int ps = 0; ps < 2 * RL_TAPS; ++ps, ++it) {
             const uint32_t st = it % CT_STAGES;
             const int t = ps >> 1, lo_plane = ps & 1;
@@ -326,7 +331,7 @@ __global__ void __launch_bounds__(256, 1) rl_conv17_tc_kernel(const int8_t *__re
             for (int ks = 0; ks < RL_C / 16; ++ks) {
                 const uint64_t ad = make_smem_desc(a0 + ks * 2 * (RL_C * 16), RL_C * 16, 128);
                 const uint64_t bh = make_smem_desc(bb0 + ks * 2 * (CT_ROWS * 16), CT_ROWS * 16, 128);
-                Wgmma<128>::ss(acc, ad, bh, (ps | ks) ? 1u : 0u);
+                Wgmma<128>::ss(acc, ad, bh, ks ? 1u : 0u);
                 if (!lo_plane) Wgmma<128>::ss(acc, ad, make_smem_desc(bb0 + CT_BPLANE + ks * 2 * (CT_ROWS * 16), CT_ROWS * 16, 128), 1u);
             }
             wg_commit();
@@ -334,11 +339,13 @@ __global__ void __launch_bounds__(256, 1) rl_conv17_tc_kernel(const int8_t *__re
             wg_hold(acc);
             __syncthreads();                                       // both warpgroups have read stage st
             if (tid == 0 && ps + 2 < 2 * RL_TAPS) issue(it + 2);
+#pragma unroll
+            for (int k = 0; k < 64; ++k) sum[k] += acc[k];
         }
 #pragma unroll
         for (int k = 0; k < 64; ++k) {
             const int hb = (k >> 1) & 1;
-            const float av = fmaxf(acc[k] + b2[hb], 0.f);
+            const float av = fmaxf(sum[k] + b2[hb], 0.f);
             pooled[k] += (av - m2[hb]) * s2[hb] * g2[hb] + o2[hb];
         }
     }
@@ -755,9 +762,11 @@ __global__ void __launch_bounds__(256, 1) rl_proj_tc_kernel(const float *__restr
             *reinterpret_cast<uint2 *>(xs + PJ_XPLANE + off) = *reinterpret_cast<uint2 *>(lv);
         }
     };
-    float acc[64];
+    // each 64-wide K chunk runs in a fresh accumulator (12 MMAs) that is added into the fp32 sum on the CUDA cores: one
+    // chain over all of K (144 MMAs at K = 768) lost accuracy in the tensor core's accumulation
+    float acc[64], sum[64];
 #pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    for (int i = 0; i < 64; ++i) sum[i] = 0.f;
     if (tid == 0) issue_w(0);
     stage_x(0);
     fence_proxy_async_smem();
@@ -775,7 +784,7 @@ __global__ void __launch_bounds__(256, 1) rl_proj_tc_kernel(const float *__restr
             const uint64_t al = make_smem_desc(wbase + PJ_WPLANE + ks * 2 * (PJ_M * 16), PJ_M * 16, 128);
             const uint64_t bh = make_smem_desc(xbase + ks * 2 * (PJ_N * 16), PJ_N * 16, 128);
             const uint64_t bl = make_smem_desc(xbase + PJ_XPLANE + ks * 2 * (PJ_N * 16), PJ_N * 16, 128);
-            Wgmma<128>::ss(acc, ah, bh, (c | ks) ? 1u : 0u);
+            Wgmma<128>::ss(acc, ah, bh, ks ? 1u : 0u);
             Wgmma<128>::ss(acc, ah, bl, 1u);
             Wgmma<128>::ss(acc, al, bh, 1u);
         }
@@ -786,6 +795,8 @@ __global__ void __launch_bounds__(256, 1) rl_proj_tc_kernel(const float *__restr
         }
         wg_wait_all();
         wg_hold(acc);
+#pragma unroll
+        for (int i = 0; i < 64; ++i) sum[i] += acc[i];
     }
     // accumulator element k = 4i + 2hb + e: gate row 64wg + 16warp + gq + 8hb, position 8i + 2cq + e
     const int r0 = rb * PJ_M + wg * 64 + warp * 16 + gq;
@@ -794,7 +805,7 @@ __global__ void __launch_bounds__(256, 1) rl_proj_tc_kernel(const float *__restr
     for (int k = 0; k < 64; ++k) {
         const int64_t p = m0 + 8 * (k >> 2) + 2 * cq + (k & 1);
         const int hb = (k >> 1) & 1;
-        if (p < M) C[p * N + r0 + 8 * hb] = acc[k] + (hb ? bias1 : bias0);
+        if (p < M) C[p * N + r0 + 8 * hb] = sum[k] + (hb ? bias1 : bias0);
     }
 }
 
@@ -892,20 +903,26 @@ __global__ void __cluster_dims__(L3_CL, 1, 1) __launch_bounds__(L3_THREADS, 1)
         const int buf = (int)(step & 1);
         const uint32_t h_hi = smem_u32(sh + buf * 2 * L3_HPLANE), h_lo = h_hi + L3_HPLANE;
         wg_fence();
+        // three accumulator chains of 24 MMAs (k-steps 0-7 onto the pre-activations, 8-15 and 16-23 from zero), added on
+        // the CUDA cores: one chain of 72 lost accuracy in the tensor core's accumulation
+        float acc2[8], acc3[8];
 #pragma unroll
         for (int ks = 0; ks < L3_KS; ++ks) {
+            float (&a)[8] = ks < L3_KS / 3 ? acc : ks < 2 * L3_KS / 3 ? acc2 : acc3;
             const uint64_t bh = make_smem_desc(h_hi + ks * 2 * L3_KG, L3_KG, 128);
-            Wgmma<16>::rs(acc, whi[ks], bh, 1u);
-            Wgmma<16>::rs(acc, whi[ks], make_smem_desc(h_lo + ks * 2 * L3_KG, L3_KG, 128), 1u);
-            Wgmma<16>::ss(acc, make_smem_desc(wl + ks * 2 * (64 * 16), 64 * 16, 128), bh, 1u);
+            Wgmma<16>::rs(a, whi[ks], bh, (ks == L3_KS / 3 || ks == 2 * L3_KS / 3) ? 0u : 1u);
+            Wgmma<16>::rs(a, whi[ks], make_smem_desc(h_lo + ks * 2 * L3_KG, L3_KG, 128), 1u);
+            Wgmma<16>::ss(a, make_smem_desc(wl + ks * 2 * (64 * 16), 64 * 16, 128), bh, 1u);
         }
         wg_commit();
         wg_wait_all();
         wg_hold(acc);
+        wg_hold(acc2);
+        wg_hold(acc3);
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
             const int wdw = 8 * (k >> 2) + 2 * cq + (k & 1);
-            xw[(warp * LT_N + wdw) * L3_XS + gq + 8 * ((k >> 1) & 1)] = acc[k];
+            xw[(warp * LT_N + wdw) * L3_XS + gq + 8 * ((k >> 1) & 1)] = acc[k] + (acc2[k] + acc3[k]);
         }
         if (step + 1 < P) fetch(dir ? (t - 1) : (t + 1));           // the next pre-activations load under the gate math
         named_bar_sync(1 + wg, 128);
@@ -1075,6 +1092,8 @@ struct mdk_rl_engine {
     std::vector<void *> allocs;
     uint8_t *scratch = nullptr;    // per-call intermediates, grown on demand and kept
     size_t scratch_bytes = 0;
+    int64_t last_B = 0, last_P = 0;                  // the last completed forward (mdk_rl_debug_read), 0 = none yet
+    size_t last_off[3] = {0, 0, 0};                  // its z, h0, h1 in the scratch
     cudaStream_t stream = nullptr;
 };
 
@@ -1392,6 +1411,7 @@ int mdk_rl_forward(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P,
                  o_part = take((size_t)B * n_groups * P * RL_C * 4), o_z = take((size_t)BP * HH * 4),
                  o_gi = take((size_t)BP * 2 * 4 * HH * 4), o_h0 = take((size_t)BP * 2 * HH * 4),
                  o_h1 = take((size_t)BP * 2 * HH * 4), o_probs = take((size_t)BP * NCLS * 4);
+    e->last_B = e->last_P = 0;                         // the scratch is about to be overwritten
     if (off > e->scratch_bytes) {
         if (e->scratch) cudaFree(e->scratch);
         e->scratch = nullptr;
@@ -1481,6 +1501,24 @@ int mdk_rl_forward(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P,
     MDK_CUDA(cudaStreamSynchronize(s));
     if (e->timing)   // convolution (mask + conv + pooling Linear), projection / recurrence of each layer, head
         for (int i = 0; i < 6; ++i) MDK_CUDA(cudaEventElapsedTime(&e->stage_ms[i], e->ev[i], e->ev[i + 1]));
+    e->last_B = B;
+    e->last_P = P;
+    e->last_off[0] = o_z;
+    e->last_off[1] = o_h0;
+    e->last_off[2] = o_h1;
+    return MDK_OK;
+}
+
+int mdk_rl_debug_read(mdk_rl_engine *e, int which, float *out_host, int64_t n_floats) {
+    MDK_REQUIRE(e && out_host, MDK_ERR_ARG, "rl_debug_read: NULL argument");
+    MDK_REQUIRE(which >= 0 && which <= 2, MDK_ERR_ARG, "rl_debug_read: which must be 0 (z), 1 (h0) or 2 (h1)");
+    MDK_REQUIRE(e->last_B > 0, MDK_ERR_STATE, "rl_debug_read: no completed forward to read from");
+    const int64_t want = e->last_B * e->last_P * (which == 0 ? e->H : 2 * e->H);
+    MDK_REQUIRE(n_floats == want, MDK_ERR_ARG,
+                "rl_debug_read: n_floats must be " + std::to_string(want) + " (B * P * H for z, B * P * 2H for h0 / h1)");
+    MDK_CUDA(cudaSetDevice(e->device));
+    MDK_CUDA(cudaStreamSynchronize(e->stream));
+    MDK_CUDA(cudaMemcpy(out_host, e->scratch + e->last_off[which], (size_t)n_floats * sizeof(float), cudaMemcpyDeviceToHost));
     return MDK_OK;
 }
 

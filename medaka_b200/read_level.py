@@ -106,15 +106,42 @@ class LatentSpaceLSTM(object):
         B, P, D, F = x.shape
         lib, ffi = _lm.lib, _lm.ffi
         probs = np.empty((B, P, 5), dtype=np.float32)
-        # windows per device call: bounded in cells and in scratch bytes (at lstm_size 384, gi alone takes 12 KiB per
-        # position); the windows are independent, so the split does not change the outputs
-        step = max(1, min(int(self.max_cells // max(P * D, 1)), int(self.max_bytes // self.scratch_bytes_per_window(P, D, F))))
+        step = self.windows_per_call(P, D, F)
+        self._last_call = None
         for b0 in range(0, B, step):
             xb = np.ascontiguousarray(x[b0:b0 + step])
             pb = probs[b0:b0 + step]
             _lm.check(lib.mdk_rl_forward(self._engine, ffi.cast("const int8_t *", ffi.from_buffer(xb)), len(xb), P, D, F,
                                          ffi.cast("float *", ffi.from_buffer(pb))))
+            self._last_call = (len(xb), P)
         return probs
+
+    MAX_WINDOWS_PER_CALL = 65535            # mdk_rl_forward's limit on B
+
+    def windows_per_call(self, P, D, F):
+        """Windows per device call of forward_arrays: bounded in cells (max_cells), in scratch bytes (max_bytes; at
+        lstm_size 384, gi alone takes 12 KiB per position) and by mdk_rl_forward's B <= 65535.  The windows are
+        independent, so the split does not change the outputs."""
+        step = min(int(self.max_cells // max(P * D, 1)), int(self.max_bytes // self.scratch_bytes_per_window(P, D, F)))
+        return max(1, min(step, self.MAX_WINDOWS_PER_CALL))
+
+    STAGE_INDEX = {"z": 0, "h0": 1, "h1": 2}
+
+    def read_stage(self, name):
+        """An intermediate of the last device call, float32: "z" [B, P, H] (pooled pre_pool_expansion_layer output, the
+        LSTM input), "h0" / "h1" [B, P, 2H] (the LSTM layers' outputs, forward direction in the first H columns).
+
+        B and P are those of the last mdk_rl_forward call, so this covers the whole batch only when the last
+        forward_arrays ran as ONE device call (B <= windows_per_call(P, D, F)); otherwise it holds the last slice."""
+        last = getattr(self, "_last_call", None)
+        if last is None:
+            raise RuntimeError("read_stage: no forward has completed on this model")
+        B, P = last
+        width = self.lstm_size if name == "z" else 2 * self.lstm_size
+        out = np.empty((B, P, width), dtype=np.float32)
+        _lm.check(_lm.lib.mdk_rl_debug_read(self._engine, self.STAGE_INDEX[name],
+                                            _lm.ffi.cast("float *", _lm.ffi.from_buffer(out)), out.size))
+        return out
 
     def predict_on_batch(self, batch):
         import torch

@@ -34,7 +34,7 @@ CASES = {            # name: (seed, B, P, D, use_dwells, gain)
 
 
 def build_oracle(sd, use_dwells):
-    """The restatement at lstm_size = 384 (rl_oracle.build constructs the 128 model)."""
+    """The restatement at lstm_size = 384 (what rl_oracle.build makes of a 384 state dict)."""
     m = rl_oracle.LatentSpaceLSTM(lstm_size=LSTM_SIZE, use_dwells=use_dwells)
     m.load_state_dict(sd)
     m.eval()
