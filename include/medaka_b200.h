@@ -116,7 +116,8 @@ int mdk_engine_load_linear(mdk_engine *e, const float *w, const float *b);
 /* TorchModel.half() / --full_precision (medaka/prediction.py:164-168): MDK_PREC_* */
 int mdk_engine_set_precision(mdk_engine *e, int mode);
 int mdk_engine_get_precision(mdk_engine *e, int *mode);
-/* fp16 products per tensor-core contraction, a bit set: 1 = W_hi.x_hi (required), 2 = W_hi.x_lo, 4 = W_lo.x_hi.
+/* fp16 products per tensor-core contraction (the GRU recurrences and the layer-1 input projection; the linear head is
+ * fp32 on the CUDA cores and does not change), a bit set: 1 = W_hi.x_hi (required), 2 = W_hi.x_lo, 4 = W_lo.x_hi.
  * 7 (default) reproduces fp32 to ~2e-6; the 2- and 1-product sets trade parity for tensor time - tabulated by
  * tools/precision_table.py; they do NOT meet the labels-bit-exact bar and are never selected automatically. */
 int mdk_engine_set_products(mdk_engine *e, int mask);

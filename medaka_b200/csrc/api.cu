@@ -76,12 +76,6 @@ static int prepare_weights(mdk_engine *e) {
         MDK_CUDA(launch_prepare_layer(lw, in, l == 1, e->stream));
         e->launches++;
     }
-    {
-        int rc;
-        if (!e->lin_w_tc && (rc = dev_alloc(&e->lin_w_tc, (size_t)NDIR * 2 * 16 * 64 * 8))) return rc;
-        MDK_CUDA(launch_pack_linear(e->lin_w, e->lin_w_tc, e->stream));
-        e->launches++;
-    }
     MDK_CUDA(cudaStreamSynchronize(e->stream));
     e->prepared = true;
     return MDK_OK;
@@ -159,9 +153,9 @@ static int run_forward(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int64_
     int launches = 0;
     const bool fuse_x = tc && e->fuse_x && e->layer[0].w_x_tm != nullptr;
     const bool pp = tc && use_pingpong(e, B);
-    // the linear head rides inside the layer-1 recurrence as extra MMAs (40 B/position of partial logits reach HBM
-    // instead of the 1 KiB/position h1 round trip): always on the ping-pong path, on the one-tile path when the batch
-    // is one tile per CTA
+    // the linear head rides inside the layer-1 recurrence, fp32 on the CUDA cores (40 B/position of partial logits
+    // reach HBM instead of the 1 KiB/position h1 round trip): always on the ping-pong path, on the one-tile path when
+    // the batch is one tile per CTA
     const bool fuse_head = tc && !e->keep_act && (pp || rec_tc_can_fuse_logits(B, e->sm_count));
     if (!fuse_head && (rc = ensure_h1(ws))) return rc;
     MDK_CUDA(cudaEventRecord(e->ev[1], s));
@@ -189,9 +183,9 @@ static int run_forward(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int64_
     MDK_CUDA(cudaEventRecord(e->ev[4], s));
     if (tc) {
         if (pp && fuse_head) MDK_CUDA(launch_rec_pp(1, ws.gi, nullptr, e->layer[1].w_hh_tm, e->layer[1].b_hn_tc, nullptr, B, T, s,
-                                                    e->lin_w_tc, ws.plog, e->prod_mask));
+                                                    e->lin_w, ws.plog, e->prod_mask));
         else MDK_CUDA(launch_rec_tc(ws.gi, nullptr, e->layer[1].w_hh_tm, e->layer[1].b_hn_tc, ws.h1, 0, B, T, e->sm_count, s,
-                                    fuse_head ? e->lin_w_tc : nullptr, fuse_head ? ws.plog : nullptr, e->prod_mask));
+                                    fuse_head ? e->lin_w : nullptr, fuse_head ? ws.plog : nullptr, e->prod_mask));
     } else {
         MDK_CUDA(launch_rec_fp32(ws.gi, e->layer[1].w_hh_t, e->layer[1].b_hn, ws.h1, B, T, s));
     }
@@ -473,7 +467,7 @@ int mdk_engine_destroy(mdk_engine *e) {
         dev_free(lw.bias_gi_tc); dev_free(lw.b_hn_tc);
         dev_free(lw.w_hh_tm); dev_free(lw.w_x_tm); dev_free(lw.w_in_tc);
     }
-    dev_free(e->lin_w); dev_free(e->lin_b); dev_free(e->lin_w_tc);
+    dev_free(e->lin_w); dev_free(e->lin_b);
     for (auto &ws : e->ws) {
         dev_free(ws.gi); dev_free(ws.h1); dev_free(ws.plog);
         if (ws.h0) cudaFree(ws.h0);

@@ -165,8 +165,6 @@ struct mdk_engine {
     mdk::LayerWeights layer[2];
     float *lin_w = nullptr, *lin_b = nullptr;
     bool lin_loaded = false;
-    __half *lin_w_tc = nullptr;   // [dir][hi/lo][k-group 16][row 64][8 halfs]: W_lin half of one direction as an M=64 smem A
-                                  // operand (rows >= 5 zero) for the logits MMAs fused into the layer-1 recurrence
     bool keep_act = false;        // debugging: keep h1 (layer-1 output) in HBM, i.e. run the unfused head
     bool prepared = false;
     cudaStream_t copy_in = nullptr, copy_out = nullptr;
@@ -210,22 +208,21 @@ struct RecXArgs {            // fused layer-0 input projection (rec_tc FUSE_X)
     const float *bias;       // LayerWeights::bias_gi
     int F;
 };
-// lin_w_tc != nullptr (layer 1, one tile per CTA): the 5-class linear head runs inside the recurrence as extra MMAs and
-// the kernel writes partial logits to plog instead of h_out; *fused_logits tells the caller whether it did
+// lin_w != nullptr (layer 1, one tile per CTA): the 5-class linear head (fp32 W_lin [5][256]) runs inside the recurrence
+// in fp32 on the CUDA cores and the kernel writes partial logits to plog instead of h_out
 bool rec_tc_can_fuse_logits(int64_t B, int sm_count);
 cudaError_t launch_rec_tc(const float *gi, const RecXArgs *fuse, const __half *w_hh_tm, const float *b_hn,
                           void *h_out, int out_tiles, int64_t B, int64_t T, int sm_count, cudaStream_t s,
-                          const __half *lin_w_tc = nullptr, float *plog = nullptr, uint32_t prod_mask = 7u);
+                          const float *lin_w = nullptr, float *plog = nullptr, uint32_t prod_mask = 7u);
 // two tiles per CTA.  layer 0: fused projection when `fuse` is given (F <= 16), else gi in; operand
-// tiles out.  layer 1: gi in, partial logits out (lin_w_tc, plog required).  prod_mask: fp16 products per contraction
-// (bit 0 W_hi.h_hi, bit 1 W_hi.h_lo, bit 2 W_lo.h_hi; 7 = fp32-faithful)
+// tiles out.  layer 1: gi in, partial logits out (lin_w, plog required).  prod_mask: fp16 products per contraction of the
+// recurrence (bit 0 W_hi.h_hi, bit 1 W_hi.h_lo, bit 2 W_lo.h_hi; 7 = fp32-faithful)
 cudaError_t launch_rec_pp(int layer, const float *gi, const RecXArgs *fuse, const __half *w_hh_tm, const float *b_hn,
-                          void *h_out, int64_t B, int64_t T, cudaStream_t s, const __half *lin_w_tc, float *plog,
+                          void *h_out, int64_t B, int64_t T, cudaStream_t s, const float *lin_w, float *plog,
                           uint32_t prod_mask);
 // head on the partial logits of the fused path: sum of the two directions + bias -> softmax / argmax
 cudaError_t launch_head_plog(const float *plog, const float *lin_b, int64_t B, int64_t T, float *probs, float *logits,
                              uint8_t *labels, cudaStream_t s);
-cudaError_t launch_pack_linear(const float *lin_w, __half *lin_w_tc, cudaStream_t s);
 constexpr int PLOG_TS_FLOATS = NCLS * WT;     // 80 floats per (tile-step, direction)
 cudaError_t launch_gemm_tc(const void *x_tiles, const __half *w_in_tm, const float *bias, float *gi, int64_t P,
                            int sm_count, cudaStream_t s, uint32_t prod_mask);

@@ -30,14 +30,12 @@ namespace mdk {
 // n gate needs W_in.x and W_hn.h apart, so its input part sits in registers of its own.
 // FUSE_X (layer 0, F <= 16): the input projection W_ih . x_t is three more products per gate on a 16-column x tile,
 // so layer 0 needs no gi buffer.  OUT: fp16 hi/lo operand tiles of the projection GEMM (layer 0), fp32 rows, or
-// (layer 1) partial logits: the 5-row linear head as three more products on the h tile, one step behind (the tile it
-// reads is the previous step's h); both warpgroups issue them (a warpgroup-dependent branch around a wgmma makes ptxas
-// serialise them all), warpgroup 0 stores rows 0..4.
+// (layer 1) partial logits: the 5-row linear head in fp32 on the CUDA cores, from the h values the threads already hold,
+// while the next step's MMAs run (see head_partials).
 // =====================================================================================================
 constexpr int RW_THREADS = 256;
 constexpr int RW_ABLK = (H / 8) * 64 * 16;          // W_hh lo of one (gate, warpgroup): [kg 16][row 64][8] = 16 KiB
 constexpr int RW_XBLK = 2 * 64 * 16;                // W_ih lo (K = 16) of one (gate, warpgroup): 2 KiB
-constexpr int RW_WL_PLANE = 16 * 64 * 16;           // one plane of W_lin: [kg 16][row 64][8] = 16 KiB
 enum { OUT_TILES = 0, OUT_ROWS = 1, OUT_LOGITS = 2 };
 
 template <int NT, bool FUSE_X, int OUT>
@@ -47,12 +45,13 @@ struct RwCfg {
                                                     // stores of one k-group over the banks)
     static constexpr int HPLANE = (H / 8) * KG;
     static constexpr int XPLANE = 2 * KG;
+    static constexpr int RED = (RW_THREADS / 32) * NCLS * N;                     // head partials of one step (floats)
     static constexpr int wlo_off = 0;                                            // [gate 3][wg 2] RW_ABLK
     static constexpr int wxlo_off = wlo_off + 6 * RW_ABLK;                       // [gate 3][wg 2] RW_XBLK
-    static constexpr int wl_off = wxlo_off + (FUSE_X ? 6 * RW_XBLK : 0);         // [plane 2] RW_WL_PLANE
-    static constexpr int h_off = wl_off + (OUT == OUT_LOGITS ? 2 * RW_WL_PLANE : 0);   // [buf 2][plane 2] HPLANE
+    static constexpr int h_off = wxlo_off + (FUSE_X ? 6 * RW_XBLK : 0);          // [buf 2][plane 2] HPLANE
     static constexpr int x_off = h_off + 4 * HPLANE;                             // [buf 2][plane 2] XPLANE
-    static constexpr int total = x_off + (FUSE_X ? 4 * XPLANE : 0);
+    static constexpr int red_off = x_off + (FUSE_X ? 4 * XPLANE : 0);            // [buf 2][warp 8][class 5][N] fp32
+    static constexpr int total = red_off + (OUT == OUT_LOGITS ? 2 * RED * 4 : 0);
     static_assert(total <= 227 * 1024, "smem budget");
 };
 
@@ -64,7 +63,7 @@ __device__ __forceinline__ uint32_t ld_u32(const __half *p) { return *reinterpre
 template <int NT, bool FUSE_X, int OUT, bool ALL3>
 __global__ void __launch_bounds__(RW_THREADS, 1)
 rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__ w_hh, const float *__restrict__ b_hn,
-              void *__restrict__ h_out, int64_t B, int64_t T, const __half *__restrict__ lin_w_tc,
+              void *__restrict__ h_out, int64_t B, int64_t T, const float *__restrict__ lin_w,
               float *__restrict__ plog, uint32_t prod_mask_rt) {
     const uint32_t prod_mask = ALL3 ? 7u : prod_mask_rt;
     using L = RwCfg<NT, FUSE_X, OUT>;
@@ -95,9 +94,12 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
             *reinterpret_cast<uint4 *>(smem + L::wxlo_off + (gate * 2 + (r >> 6)) * RW_XBLK + kg * 1024 + (r & 63) * 16) = v;
         }
     }
-    if (LOGITS) {   // this direction's half of W_lin, already in operand layout [plane][kg][row 64][8]
-        const int4 *src = reinterpret_cast<const int4 *>(lin_w_tc + (size_t)dir * 2 * (RW_WL_PLANE / 2));
-        for (int i = tid; i < 2 * RW_WL_PLANE / 16; i += RW_THREADS) reinterpret_cast<int4 *>(smem + L::wl_off)[i] = src[i];
+    float wlin[2][NCLS];                            // LOGITS: W_lin[c][dir * H + j0 + 8 hb], fp32
+    if (LOGITS) {
+#pragma unroll
+        for (int hb = 0; hb < 2; ++hb)
+#pragma unroll
+            for (int c = 0; c < NCLS; ++c) wlin[hb][c] = lin_w[c * H2 + dir * H + j0 + 8 * hb];
     }
     uint32_t whi[3][H / 16][4];
 #pragma unroll
@@ -127,7 +129,7 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
     const float bhn[2] = {b_hn[dir * H + j0], b_hn[dir * H + j0 + 8]};
 
     // Accumulator element k = 4i + 2hb + e: hidden unit j0 + 8hb, window n = 8i + 2cq + e of tile wtile0 + i/2.
-    float ar[NA], az[NA], an[NA], axn[NA], hp[NA], alg[NA];
+    float ar[NA], az[NA], an[NA], axn[NA], hp[NA];
 #pragma unroll
     for (int k = 0; k < NA; ++k) hp[k] = 0.f;
     // pre-activations of time t into the accumulators (gi in quad layout, common.cuh: the pair e = 0, 1 is contiguous)
@@ -185,29 +187,62 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
     fence_proxy_async_smem();   // generic-proxy writes above (weights, zeroed tiles, x_0) -> visible to wgmma reads
     __syncthreads();            // h_{-1} = 0, x_0 and the weights are in shared memory
 
-    // logits of h in buffer `buf` (warpgroup 0): class c = row gq of warp 0, c < 5
-    auto issue_logits = [&](int buf) {
-        const uint32_t hb_addr = sbase + L::h_off + buf * 2 * L::HPLANE;
+    // ---- fused linear head (LOGITS), fp32 on the CUDA cores ----
+    // head_partials(rb): this direction's logits of the h in hp, summed over the thread's 2 hidden units, then over the 8
+    // gq lanes of its cq group (shuffles), into red[rb][warp][class][n].  A thread holds NW = N / 4 windows, wl = 2i + e
+    // (window n = 8i + 2cq + e); while more than one is left, each shuffle level hands half of them to the partner lane
+    // and keeps the sums of the other half (a reduce-scatter: 5 NW / 2 + 5 NW / 4 + ... shuffles instead of 15 NW);
+    // below one window the level is an all-reduce.  Every window's sum runs through the same tree over gq and the same
+    // warp order in head_store, whatever its slot in the tile or NT.
+    constexpr int NW = N / 4;
+    auto head_partials = [&](int rb) {
+        float v[NW][NCLS];
 #pragma unroll
-        for (int ks = 0; ks < H / 16; ++ks) {
-            const uint64_t bh = make_smem_desc(hb_addr + ks * 2 * L::KG, L::KG, 128);
-            const uint64_t bl = make_smem_desc(hb_addr + L::HPLANE + ks * 2 * L::KG, L::KG, 128);
-            const uint64_t wh = make_smem_desc(sbase + L::wl_off + ks * 2 * 1024, 1024, 128);
-            const uint64_t wl = make_smem_desc(sbase + L::wl_off + RW_WL_PLANE + ks * 2 * 1024, 1024, 128);
-            MMA::ss(alg, wh, bh, ks ? 1u : 0u);
-            if (prod_mask & 2u) MMA::ss(alg, wh, bl, 1u);
-            if (prod_mask & 4u) MMA::ss(alg, wl, bh, 1u);
+        for (int wl = 0; wl < NW; ++wl) {
+            const int k = 4 * (wl >> 1) + (wl & 1);             // hidden unit j0 at k, j0 + 8 at k + 2
+#pragma unroll
+            for (int c = 0; c < NCLS; ++c) v[wl][c] = fmaf(wlin[1][c], hp[k + 2], wlin[0][c] * hp[k]);
+        }
+        int wbase = 0;                                          // window of v[0]
+#pragma unroll
+        for (int lvl = 0; lvl < 3; ++lvl) {
+            const int mask = 16 >> lvl;                         // lane bit of gq bit 2 - lvl
+            const int half = (NW >> lvl) / 2;
+            if (half > 0) {
+                const bool up = lane & mask;
+#pragma unroll
+                for (int w = 0; w < NW / 2; ++w) {      // (a constant trip count, so that v stays in registers)
+                    if (w >= half) continue;
+#pragma unroll
+                    for (int c = 0; c < NCLS; ++c) {
+                        const float send = up ? v[w][c] : v[w + half][c];
+                        const float keep = up ? v[w + half][c] : v[w][c];
+                        v[w][c] = keep + __shfl_xor_sync(0xffffffffu, send, mask);
+                    }
+                }
+                if (up) wbase += half;
+            } else {
+#pragma unroll
+                for (int c = 0; c < NCLS; ++c) v[0][c] += __shfl_xor_sync(0xffffffffu, v[0][c], mask);
+            }
+        }
+        if (NW >= 8 || !(lane & 4)) {                           // NW = 4: the lanes of a gq pair hold the same sums
+            float *red = reinterpret_cast<float *>(smem + L::red_off) + rb * L::RED + (tid >> 5) * NCLS * N;
+            const int n = 8 * (wbase >> 1) + 2 * cq + (wbase & 1);
+#pragma unroll
+            for (int c = 0; c < NCLS; ++c) red[c * N + n] = v[0][c];
         }
     };
-    auto store_logits = [&](int64_t t) {
-        if (warp != 0 || gq >= NCLS) return;
+    // head_store(rb, t): the 8 warps' partials of red[rb] (published by a __syncthreads), summed in warp order -> plog row t
+    auto head_store = [&](int rb, int64_t t) {
+        if (tid >= NCLS * N) return;
+        const int c = tid / N, n = tid % N;
+        const float *red = reinterpret_cast<const float *>(smem + L::red_off) + rb * L::RED + c * N + n;
+        float s = red[0];
 #pragma unroll
-        for (int k = 0; k < NA; ++k) {
-            if ((k >> 1) & 1) continue;             // rows 8..15 are padding
-            const int i = k >> 2, n = 8 * i + 2 * cq + (k & 1);
-            const int64_t wt = wtile0 + (i >> 1);
-            if (wt < ntiles) plog[((dir * ntiles + wt) * T + t) * PLOG_TS_FLOATS + gq * RT_N + (n & 15)] = alg[k];
-        }
+        for (int w = 1; w < RW_THREADS / 32; ++w) s += red[w * NCLS * N];
+        const int64_t wt = wtile0 + n / RT_N;
+        if (wt < ntiles) plog[((dir * ntiles + wt) * T + t) * PLOG_TS_FLOATS + c * RT_N + (n & 15)] = s;
     };
 
 #pragma unroll 1
@@ -239,9 +274,6 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
                 if (prod_mask & 4u) MMA::ss(acc, make_smem_desc(sbase + L::wxlo_off + (gate * 2 + wg) * RW_XBLK, 1024, 128), bh, 1u);
             }
         }
-        // the tile holds h of the previous step (zeros at step 0: not stored).  Both warpgroups issue the same chain and
-        // only warpgroup 0 stores: issued under a warpgroup-dependent branch, ptxas serialises every wgmma of the kernel
-        if (LOGITS) issue_logits(buf);
         wg_commit();
         // the next step's L2 prefetch and feature loads run under the MMAs
         if (!FUSE_X && tid == 0 && step + GI_PREFETCH_STEPS < T) {
@@ -254,9 +286,14 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
                 for (int i = 0; i < 12; ++i) bulk_prefetch_l2(blk + i * 512, 2048);
             }
         }
+        // the head runs under the MMAs too: hp still holds h of the previous step (zeros at step 0: nothing to do); the
+        // sums of the step before that, published by the last barrier, go out to plog
+        if (LOGITS && step > 0) {
+            if (step > 1) head_store((int)((step - 1) & 1), dir ? t + 2 : t - 2);
+            head_partials((int)(step & 1));
+        }
         wg_wait_all();
         wg_hold(ar); wg_hold(az); wg_hold(an); wg_hold(axn);
-        if (LOGITS) wg_hold(alg);
 
         // ---- gate math (weights and biases carry the exp2 scale factors, common.cuh gate_scale) ----
         uint8_t *hw = smem + L::h_off + (buf ^ 1) * 2 * L::HPLANE;
@@ -282,9 +319,7 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
             }
         }
         // ---- outputs of this step ----
-        if (LOGITS) {
-            if (wg == 0 && step > 0) store_logits(dir ? t + 1 : t - 1);
-        } else {
+        if (!LOGITS) {
 #pragma unroll
             for (int k = 0; k < NA; ++k) {
                 const int i = k >> 2, n = 8 * i + 2 * cq + (k & 1);
@@ -308,13 +343,11 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
         fence_proxy_async_smem();     // h / x tile writes -> visible to the next step's wgmma operand reads
         __syncthreads();
     }
-    if (LOGITS) {                     // h of the last step (made visible by the last barrier)
-        wg_fence();
-        issue_logits((int)(T & 1));
-        wg_commit();
-        wg_wait_all();
-        wg_hold(alg);
-        if (wg == 0) store_logits(dir ? 0 : T - 1);
+    if (LOGITS) {                     // the last two steps' logits: step T - 2 (partials in red), step T - 1 (in hp)
+        if (T > 1) head_store((int)((T - 1) & 1), dir ? 1 : T - 2);
+        head_partials((int)(T & 1));
+        __syncthreads();
+        head_store((int)(T & 1), dir ? 0 : T - 1);
     }
 }
 
@@ -325,7 +358,7 @@ bool rec_tc_can_fuse_logits(int64_t B, int sm_count) {
 
 template <int NT, bool FX, int OUT>
 static cudaError_t launch_rec(const float *gi, const RecX &xin, const __half *w_hh_tm, const float *b_hn, void *h_out,
-                              int64_t B, int64_t T, cudaStream_t s, const __half *lin_w_tc, float *plog, uint32_t prod_mask) {
+                              int64_t B, int64_t T, cudaStream_t s, const float *lin_w, float *plog, uint32_t prod_mask) {
     prod_mask = (prod_mask & 7u) | 1u;
     auto kern = prod_mask == 7u ? rec_tc_kernel<NT, FX, OUT, true> : rec_tc_kernel<NT, FX, OUT, false>;
     constexpr int smem_bytes = RwCfg<NT, FX, OUT>::total;
@@ -334,23 +367,23 @@ static cudaError_t launch_rec(const float *gi, const RecX &xin, const __half *w_
     if (e != cudaSuccess) return e;
     const int64_t tiles = (B + RT_N - 1) / RT_N;
     dim3 grid((unsigned)((tiles + NT - 1) / NT), NDIR);
-    kern<<<grid, RW_THREADS, smem_bytes, s>>>(gi, xin, w_hh_tm, b_hn, h_out, B, T, lin_w_tc, plog, prod_mask);
+    kern<<<grid, RW_THREADS, smem_bytes, s>>>(gi, xin, w_hh_tm, b_hn, h_out, B, T, lin_w, plog, prod_mask);
     return cudaGetLastError();
 }
 
 cudaError_t launch_rec_tc(const float *gi, const RecXArgs *fuse, const __half *w_hh_tm, const float *b_hn,
                           void *h_out, int out_tiles, int64_t B, int64_t T, int sm_count, cudaStream_t s,
-                          const __half *lin_w_tc, float *plog, uint32_t prod_mask) {
+                          const float *lin_w, float *plog, uint32_t prod_mask) {
     if (B == 0 || T == 0) return cudaSuccess;
     const int64_t tiles = (B + RT_N - 1) / RT_N;
     // two tiles per CTA only once there are more tiles than SMs to run them one per CTA
     const bool two = tiles * NDIR > (int64_t)sm_count;
     RecX xin{nullptr, nullptr, nullptr, 0};
     if (fuse) xin = RecX{fuse->feats, fuse->w_x, fuse->bias, fuse->F};
-    if (lin_w_tc) {
+    if (lin_w) {
         // layer 1 with the linear head fused in (partial logits instead of h1)
         if (fuse || out_tiles || two || !plog) return cudaErrorInvalidValue;
-        return launch_rec<1, false, OUT_LOGITS>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, lin_w_tc, plog, prod_mask);
+        return launch_rec<1, false, OUT_LOGITS>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, lin_w, plog, prod_mask);
     }
     if (fuse) {
         if (!out_tiles) return cudaErrorInvalidValue;   // the fused projection is layer 0, which feeds the GEMM
@@ -365,7 +398,7 @@ cudaError_t launch_rec_tc(const float *gi, const RecXArgs *fuse, const __half *w
 }
 
 cudaError_t launch_rec_pp(int layer, const float *gi, const RecXArgs *fuse, const __half *w_hh_tm, const float *b_hn,
-                          void *h_out, int64_t B, int64_t T, cudaStream_t s, const __half *lin_w_tc, float *plog,
+                          void *h_out, int64_t B, int64_t T, cudaStream_t s, const float *lin_w, float *plog,
                           uint32_t prod_mask) {
     if (B == 0 || T == 0) return cudaSuccess;
     RecX xin{nullptr, nullptr, nullptr, 0};
@@ -373,8 +406,8 @@ cudaError_t launch_rec_pp(int layer, const float *gi, const RecXArgs *fuse, cons
     if (layer == 0)
         return fuse ? launch_rec<2, true, OUT_TILES>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, nullptr, nullptr, prod_mask)
                     : launch_rec<2, false, OUT_TILES>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, nullptr, nullptr, prod_mask);
-    if (fuse || !lin_w_tc || !plog) return cudaErrorInvalidValue;
-    return launch_rec<2, false, OUT_LOGITS>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, lin_w_tc, plog, prod_mask);
+    if (fuse || !lin_w || !plog) return cudaErrorInvalidValue;
+    return launch_rec<2, false, OUT_LOGITS>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, lin_w, plog, prod_mask);
 }
 
 // =====================================================================================================

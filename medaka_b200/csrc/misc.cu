@@ -535,24 +535,6 @@ cudaError_t launch_prepare_layer(const LayerWeights &lw, int in_features, bool b
     return cudaGetLastError();
 }
 
-// W_lin [5][256] -> per direction an M = 64 (rows >= 5 zero), K = 128 K-major shared-memory A operand image, fp16 hi/lo
-__global__ void pack_linear_kernel(const float *__restrict__ lin_w, __half *__restrict__ out) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;     // [dir 2][kg 16][row 64][8]
-    if (i >= NDIR * 16 * 64 * 8) return;
-    const int k8 = i & 7, row = (i >> 3) & 63, kg = (i >> 9) & 15, d = i >> 13;
-    const float v = row < NCLS ? lin_w[row * H2 + d * H + kg * 8 + k8] : 0.f;
-    __half hi, lo;
-    split_f16(v, hi, lo);
-    const int plane = 16 * 64 * 8;
-    out[(d * 2 + 0) * plane + (i & (plane - 1))] = hi;
-    out[(d * 2 + 1) * plane + (i & (plane - 1))] = lo;
-}
-
-cudaError_t launch_pack_linear(const float *lin_w, __half *lin_w_tc, cudaStream_t s) {
-    pack_linear_kernel<<<(NDIR * 16 * 64 * 8 + 255) / 256, 256, 0, s>>>(lin_w, lin_w_tc);
-    return cudaGetLastError();
-}
-
 // Head of the fused path (gru.py:53-55,67-71): logits = fwd partial + rev partial + bias, softmax, first-max argmax.
 // One thread per (window of the tile, time step); blockIdx.y = window tile.  41 B written per position, 40 B read.
 __global__ void __launch_bounds__(256) head_plog_kernel(const float *__restrict__ plog, const float *__restrict__ lin_b,

@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """On-device measurement of the fp16 product sets (VERDICT r01 item 2): for each set of products per contraction
 {hi.hi} / {hi.hi + W_hi.x_lo} / {hi.hi + W_lo.x_hi} / {all three} the real kernels (fused layer-0 projection, both
-recurrences, the layer-1 GEMM, the fused logits) are run on the golden cases, a T = 10 000 batch and two "hot"
-recurrent-gain models, against the fp32 CPU reference.  Writes markdown to stdout."""
+recurrences, the layer-1 GEMM; the fused linear head is fp32 on the CUDA cores whatever the set) are run on the golden
+cases, a T = 10 000 batch and two "hot" recurrent-gain models, against the fp32 CPU reference.  Writes markdown to
+stdout."""
 import json
 import os
 import sys
