@@ -44,10 +44,10 @@ extern "C" {
 #define MDK_PREC_TC 0    /* wgmma tensor cores, fp16 hi/lo split operands (3 MMAs), fp32 accumulate */
 #define MDK_PREC_FP32 1  /* CUDA-core fp32 FFMA path: validation / --full_precision */
 
-/* which recurrent kernel the tensor-core path runs (mdk_engine_set_rec_mode) */
-#define MDK_REC_AUTO 0      /* ping-pong from half a wave of 16-window tiles up, else one tile per CTA */
-#define MDK_REC_ONE_TILE 1  /* rec_tc_kernel: one (two beyond a wave) 16-window tile per CTA */
-#define MDK_REC_PINGPONG 2  /* rec_pp_kernel: two tiles per CTA, their MMA and gate phases interleaved */
+/* how many 16-window tiles each CTA of the tensor-core recurrences runs (mdk_engine_set_rec_mode) */
+#define MDK_REC_AUTO 0      /* two once the tiles of both directions outnumber the SMs (beyond one wave), else one */
+#define MDK_REC_ONE_TILE 1  /* one tile per CTA, over several waves when the batch needs more CTAs than there are SMs */
+#define MDK_REC_PINGPONG 2  /* two tiles per CTA (one N = 32 MMA chain), whatever the batch size */
 
 /* count normalisation modes: CountsFeatureEncoder._norm_modes_ (medaka/features.py:816) */
 #define MDK_NORM_TOTAL 0
@@ -116,12 +116,7 @@ int mdk_engine_load_linear(mdk_engine *e, const float *w, const float *b);
 /* TorchModel.half() / --full_precision (medaka/prediction.py:164-168): MDK_PREC_* */
 int mdk_engine_set_precision(mdk_engine *e, int mode);
 int mdk_engine_get_precision(mdk_engine *e, int *mode);
-/* fp16 products per tensor-core contraction (the GRU recurrences and the layer-1 input projection; the linear head is
- * fp32 on the CUDA cores and does not change), a bit set: 1 = W_hi.x_hi (required), 2 = W_hi.x_lo, 4 = W_lo.x_hi.
- * 7 (default) reproduces fp32 to ~2e-6; the 2- and 1-product sets trade parity for tensor time - tabulated by
- * tools/precision_table.py; they do NOT meet the labels-bit-exact bar and are never selected automatically. */
-int mdk_engine_set_products(mdk_engine *e, int mask);
-/* MDK_REC_*: recurrent-kernel selection (A/B measurements; AUTO is the default) */
+/* MDK_REC_*: tiles per CTA of the recurrent kernels (A/B measurements; AUTO is the default) */
 int mdk_engine_set_rec_mode(mdk_engine *e, int mode);
 /* pre-size the compute lanes (workspace + staging) for groups of up to B windows of T columns (otherwise grown on
  * demand, to the size of the batch that opens a group - i.e. without a reserve call nothing is coalesced) */
@@ -172,7 +167,7 @@ int mdk_engine_timer_stop(mdk_engine *e, float *elapsed_ms);
  * which: 0 = layer-0 output [B][T][2H] fp32, 1 = layer-1 output [B][T][2H] fp32 */
 int mdk_engine_read_activation(mdk_engine *e, int which, float *out_host, int64_t n_floats);
 /* keep != 0: leave the layer-1 output in HBM (for mdk_engine_read_activation(e, 1, ...)) by running the 5-class head as
- * its own kernel; default 0: the head is fused into the layer-1 recurrence whenever the batch is one tile per CTA */
+ * its own kernel; default 0: the tensor-core path fuses the head into the layer-1 recurrence */
 int mdk_engine_keep_activations(mdk_engine *e, int keep);
 /* number of kernels launched by this engine since creation (bench.py "gpu_launches") */
 int64_t mdk_engine_launch_count(mdk_engine *e);

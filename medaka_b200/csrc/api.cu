@@ -131,16 +131,6 @@ static int ensure_io(mdk_engine *e, mdk_lane &ln, int64_t B, int64_t T) {
     return MDK_OK;
 }
 
-// Which recurrent kernel runs a batch of B windows (tensor-core path).  One tile per CTA (NT = 1) is a single dependent
-// chain per SM; two tiles per CTA (NT = 2, one N = 32 MMA chain) need half as many CTAs.  AUTO: two tiles per CTA only
-// once the tiles of both directions outnumber the SMs.
-static bool use_pingpong(const mdk_engine *e, int64_t B) {
-    const int64_t tiles = (B + WT - 1) / WT;
-    if (e->rec_mode == MDK_REC_PINGPONG) return true;
-    if (e->rec_mode == MDK_REC_ONE_TILE) return false;
-    return tiles * NDIR > (int64_t)e->sm_count;
-}
-
 // The forward pipeline on the workspace's stream.  ev[1..6] bracket the stages for mdk_timings.
 static int run_forward(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int64_t B, int64_t T, float *probs_dev,
                        float *logits_dev, uint8_t *labels_dev) {
@@ -151,12 +141,16 @@ static int run_forward(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int64_
     cudaStream_t s = ws.stream;
     const bool tc = e->precision == MDK_PREC_TC;
     int launches = 0;
-    const bool fuse_x = tc && e->fuse_x && e->layer[0].w_x_tm != nullptr;
-    const bool pp = tc && use_pingpong(e, B);
-    // the linear head rides inside the layer-1 recurrence, fp32 on the CUDA cores (40 B/position of partial logits
-    // reach HBM instead of the 1 KiB/position h1 round trip): always on the ping-pong path, on the one-tile path when
-    // the batch is one tile per CTA
-    const bool fuse_head = tc && !e->keep_act && (pp || rec_tc_can_fuse_logits(B, e->sm_count));
+    const bool fuse_x = tc && e->layer[0].w_x_tm != nullptr;     // F <= 16
+    // Recurrent kernels of the tensor-core path.  One 16-window tile per CTA is a single dependent chain per SM; two tiles
+    // per CTA (one N = 32 MMA chain) need half as many CTAs, so AUTO takes two only once the tiles of both directions
+    // outnumber the SMs.  The linear head rides inside the layer-1 recurrence, fp32 on the CUDA cores (40 B/position of
+    // partial logits reach HBM instead of the 1 KiB/position h1 round trip), unless h1 is to be kept.
+    const int64_t tiles = (B + WT - 1) / WT;
+    const int tiles_per_cta = e->rec_mode == MDK_REC_PINGPONG ? 2
+                            : e->rec_mode == MDK_REC_ONE_TILE ? 1
+                            : tiles * NDIR > (int64_t)e->sm_count ? 2 : 1;
+    const bool fuse_head = tc && !e->keep_act;
     if (!fuse_head && (rc = ensure_h1(ws))) return rc;
     MDK_CUDA(cudaEventRecord(e->ev[1], s));
     if (!fuse_x) {
@@ -166,26 +160,21 @@ static int run_forward(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int64_
     }
     MDK_CUDA(cudaEventRecord(e->ev[2], s));
     if (tc) {
-        const RecXArgs fx{feats_dev, e->layer[0].w_x_tm, e->layer[0].bias_gi_tc, e->desc.num_features};
-        if (pp) MDK_CUDA(launch_rec_pp(0, ws.gi, fuse_x ? &fx : nullptr, e->layer[0].w_hh_tm, e->layer[0].b_hn_tc, ws.h0, B, T, s,
-                                       nullptr, nullptr, e->prod_mask));
-        else MDK_CUDA(launch_rec_tc(ws.gi, fuse_x ? &fx : nullptr, e->layer[0].w_hh_tm, e->layer[0].b_hn_tc, ws.h0, 1, B, T,
-                                    e->sm_count, s, nullptr, nullptr, e->prod_mask));
+        const RecX fx{feats_dev, e->layer[0].w_x_tm, e->layer[0].bias_gi_tc, e->desc.num_features};
+        MDK_CUDA(launch_rec_tc(ws.gi, fuse_x ? &fx : nullptr, e->layer[0].w_hh_tm, e->layer[0].b_hn_tc, tiles_per_cta,
+                               OUT_TILES, ws.h0, nullptr, B, T, s));
     } else {
         MDK_CUDA(launch_rec_fp32(ws.gi, e->layer[0].w_hh_t, e->layer[0].b_hn, (float *)ws.h0, B, T, s));
     }
     launches++;
     MDK_CUDA(cudaEventRecord(e->ev[3], s));
-    if (tc) MDK_CUDA(launch_gemm_tc(ws.h0, e->layer[1].w_in_tc, e->layer[1].bias_gi_tc, ws.gi, tiled_rows(B, T), e->sm_count, s,
-                                    e->prod_mask));
+    if (tc) MDK_CUDA(launch_gemm_tc(ws.h0, e->layer[1].w_in_tc, e->layer[1].bias_gi_tc, ws.gi, tiled_rows(B, T), e->sm_count, s));
     else MDK_CUDA(launch_gemm_fp32((const float *)ws.h0, e->layer[1].w_in_packed, e->layer[1].bias_gi, ws.gi, P, s));
     launches++;
     MDK_CUDA(cudaEventRecord(e->ev[4], s));
     if (tc) {
-        if (pp && fuse_head) MDK_CUDA(launch_rec_pp(1, ws.gi, nullptr, e->layer[1].w_hh_tm, e->layer[1].b_hn_tc, nullptr, B, T, s,
-                                                    e->lin_w, ws.plog, e->prod_mask));
-        else MDK_CUDA(launch_rec_tc(ws.gi, nullptr, e->layer[1].w_hh_tm, e->layer[1].b_hn_tc, ws.h1, 0, B, T, e->sm_count, s,
-                                    fuse_head ? e->lin_w : nullptr, fuse_head ? ws.plog : nullptr, e->prod_mask));
+        MDK_CUDA(launch_rec_tc(ws.gi, nullptr, e->layer[1].w_hh_tm, e->layer[1].b_hn_tc, tiles_per_cta,
+                               fuse_head ? OUT_LOGITS : OUT_ROWS, fuse_head ? (void *)ws.plog : ws.h1, e->lin_w, B, T, s));
     } else {
         MDK_CUDA(launch_rec_fp32(ws.gi, e->layer[1].w_hh_t, e->layer[1].b_hn, ws.h1, B, T, s));
     }
@@ -424,15 +413,6 @@ int mdk_engine_create(int device, const mdk_model_desc *desc, mdk_engine **out) 
     e->device = device;
     e->desc = *desc;
     e->sm_count = prop.multiProcessorCount;
-    {
-        const char *v = getenv("MDK_NO_FUSE_X");
-        e->fuse_x = !(v && v[0] == '1');
-        v = getenv("MDK_REC_MODE");          // A/B measurements: "one" / "pp"
-        if (v && v[0] == 'o') e->rec_mode = MDK_REC_ONE_TILE;
-        else if (v && v[0] == 'p') e->rec_mode = MDK_REC_PINGPONG;
-        v = getenv("MDK_PRODUCTS");
-        if (v && v[0] >= '1' && v[0] <= '7') e->prod_mask = ((uint32_t)(v[0] - '0') & 7u) | 1u;
-    }
     for (auto &ws : e->ws) {
         cudaError_t err = cudaStreamCreateWithFlags(&ws.stream, cudaStreamNonBlocking);
         if (err != cudaSuccess) { mdk_engine_destroy(e); return cuda_fail(err, "cudaStreamCreate", __FILE__, __LINE__); }
@@ -537,14 +517,6 @@ int mdk_engine_set_precision(mdk_engine *e, int mode) {
 int mdk_engine_get_precision(mdk_engine *e, int *mode) {
     MDK_REQUIRE(e && mode, MDK_ERR_ARG, "NULL argument");
     *mode = e->precision;
-    return MDK_OK;
-}
-
-int mdk_engine_set_products(mdk_engine *e, int mask) {
-    MDK_REQUIRE(e, MDK_ERR_ARG, "engine is NULL");
-    MDK_REQUIRE(mask >= 1 && mask <= 7 && (mask & 1), MDK_ERR_ARG,
-                "set_products: mask is a bit set of {1: W_hi.x_hi (required), 2: W_hi.x_lo, 4: W_lo.x_hi}");
-    e->prod_mask = (uint32_t)mask;
     return MDK_OK;
 }
 

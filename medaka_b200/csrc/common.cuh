@@ -143,9 +143,7 @@ struct mdk_engine {
     mdk_model_desc desc{};
     int precision = MDK_PREC_TC;
     int sm_count = 132;
-    bool fuse_x = true;           // layer-0 input projection fused into the recurrence (F <= 16); MDK_NO_FUSE_X=1 disables
-    int rec_mode = MDK_REC_AUTO;  // which recurrent kernel the tensor-core path runs (MDK_REC_*)
-    uint32_t prod_mask = 7u;      // fp16 products per contraction (mdk_engine_set_products)
+    int rec_mode = MDK_REC_AUTO;  // tiles per CTA of the tensor-core recurrences (MDK_REC_*)
     static constexpr int BIG_WS = 1, BIG_LANES = 4, SMALL_LANES = 14;
     static constexpr int N_LANES = BIG_LANES + SMALL_LANES, N_WS = BIG_WS + SMALL_LANES;
     static constexpr int64_t SMALL_POS = 1 << 18;   // forwards up to this many positions run on the small lanes
@@ -202,30 +200,26 @@ cudaError_t launch_rec_fp32(const float *gi, const float *w_hh_t, const float *b
 cudaError_t launch_gemm_fp32(const float *A, const float *W, const float *bias, float *C, int64_t P,
                              cudaStream_t s);
 // gru_wg.cu
-struct RecXArgs {            // fused layer-0 input projection (rec_tc FUSE_X)
-    const float *feats;      // [B][T][F]
-    const __half *w_x;       // LayerWeights::w_x_tm
-    const float *bias;       // LayerWeights::bias_gi
+struct RecX {               // fused layer-0 input projection (rec_tc_kernel FUSE_X, F <= 16)
+    const float *feats;     // [B][T][F]
+    const __half *w_x;      // LayerWeights::w_x_tm: [dir][part][gate][row 128][16] fp16, K zero-padded to 16
+    const float *bias;      // LayerWeights::bias_gi_tc: [768]: r,z: b_ih + b_hh ; n: b_ih
     int F;
 };
-// lin_w != nullptr (layer 1, one tile per CTA): the 5-class linear head (fp32 W_lin [5][256]) runs inside the recurrence
-// in fp32 on the CUDA cores and the kernel writes partial logits to plog instead of h_out
-bool rec_tc_can_fuse_logits(int64_t B, int sm_count);
-cudaError_t launch_rec_tc(const float *gi, const RecXArgs *fuse, const __half *w_hh_tm, const float *b_hn,
-                          void *h_out, int out_tiles, int64_t B, int64_t T, int sm_count, cudaStream_t s,
-                          const float *lin_w = nullptr, float *plog = nullptr, uint32_t prod_mask = 7u);
-// two tiles per CTA.  layer 0: fused projection when `fuse` is given (F <= 16), else gi in; operand
-// tiles out.  layer 1: gi in, partial logits out (lin_w, plog required).  prod_mask: fp16 products per contraction of the
-// recurrence (bit 0 W_hi.h_hi, bit 1 W_hi.h_lo, bit 2 W_lo.h_hi; 7 = fp32-faithful)
-cudaError_t launch_rec_pp(int layer, const float *gi, const RecXArgs *fuse, const __half *w_hh_tm, const float *b_hn,
-                          void *h_out, int64_t B, int64_t T, cudaStream_t s, const float *lin_w, float *plog,
-                          uint32_t prod_mask);
+// what the recurrent kernel writes: h as the fp16 hi/lo operand tiles of the layer-1 GEMM (layer 0), h as fp32 tiled rows
+// [row][256] (layer 1, unfused head), or the partial logits of the 5-class linear head (fp32 W_lin [5][256] in lin_w),
+// which runs inside the layer-1 recurrence in fp32 on the CUDA cores (plog layout)
+enum { OUT_TILES = 0, OUT_ROWS = 1, OUT_LOGITS = 2 };
+// one layer's recurrence, both directions, tiles_per_cta (1 or 2) 16-window tiles per CTA.  xin: the fused layer-0 input
+// projection (OUT_TILES only), or nullptr to read the pre-activations from gi.  out: h0 tiles, h1 rows or plog (out_kind).
+cudaError_t launch_rec_tc(const float *gi, const RecX *xin, const __half *w_hh_tm, const float *b_hn, int tiles_per_cta,
+                          int out_kind, void *out, const float *lin_w, int64_t B, int64_t T, cudaStream_t s);
 // head on the partial logits of the fused path: sum of the two directions + bias -> softmax / argmax
 cudaError_t launch_head_plog(const float *plog, const float *lin_b, int64_t B, int64_t T, float *probs, float *logits,
                              uint8_t *labels, cudaStream_t s);
 constexpr int PLOG_TS_FLOATS = NCLS * WT;     // 80 floats per (tile-step, direction)
 cudaError_t launch_gemm_tc(const void *x_tiles, const __half *w_in_tm, const float *bias, float *gi, int64_t P,
-                           int sm_count, cudaStream_t s, uint32_t prod_mask);
+                           int sm_count, cudaStream_t s);
 int selftest_umma(int device, const float *A, const float *B, float *D, int N, int K, int variant);
 // pileup.cu
 cudaError_t plp_scratch(size_t bytes, uint8_t **out, int slot);   // per-host-thread cached device buffers (slot 0 / 1)

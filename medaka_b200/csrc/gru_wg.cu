@@ -36,7 +36,6 @@ namespace mdk {
 constexpr int RW_THREADS = 256;
 constexpr int RW_ABLK = (H / 8) * 64 * 16;          // W_hh lo of one (gate, warpgroup): [kg 16][row 64][8] = 16 KiB
 constexpr int RW_XBLK = 2 * 64 * 16;                // W_ih lo (K = 16) of one (gate, warpgroup): 2 KiB
-enum { OUT_TILES = 0, OUT_ROWS = 1, OUT_LOGITS = 2 };
 
 template <int NT, bool FUSE_X, int OUT>
 struct RwCfg {
@@ -57,15 +56,11 @@ struct RwCfg {
 
 __device__ __forceinline__ uint32_t ld_u32(const __half *p) { return *reinterpret_cast<const uint32_t *>(p); }
 
-// ALL3: the product set is the full one (the production path) and known at compile time.  A run-time product set puts a
-// branch between the wgmmas of one accumulator chain, and ptxas then inserts a warpgroup.arrive in front of each of them
-// (warning C7519); the run-time form is kept for the precision experiments of mdk_engine_set_products.
-template <int NT, bool FUSE_X, int OUT, bool ALL3>
+template <int NT, bool FUSE_X, int OUT>
 __global__ void __launch_bounds__(RW_THREADS, 1)
 rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__ w_hh, const float *__restrict__ b_hn,
               void *__restrict__ h_out, int64_t B, int64_t T, const float *__restrict__ lin_w,
-              float *__restrict__ plog, uint32_t prod_mask_rt) {
-    const uint32_t prod_mask = ALL3 ? 7u : prod_mask_rt;
+              float *__restrict__ plog) {
     using L = RwCfg<NT, FUSE_X, OUT>;
     constexpr int N = L::N, NA = N / 2;             // accumulator values per thread and gate
     using MMA = Wgmma<N>;
@@ -258,9 +253,8 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
             for (int ks = 0; ks < H / 16; ++ks) {
                 const uint64_t bh = make_smem_desc(hb_addr + ks * 2 * L::KG, L::KG, 128);
                 MMA::rs(acc, whi[gate][ks], bh, 1u);
-                if (prod_mask & 2u) MMA::rs(acc, whi[gate][ks], make_smem_desc(hb_addr + L::HPLANE + ks * 2 * L::KG, L::KG, 128), 1u);
-                if (prod_mask & 4u)
-                    MMA::ss(acc, make_smem_desc(sbase + L::wlo_off + (gate * 2 + wg) * RW_ABLK + ks * 2 * 1024, 1024, 128), bh, 1u);
+                MMA::rs(acc, whi[gate][ks], make_smem_desc(hb_addr + L::HPLANE + ks * 2 * L::KG, L::KG, 128), 1u);
+                MMA::ss(acc, make_smem_desc(sbase + L::wlo_off + (gate * 2 + wg) * RW_ABLK + ks * 2 * 1024, 1024, 128), bh, 1u);
             }
         }
         if (FUSE_X) {
@@ -270,8 +264,8 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
             for (int gate = 0; gate < 3; ++gate) {
                 float(&acc)[NA] = gate == 0 ? ar : (gate == 1 ? az : axn);
                 MMA::rs(acc, wxhi[gate], bh, 1u);
-                if (prod_mask & 2u) MMA::rs(acc, wxhi[gate], bl, 1u);
-                if (prod_mask & 4u) MMA::ss(acc, make_smem_desc(sbase + L::wxlo_off + (gate * 2 + wg) * RW_XBLK, 1024, 128), bh, 1u);
+                MMA::rs(acc, wxhi[gate], bl, 1u);
+                MMA::ss(acc, make_smem_desc(sbase + L::wxlo_off + (gate * 2 + wg) * RW_XBLK, 1024, 128), bh, 1u);
             }
         }
         wg_commit();
@@ -351,63 +345,46 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
     }
 }
 
-bool rec_tc_can_fuse_logits(int64_t B, int sm_count) {
-    const int64_t tiles = (B + RT_N - 1) / RT_N;
-    return tiles > 0 && tiles * NDIR <= (int64_t)sm_count;      // one tile per CTA (NT == 1)
-}
-
 template <int NT, bool FX, int OUT>
-static cudaError_t launch_rec(const float *gi, const RecX &xin, const __half *w_hh_tm, const float *b_hn, void *h_out,
-                              int64_t B, int64_t T, cudaStream_t s, const float *lin_w, float *plog, uint32_t prod_mask) {
-    prod_mask = (prod_mask & 7u) | 1u;
-    auto kern = prod_mask == 7u ? rec_tc_kernel<NT, FX, OUT, true> : rec_tc_kernel<NT, FX, OUT, false>;
+static cudaError_t launch_rec(const float *gi, const RecX &xin, const __half *w_hh_tm, const float *b_hn, void *out,
+                              const float *lin_w, int64_t B, int64_t T, cudaStream_t s) {
+    auto kern = rec_tc_kernel<NT, FX, OUT>;
     constexpr int smem_bytes = RwCfg<NT, FX, OUT>::total;
     // (the attribute is per device: set it on every launch, a process may drive several GPUs)
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
     if (e != cudaSuccess) return e;
     const int64_t tiles = (B + RT_N - 1) / RT_N;
     dim3 grid((unsigned)((tiles + NT - 1) / NT), NDIR);
-    kern<<<grid, RW_THREADS, smem_bytes, s>>>(gi, xin, w_hh_tm, b_hn, h_out, B, T, lin_w, plog, prod_mask);
+    constexpr bool LOGITS = OUT == OUT_LOGITS;
+    kern<<<grid, RW_THREADS, smem_bytes, s>>>(gi, xin, w_hh_tm, b_hn, LOGITS ? nullptr : out, B, T, lin_w,
+                                              LOGITS ? static_cast<float *>(out) : nullptr);
     return cudaGetLastError();
 }
 
-cudaError_t launch_rec_tc(const float *gi, const RecXArgs *fuse, const __half *w_hh_tm, const float *b_hn,
-                          void *h_out, int out_tiles, int64_t B, int64_t T, int sm_count, cudaStream_t s,
-                          const float *lin_w, float *plog, uint32_t prod_mask) {
-    if (B == 0 || T == 0) return cudaSuccess;
-    const int64_t tiles = (B + RT_N - 1) / RT_N;
-    // two tiles per CTA only once there are more tiles than SMs to run them one per CTA
-    const bool two = tiles * NDIR > (int64_t)sm_count;
-    RecX xin{nullptr, nullptr, nullptr, 0};
-    if (fuse) xin = RecX{fuse->feats, fuse->w_x, fuse->bias, fuse->F};
-    if (lin_w) {
-        // layer 1 with the linear head fused in (partial logits instead of h1)
-        if (fuse || out_tiles || two || !plog) return cudaErrorInvalidValue;
-        return launch_rec<1, false, OUT_LOGITS>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, lin_w, plog, prod_mask);
+template <int NT>
+static cudaError_t launch_rec_nt(const float *gi, const RecX *xin, const __half *w_hh_tm, const float *b_hn, int out_kind,
+                                 void *out, const float *lin_w, int64_t B, int64_t T, cudaStream_t s) {
+    if (xin)    // the fused projection is layer 0, which feeds the GEMM
+        return out_kind == OUT_TILES ? launch_rec<NT, true, OUT_TILES>(gi, *xin, w_hh_tm, b_hn, out, nullptr, B, T, s)
+                                     : cudaErrorInvalidValue;
+    const RecX none{nullptr, nullptr, nullptr, 0};
+    switch (out_kind) {
+    case OUT_TILES: return launch_rec<NT, false, OUT_TILES>(gi, none, w_hh_tm, b_hn, out, nullptr, B, T, s);
+    case OUT_ROWS: return launch_rec<NT, false, OUT_ROWS>(gi, none, w_hh_tm, b_hn, out, nullptr, B, T, s);
+    case OUT_LOGITS:
+        return lin_w ? launch_rec<NT, false, OUT_LOGITS>(gi, none, w_hh_tm, b_hn, out, lin_w, B, T, s) : cudaErrorInvalidValue;
     }
-    if (fuse) {
-        if (!out_tiles) return cudaErrorInvalidValue;   // the fused projection is layer 0, which feeds the GEMM
-        return two ? launch_rec<2, true, OUT_TILES>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, nullptr, nullptr, prod_mask)
-                   : launch_rec<1, true, OUT_TILES>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, nullptr, nullptr, prod_mask);
-    }
-    if (two)
-        return out_tiles ? launch_rec<2, false, OUT_TILES>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, nullptr, nullptr, prod_mask)
-                         : launch_rec<2, false, OUT_ROWS>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, nullptr, nullptr, prod_mask);
-    return out_tiles ? launch_rec<1, false, OUT_TILES>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, nullptr, nullptr, prod_mask)
-                     : launch_rec<1, false, OUT_ROWS>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, nullptr, nullptr, prod_mask);
+    return cudaErrorInvalidValue;
 }
 
-cudaError_t launch_rec_pp(int layer, const float *gi, const RecXArgs *fuse, const __half *w_hh_tm, const float *b_hn,
-                          void *h_out, int64_t B, int64_t T, cudaStream_t s, const float *lin_w, float *plog,
-                          uint32_t prod_mask) {
+cudaError_t launch_rec_tc(const float *gi, const RecX *xin, const __half *w_hh_tm, const float *b_hn, int tiles_per_cta,
+                          int out_kind, void *out, const float *lin_w, int64_t B, int64_t T, cudaStream_t s) {
     if (B == 0 || T == 0) return cudaSuccess;
-    RecX xin{nullptr, nullptr, nullptr, 0};
-    if (fuse) xin = RecX{fuse->feats, fuse->w_x, fuse->bias, fuse->F};
-    if (layer == 0)
-        return fuse ? launch_rec<2, true, OUT_TILES>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, nullptr, nullptr, prod_mask)
-                    : launch_rec<2, false, OUT_TILES>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, nullptr, nullptr, prod_mask);
-    if (fuse || !lin_w || !plog) return cudaErrorInvalidValue;
-    return launch_rec<2, false, OUT_LOGITS>(gi, xin, w_hh_tm, b_hn, h_out, B, T, s, lin_w, plog, prod_mask);
+    switch (tiles_per_cta) {
+    case 1: return launch_rec_nt<1>(gi, xin, w_hh_tm, b_hn, out_kind, out, lin_w, B, T, s);
+    case 2: return launch_rec_nt<2>(gi, xin, w_hh_tm, b_hn, out_kind, out, lin_w, B, T, s);
+    }
+    return cudaErrorInvalidValue;
 }
 
 // =====================================================================================================
@@ -426,11 +403,9 @@ constexpr int GW_X_OFF = XT_TILE_BYTES;                         // behind the we
 constexpr int GW_BAR_OFF = GW_X_OFF + 2 * GW_STAGE;
 constexpr int GW_SMEM = GW_BAR_OFF + 16;
 
-template <bool ALL3>   // as in rec_tc_kernel: the full product set known at compile time
 __global__ void __launch_bounds__(GW_THREADS, 1)
 gemm_tc_kernel(const uint8_t *__restrict__ x_tiles, const __half *__restrict__ w_in_tm, const float *__restrict__ bias,
-               float *__restrict__ gi, int64_t P, int64_t ntiles, uint32_t prod_mask_rt) {
-    const uint32_t prod_mask = ALL3 ? 7u : prod_mask_rt;
+               float *__restrict__ gi, int64_t P, int64_t ntiles) {
     extern __shared__ __align__(128) uint8_t smem[];
     uint64_t *full = reinterpret_cast<uint64_t *>(smem + GW_BAR_OFF);
     const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
@@ -473,7 +448,6 @@ gemm_tc_kernel(const uint8_t *__restrict__ x_tiles, const __half *__restrict__ w
         wg_fence();
 #pragma unroll
         for (int prod = 0; prod < 3; ++prod) {
-            if (prod && !(prod_mask & (1u << prod))) continue;
             const int pa = prod == 2, pb = prod == 1;   // W part hi, hi, lo ; x part hi, lo, hi
 #pragma unroll
             for (int kk = 0; kk < GW_QK / 2; ++kk) {
@@ -506,19 +480,16 @@ gemm_tc_kernel(const uint8_t *__restrict__ x_tiles, const __half *__restrict__ w
 }
 
 cudaError_t launch_gemm_tc(const void *x_tiles, const __half *w_in_tm, const float *bias, float *gi, int64_t P,
-                           int sm_count, cudaStream_t s, uint32_t prod_mask) {
+                           int sm_count, cudaStream_t s) {
     if (P == 0) return cudaSuccess;
     const int64_t ntiles = (P + XT_ROWS - 1) / XT_ROWS;
-    prod_mask = (prod_mask & 7u) | 1u;
-    auto kern = prod_mask == 7u ? gemm_tc_kernel<true> : gemm_tc_kernel<false>;
-    cudaError_t ea = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GW_SMEM);
+    cudaError_t ea = cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GW_SMEM);
     if (ea != cudaSuccess) return ea;
     int64_t ct = sm_count / 6;
     if (ct < 1) ct = 1;
     if (ct > ntiles) ct = ntiles;
     dim3 grid(6, (unsigned)ct);
-    kern<<<grid, GW_THREADS, GW_SMEM, s>>>(reinterpret_cast<const uint8_t *>(x_tiles), w_in_tm, bias, gi, P, ntiles,
-                                           prod_mask);
+    gemm_tc_kernel<<<grid, GW_THREADS, GW_SMEM, s>>>(reinterpret_cast<const uint8_t *>(x_tiles), w_in_tm, bias, gi, P, ntiles);
     return cudaGetLastError();
 }
 

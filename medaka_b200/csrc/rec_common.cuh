@@ -21,12 +21,4 @@ constexpr int RT_N = 16;                                 // windows per tile
 constexpr int GI_PREFETCH_STEPS = 3;
 constexpr float EXP_CLAMP = 60.0f;
 
-// arguments of the fused input projection (layer 0)
-struct RecX {
-    const float *feats;     // [B][T][F]
-    const __half *w_x;      // [dir][part][gate][row 128][16] fp16, K zero-padded to 16
-    const float *bias;      // [768]: r,z: b_ih + b_hh ; n: b_ih
-    int F;
-};
-
 }  // namespace mdk

@@ -284,12 +284,8 @@ class GRUModel(object):
     def flush(self):
         _lm.check(_lm.lib.mdk_engine_flush(self._engine))
 
-    def set_products(self, mask):
-        """fp16 products per contraction (precision experiments; 7 = fp32-faithful default)."""
-        _lm.check(_lm.lib.mdk_engine_set_products(self._engine, int(mask)))
-
     def set_rec_mode(self, mode):
-        """'auto' | 'one' | 'pp': recurrent-kernel selection (mdk_engine_set_rec_mode)."""
+        """'auto' | 'one' | 'pp': tiles per CTA of the recurrent kernels (mdk_engine_set_rec_mode)."""
         code = {"auto": _lm.lib.MDK_REC_AUTO, "one": _lm.lib.MDK_REC_ONE_TILE, "pp": _lm.lib.MDK_REC_PINGPONG}[mode]
         _lm.check(_lm.lib.mdk_engine_set_rec_mode(self._engine, code))
 

@@ -127,18 +127,23 @@ def test_forward_ragged_shapes(B, T):
         m.close()
 
 
-@pytest.mark.parametrize("B,T,F", [(1200, 24, 10), (1217, 33, 10), (1217, 20, 20)])
-def test_forward_pingpong_path(B, T, F):
-    """More window tiles than SMs: the recurrent kernel runs two tiles per CTA (NT = 2, ping-pong).  1217 windows = 77
-    tiles: the last CTA's second tile does not exist; F = 20 takes the unfused layer-0 path (gi in quad layout)."""
+@pytest.mark.parametrize("B,T,F,rec_mode", [(1200, 24, 10, "auto"), (1217, 33, 10, "auto"), (1217, 20, 20, "auto"),
+                                            (1200, 24, 10, "one"), (1217, 33, 10, "one")],
+                         ids=["1200-24-10", "1217-33-10", "1217-20-20", "one-1200-24-10", "one-1217-33-10"])
+def test_forward_pingpong_path(B, T, F, rec_mode):
+    """More window tiles than SMs: "auto" runs two tiles per CTA (NT = 2), "one" runs one tile per CTA over more than one
+    wave.  1217 windows = 77 tiles: the last CTA's second tile does not exist; F = 20 takes the unfused layer-0 path (gi in
+    quad layout)."""
     sd = synth.synth_state_dict(11, num_features=F)
     feats = synth.synth_features(B, T, F, seed=B + T)
     ref_probs, ref_logits = gru_oracle.predict_on_batch(gru_oracle.build(sd, num_features=F), feats)
     m = _make_model(sd, F, "tc")
+    m.set_rec_mode(rec_mode)
     out = m.forward_arrays(feats, want_logits=True)
     err = _scaled_err(out.logits, ref_logits)
     flips, tie_flips, ties = label_parity(out.labels, ref_probs)
-    print("NT=2 %dx%dx%d: scaled logit err %.3e, label mismatches %d (+%d among %d near-ties)" % (B, T, F, err, flips, tie_flips, ties))
+    print("%s %dx%dx%d: scaled logit err %.3e, label mismatches %d (+%d among %d near-ties)" % (
+        rec_mode, B, T, F, err, flips, tie_flips, ties))
     assert err <= LOGIT_TOL and flips == 0
     m.close()
 
