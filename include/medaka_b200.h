@@ -264,7 +264,9 @@ int mdk_read_matrix(int device, int64_t n_rec, const int32_t *pos, const uint16_
  *                   torch's own layouts; tensors the forward does not use (num_batches_tracked,
  *                   read_level_conv.expansion_layer.*) may be skipped
  *   mdk_rl_forward  x int8 [B][P][D][F] host (the padded read-level feature tensor, torch_ext.py:127-136: F = 4, or 5 with
- *                   dwells) -> probs float32 [B][P][5] host (softmax output, normalise = True as at inference) */
+ *                   dwells) -> probs float32 [B][P][5] host (softmax output, normalise = True as at inference); returns
+ *                   when the probabilities are in host memory.  It is mdk_rl_submit + mdk_rl_wait, except that the open
+ *                   group is launched first and the call runs as one group of its own, whatever its B */
 typedef struct mdk_rl_engine mdk_rl_engine;
 int mdk_rl_create(int device, int32_t lstm_size, int32_t cnn_size, int32_t use_dwells, int32_t num_classes,
                   mdk_rl_engine **out);
@@ -276,9 +278,37 @@ int mdk_rl_load(mdk_rl_engine *e, const char *name, const float *data, int64_t n
 int mdk_rl_set_conv(mdk_rl_engine *e, int tensor_cores);
 int mdk_rl_forward(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P, int64_t D, int64_t F,
                    float *probs_host);
-/* per-stage device times of the forwards that follow mdk_rl_set_timing(e, 1) (CUDA events on the engine's stream);
- * mdk_rl_stage_ms writes the last forward's 6 times in ms: convolution (mask, k = 1 and k = 17 convolutions, pooling
- * Linear), layer-0 projection, layer-0 recurrence, layer-1 projection, layer-1 recurrence, head */
+/* asynchronous form of mdk_rl_forward: returns once the call is queued; labels_host uint8 [B][P] (may be NULL) receives
+ * the argmax of each position's probabilities, first maximum wins (labels.py:1063).  x_host, probs_host and labels_host
+ * must stay valid and untouched until mdk_rl_wait(ticket) returns (page-locked memory from mdk_host_alloc makes the
+ * copies asynchronous).
+ * Calls are PACKED: each call's convolution (which depends on its read depth D) runs when it is submitted, in slices of
+ * a fixed scratch budget, and leaves the pooled LSTM input of its windows in the open group; the LSTM input
+ * projections, both recurrences and the head then run ONCE per group over all of its windows - the recurrences take as
+ * long for one window as for a full wave, so a 100-window batch that runs alone pays the whole 2 x P-step chain.  Calls
+ * of different D share a group; a call with another P seals the group first; a call that does not fit what is left of
+ * the group is split, and its ticket follows its last piece.  A group is launched when it is full
+ * (mdk_rl_preferred_windows at P = 10 000, in general one recurrence wave capped by a 24 GiB budget for the group
+ * buffers), when P changes, on mdk_rl_flush, or when somebody waits for one of its tickets.  Without mdk_rl_reserve a
+ * group collects calls only as far as the group buffers reach (they grow to the call that opens a group).  Groups
+ * complete, and tickets with them, in submission order.  Results are bit-identical to each window run alone through
+ * mdk_rl_forward: windows never interact. */
+int mdk_rl_submit(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P, int64_t D, int64_t F,
+                  float *probs_host, uint8_t *labels_host, int64_t *ticket);
+int mdk_rl_wait(mdk_rl_engine *e, int64_t ticket);
+/* launch the group that is still collecting calls (if any) without waiting for it */
+int mdk_rl_flush(mdk_rl_engine *e);
+/* size the group buffers for groups of up to min(windows, the group limit at P) windows of P positions (launches the
+ * open group first): a submitted group never holds more, so the reservation stays within the 24 GiB budget */
+int mdk_rl_reserve(mdk_rl_engine *e, int64_t windows, int64_t P);
+/* windows one group holds at P = 10 000 (the reference's chunk_len): one wave of the tensor-core recurrence (16 windows
+ * per CTA at lstm_size 128, 16 per 8-CTA cluster at 384, both directions), capped by the group buffers' 24 GiB budget -
+ * 112 at 384 (14 clusters of 8 CTAs fit an H100 at once) and 384 at 128.  Callers that own the batching should coalesce to this size. */
+int64_t mdk_rl_preferred_windows(mdk_rl_engine *e);
+/* per-stage device times of the groups that follow mdk_rl_set_timing(e, 1) (CUDA events on the engine's compute
+ * stream); mdk_rl_stage_ms writes the last launched group's 6 times in ms: convolution (mask, k = 1 and k = 17
+ * convolutions, pooling Linear, of all of the group's calls), layer-0 projection, layer-0 recurrence, layer-1
+ * projection, layer-1 recurrence, head */
 int mdk_rl_set_timing(mdk_rl_engine *e, int on);
 int mdk_rl_stage_ms(mdk_rl_engine *e, float *ms);
 

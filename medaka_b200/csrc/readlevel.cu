@@ -1012,10 +1012,11 @@ __global__ void __launch_bounds__(RL_H3) rl_lstm384_kernel(const float *__restri
     }
 }
 
-// Linear(2H = 768 -> 5) + softmax: one warp per position, 24 inputs per lane, the weights in shared memory
+// Linear(2H = 768 -> 5) + softmax + argmax: one warp per position, 24 inputs per lane, the weights in shared memory.
+// labels (may be NULL): argmax of the five probabilities as written, first maximum wins (np.argmax, labels.py:1063)
 __global__ void __launch_bounds__(256) rl_head768_kernel(const float *__restrict__ h1, const float *__restrict__ lin_w,
                                                          const float *__restrict__ lin_b, int64_t n_pos,
-                                                         float *__restrict__ probs) {
+                                                         float *__restrict__ probs, uint8_t *__restrict__ labels) {
     constexpr int W2 = 2 * RL_H3;
     __shared__ __align__(16) float ws[NCLS * W2];
     for (int i = threadIdx.x; i < NCLS * W2; i += blockDim.x) ws[i] = lin_w[i];
@@ -1046,11 +1047,21 @@ __global__ void __launch_bounds__(256) rl_head768_kernel(const float *__restrict
         float sum = 0.f;
 #pragma unroll
         for (int c = 0; c < NCLS; ++c) { s[c] = expf(s[c] - mx); sum += s[c]; }
-        if (lane < NCLS) {
-            float v = s[0];
+        float v = s[0];
 #pragma unroll
-            for (int c = 1; c < NCLS; ++c) if (lane == c) v = s[c];
-            probs[p * NCLS + lane] = v / sum;
+        for (int c = 1; c < NCLS; ++c) if (lane == c) v = s[c];
+        const float pr = v / sum;                  // lane c < 5: probability of class c
+        if (lane < NCLS) probs[p * NCLS + lane] = pr;
+        if (labels) {                              // argmax over lanes 0..4, first maximum wins
+            float best = lane < NCLS ? pr : -1.f;
+            int arg = lane;
+#pragma unroll
+            for (int m = 4; m >= 1; m >>= 1) {
+                const float ob = __shfl_xor_sync(0xffffffffu, best, m);
+                const int oa = __shfl_xor_sync(0xffffffffu, arg, m);
+                if (ob > best || (ob == best && oa < arg)) { best = ob; arg = oa; }
+            }
+            if (lane == 0) labels[p] = (uint8_t)arg;
         }
     }
 }
@@ -1070,13 +1081,25 @@ struct RlLstmLayer {
 
 using namespace mdk;
 
+// Submitted calls are packed into GROUPS (DESIGN §4).  Each call's convolution runs when it is submitted, in slices of
+// windows bounded by RL_CONV_BUDGET, and writes z (the pooled pre_pool_expansion_layer output) for its windows into the
+// open group's z at their window offset; the projections, both recurrences and the head run once per group over all of
+// its windows.  One set of group buffers, one compute stream: the convolutions of the next group queue behind the
+// group in flight; only the feature copies (copy_in) and the result copies (copy_out) run beside the compute.
+// (The ticket bookkeeping is the counts engine's idea without its lanes: one group buffer set here, so a ticket maps to
+// a group serial number alone.)
+constexpr size_t RL_CONV_BUDGET = (size_t)2 << 30;     // feature staging + convolution scratch of one slice, bytes
+constexpr size_t RL_GROUP_BUDGET = (size_t)24 << 30;   // z, gi, h0, h1, probs, labels of one group, bytes
+constexpr int64_t RL_PREFERRED_P = 10000;              // window length mdk_rl_preferred_windows sizes for (chunk_len)
+
 struct mdk_rl_engine {
     int device = 0;
     int use_dwells = 0;
     int H = RL_H;                  // lstm_size: 128 or 384
-    int timing = 0;                // record per-stage CUDA events in mdk_rl_forward
-    cudaEvent_t ev[7] = {};
-    float stage_ms[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    int sm_count = 132;
+    int wave = 0;                  // windows of one recurrence wave (0: not computed yet)
+    int timing = 0;                // record per-stage CUDA events in each group
+    cudaEvent_t ev[2][7] = {};     // stage events, by group parity: one group's may be read while the next collects
     std::unordered_map<std::string, std::vector<float>> host;     // state-dict tensors as loaded
     bool prepared = false;
     // device parameters
@@ -1090,11 +1113,38 @@ struct mdk_rl_engine {
     RlLstmLayer lstm[2];
     float *lin_w = nullptr, *lin_b = nullptr;
     std::vector<void *> allocs;
-    uint8_t *scratch = nullptr;    // per-call intermediates, grown on demand and kept
-    size_t scratch_bytes = 0;
-    int64_t last_B = 0, last_P = 0;                  // the last completed forward (mdk_rl_debug_read), 0 = none yet
-    size_t last_off[3] = {0, 0, 0};                  // its z, h0, h1 in the scratch
-    cudaStream_t stream = nullptr;
+    cudaStream_t stream = nullptr;                   // compute: convolutions, then each group's LSTM and head
+    cudaStream_t copy_in = nullptr, copy_out = nullptr;
+    // convolution of one slice: features in two staging slots (the copy of the next slice runs under this one's
+    // convolution), then mask | y1 (fp32 path only) | partial sums on the compute stream
+    int8_t *xbuf[2] = {nullptr, nullptr};
+    size_t xcap[2] = {0, 0};
+    cudaEvent_t ev_xin[2] = {}, ev_xfree[2] = {};
+    int xslot = 0;
+    uint8_t *conv = nullptr;
+    size_t conv_cap = 0;
+    // group buffers, [window][P][...] for up to cap_pos positions
+    int64_t cap_pos = 0;
+    float *z = nullptr, *gi = nullptr, *h0 = nullptr, *h1 = nullptr, *probs = nullptr;
+    uint8_t *labels = nullptr;
+    // the open group: its calls' output buffers (host), its windows so far and its window length
+    struct Item {
+        float *probs;
+        uint8_t *labels;
+        int64_t B;
+    };
+    std::vector<Item> items;
+    bool open = false;
+    int64_t gB = 0, gP = 0;
+    int64_t group = -1;                              // serial number of the open or last launched group
+    int64_t launched = -1;                           // serial number of the last launched group
+    static constexpr int OUT_RING = 8;
+    cudaEvent_t ev_done = nullptr;                   // compute -> copy_out
+    cudaEvent_t ev_out[OUT_RING] = {};               // results of group g in its callers' buffers: ev_out[g % OUT_RING]
+    static constexpr int TICKET_RING = 4096;
+    int64_t ticket_group[TICKET_RING] = {};
+    int64_t submit_count = 0;
+    int64_t last_B = 0, last_P = 0;                  // the last completed mdk_rl_forward (mdk_rl_debug_read), 0 = none
 };
 
 namespace {
@@ -1180,12 +1230,14 @@ int rl_prepare_lstm384(mdk_rl_engine *e) {
     return MDK_OK;
 }
 
-int rl_prepare(mdk_rl_engine *e) {
-    if (e->prepared) return MDK_OK;
-    const int nin = RL_EMB + 1 + (e->use_dwells ? 1 : 0);
-    const int HH = e->H;
-    int rc;
-    if (HH == RL_H3) {   // one 8-CTA cluster of the recurrence must fit the device
+// Windows of one wave of the tensor-core recurrence: one CTA per (16-window tile, direction) at lstm_size 128, one
+// 8-CTA cluster per (tile, direction) at 384, as many clusters as fit the device at once (cudaOccupancyMaxActiveClusters;
+// MDK_ERR_UNSUPPORTED when none does).
+int rl_wave_windows(mdk_rl_engine *e, int *out) {
+    if (e->wave > 0) { *out = e->wave; return MDK_OK; }
+    if (e->H == RL_H) {
+        e->wave = LT_N * (e->sm_count / 2);
+    } else {
         MDK_CUDA(cudaFuncSetAttribute(rl_lstm384_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L3_SMEM));
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3(L3_CL, 2);
@@ -1203,6 +1255,33 @@ int rl_prepare(mdk_rl_engine *e) {
         MDK_REQUIRE(clusters >= 1, MDK_ERR_UNSUPPORTED,
                     "read-level model: lstm_size = 384 needs a cluster of 8 CTAs with 210 KiB of shared memory each; "
                     "none fits this device");
+        e->wave = LT_N * std::max(1, clusters / 2);
+    }
+    *out = e->wave;
+    return MDK_OK;
+}
+
+// Most windows of window length P one group holds: one recurrence wave, capped by RL_GROUP_BUDGET (a multiple of the
+// 16-window tile when the cap allows one).
+int rl_group_limit(mdk_rl_engine *e, int64_t P, int64_t *out) {
+    int wave = 0;
+    int rc = rl_wave_windows(e, &wave);
+    if (rc) return rc;
+    const int64_t per_pos = (int64_t)52 * e->H + 4 * NCLS + 1;      // z 4H + gi 32H + h0 8H + h1 8H bytes, probs, label
+    int64_t cap = (int64_t)(RL_GROUP_BUDGET / (size_t)(P * per_pos));
+    if (cap >= LT_N) cap -= cap % LT_N;
+    *out = std::max<int64_t>(1, std::min<int64_t>(wave, cap));
+    return MDK_OK;
+}
+
+int rl_prepare(mdk_rl_engine *e) {
+    if (e->prepared) return MDK_OK;
+    const int nin = RL_EMB + 1 + (e->use_dwells ? 1 : 0);
+    const int HH = e->H;
+    int rc;
+    {   // at 384: one 8-CTA cluster of the recurrence must fit the device
+        int wave = 0;
+        if ((rc = rl_wave_windows(e, &wave))) return rc;
     }
 #define RL_NEED(var, name, n) const std::vector<float> *var = rl_get(e, name, (size_t)(n)); if (!var) return MDK_ERR_STATE;
     RL_NEED(eb, "base_embedder.weight", 6 * RL_EMB)
@@ -1321,6 +1400,235 @@ int rl_prepare(mdk_rl_engine *e) {
     return MDK_OK;
 }
 
+size_t rl_round(size_t bytes) { return (bytes + 255) / 256 * 256; }
+
+// Device buffer of at least `need` bytes (grown by 1/8 to spare regrowth); the caller has drained its users
+template <class T>
+int rl_grow(T **p, size_t *cap, size_t need) {
+    if (need <= *cap) return MDK_OK;
+    if (*p) cudaFree(*p);
+    *p = nullptr;
+    *cap = 0;
+    void *q = nullptr;
+    MDK_CUDA(cudaMalloc(&q, need + need / 8));
+    *p = static_cast<T *>(q);
+    *cap = need + need / 8;
+    return MDK_OK;
+}
+
+// Group buffers for `pos` positions.  Only called when no group is open: the compute and copy-out streams are drained
+// before the old buffers go.
+int rl_ensure_group(mdk_rl_engine *e, int64_t pos) {
+    if (pos <= e->cap_pos) return MDK_OK;
+    MDK_CUDA(cudaStreamSynchronize(e->stream));
+    MDK_CUDA(cudaStreamSynchronize(e->copy_out));
+    e->last_B = e->last_P = 0;                       // the last mdk_rl_forward's stages go with the old buffers
+    float **fb[5] = {&e->z, &e->gi, &e->h0, &e->h1, &e->probs};
+    for (float **p : fb) { if (*p) cudaFree(*p); *p = nullptr; }
+    if (e->labels) cudaFree(e->labels);
+    e->labels = nullptr;
+    e->cap_pos = 0;
+    const size_t n = (size_t)pos, H = (size_t)e->H;
+    const size_t floats[5] = {n * H, n * 8 * H, n * 2 * H, n * 2 * H, n * NCLS};
+    for (int i = 0; i < 5; ++i) MDK_CUDA(cudaMalloc(fb[i], floats[i] * sizeof(float)));
+    MDK_CUDA(cudaMalloc(&e->labels, n));
+    e->cap_pos = pos;
+    return MDK_OK;
+}
+
+void rl_mark(mdk_rl_engine *e, int i) {
+    if (e->timing) cudaEventRecord(e->ev[e->group & 1][i], e->stream);
+}
+
+// The convolution of n windows of one call (host features x [n][P][D][F]) into z of the open group at window woff:
+// mask, k = 1 and k = 17 convolutions, pooled Linear, in slices whose scratch RL_CONV_BUDGET bounds (one window at
+// least).  Each slice's features go to a staging slot on copy_in; a slot is refilled once the convolution that read it
+// is done.  Every window is its own grid slice of each kernel, so the slicing does not change any output bit.
+int rl_conv(mdk_rl_engine *e, const int8_t *x, int64_t n, int64_t P, int64_t D, int64_t F, int64_t woff) {
+    const int dgroup = 4;
+    const int n_groups = (int)((D + dgroup - 1) / dgroup);
+    const size_t xw = (size_t)P * D * F, yw = e->conv_tc ? 0 : (size_t)D * P * RL_C * 4, pw = (size_t)n_groups * P * RL_C * 4;
+    const size_t per_window = 2 * xw + (size_t)D + yw + pw;
+    const int64_t slice = std::max<int64_t>(1, std::min<int64_t>(n, (int64_t)(RL_CONV_BUDGET / per_window)));
+    const size_t o_y1 = rl_round((size_t)slice * D), o_part = o_y1 + rl_round((size_t)slice * yw);
+    int rc;
+    if (o_part + (size_t)slice * pw > e->conv_cap) {
+        MDK_CUDA(cudaStreamSynchronize(e->stream));
+        if ((rc = rl_grow(&e->conv, &e->conv_cap, o_part + (size_t)slice * pw))) return rc;
+    }
+    cudaStream_t s = e->stream;
+    uint8_t *d_mask = e->conv;
+    float *d_y1 = (float *)(e->conv + o_y1), *d_part = (float *)(e->conv + o_part);
+    RlConv1 c1{e->emb_base, e->emb_strand, e->c1_w, e->c1_b, e->bn1[0], e->bn1[1], e->bn1[2], e->bn1[3]};
+    RlConv17 c17{e->c17_wt, e->c17_b, e->bn2[0], e->bn2[1], e->bn2[2], e->bn2[3]};
+    if (e->conv_tc) MDK_CUDA(cudaFuncSetAttribute(rl_conv17_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CT_SMEM));
+    else MDK_CUDA(cudaFuncSetAttribute(rl_conv17_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RL_CONV_SMEM));
+    for (int64_t s0 = 0; s0 < n; s0 += slice) {
+        const int64_t B = std::min(slice, n - s0);
+        const int k = e->xslot;
+        e->xslot ^= 1;
+        if ((size_t)B * xw > e->xcap[k]) {
+            MDK_CUDA(cudaStreamSynchronize(e->stream));
+            MDK_CUDA(cudaStreamSynchronize(e->copy_in));
+            if ((rc = rl_grow(&e->xbuf[k], &e->xcap[k], (size_t)B * xw))) return rc;
+        }
+        MDK_CUDA(cudaStreamWaitEvent(e->copy_in, e->ev_xfree[k], 0));
+        MDK_CUDA(cudaMemcpyAsync(e->xbuf[k], x + (size_t)s0 * xw, (size_t)B * xw, cudaMemcpyHostToDevice, e->copy_in));
+        MDK_CUDA(cudaEventRecord(e->ev_xin[k], e->copy_in));
+        MDK_CUDA(cudaStreamWaitEvent(s, e->ev_xin[k], 0));
+        if (woff + s0 == 0) rl_mark(e, 0);
+        const int8_t *d_x = e->xbuf[k];
+        rl_mask_kernel<<<(unsigned)(B * D), 256, 0, s>>>(d_x, P, (int)D, (int)F, d_mask);
+        if (e->conv_tc) {
+            rl_conv17_tc_kernel<<<dim3((unsigned)((P + CT_NPOS - 1) / CT_NPOS), (unsigned)n_groups, (unsigned)B), 256, CT_SMEM, s>>>(
+                d_x, d_mask, c1, c17, e->c17_tc, P, (int)D, (int)F, e->use_dwells, dgroup, d_part);
+        } else {
+            rl_embed_conv1_kernel<<<dim3((unsigned)((P + 31) / 32), (unsigned)(B * D)), RL_C, 0, s>>>(d_x, d_mask, c1, P, (int)D, (int)F,
+                                                                                                 e->use_dwells, d_y1);
+            rl_conv17_pool_kernel<<<dim3((unsigned)((P + RL_PT - 1) / RL_PT), (unsigned)n_groups, (unsigned)B), 256, RL_CONV_SMEM, s>>>(
+                d_y1, d_mask, c17, P, (int)D, dgroup, d_part);
+        }
+        MDK_CUDA(cudaEventRecord(e->ev_xfree[k], s));
+        float *z = e->z + (size_t)(woff + s0) * P * e->H;
+        if (e->H == RL_H3)
+            rl_pool_linear_kernel<RL_H3><<<dim3((unsigned)((P + RL_PLT - 1) / RL_PLT), (unsigned)B), RL_C, 0, s>>>(
+                d_part, d_mask, e->pool_w, e->pool_b, P, (int)D, n_groups, z);
+        else
+            rl_pool_linear_kernel<RL_H><<<dim3((unsigned)((P + RL_PLT - 1) / RL_PLT), (unsigned)B), RL_C, 0, s>>>(
+                d_part, d_mask, e->pool_w, e->pool_b, P, (int)D, n_groups, z);
+        MDK_CUDA(cudaGetLastError());
+    }
+    return MDK_OK;
+}
+
+// Seal the open group: the projections, both recurrences and the head over all of its windows on the compute stream,
+// then each call's probabilities (and labels) from the group buffers to its own buffers on copy_out.
+int rl_launch(mdk_rl_engine *e) {
+    if (!e->open) return MDK_OK;
+    e->open = false;
+    if (e->items.empty()) return MDK_OK;
+    e->last_B = e->last_P = 0;                       // the group buffers are about to be overwritten
+    const int64_t B = e->gB, P = e->gP, BP = B * P;
+    cudaStream_t s = e->stream;
+    rl_mark(e, 1);
+    const float *layer_in = e->z;
+    float *layer_out[2] = {e->h0, e->h1};
+    float *d_gi = e->gi;
+    if (e->H == RL_H3) {
+        for (int l = 0; l < 2; ++l) {
+            const int in = l == 0 ? RL_H3 : 2 * RL_H3;
+            if (e->lstm_tc) {
+                MDK_CUDA(cudaFuncSetAttribute(rl_proj_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PJ_SMEM));
+                rl_proj_tc_kernel<<<dim3((unsigned)((BP + PJ_N - 1) / PJ_N), 2 * RL_G43 / PJ_M), 256, PJ_SMEM, s>>>(
+                    layer_in, e->lstm[l].w_ih_tc, e->lstm[l].bias, d_gi, BP, in, 2 * RL_G43);
+                rl_mark(e, 2 + 2 * l);
+                rl_lstm384_tc_kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N * L3_CL), 2), L3_THREADS, L3_SMEM, s>>>(
+                    d_gi, e->lstm[l].w_hi, e->lstm[l].w_lo, layer_out[l], B, P);
+            } else {
+                rl_gemm_kernel<<<dim3((unsigned)((BP + 127) / 128), 2 * RL_G43 / 128), 256, 0, s>>>(
+                    layer_in, e->lstm[l].w_ih, e->lstm[l].bias, d_gi, BP, in, 2 * RL_G43);
+                rl_mark(e, 2 + 2 * l);
+                rl_lstm384_kernel<<<dim3((unsigned)((B + R3_NB - 1) / R3_NB), 2), RL_H3, 0, s>>>(d_gi, e->lstm[l].w3t,
+                                                                                               layer_out[l], B, P);
+            }
+            rl_mark(e, 3 + 2 * l);
+            layer_in = layer_out[l];
+        }
+    } else {
+        MDK_CUDA(cudaFuncSetAttribute(rl_lstm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RL_LSTM_SMEM));
+        for (int l = 0; l < 2; ++l) {
+            const int in = l == 0 ? RL_H : 2 * RL_H;
+            rl_gemm_kernel<<<dim3((unsigned)((BP + 127) / 128), 2 * RL_G4 / 128), 256, 0, s>>>(layer_in, e->lstm[l].w_ih, e->lstm[l].bias,
+                                                                                           d_gi, BP, in, 2 * RL_G4);
+            rl_mark(e, 2 + 2 * l);
+            if (e->lstm_tc) {
+                MDK_CUDA(cudaFuncSetAttribute(rl_lstm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LT_SMEM));
+                rl_lstm_tc_kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N), 2), LT_THREADS, LT_SMEM, s>>>(d_gi, e->lstm[l].w_hi, e->lstm[l].w_lo,
+                                                                                                layer_out[l], B, P);
+            } else {
+                rl_lstm_kernel<<<dim3((unsigned)((B + RL_NB - 1) / RL_NB), 2), 256, RL_LSTM_SMEM, s>>>(d_gi, e->lstm[l].w3t, e->lstm[l].wo,
+                                                                                                    layer_out[l], B, P);
+            }
+            rl_mark(e, 3 + 2 * l);
+            layer_in = layer_out[l];
+        }
+    }
+    MDK_CUDA(cudaGetLastError());
+    // the previous group's results must have left probs / labels before the head rewrites them
+    if (e->launched >= 0) MDK_CUDA(cudaStreamWaitEvent(s, e->ev_out[e->launched % mdk_rl_engine::OUT_RING], 0));
+    if (e->H == RL_H3) {
+        int64_t blocks = (BP + 7) / 8;
+        if (blocks > 132 * 8) blocks = 132 * 8;
+        rl_head768_kernel<<<(unsigned)blocks, 256, 0, s>>>(e->h1, e->lin_w, e->lin_b, BP, e->probs, e->labels);
+        MDK_CUDA(cudaGetLastError());
+    } else {
+        MDK_CUDA(launch_head(e->h1, e->lin_w, e->lin_b, B, P, 0, e->probs, nullptr, e->labels, s));
+    }
+    rl_mark(e, 6);
+    MDK_CUDA(cudaEventRecord(e->ev_done, s));
+    MDK_CUDA(cudaStreamWaitEvent(e->copy_out, e->ev_done, 0));
+    int64_t w0 = 0;
+    for (const mdk_rl_engine::Item &it : e->items) {
+        const size_t n = (size_t)it.B * P, off = (size_t)w0 * P;
+        MDK_CUDA(cudaMemcpyAsync(it.probs, e->probs + off * NCLS, n * NCLS * sizeof(float), cudaMemcpyDeviceToHost, e->copy_out));
+        if (it.labels) MDK_CUDA(cudaMemcpyAsync(it.labels, e->labels + off, n, cudaMemcpyDeviceToHost, e->copy_out));
+        w0 += it.B;
+    }
+    MDK_CUDA(cudaEventRecord(e->ev_out[e->group % mdk_rl_engine::OUT_RING], e->copy_out));
+    e->launched = e->group;
+    return MDK_OK;
+}
+
+// One call into the open group, window by window: a new P seals the open group, a call that does not fit what is left
+// of the group is split (windows are independent), a full group is launched at once.  The group buffers grow, when a
+// group opens, to this call's windows (at most gmax): without mdk_rl_reserve a group collects calls only as far as the
+// buffers reach.  ticket (may be NULL) follows the call's last piece.
+int rl_enqueue(mdk_rl_engine *e, const int8_t *x, int64_t B, int64_t P, int64_t D, int64_t F, float *probs,
+               uint8_t *labels, int64_t gmax, int64_t *ticket) {
+    int rc;
+    if (e->open && e->gP != P && (rc = rl_launch(e))) return rc;
+    int64_t done = 0;
+    while (done < B) {
+        if (!e->open) {
+            if ((rc = rl_ensure_group(e, std::min(B - done, gmax) * P))) return rc;
+            e->items.clear();
+            e->gB = 0;
+            e->gP = P;
+            e->open = true;
+            e->group++;
+            e->last_B = e->last_P = 0;               // this group's convolutions overwrite z of the last mdk_rl_forward
+        }
+        const int64_t room = std::min(gmax, e->cap_pos / P) - e->gB;
+        if (room < 1) {
+            if ((rc = rl_launch(e))) return rc;
+            continue;
+        }
+        const int64_t n = std::min(room, B - done);
+        if ((rc = rl_conv(e, x + (size_t)done * P * D * F, n, P, D, F, e->gB))) return rc;
+        e->items.push_back(mdk_rl_engine::Item{probs + (size_t)done * P * NCLS, labels ? labels + (size_t)done * P : nullptr, n});
+        e->gB += n;
+        done += n;
+        if (done == B && ticket) {
+            const int64_t tk = e->submit_count++;
+            e->ticket_group[tk % mdk_rl_engine::TICKET_RING] = e->group;
+            *ticket = tk;
+        }
+        if (n == room && (rc = rl_launch(e))) return rc;
+    }
+    return MDK_OK;
+}
+
+int rl_check(mdk_rl_engine *e, const int8_t *x, int64_t B, int64_t P, int64_t D, int64_t F, const float *probs,
+             const char *who) {
+    const std::string w(who);
+    MDK_REQUIRE(e && x && probs, MDK_ERR_ARG, w + ": NULL argument");
+    MDK_REQUIRE(B >= 1 && P >= 1 && D >= 1, MDK_ERR_ARG, w + ": need B, P, D >= 1");
+    MDK_REQUIRE(F == (e->use_dwells ? 5 : 4) || (!e->use_dwells && F >= 4), MDK_ERR_ARG,
+                w + ": feature vector length does not match the model (4, or 5 with dwells)");
+    MDK_REQUIRE(D <= 65535 && B <= 65535, MDK_ERR_ARG, w + ": B, D <= 65535");
+    return MDK_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1333,17 +1641,29 @@ int mdk_rl_create(int device, int32_t lstm_size, int32_t cnn_size, int32_t use_d
                 "rl_create: supported sizes are lstm_size 128 or 384 with cnn_size 128");
     MDK_REQUIRE(num_classes == NCLS, MDK_ERR_UNSUPPORTED, "rl_create: 5 classes only");
     MDK_CUDA(cudaSetDevice(device));
+    int sms = 0;
+    MDK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
     mdk_rl_engine *e = new (std::nothrow) mdk_rl_engine();
     MDK_REQUIRE(e, MDK_ERR_NOMEM, "rl_create: out of host memory");
     e->device = device;
     e->use_dwells = use_dwells ? 1 : 0;
     e->H = lstm_size;
+    e->sm_count = sms;
     {
         const char *v = getenv("MDK_RL_CONV");      // "fp32": CUDA-core convolution (validation)
         if (v && v[0] == 'f') { e->conv_tc = 0; e->lstm_tc = 0; }
     }
     cudaError_t err = cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking);
-    if (err != cudaSuccess) { delete e; return cuda_fail(err, "cudaStreamCreate", __FILE__, __LINE__); }
+    if (err == cudaSuccess) err = cudaStreamCreateWithFlags(&e->copy_in, cudaStreamNonBlocking);
+    if (err == cudaSuccess) err = cudaStreamCreateWithFlags(&e->copy_out, cudaStreamNonBlocking);
+    for (int i = 0; i < 2 && err == cudaSuccess; ++i) {
+        err = cudaEventCreateWithFlags(&e->ev_xin[i], cudaEventDisableTiming);
+        if (err == cudaSuccess) err = cudaEventCreateWithFlags(&e->ev_xfree[i], cudaEventDisableTiming);
+    }
+    if (err == cudaSuccess) err = cudaEventCreateWithFlags(&e->ev_done, cudaEventDisableTiming);
+    for (int i = 0; i < mdk_rl_engine::OUT_RING && err == cudaSuccess; ++i)
+        err = cudaEventCreateWithFlags(&e->ev_out[i], cudaEventDisableTiming);
+    if (err != cudaSuccess) { mdk_rl_destroy(e); return cuda_fail(err, "rl_create: streams / events", __FILE__, __LINE__); }
     *out = e;
     return MDK_OK;
 }
@@ -1351,11 +1671,19 @@ int mdk_rl_create(int device, int32_t lstm_size, int32_t cnn_size, int32_t use_d
 int mdk_rl_destroy(mdk_rl_engine *e) {
     if (!e) return MDK_OK;
     cudaSetDevice(e->device);
-    if (e->stream) { cudaStreamSynchronize(e->stream); cudaStreamDestroy(e->stream); }
-    for (cudaEvent_t ev : e->ev)
+    for (cudaStream_t s : {e->copy_in, e->stream, e->copy_out})
+        if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); }
+    for (auto &set : e->ev)
+        for (cudaEvent_t ev : set)
+            if (ev) cudaEventDestroy(ev);
+    for (cudaEvent_t ev : {e->ev_xin[0], e->ev_xin[1], e->ev_xfree[0], e->ev_xfree[1], e->ev_done})
+        if (ev) cudaEventDestroy(ev);
+    for (cudaEvent_t ev : e->ev_out)
         if (ev) cudaEventDestroy(ev);
     for (void *p : e->allocs) cudaFree(p);
-    if (e->scratch) cudaFree(e->scratch);
+    for (void *p : {(void *)e->xbuf[0], (void *)e->xbuf[1], (void *)e->conv, (void *)e->z, (void *)e->gi, (void *)e->h0,
+                    (void *)e->h1, (void *)e->probs, (void *)e->labels})
+        if (p) cudaFree(p);
     delete e;
     cudaGetLastError();
     return MDK_OK;
@@ -1377,9 +1705,10 @@ int mdk_rl_set_conv(mdk_rl_engine *e, int tensor_cores) {
 
 int mdk_rl_set_timing(mdk_rl_engine *e, int on) {
     MDK_REQUIRE(e, MDK_ERR_ARG, "rl_set_timing: engine is NULL");
-    if (on && !e->ev[0]) {
+    if (on && !e->ev[0][0]) {
         MDK_CUDA(cudaSetDevice(e->device));
-        for (cudaEvent_t &ev : e->ev) MDK_CUDA(cudaEventCreate(&ev));
+        for (auto &set : e->ev)
+            for (cudaEvent_t &ev : set) MDK_CUDA(cudaEventCreate(&ev));
     }
     e->timing = on ? 1 : 0;
     return MDK_OK;
@@ -1387,125 +1716,84 @@ int mdk_rl_set_timing(mdk_rl_engine *e, int on) {
 
 int mdk_rl_stage_ms(mdk_rl_engine *e, float *ms) {
     MDK_REQUIRE(e && ms, MDK_ERR_ARG, "rl_stage_ms: NULL argument");
-    for (int i = 0; i < 6; ++i) ms[i] = e->stage_ms[i];
+    for (int i = 0; i < 6; ++i) ms[i] = 0.f;
+    if (e->launched < 0 || !e->ev[0][0]) return MDK_OK;
+    MDK_CUDA(cudaSetDevice(e->device));
+    cudaEvent_t *ev = e->ev[e->launched & 1];
+    MDK_CUDA(cudaEventSynchronize(ev[6]));
+    for (int i = 0; i < 6; ++i) MDK_CUDA(cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]));
     return MDK_OK;
 }
 
-int mdk_rl_forward(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P, int64_t D, int64_t F, float *probs_host) {
-    MDK_REQUIRE(e && x_host && probs_host, MDK_ERR_ARG, "rl_forward: NULL argument");
-    MDK_REQUIRE(B >= 1 && P >= 1 && D >= 1, MDK_ERR_ARG, "rl_forward: need B, P, D >= 1");
-    MDK_REQUIRE(F == (e->use_dwells ? 5 : 4) || (!e->use_dwells && F >= 4), MDK_ERR_ARG,
-                "rl_forward: feature vector length does not match the model (4, or 5 with dwells)");
-    MDK_REQUIRE(D <= 65535 && B <= 65535, MDK_ERR_ARG, "rl_forward: B, D <= 65535");
+// A submitted group never holds more than rl_group_limit windows, so the reservation is capped there: asking for a
+// 200-window batch at lstm_size 384 and P = 10 000 must not allocate 40 GB of which 22 GB could ever be used.
+int mdk_rl_reserve(mdk_rl_engine *e, int64_t windows, int64_t P) {
+    MDK_REQUIRE(e && windows >= 1 && P >= 1, MDK_ERR_ARG, "rl_reserve: bad arguments");
     MDK_CUDA(cudaSetDevice(e->device));
-    int rc = rl_prepare(e);
+    int64_t gmax = 0;
+    int rc = rl_group_limit(e, P, &gmax);
     if (rc) return rc;
-    cudaStream_t s = e->stream;
-    const int dgroup = 4;
-    const int n_groups = (int)((D + dgroup - 1) / dgroup);
-    const int64_t BP = B * P;
-    const int HH = e->H;
-    size_t off = 0;
-    auto take = [&off](size_t bytes) { size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
-    const size_t o_x = take((size_t)BP * D * F), o_mask = take((size_t)B * D), o_y1 = take(e->conv_tc ? 256 : (size_t)B * D * P * RL_C * 4),
-                 o_part = take((size_t)B * n_groups * P * RL_C * 4), o_z = take((size_t)BP * HH * 4),
-                 o_gi = take((size_t)BP * 2 * 4 * HH * 4), o_h0 = take((size_t)BP * 2 * HH * 4),
-                 o_h1 = take((size_t)BP * 2 * HH * 4), o_probs = take((size_t)BP * NCLS * 4);
-    e->last_B = e->last_P = 0;                         // the scratch is about to be overwritten
-    if (off > e->scratch_bytes) {
-        if (e->scratch) cudaFree(e->scratch);
-        e->scratch = nullptr;
-        e->scratch_bytes = 0;
-        MDK_CUDA(cudaMalloc(&e->scratch, off + off / 8));
-        e->scratch_bytes = off + off / 8;
+    if ((rc = rl_launch(e))) return rc;
+    return rl_ensure_group(e, std::min(windows, gmax) * P);
+}
+
+int64_t mdk_rl_preferred_windows(mdk_rl_engine *e) {
+    int64_t n = 0;
+    if (!e || cudaSetDevice(e->device) != cudaSuccess || rl_group_limit(e, RL_PREFERRED_P, &n)) return 1;
+    return n;
+}
+
+int mdk_rl_submit(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P, int64_t D, int64_t F, float *probs_host,
+                  uint8_t *labels_host, int64_t *ticket) {
+    int rc = rl_check(e, x_host, B, P, D, F, probs_host, "rl_submit");
+    if (rc) return rc;
+    MDK_REQUIRE(ticket, MDK_ERR_ARG, "rl_submit: ticket is NULL");
+    MDK_CUDA(cudaSetDevice(e->device));
+    if ((rc = rl_prepare(e))) return rc;
+    int64_t gmax = 0;
+    if ((rc = rl_group_limit(e, P, &gmax))) return rc;
+    return rl_enqueue(e, x_host, B, P, D, F, probs_host, labels_host, gmax, ticket);
+}
+
+int mdk_rl_flush(mdk_rl_engine *e) {
+    MDK_REQUIRE(e, MDK_ERR_ARG, "rl_flush: engine is NULL");
+    MDK_CUDA(cudaSetDevice(e->device));
+    return rl_launch(e);
+}
+
+int mdk_rl_wait(mdk_rl_engine *e, int64_t ticket) {
+    MDK_REQUIRE(e, MDK_ERR_ARG, "rl_wait: engine is NULL");
+    MDK_REQUIRE(ticket >= 0 && ticket < e->submit_count, MDK_ERR_ARG, "rl_wait: unknown ticket");
+    MDK_CUDA(cudaSetDevice(e->device));
+    if (ticket < e->submit_count - mdk_rl_engine::TICKET_RING) {   // long done, or at least queued before all of copy_out
+        MDK_CUDA(cudaStreamSynchronize(e->copy_out));
+        return MDK_OK;
     }
-    uint8_t *buf = e->scratch;
-    int8_t *d_x = (int8_t *)(buf + o_x);
-    uint8_t *d_mask = buf + o_mask;
-    float *d_y1 = (float *)(buf + o_y1), *d_part = (float *)(buf + o_part), *d_z = (float *)(buf + o_z),
-          *d_gi = (float *)(buf + o_gi), *d_h0 = (float *)(buf + o_h0), *d_h1 = (float *)(buf + o_h1),
-          *d_probs = (float *)(buf + o_probs);
-    MDK_CUDA(cudaMemcpyAsync(d_x, x_host, (size_t)BP * D * F, cudaMemcpyHostToDevice, s));
-    auto mark = [e, s](int i) { if (e->timing) cudaEventRecord(e->ev[i], s); };
-    mark(0);
-    rl_mask_kernel<<<(unsigned)(B * D), 256, 0, s>>>(d_x, P, (int)D, (int)F, d_mask);
-    RlConv1 c1{e->emb_base, e->emb_strand, e->c1_w, e->c1_b, e->bn1[0], e->bn1[1], e->bn1[2], e->bn1[3]};
-    RlConv17 c17{e->c17_wt, e->c17_b, e->bn2[0], e->bn2[1], e->bn2[2], e->bn2[3]};
-    if (e->conv_tc) {
-        MDK_CUDA(cudaFuncSetAttribute(rl_conv17_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CT_SMEM));
-        rl_conv17_tc_kernel<<<dim3((unsigned)((P + CT_NPOS - 1) / CT_NPOS), (unsigned)n_groups, (unsigned)B), 256, CT_SMEM, s>>>(
-            d_x, d_mask, c1, c17, e->c17_tc, P, (int)D, (int)F, e->use_dwells, dgroup, d_part);
-    } else {
-        rl_embed_conv1_kernel<<<dim3((unsigned)((P + 31) / 32), (unsigned)(B * D)), RL_C, 0, s>>>(d_x, d_mask, c1, P, (int)D, (int)F,
-                                                                                             e->use_dwells, d_y1);
-        MDK_CUDA(cudaFuncSetAttribute(rl_conv17_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RL_CONV_SMEM));
-        rl_conv17_pool_kernel<<<dim3((unsigned)((P + RL_PT - 1) / RL_PT), (unsigned)n_groups, (unsigned)B), 256, RL_CONV_SMEM, s>>>(
-            d_y1, d_mask, c17, P, (int)D, dgroup, d_part);
+    const int64_t g = e->ticket_group[ticket % mdk_rl_engine::TICKET_RING];
+    if (e->open && g == e->group) {                  // still collecting: the caller wants the result now
+        int rc = rl_launch(e);
+        if (rc) return rc;
     }
-    const float *layer_in = d_z;
-    float *layer_out[2] = {d_h0, d_h1};
-    if (HH == RL_H3) {
-        rl_pool_linear_kernel<RL_H3><<<dim3((unsigned)((P + RL_PLT - 1) / RL_PLT), (unsigned)B), RL_C, 0, s>>>(
-            d_part, d_mask, e->pool_w, e->pool_b, P, (int)D, n_groups, d_z);
-        mark(1);
-        for (int l = 0; l < 2; ++l) {
-            const int in = l == 0 ? RL_H3 : 2 * RL_H3;
-            if (e->lstm_tc) {
-                MDK_CUDA(cudaFuncSetAttribute(rl_proj_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PJ_SMEM));
-                rl_proj_tc_kernel<<<dim3((unsigned)((BP + PJ_N - 1) / PJ_N), 2 * RL_G43 / PJ_M), 256, PJ_SMEM, s>>>(
-                    layer_in, e->lstm[l].w_ih_tc, e->lstm[l].bias, d_gi, BP, in, 2 * RL_G43);
-                mark(2 + 2 * l);
-                rl_lstm384_tc_kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N * L3_CL), 2), L3_THREADS, L3_SMEM, s>>>(
-                    d_gi, e->lstm[l].w_hi, e->lstm[l].w_lo, layer_out[l], B, P);
-            } else {
-                rl_gemm_kernel<<<dim3((unsigned)((BP + 127) / 128), 2 * RL_G43 / 128), 256, 0, s>>>(
-                    layer_in, e->lstm[l].w_ih, e->lstm[l].bias, d_gi, BP, in, 2 * RL_G43);
-                mark(2 + 2 * l);
-                rl_lstm384_kernel<<<dim3((unsigned)((B + R3_NB - 1) / R3_NB), 2), RL_H3, 0, s>>>(d_gi, e->lstm[l].w3t,
-                                                                                               layer_out[l], B, P);
-            }
-            mark(3 + 2 * l);
-            layer_in = layer_out[l];
-        }
-        MDK_CUDA(cudaGetLastError());
-        int64_t blocks = (BP + 7) / 8;
-        if (blocks > 132 * 8) blocks = 132 * 8;
-        rl_head768_kernel<<<(unsigned)blocks, 256, 0, s>>>(d_h1, e->lin_w, e->lin_b, BP, d_probs);
-        MDK_CUDA(cudaGetLastError());
-    } else {
-        rl_pool_linear_kernel<RL_H><<<dim3((unsigned)((P + RL_PLT - 1) / RL_PLT), (unsigned)B), RL_H, 0, s>>>(d_part, d_mask, e->pool_w, e->pool_b, P,
-                                                                                                     (int)D, n_groups, d_z);
-        mark(1);
-        MDK_CUDA(cudaFuncSetAttribute(rl_lstm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RL_LSTM_SMEM));
-        for (int l = 0; l < 2; ++l) {
-            const int in = l == 0 ? RL_H : 2 * RL_H;
-            rl_gemm_kernel<<<dim3((unsigned)((BP + 127) / 128), 2 * RL_G4 / 128), 256, 0, s>>>(layer_in, e->lstm[l].w_ih, e->lstm[l].bias,
-                                                                                           d_gi, BP, in, 2 * RL_G4);
-            mark(2 + 2 * l);
-            if (e->lstm_tc) {
-                MDK_CUDA(cudaFuncSetAttribute(rl_lstm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LT_SMEM));
-                rl_lstm_tc_kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N), 2), LT_THREADS, LT_SMEM, s>>>(d_gi, e->lstm[l].w_hi, e->lstm[l].w_lo,
-                                                                                                layer_out[l], B, P);
-            } else {
-                rl_lstm_kernel<<<dim3((unsigned)((B + RL_NB - 1) / RL_NB), 2), 256, RL_LSTM_SMEM, s>>>(d_gi, e->lstm[l].w3t, e->lstm[l].wo,
-                                                                                                    layer_out[l], B, P);
-            }
-            mark(3 + 2 * l);
-            layer_in = layer_out[l];
-        }
-        MDK_CUDA(cudaGetLastError());
-        MDK_CUDA(launch_head(d_h1, e->lin_w, e->lin_b, B, P, 0, d_probs, nullptr, nullptr, s));
-    }
-    mark(6);
-    MDK_CUDA(cudaMemcpyAsync(probs_host, d_probs, (size_t)BP * NCLS * 4, cudaMemcpyDeviceToHost, s));
-    MDK_CUDA(cudaStreamSynchronize(s));
-    if (e->timing)   // convolution (mask + conv + pooling Linear), projection / recurrence of each layer, head
-        for (int i = 0; i < 6; ++i) MDK_CUDA(cudaEventElapsedTime(&e->stage_ms[i], e->ev[i], e->ev[i + 1]));
+    // groups leave copy_out in order: a later group's event also covers g once g's own has been reused
+    if (g > e->launched - mdk_rl_engine::OUT_RING) MDK_CUDA(cudaEventSynchronize(e->ev_out[g % mdk_rl_engine::OUT_RING]));
+    else MDK_CUDA(cudaStreamSynchronize(e->copy_out));
+    return MDK_OK;
+}
+
+// The one-call form: the open group is sealed, then this call runs as one group of its own (however many windows it
+// has), so that mdk_rl_debug_read sees all of it.
+int mdk_rl_forward(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P, int64_t D, int64_t F, float *probs_host) {
+    int rc = rl_check(e, x_host, B, P, D, F, probs_host, "rl_forward");
+    if (rc) return rc;
+    MDK_CUDA(cudaSetDevice(e->device));
+    if ((rc = rl_prepare(e))) return rc;
+    if ((rc = rl_launch(e))) return rc;
+    int64_t gmax = 0, ticket = -1;
+    if ((rc = rl_group_limit(e, P, &gmax))) return rc;
+    if ((rc = rl_enqueue(e, x_host, B, P, D, F, probs_host, nullptr, std::max(B, gmax), &ticket))) return rc;
+    if ((rc = mdk_rl_wait(e, ticket))) return rc;
     e->last_B = B;
     e->last_P = P;
-    e->last_off[0] = o_z;
-    e->last_off[1] = o_h0;
-    e->last_off[2] = o_h1;
     return MDK_OK;
 }
 
@@ -1518,7 +1806,8 @@ int mdk_rl_debug_read(mdk_rl_engine *e, int which, float *out_host, int64_t n_fl
                 "rl_debug_read: n_floats must be " + std::to_string(want) + " (B * P * H for z, B * P * 2H for h0 / h1)");
     MDK_CUDA(cudaSetDevice(e->device));
     MDK_CUDA(cudaStreamSynchronize(e->stream));
-    MDK_CUDA(cudaMemcpy(out_host, e->scratch + e->last_off[which], (size_t)n_floats * sizeof(float), cudaMemcpyDeviceToHost));
+    const float *src = which == 0 ? e->z : which == 1 ? e->h0 : e->h1;
+    MDK_CUDA(cudaMemcpy(out_host, src, (size_t)n_floats * sizeof(float), cudaMemcpyDeviceToHost));
     return MDK_OK;
 }
 

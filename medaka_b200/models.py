@@ -55,6 +55,18 @@ class PinnedArray(object):
             pass
 
 
+def pinned_array(cache, key, shape, dtype):
+    """A view of shape ``shape`` on the page-locked array ``cache[key]``, which is (re)allocated when it is too small."""
+    need = int(np.prod(shape))
+    cur = cache.get(key)
+    if cur is None or cur.dtype != np.dtype(dtype) or int(np.prod(cur.shape)) < need:
+        if cur is not None:
+            cur.close()
+        cur = PinnedArray((need,), dtype)
+        cache[key] = cur
+    return cur.array[:need].reshape(shape)
+
+
 class GRUModel(object):
     """Bidirectional GRU consensus model (gru.py:10-72) executing on an H100.
 
@@ -189,14 +201,7 @@ class GRUModel(object):
 
     def pinned(self, key, shape, dtype):
         """Reusable page-locked staging array, grown on demand."""
-        need = int(np.prod(shape))
-        cur = self._pinned.get(key)
-        if cur is None or cur.dtype != np.dtype(dtype) or int(np.prod(cur.shape)) < need:
-            if cur is not None:
-                cur.close()
-            cur = PinnedArray((need,), dtype)
-            self._pinned[key] = cur
-        return cur.array[:need].reshape(shape)
+        return pinned_array(self._pinned, key, shape, dtype)
 
     def forward_arrays(self, feats, want_logits=False, want_labels=True):
         """feats float32 [B,T,F] (host) -> ForwardOutput of numpy arrays (copies out of pinned staging)."""

@@ -36,8 +36,10 @@ class LatentSpaceLSTM(object):
         _lm.check(lib.mdk_rl_create(device, lstm_size, cnn_size, 1 if use_dwells else 0, num_classes, pe))
         self._engine = pe[0]
         self.max_cells = 1 << 26            # positions x reads per device call
-        self.max_bytes = 8 << 30            # device scratch per call (mdk_rl_forward's intermediates), bytes
+        self.max_bytes = 8 << 30            # forward_arrays' call size in scratch_bytes_per_window units, bytes
         self._fp32_conv = False
+        self._pinned = {}
+        self._async_n = 0
 
     # ---- TorchModel interface (medaka/models.py:233-313) ----
     def load_state_dict(self, state_dict, strict=True):
@@ -69,7 +71,10 @@ class LatentSpaceLSTM(object):
         return dict(zip(self.STAGES, (float(v) for v in ms)))
 
     def scratch_bytes_per_window(self, P, D, F):
-        """Device scratch one window of P positions and D reads takes in mdk_rl_forward (its intermediates)."""
+        """Bytes per window that windows_per_call budgets against max_bytes: every intermediate of the window at once
+        (features, conv partial sums, z, gi, h0, h1, probabilities).  The engine no longer holds them all: a call's
+        convolution runs in slices of a fixed 2 GiB scratch and the group buffers take 52 H + 21 bytes per position
+        (DESIGN §4).  The formula is kept so that forward_arrays cuts batches into the same calls as before."""
         H, groups = self.lstm_size, -(-D // 4)
         per_pos = D * F + groups * 512 + 4 * H + 32 * H + 16 * H + 20 + (D * 512 if self._fp32_conv else 0)
         return P * per_pos + D
@@ -143,9 +148,78 @@ class LatentSpaceLSTM(object):
                                             _lm.ffi.cast("float *", _lm.ffi.from_buffer(out)), out.size))
         return out
 
-    def predict_on_batch(self, batch):
+    # ---- packed asynchronous calls (mdk_rl_submit / wait / flush / reserve) ----
+    def pinned(self, key, shape, dtype):
+        """Reusable page-locked staging array, grown on demand."""
+        from medaka_b200 import models
+        return models.pinned_array(self._pinned, key, shape, dtype)
+
+    def predict_async(self, batch, slots=2):
+        """Asynchronous predict_on_batch: returns a handle whose ``result()`` is the CPU tensor [B, P, 5] and which then
+        carries the argmax labels (uint8 [B, P]) as ``.labels``.
+
+        Up to ``slots`` calls may be in flight, each with its own page-locked staging for the int8 features and the
+        outputs.  The engine runs each call's convolution when it is submitted and packs the calls' windows into groups
+        of ``preferred_batch_size()`` windows whose LSTM runs once (mdk_rl_submit), so the reference's 100-window
+        batches share recurrence waves instead of paying the P-step chain each.
+        """
+        slot = self._async_n % max(int(slots), 1)
+        self._async_n += 1
+        return self._submit(batch, "a%d" % slot)
+
+    def _submit(self, batch, key):
+        """Submit the batch's features through the page-locked staging arrays named `key`; returns the handle."""
         import torch
-        return torch.from_numpy(self.forward_arrays(self.get_model_input_features(batch)))
+        x = self.get_model_input_features(batch)
+        x = x.detach().cpu().numpy() if hasattr(x, "detach") else np.asarray(x)
+        if x.ndim != 4:
+            raise ValueError("expected read-level features [batch, positions, reads, features]")
+        B, P, D, F = x.shape
+        lib, ffi = _lm.lib, _lm.ffi
+        self._last_call = None                               # this call's group overwrites the stages read_stage reads
+        xin = self.pinned(key + "feats", (B, P, D, F), np.int8)
+        np.copyto(xin, x, casting="unsafe")                  # collated batches are uint8 (torch_ext.Batch.collate)
+        probs = self.pinned(key + "probs", (B, P, 5), np.float32)
+        labels = self.pinned(key + "labels", (B, P), np.uint8)
+        ticket = ffi.new("int64_t *")
+        _lm.check(lib.mdk_rl_submit(self._engine, ffi.cast("const int8_t *", ffi.from_buffer(xin)), B, P, D, F,
+                                    ffi.cast("float *", ffi.from_buffer(probs)),
+                                    ffi.cast("uint8_t *", ffi.from_buffer(labels)), ticket))
+        ticket = int(ticket[0])
+        model = self
+
+        class _Handle(object):
+            def result(self_inner):
+                _lm.check(_lm.lib.mdk_rl_wait(model._engine, ticket))
+                model.last_labels = labels.copy()
+                self_inner.labels = model.last_labels
+                return torch.from_numpy(probs.copy())
+
+        return _Handle()
+
+    def preferred_batch_size(self):
+        """Windows one packed group holds at the reference's 10 000-position chunks (mdk_rl_preferred_windows: one
+        recurrence wave within the group buffers' memory budget, 112 at lstm_size 384 on an H100);
+        ``batch_size="auto"`` in ``prediction.run_prediction`` resolves to this."""
+        return int(_lm.lib.mdk_rl_preferred_windows(self._engine))
+
+    def lookahead(self, batch_size, window_len=None):
+        """How many ``predict_async`` calls of ``batch_size`` windows to keep in flight: enough to fill the group that
+        computes and to start filling the next one (its convolutions queue behind the group in flight)."""
+        pref = self.preferred_batch_size()
+        return int(max(2, min(64, 2 * ((pref + batch_size - 1) // max(batch_size, 1)) + 1)))
+
+    def reserve(self, windows, window_len):
+        """Size the group buffers for packed groups of up to ``windows`` windows (mdk_rl_reserve)."""
+        _lm.check(_lm.lib.mdk_rl_reserve(self._engine, int(windows), int(window_len)))
+
+    def flush(self):
+        _lm.check(_lm.lib.mdk_rl_flush(self._engine))
+
+    def predict_on_batch(self, batch):
+        """TorchModel.predict_on_batch (models.py:303-313): CPU float32 tensor [B, P, 5].  Runs through the packed path
+        (one submit, then wait), and keeps the argmax labels of the call on ``self.last_labels`` (uint8 [B, P])."""
+        return self._submit(batch, "sync").result()
 
     def to_dict(self):
         return {"type": "LatentSpaceLSTM", "kwargs": {
@@ -158,6 +232,9 @@ class LatentSpaceLSTM(object):
         if getattr(self, "_engine", None) is not None and _lm.lib is not None:
             _lm.lib.mdk_rl_destroy(self._engine)
             self._engine = None
+        for p in getattr(self, "_pinned", {}).values():
+            p.close()
+        self._pinned = {}
 
     def __del__(self):
         try:
