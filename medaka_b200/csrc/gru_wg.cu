@@ -28,10 +28,18 @@ namespace mdk {
 // thread), W_hh lo is a shared-memory A operand, so per step shared memory feeds only one of the three weight planes.
 // The pre-activations of the next step are loaded straight into the accumulators (r, z) while the step ends; the
 // n gate needs W_in.x and W_hn.h apart, so its input part sits in registers of its own.
-// FUSE_X (layer 0, F <= 16): the input projection W_ih . x_t is three more products per gate on a 16-column x tile,
-// so layer 0 needs no gi buffer.  OUT: fp16 hi/lo operand tiles of the projection GEMM (layer 0), fp32 rows, or
-// (layer 1) partial logits: the 5-row linear head in fp32 on the CUDA cores, from the h values the threads already hold,
-// while the next step's MMAs run (see head_partials).
+// Products per (gate, k-step):
+//   NT = 1: the h tile holds hi and lo as ONE operand of 32 rows (rows 0-15 h_hi of the 16 windows, 16-31 their h_lo).
+//           One RS m64n32k16 gives W_hi.h_hi in accumulator columns 0-15 and W_hi.h_lo in columns 16-31, one SS
+//           m64n16k16 adds W_lo.h_hi (the same descriptor at N = 16 reads rows 0-15) into columns 0-15 (d[0..7]); the
+//           pre-activation is d[k] + d[k + 8].  48 MMAs per warpgroup-step instead of 72, and r and z share one
+//           reciprocal (5 MUFU operations per value instead of 6).
+//   NT = 2: hi and lo planes of N = 32 rows each and three m64n32k16 MMAs (no registers left for accumulators twice as
+//           wide: 239-252 of 255).
+// FUSE_X (layer 0, F <= 16): the input projection W_ih . x_t is the same products per gate on an x tile laid out like
+// the h tile (K = 16), so layer 0 needs no gi buffer.  OUT: fp16 hi/lo operand tiles of the projection GEMM (layer 0),
+// fp32 rows, or (layer 1) partial logits: the 5-row linear head in fp32 on the CUDA cores, from the h values the threads
+// already hold, while the next step's MMAs run (see head_partials).
 // =====================================================================================================
 constexpr int RW_THREADS = 256;
 constexpr int RW_ABLK = (H / 8) * 64 * 16;          // W_hh lo of one (gate, warpgroup): [kg 16][row 64][8] = 16 KiB
@@ -40,16 +48,21 @@ constexpr int RW_XBLK = 2 * 64 * 16;                // W_ih lo (K = 16) of one (
 template <int NT, bool FUSE_X, int OUT>
 struct RwCfg {
     static constexpr int N = NT * RT_N;
-    static constexpr int KG = N * 16 + 16;          // k-group stride of an activation tile (+16 B spreads the 2-byte
+    static constexpr bool HL = NT == 1;             // hi and lo in one operand of 2N rows (see the kernel's header)
+    static constexpr int ROWS = HL ? 2 * N : N;     // rows of an activation operand
+    static constexpr int PLANES = HL ? 1 : 2;       // operands per tile buffer
+    static constexpr int KG = ROWS * 16 + 16;       // k-group stride of an activation tile (+16 B spreads the 2-byte
                                                     // stores of one k-group over the banks)
     static constexpr int HPLANE = (H / 8) * KG;
     static constexpr int XPLANE = 2 * KG;
+    static constexpr int HLO = HL ? N * 16 : HPLANE;   // bytes from an h value's hi half to its lo half
+    static constexpr int XLO = HL ? N * 16 : XPLANE;   // the same in the x tile
     static constexpr int RED = (RW_THREADS / 32) * NCLS * N;                     // head partials of one step (floats)
     static constexpr int wlo_off = 0;                                            // [gate 3][wg 2] RW_ABLK
     static constexpr int wxlo_off = wlo_off + 6 * RW_ABLK;                       // [gate 3][wg 2] RW_XBLK
-    static constexpr int h_off = wxlo_off + (FUSE_X ? 6 * RW_XBLK : 0);          // [buf 2][plane 2] HPLANE
-    static constexpr int x_off = h_off + 4 * HPLANE;                             // [buf 2][plane 2] XPLANE
-    static constexpr int red_off = x_off + (FUSE_X ? 4 * XPLANE : 0);            // [buf 2][warp 8][class 5][N] fp32
+    static constexpr int h_off = wxlo_off + (FUSE_X ? 6 * RW_XBLK : 0);          // [buf 2][plane PLANES] HPLANE
+    static constexpr int x_off = h_off + 2 * PLANES * HPLANE;                    // [buf 2][plane PLANES] XPLANE
+    static constexpr int red_off = x_off + (FUSE_X ? 2 * PLANES * XPLANE : 0);   // [buf 2][warp 8][class 5][N] fp32
     static constexpr int total = red_off + (OUT == OUT_LOGITS ? 2 * RED * 4 : 0);
     static_assert(total <= 227 * 1024, "smem budget");
 };
@@ -62,8 +75,11 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
               void *__restrict__ h_out, int64_t B, int64_t T, const float *__restrict__ lin_w,
               float *__restrict__ plog) {
     using L = RwCfg<NT, FUSE_X, OUT>;
-    constexpr int N = L::N, NA = N / 2;             // accumulator values per thread and gate
-    using MMA = Wgmma<N>;
+    constexpr int N = L::N, NA = N / 2;             // values per thread and gate (hidden unit x window)
+    constexpr int NACC = L::ROWS / 2;               // accumulator registers per gate (HL: NA more for the W_hi.h_lo columns)
+    constexpr int NX = FUSE_X ? NACC : NA;          // axn: an accumulator only when the x projection is fused
+    using MMA = Wgmma<N>;                           // SS: W_lo . h_hi (x_hi)
+    using MMA_H = Wgmma<L::ROWS>;                   // RS: W_hi . the whole h (x) operand
     constexpr bool LOGITS = OUT == OUT_LOGITS;
     extern __shared__ __align__(128) uint8_t smem[];
     const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
@@ -123,8 +139,9 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
     }
     const float bhn[2] = {b_hn[dir * H + j0], b_hn[dir * H + j0 + 8]};
 
-    // Accumulator element k = 4i + 2hb + e: hidden unit j0 + 8hb, window n = 8i + 2cq + e of tile wtile0 + i/2.
-    float ar[NA], az[NA], an[NA], axn[NA], hp[NA];
+    // Accumulator element k = 4i + 2hb + e: hidden unit j0 + 8hb, window n = 8i + 2cq + e of tile wtile0 + i/2
+    // (HL: k >= NA is the lo part of window n - 16, element k - NA).
+    float ar[NACC], az[NACC], an[NACC], axn[NX], hp[NA];
 #pragma unroll
     for (int k = 0; k < NA; ++k) hp[k] = 0.f;
     // pre-activations of time t into the accumulators (gi in quad layout, common.cuh: the pair e = 0, 1 is contiguous)
@@ -149,8 +166,16 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
                 axn[k] = v[2].x; axn[k + 1] = v[2].y;
                 an[k] = bhn[hb]; an[k + 1] = bhn[hb];
             }
+        if constexpr (L::HL) {
+#pragma unroll
+            for (int k = NA; k < NACC; ++k) {
+                ar[k] = 0.f; az[k] = 0.f; an[k] = 0.f;
+                if constexpr (FUSE_X) axn[k] = 0.f;
+            }
+        }
     };
-    // FUSE_X: x_t staged as the B tile [plane][kg 2][n][8]; thread entry q = tid + 256 m covers (window q / F, feature q % F)
+    // FUSE_X: x_t staged as the B tile [plane][kg 2][row][8] (hi at row n, lo XLO bytes on); thread entry q = tid + 256 m
+    // covers (window q / F, feature q % F)
     const int xF = FUSE_X ? xin.F : 1;
     const float *xsrc[NT];
     int xoff[NT];
@@ -166,8 +191,8 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
     auto stage_x = [&](int buf, int m, float v) {
         __half hi, lo;
         split_f16(v, hi, lo);
-        *reinterpret_cast<__half *>(smem + L::x_off + buf * 2 * L::XPLANE + xoff[m]) = hi;
-        *reinterpret_cast<__half *>(smem + L::x_off + buf * 2 * L::XPLANE + L::XPLANE + xoff[m]) = lo;
+        *reinterpret_cast<__half *>(smem + L::x_off + buf * L::PLANES * L::XPLANE + xoff[m]) = hi;
+        *reinterpret_cast<__half *>(smem + L::x_off + buf * L::PLANES * L::XPLANE + L::XLO + xoff[m]) = lo;
     };
     const int64_t t_first = dir ? T - 1 : 0;
     if (FUSE_X) {
@@ -244,28 +269,52 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
     for (int64_t step = 0; step < T; ++step) {
         const int64_t t = dir ? T - 1 - step : step;
         const int buf = (int)(step & 1);
-        const uint32_t hb_addr = sbase + L::h_off + buf * 2 * L::HPLANE;
+        const uint32_t hb_addr = sbase + L::h_off + buf * L::PLANES * L::HPLANE;
         wg_fence();
-#pragma unroll
-        for (int gate = 0; gate < 3; ++gate) {
-            float(&acc)[NA] = gate == 0 ? ar : (gate == 1 ? az : an);
+        if constexpr (L::HL) {
+            // k-step outer, gate inner: consecutive MMAs go to different accumulators
 #pragma unroll
             for (int ks = 0; ks < H / 16; ++ks) {
                 const uint64_t bh = make_smem_desc(hb_addr + ks * 2 * L::KG, L::KG, 128);
-                MMA::rs(acc, whi[gate][ks], bh, 1u);
-                MMA::rs(acc, whi[gate][ks], make_smem_desc(hb_addr + L::HPLANE + ks * 2 * L::KG, L::KG, 128), 1u);
-                MMA::ss(acc, make_smem_desc(sbase + L::wlo_off + (gate * 2 + wg) * RW_ABLK + ks * 2 * 1024, 1024, 128), bh, 1u);
+#pragma unroll
+                for (int gate = 0; gate < 3; ++gate) MMA_H::rs(gate == 0 ? ar : (gate == 1 ? az : an), whi[gate][ks], bh, 1u);
+#pragma unroll
+                for (int gate = 0; gate < 3; ++gate)
+                    MMA::ss(gate == 0 ? ar : (gate == 1 ? az : an),
+                            make_smem_desc(sbase + L::wlo_off + (gate * 2 + wg) * RW_ABLK + ks * 2 * 1024, 1024, 128), bh, 1u);
             }
-        }
-        if (FUSE_X) {
-            const uint32_t xa = sbase + L::x_off + buf * 2 * L::XPLANE;
-            const uint64_t bh = make_smem_desc(xa, L::KG, 128), bl = make_smem_desc(xa + L::XPLANE, L::KG, 128);
+        } else {
 #pragma unroll
             for (int gate = 0; gate < 3; ++gate) {
-                float(&acc)[NA] = gate == 0 ? ar : (gate == 1 ? az : axn);
-                MMA::rs(acc, wxhi[gate], bh, 1u);
-                MMA::rs(acc, wxhi[gate], bl, 1u);
-                MMA::ss(acc, make_smem_desc(sbase + L::wxlo_off + (gate * 2 + wg) * RW_XBLK, 1024, 128), bh, 1u);
+                float(&acc)[NACC] = gate == 0 ? ar : (gate == 1 ? az : an);
+#pragma unroll
+                for (int ks = 0; ks < H / 16; ++ks) {
+                    const uint64_t bh = make_smem_desc(hb_addr + ks * 2 * L::KG, L::KG, 128);
+                    MMA::rs(acc, whi[gate][ks], bh, 1u);
+                    MMA::rs(acc, whi[gate][ks], make_smem_desc(hb_addr + L::HPLANE + ks * 2 * L::KG, L::KG, 128), 1u);
+                    MMA::ss(acc, make_smem_desc(sbase + L::wlo_off + (gate * 2 + wg) * RW_ABLK + ks * 2 * 1024, 1024, 128), bh, 1u);
+                }
+            }
+        }
+        if constexpr (FUSE_X) {
+            const uint32_t xa = sbase + L::x_off + buf * L::PLANES * L::XPLANE;
+            const uint64_t bh = make_smem_desc(xa, L::KG, 128);
+            if constexpr (L::HL) {
+#pragma unroll
+                for (int gate = 0; gate < 3; ++gate) MMA_H::rs(gate == 0 ? ar : (gate == 1 ? az : axn), wxhi[gate], bh, 1u);
+#pragma unroll
+                for (int gate = 0; gate < 3; ++gate)
+                    MMA::ss(gate == 0 ? ar : (gate == 1 ? az : axn),
+                            make_smem_desc(sbase + L::wxlo_off + (gate * 2 + wg) * RW_XBLK, 1024, 128), bh, 1u);
+            } else {
+                const uint64_t bl = make_smem_desc(xa + L::XPLANE, L::KG, 128);
+#pragma unroll
+                for (int gate = 0; gate < 3; ++gate) {
+                    float(&acc)[NACC] = gate == 0 ? ar : (gate == 1 ? az : axn);
+                    MMA::rs(acc, wxhi[gate], bh, 1u);
+                    MMA::rs(acc, wxhi[gate], bl, 1u);
+                    MMA::ss(acc, make_smem_desc(sbase + L::wxlo_off + (gate * 2 + wg) * RW_XBLK, 1024, 128), bh, 1u);
+                }
             }
         }
         wg_commit();
@@ -290,19 +339,31 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
         wg_hold(ar); wg_hold(az); wg_hold(an); wg_hold(axn);
 
         // ---- gate math (weights and biases carry the exp2 scale factors, common.cuh gate_scale) ----
-        uint8_t *hw = smem + L::h_off + (buf ^ 1) * 2 * L::HPLANE;
+        uint8_t *hw = smem + L::h_off + (buf ^ 1) * L::PLANES * L::HPLANE;
 #pragma unroll
         for (int k = 0; k < NA; ++k) {
-            const float r = rcp_approx(1.f + ex2_approx(fminf(ar[k], EXP_CLAMP)));
-            const float z = rcp_approx(1.f + ex2_approx(fminf(az[k], EXP_CLAMP)));
-            const float en = ex2_approx(fminf(fmaf(r, an[k], axn[k]), EXP_CLAMP));
+            float pr = ar[k], pz = az[k], pn = an[k], px = axn[k], r, z;
+            if constexpr (L::HL) {
+                pr += ar[k + NA]; pz += az[k + NA]; pn += an[k + NA];
+                if constexpr (FUSE_X) px += axn[k + NA];
+                // one reciprocal for r and z: r = 1 / a = b / (a b), z = 1 / b = a / (a b); a, b <= 1 + 2^EXP_CLAMP, so
+                // the product stays finite
+                const float a = 1.f + ex2_approx(fminf(pr, EXP_CLAMP)), b = 1.f + ex2_approx(fminf(pz, EXP_CLAMP));
+                const float q = rcp_approx(a * b);
+                r = b * q;
+                z = a * q;
+            } else {
+                r = rcp_approx(1.f + ex2_approx(fminf(pr, EXP_CLAMP)));
+                z = rcp_approx(1.f + ex2_approx(fminf(pz, EXP_CLAMP)));
+            }
+            const float en = ex2_approx(fminf(fmaf(r, pn, px), EXP_CLAMP));
             const float n = (en - 1.f) * rcp_approx(en + 1.f);
             hp[k] = fmaf(z, hp[k] - n, n);
             const int j = j0 + 8 * ((k >> 1) & 1), col = 8 * (k >> 2) + 2 * cq + (k & 1);
             __half hi, lo;
             split_f16(hp[k], hi, lo);
             *reinterpret_cast<__half *>(hw + (j >> 3) * L::KG + col * 16 + (j & 7) * 2) = hi;
-            *reinterpret_cast<__half *>(hw + L::HPLANE + (j >> 3) * L::KG + col * 16 + (j & 7) * 2) = lo;
+            *reinterpret_cast<__half *>(hw + L::HLO + (j >> 3) * L::KG + col * 16 + (j & 7) * 2) = lo;
         }
         if (FUSE_X && step + 1 < T) {
 #pragma unroll

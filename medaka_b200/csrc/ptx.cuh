@@ -163,6 +163,14 @@ template <> struct Wgmma<16> {
             : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
             : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(accumulate));
     }
+    // the same SS MMA into columns 0-15 of an m64n32 accumulator: its d[0..7] (the fragment layout above is that of n16)
+    __device__ __forceinline__ static void ss(float (&d)[16], uint64_t a, uint64_t b, uint32_t accumulate) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+            : "l"(a), "l"(b), "r"(accumulate));
+    }
 };
 template <> struct Wgmma<32> {
     __device__ __forceinline__ static void ss(float (&d)[16], uint64_t a, uint64_t b, uint32_t accumulate) {
