@@ -169,7 +169,7 @@ static int run_forward(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int64_
     launches++;
     MDK_CUDA(cudaEventRecord(e->ev[3], s));
     if (tc) MDK_CUDA(launch_gemm_tc(ws.h0, e->layer[1].w_in_tc, e->layer[1].bias_gi_tc, ws.gi, tiled_rows(B, T), e->sm_count, s));
-    else MDK_CUDA(launch_gemm_fp32((const float *)ws.h0, e->layer[1].w_in_packed, e->layer[1].bias_gi, ws.gi, P, s));
+    else MDK_CUDA(launch_gemm_fp32((const float *)ws.h0, e->layer[1].w_in_packed, e->layer[1].bias_gi, ws.gi, P, H2, GI_COLS, s));
     launches++;
     MDK_CUDA(cudaEventRecord(e->ev[4], s));
     if (tc) {

@@ -197,7 +197,8 @@ cudaError_t launch_unpack_h0(const void *h0_tiles, float *out, int64_t B, int64_
 // gru_fp32.cu
 cudaError_t launch_rec_fp32(const float *gi, const float *w_hh_t, const float *b_hn, float *h_out, int64_t B,
                             int64_t T, cudaStream_t s);
-cudaError_t launch_gemm_fp32(const float *A, const float *W, const float *bias, float *C, int64_t P,
+// C[M][N] = A[M][K] . W[N][K]^T + bias[N], fp32 (K % 16 == 0, N % 128 == 0)
+cudaError_t launch_gemm_fp32(const float *A, const float *W, const float *bias, float *C, int64_t M, int K, int N,
                              cudaStream_t s);
 // gru_wg.cu
 struct RecX {               // fused layer-0 input projection (rec_tc_kernel FUSE_X, F <= 16)

@@ -1,6 +1,6 @@
 // fp32 CUDA-core (FFMA) implementation of the GRU layer: the --full_precision / validation path
 // (MDK_PREC_FP32).  Same data flow as the tensor-core path (gru_wg.cu) with fp32 operands:
-//   gi  = X . W_ih^T + folded bias           (time-parallel GEMM, gemm_fp32)
+//   gi  = X . W_ih^T + folded bias           (time-parallel GEMM, gemm_fp32; the read-level LSTM's fp32 projections too)
 //   h_t = GRU cell(gi_t, h_{t-1} . W_hh^T)   (persistent recurrent kernel, rec_fp32)
 // Reference arithmetic: torch.nn.GRU as used by medaka/architectures/gru.py:46-52,66.
 #include "common.cuh"
@@ -125,14 +125,15 @@ cudaError_t launch_rec_fp32(const float *gi, const float *w_hh_t, const float *b
 }
 
 // -------------------------------------------------------------------------------------
-// Layer-1 input projection, fp32: C[P][768] = A[P][256] . W[768][256]^T + bias.
+// Input projections, fp32: C[M][N] = A[M][K] . W[N][K]^T + bias[N];  K % 16 == 0, N % 128 == 0.
+// The GRU's layer 1 (K = 256, N = 768) and both layers of the read-level LSTM at either size.
 // Classic 128x128x16 shared-memory tiling, 256 threads, 8x8 register tile.
 // -------------------------------------------------------------------------------------
 constexpr int GM = 128, GN = 128, GK = 16;
 
 __global__ void __launch_bounds__(256) gemm_fp32_kernel(const float *__restrict__ A, const float *__restrict__ W,
-                                                        const float *__restrict__ bias, float *__restrict__ C,
-                                                        int64_t P) {
+                                                        const float *__restrict__ bias, float *__restrict__ C, int64_t M,
+                                                        int K, int N) {
     __shared__ float As[GK][GM + 4];
     __shared__ float Ws[GK][GN + 4];
     const int tid = threadIdx.x;
@@ -143,57 +144,55 @@ __global__ void __launch_bounds__(256) gemm_fp32_kernel(const float *__restrict_
 #pragma unroll
     for (int i = 0; i < 8; ++i)
 #pragma unroll
-        for (int jx = 0; jx < 8; ++jx) acc[i][jx] = 0.f;
+        for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
     // loader mapping: 128 rows x 16 k = 512 float4; thread loads 2 float4 per operand
-    const int lrow = tid / 4;            // 0..63
-    const int lk = (tid % 4) * 4;        // 0,4,8,12
-    for (int k0 = 0; k0 < H2; k0 += GK) {
+    const int lrow = tid / 4, lk = (tid % 4) * 4;
+    for (int k0 = 0; k0 < K; k0 += GK) {
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
             const int r = lrow + half * 64;
             const int64_t gm = m0 + r;
-            float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (gm < P) a = *reinterpret_cast<const float4 *>(A + gm * H2 + k0 + lk);
-            As[lk + 0][r] = a.x; As[lk + 1][r] = a.y; As[lk + 2][r] = a.z; As[lk + 3][r] = a.w;
-            const float4 w = *reinterpret_cast<const float4 *>(W + (int64_t)(n0 + r) * H2 + k0 + lk);
-            Ws[lk + 0][r] = w.x; Ws[lk + 1][r] = w.y; Ws[lk + 2][r] = w.z; Ws[lk + 3][r] = w.w;
+            float4 av = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (gm < M) av = *reinterpret_cast<const float4 *>(A + gm * K + k0 + lk);
+            As[lk + 0][r] = av.x; As[lk + 1][r] = av.y; As[lk + 2][r] = av.z; As[lk + 3][r] = av.w;
+            const float4 wv = *reinterpret_cast<const float4 *>(W + (int64_t)(n0 + r) * K + k0 + lk);
+            Ws[lk + 0][r] = wv.x; Ws[lk + 1][r] = wv.y; Ws[lk + 2][r] = wv.z; Ws[lk + 3][r] = wv.w;
         }
         __syncthreads();
 #pragma unroll
         for (int k = 0; k < GK; ++k) {
-            float a[8], b[8];
             // rows {ty*4..+3, 64+ty*4..+3}, cols {tx*4..+3, 64+tx*4..+3}: conflict-free float4 smem reads
             const float4 a0 = *reinterpret_cast<const float4 *>(&As[k][ty * 4]);
             const float4 a1 = *reinterpret_cast<const float4 *>(&As[k][64 + ty * 4]);
             const float4 b0 = *reinterpret_cast<const float4 *>(&Ws[k][tx * 4]);
             const float4 b1 = *reinterpret_cast<const float4 *>(&Ws[k][64 + tx * 4]);
-            a[0] = a0.x; a[1] = a0.y; a[2] = a0.z; a[3] = a0.w; a[4] = a1.x; a[5] = a1.y; a[6] = a1.z; a[7] = a1.w;
-            b[0] = b0.x; b[1] = b0.y; b[2] = b0.z; b[3] = b0.w; b[4] = b1.x; b[5] = b1.y; b[6] = b1.z; b[7] = b1.w;
+            const float av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+            const float bv[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
 #pragma unroll
             for (int i = 0; i < 8; ++i)
 #pragma unroll
-                for (int jx = 0; jx < 8; ++jx) acc[i][jx] = fmaf(a[i], b[jx], acc[i][jx]);
+                for (int j = 0; j < 8; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
         }
         __syncthreads();
     }
     float bv[8];
 #pragma unroll
-    for (int jx = 0; jx < 8; ++jx) bv[jx] = bias[n0 + (jx < 4 ? tx * 4 + jx : 64 + tx * 4 + jx - 4)];
+    for (int j = 0; j < 8; ++j) bv[j] = bias[n0 + (j < 4 ? tx * 4 + j : 64 + tx * 4 + j - 4)];
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
         const int64_t gm = m0 + (i < 4 ? ty * 4 + i : 64 + ty * 4 + i - 4);
-        if (gm >= P) continue;
-        float *dst = C + gm * GI_COLS + n0;
+        if (gm >= M) continue;
+        float *dst = C + gm * N + n0;
         *reinterpret_cast<float4 *>(dst + tx * 4) = make_float4(acc[i][0] + bv[0], acc[i][1] + bv[1], acc[i][2] + bv[2], acc[i][3] + bv[3]);
         *reinterpret_cast<float4 *>(dst + 64 + tx * 4) = make_float4(acc[i][4] + bv[4], acc[i][5] + bv[5], acc[i][6] + bv[6], acc[i][7] + bv[7]);
     }
 }
 
-cudaError_t launch_gemm_fp32(const float *A, const float *W, const float *bias, float *C, int64_t P,
+cudaError_t launch_gemm_fp32(const float *A, const float *W, const float *bias, float *C, int64_t M, int K, int N,
                              cudaStream_t s) {
-    if (P == 0) return cudaSuccess;
-    dim3 grid((unsigned)((P + GM - 1) / GM), GI_COLS / GN);
-    gemm_fp32_kernel<<<grid, 256, 0, s>>>(A, W, bias, C, P);
+    if (M == 0) return cudaSuccess;
+    dim3 grid((unsigned)((M + GM - 1) / GM), N / GN);
+    gemm_fp32_kernel<<<grid, 256, 0, s>>>(A, W, bias, C, M, K, N);
     return cudaGetLastError();
 }
 

@@ -1,6 +1,6 @@
 // Read-level consensus network: LatentSpaceLSTM.forward (medaka/architectures/latent_space_lstm.py:154-207) with
-// ReadLevelConv (read_level_modules.py:45-78) and MeanPooler (:81-100), fp32 on the CUDA cores - the first correct
-// version of SURVEY.md row f4's network half (the feature tensor comes from mdk_read_matrix, pileup.cu).
+// ReadLevelConv (read_level_modules.py:45-78) and MeanPooler (:81-100), SURVEY.md row f4's network half (the feature
+// tensor comes from mdk_read_matrix, pileup.cu).
 //
 //   x int8 [B][P][D][F]  (base, quality, strand, mapQ [, dwell])                      latent_space_lstm.py:163-183
 //   e = base_embedder[base] + strand_embedder[strand + 1]  (6) ++ q / 25 - 1 (++ dwell)          :168-183
@@ -8,32 +8,30 @@
 //   y2 = BN2(ReLU(Conv1d k=17, zero padding 8 (C -> C)))
 //   z  = mean over the non-empty reads of Linear(C -> H)(y2)                                        :192-197, MeanPooler
 //   two bidirectional LSTM layers (H), Linear(2H -> 5), softmax                                    :198-205
-// Sizes: C = cnn_size = 128 with H = lstm_size = 128 (the class defaults) or 384 (every released read-level model; its
-// LSTM kernels are in the "lstm_size = 384" section below); other sizes are refused.  BatchNorm runs in inference
-// mode (running statistics), in torch's operation order ((x - mean) * invstd * weight + bias).
+// Sizes: C = cnn_size = 128 with H = lstm_size = 128 (the class defaults) or 384 (every released read-level model);
+// other sizes are refused.  BatchNorm runs in inference mode (running statistics), in torch's operation order
+// ((x - mean) * invstd * weight + bias).
 //
-// Kernels:
+// Kernels (the tensor-core ones run by default; mdk_rl_set_conv selects the fp32 CUDA-core twins for validation):
 //   rl_mask_kernel        which (window, read) rows are non-empty (x.sum((1, -1)) != 0, :163-165)
-//   rl_embed_conv1_kernel embedding lookups + the k = 1 convolution + ReLU + BN1 -> y1 [B][D][P][C]  (non-empty rows only)
-//   rl_conv17_pool_kernel the k = 17 convolution as an implicit GEMM (64 positions x 128 channels per CTA, K = 17 x 128,
-//                         8 x 4 register tiles, weights streamed through shared memory), ReLU + BN2 and the masked SUM
-//                         over a group of reads, all in one pass: y2 never exists in memory
-//   rl_pool_linear_kernel sum of the read groups / number of reads, then Linear(C -> H).  (The reference applies the
+//   rl_conv17_tc_kernel   embedding + k = 1 convolution + ReLU + BN1 built in shared memory, the k = 17 convolution as
+//                         a wgmma implicit GEMM, ReLU + BN2 and the masked SUM over a group of reads (99 % of the FLOPs)
+//     fp32 twin:          rl_embed_conv1_kernel (-> y1 [B][D][P][C]) + rl_conv17_pool_kernel
+//   rl_pool_linear_kernel<H>  sum of the read groups / number of reads, then Linear(C -> H).  (The reference applies the
 //                         Linear before the mean; the mean of an affine map is the affine map of the mean.)
-//   rl_gemm_kernel        LSTM input projections  gi = X W_ih^T + b_ih + b_hh   (both directions in one launch)
-//   rl_lstm_kernel        the LSTM recurrence: one CTA = 4 windows of one direction, 256 threads (gate pair, unit j);
-//                         W_hh^T of gates i, f, g resident in shared memory (192 KiB), gate o's rows in registers (128
-//                         per thread of the second half); c and h stay on chip for all P steps
-//   head_kernel (misc.cu) Linear(2H -> 5) + softmax, shared with the counts models
-// All of it is CUDA-core fp32: parity first (tests/test_read_level.py against the reference's own class); the convolution
-// is 99 % of the FLOPs (557 kFLOP per read and position); the tensor-core kernels below take it and the recurrence.
-#include <cstdlib>
+//   LSTM input projections gi = X W_ih^T + b_ih + b_hh (both directions in one launch): rl_proj_tc_kernel at H = 384,
+//                         the fp32 gemm_fp32_kernel (gru_fp32.cu) at H = 128 and on the fp32 path
+//   LSTM recurrences      rl_lstm_tc_kernel (H = 128, one CTA per 16-window tile and direction), rl_lstm384_tc_kernel
+//                         (H = 384, one 8-CTA cluster per tile and direction); fp32 twin rl_lstm_fp32<H>
+//   head                  Linear(2H -> 5) + softmax + argmax: head_kernel (misc.cu, shared with the counts models) at
+//                         H = 128, rl_head768_kernel at H = 384
 #include <string>
 #include <unordered_map>
 #include <vector>
 
 #include "common.cuh"
 #include "ptx.cuh"
+#include "rec_common.cuh"
 
 namespace mdk {
 
@@ -404,189 +402,62 @@ __global__ void __launch_bounds__(RL_C) rl_pool_linear_kernel(const float *__res
             if (p0 + i < P) out[(b * P + p0 + i) * HO + h + u * RL_C] = acc[u][i];
 }
 
-// ---------------------------------------------------------------------------------------------- generic fp32 GEMM
-// C[M][N] = A[M][K] . W[N][K]^T + bias[N];  K % 16 == 0, N % 128 == 0.  128 x 128 x 16 tiles, 8 x 8 per thread.
-__global__ void __launch_bounds__(256) rl_gemm_kernel(const float *__restrict__ A, const float *__restrict__ W,
-                                                      const float *__restrict__ bias, float *__restrict__ C, int64_t M,
-                                                      int K, int N) {
-    __shared__ float As[16][128 + 4];
-    __shared__ float Ws[16][128 + 4];
-    const int tid = threadIdx.x;
-    const int64_t m0 = (int64_t)blockIdx.x * 128;
-    const int n0 = blockIdx.y * 128;
-    const int tx = tid % 16, ty = tid / 16;
-    float acc[8][8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
-    const int lrow = tid / 4, lk = (tid % 4) * 4;
-    for (int k0 = 0; k0 < K; k0 += 16) {
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-            const int r = lrow + half * 64;
-            const int64_t gm = m0 + r;
-            float4 av = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (gm < M) av = *reinterpret_cast<const float4 *>(A + gm * K + k0 + lk);
-            As[lk + 0][r] = av.x; As[lk + 1][r] = av.y; As[lk + 2][r] = av.z; As[lk + 3][r] = av.w;
-            const float4 wv = *reinterpret_cast<const float4 *>(W + (int64_t)(n0 + r) * K + k0 + lk);
-            Ws[lk + 0][r] = wv.x; Ws[lk + 1][r] = wv.y; Ws[lk + 2][r] = wv.z; Ws[lk + 3][r] = wv.w;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int k = 0; k < 16; ++k) {
-            const float4 a0 = *reinterpret_cast<const float4 *>(&As[k][ty * 4]);
-            const float4 a1 = *reinterpret_cast<const float4 *>(&As[k][64 + ty * 4]);
-            const float4 b0 = *reinterpret_cast<const float4 *>(&Ws[k][tx * 4]);
-            const float4 b1 = *reinterpret_cast<const float4 *>(&Ws[k][64 + tx * 4]);
-            const float av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-            const float bv[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-            for (int i = 0; i < 8; ++i)
-#pragma unroll
-                for (int j = 0; j < 8; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
-        }
-        __syncthreads();
-    }
-    float bv[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) bv[j] = bias[n0 + (j < 4 ? tx * 4 + j : 64 + tx * 4 + j - 4)];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        const int64_t gm = m0 + (i < 4 ? ty * 4 + i : 64 + ty * 4 + i - 4);
-        if (gm >= M) continue;
-        float *dst = C + gm * N + n0;
-        *reinterpret_cast<float4 *>(dst + tx * 4) = make_float4(acc[i][0] + bv[0], acc[i][1] + bv[1], acc[i][2] + bv[2], acc[i][3] + bv[3]);
-        *reinterpret_cast<float4 *>(dst + 64 + tx * 4) = make_float4(acc[i][4] + bv[4], acc[i][5] + bv[5], acc[i][6] + bv[6], acc[i][7] + bv[7]);
-    }
-}
-
-// ---------------------------------------------------------------------------------------------- LSTM recurrence
+// ---------------------------------------------------------------------------------------------- LSTM recurrence, fp32
 // gi  [B*P][2 dirs][4H]  (torch gate order i, f, g, o; b_ih + b_hh folded in)
 // out [B*P][2H]          (columns dir*H + j)
-// w3t [dir][H k][3H]     W_hh^T of gates i, f, g;   wo [dir][H j][H k]  W_hh rows of gate o
-// One CTA = 4 windows of one direction, 256 threads = (half, unit j).  Half 0 computes gates i and f of unit j, half 1
-// gates g and o; W_hh^T of i, f, g is resident in shared memory (192 KiB), gate o's row j lives in the 128 registers of
-// thread (1, j).  The step is bound by shared-memory wavefronts (weights: 3 x 128 per warp pair; h: one broadcast
-// 16-byte load per window and 4 k), so every load of h feeds two gates.
-constexpr int RL_NB = 4;
-constexpr int RL_LSTM_SMEM = (RL_H * 3 * RL_H + 2 * RL_NB * RL_H + 4 * RL_NB * RL_H) * 4;      // 208 KiB
-
-__global__ void __launch_bounds__(256, 1) rl_lstm_kernel(const float *__restrict__ gi, const float *__restrict__ w3t,
-                                                         const float *__restrict__ wo, float *__restrict__ out, int64_t B,
-                                                         int64_t P) {
-    extern __shared__ __align__(16) float smem_rl[];
-    float *wt = smem_rl;                                  // [128 k][384]
-    float *hs = wt + RL_H * 3 * RL_H;                     // [2][NB][128]
-    float *pre = hs + 2 * RL_NB * RL_H;                   // [4 gates][NB][128]
-    const int tid = threadIdx.x;
-    const int half = tid >> 7, j = tid & 127;
+// w_t [dir][H k][4H]     W_hh^T
+// The recurrence on the CUDA cores (validation path, both sizes): one CTA = 8 windows of one direction, thread = hidden
+// unit j with all four gates, W_hh^T read from global memory (L2-resident: 0.26 MB per direction at H = 128, 2.36 MB at
+// 384), h in shared memory.
+constexpr int LF_NB = 8;
+template <int H>
+__global__ void __launch_bounds__(H) rl_lstm_fp32(const float *__restrict__ gi, const float *__restrict__ wt,
+                                                  float *__restrict__ out, int64_t B, int64_t P) {
+    __shared__ __align__(16) float hs[LF_NB][H];
+    const int j = threadIdx.x;
     const int dir = blockIdx.y;
-    const int64_t b0 = (int64_t)blockIdx.x * RL_NB;
-    const int nb = (int)min((int64_t)RL_NB, B - b0);
-    {
-        const float *src = w3t + (size_t)dir * RL_H * 3 * RL_H;
-        for (int i = tid; i < RL_H * 3 * RL_H / 4; i += 256) reinterpret_cast<float4 *>(wt)[i] = reinterpret_cast<const float4 *>(src)[i];
-        for (int i = tid; i < 2 * RL_NB * RL_H; i += 256) hs[i] = 0.f;
-    }
-    float wq[RL_H];                                       // gate o, row j (half 1 only)
-    if (half == 1) {
+    const int64_t b0 = (int64_t)blockIdx.x * LF_NB;
+    const int nb = (int)min((int64_t)LF_NB, B - b0);
+    const float *w = wt + (size_t)dir * H * (4 * H) + j;
 #pragma unroll
-        for (int k = 0; k < RL_H; k += 4) {
-            const float4 v = *reinterpret_cast<const float4 *>(wo + ((size_t)dir * RL_H + j) * RL_H + k);
-            wq[k] = v.x; wq[k + 1] = v.y; wq[k + 2] = v.z; wq[k + 3] = v.w;
-        }
-    }
-    // update phase: thread (half, j) owns windows n = half, half + 2 of unit j
-    float c_state[RL_NB / 2];
+    for (int n = 0; n < LF_NB; ++n) hs[n][j] = 0.f;
+    float c_state[LF_NB];
 #pragma unroll
-    for (int q = 0; q < RL_NB / 2; ++q) c_state[q] = 0.f;
+    for (int n = 0; n < LF_NB; ++n) c_state[n] = 0.f;
     __syncthreads();
-    int cur = 0;
-    float gnext[RL_NB / 2][4];
-    auto fetch = [&](int64_t t, float (&dst)[RL_NB / 2][4]) {
-#pragma unroll
-        for (int q = 0; q < RL_NB / 2; ++q) {
-            const int n = half + 2 * q;
-            const bool ok = n < nb;
-            const float *row = gi + (((b0 + (ok ? n : 0)) * P + t) * 2 + dir) * RL_G4;
-#pragma unroll
-            for (int gate = 0; gate < 4; ++gate) dst[q][gate] = ok ? __ldg(row + gate * RL_H + j) : 0.f;
-        }
-    };
-    fetch(dir ? (P - 1) : 0, gnext);
     for (int64_t step = 0; step < P; ++step) {
         const int64_t t = dir ? (P - 1 - step) : step;
-        const float *hc = hs + cur * RL_NB * RL_H;
-        float gcur[RL_NB / 2][4];
+        float a[4][LF_NB];
 #pragma unroll
-        for (int q = 0; q < RL_NB / 2; ++q)
-#pragma unroll
-            for (int gate = 0; gate < 4; ++gate) gcur[q][gate] = gnext[q][gate];
-        if (step + 1 < P) fetch(dir ? (t - 1) : (t + 1), gnext);
-        float a0[RL_NB], a1[RL_NB];                       // half 0: i, f     half 1: g, o
-#pragma unroll
-        for (int n = 0; n < RL_NB; ++n) { a0[n] = 0.f; a1[n] = 0.f; }
-        if (half == 0) {
-#pragma unroll 4
-            for (int k = 0; k < RL_H; k += 4) {
-                float4 hv[RL_NB];
-#pragma unroll
-                for (int n = 0; n < RL_NB; ++n) hv[n] = *reinterpret_cast<const float4 *>(hc + n * RL_H + k);
-#pragma unroll
-                for (int kk = 0; kk < 4; ++kk) {
-                    const float wi = wt[(k + kk) * 3 * RL_H + j];
-                    const float wf = wt[(k + kk) * 3 * RL_H + RL_H + j];
-#pragma unroll
-                    for (int n = 0; n < RL_NB; ++n) {
-                        const float hvk = kk == 0 ? hv[n].x : kk == 1 ? hv[n].y : kk == 2 ? hv[n].z : hv[n].w;
-                        a0[n] = fmaf(wi, hvk, a0[n]);
-                        a1[n] = fmaf(wf, hvk, a1[n]);
-                    }
-                }
-            }
-        } else {
-#pragma unroll
-            for (int k = 0; k < RL_H; k += 4) {            // fully unrolled: wq[] must stay in registers
-                float4 hv[RL_NB];
-#pragma unroll
-                for (int n = 0; n < RL_NB; ++n) hv[n] = *reinterpret_cast<const float4 *>(hc + n * RL_H + k);
-#pragma unroll
-                for (int kk = 0; kk < 4; ++kk) {
-                    const float wg = wt[(k + kk) * 3 * RL_H + 2 * RL_H + j];
-                    const float wov = wq[k + kk];
-#pragma unroll
-                    for (int n = 0; n < RL_NB; ++n) {
-                        const float hvk = kk == 0 ? hv[n].x : kk == 1 ? hv[n].y : kk == 2 ? hv[n].z : hv[n].w;
-                        a0[n] = fmaf(wg, hvk, a0[n]);
-                        a1[n] = fmaf(wov, hvk, a1[n]);
-                    }
-                }
-            }
-        }
-#pragma unroll
-        for (int n = 0; n < RL_NB; ++n) {
-            pre[((2 * half) * RL_NB + n) * RL_H + j] = a0[n];
-            pre[((2 * half + 1) * RL_NB + n) * RL_H + j] = a1[n];
-        }
-        __syncthreads();
-        float *hn = hs + (cur ^ 1) * RL_NB * RL_H;
-#pragma unroll
-        for (int q = 0; q < RL_NB / 2; ++q) {
-            const int n = half + 2 * q;
+        for (int n = 0; n < LF_NB; ++n) {
             const bool ok = n < nb;
-            const float ig = rl_sigmoid(gcur[q][0] + pre[(0 * RL_NB + n) * RL_H + j]);
-            const float fg = rl_sigmoid(gcur[q][1] + pre[(1 * RL_NB + n) * RL_H + j]);
-            const float gg = tanhf(gcur[q][2] + pre[(2 * RL_NB + n) * RL_H + j]);
-            const float og = rl_sigmoid(gcur[q][3] + pre[(3 * RL_NB + n) * RL_H + j]);
-            const float c = fg * c_state[q] + ig * gg;
-            c_state[q] = c;
+            const float *row = gi + (((b0 + (ok ? n : 0)) * P + t) * 2 + dir) * (4 * H) + j;
+#pragma unroll
+            for (int g = 0; g < 4; ++g) a[g][n] = ok ? __ldg(row + g * H) : 0.f;
+        }
+#pragma unroll 4
+        for (int k = 0; k < H; ++k) {
+            float wv[4];
+#pragma unroll
+            for (int g = 0; g < 4; ++g) wv[g] = __ldg(w + (size_t)k * (4 * H) + g * H);
+#pragma unroll
+            for (int n = 0; n < LF_NB; ++n) {
+                const float hk = hs[n][k];
+#pragma unroll
+                for (int g = 0; g < 4; ++g) a[g][n] = fmaf(wv[g], hk, a[g][n]);
+            }
+        }
+        __syncthreads();                                     // every thread has read h of the previous step
+#pragma unroll
+        for (int n = 0; n < LF_NB; ++n) {
+            const float ig = rl_sigmoid(a[0][n]), fg = rl_sigmoid(a[1][n]), gg = tanhf(a[2][n]), og = rl_sigmoid(a[3][n]);
+            const float c = fg * c_state[n] + ig * gg;
+            c_state[n] = c;
             const float h = og * tanhf(c);
-            hn[n * RL_H + j] = h;
-            if (ok) out[((b0 + n) * P + t) * (2 * RL_H) + dir * RL_H + j] = h;
+            hs[n][j] = h;
+            if (n < nb) out[((b0 + n) * P + t) * (2 * H) + dir * H + j] = h;
         }
         __syncthreads();
-        cur ^= 1;
     }
 }
 
@@ -605,11 +476,13 @@ constexpr int LT_HPLANE = (RL_H / 8) * LT_KG;
 constexpr int LT_OFF_H = 4 * LT_WLO_GATE;
 constexpr int LT_SMEM = LT_OFF_H + 4 * LT_HPLANE;
 constexpr int LT_THREADS = 256;
+// element (direction d, gate row r, column k) of W_hh's lo plane in the tiles above: [dir][gate][k-group][row][8 halfs]
+inline size_t lt_lo_index(int d, int r, int k) {
+    return ((((size_t)d * 4 + r / RL_H) * (RL_H / 8) + k / 8) * RL_H + r % RL_H) * 8 + k % 8;
+}
 // MUFU-based gate functions (ex2.approx / rcp.approx, ~2 ulp)
-__device__ __forceinline__ float lt_ex2(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-__device__ __forceinline__ float lt_rcp(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-__device__ __forceinline__ float lt_sigmoid(float x) { return lt_rcp(1.0f + lt_ex2(-1.4426950408889634f * x)); }
-__device__ __forceinline__ float lt_tanh(float x) { return fmaf(-2.0f, lt_rcp(1.0f + lt_ex2(2.8853900817779268f * x)), 1.0f); }
+__device__ __forceinline__ float lt_sigmoid(float x) { return rcp_approx(1.0f + ex2_approx(-1.4426950408889634f * x)); }
+__device__ __forceinline__ float lt_tanh(float x) { return fmaf(-2.0f, rcp_approx(1.0f + ex2_approx(2.8853900817779268f * x)), 1.0f); }
 
 __global__ void __launch_bounds__(LT_THREADS, 1) rl_lstm_tc_kernel(const float *__restrict__ gi, const __half *__restrict__ w_hi,
                                                             const uint8_t *__restrict__ w_lo_tiles, float *__restrict__ out,
@@ -702,7 +575,8 @@ __global__ void __launch_bounds__(LT_THREADS, 1) rl_lstm_tc_kernel(const float *
 // Every released read-level model is `..._rl_lstm384_...`: H = 384 with C = 128.  The convolution and the mask are the
 // kernels above; the pooling Linear is rl_pool_linear_kernel<384>.  What changes is the LSTM: W_hh is 4H x H per
 // direction (2.25 MiB as fp16 hi + lo, more than one SM holds) and the input projections grow nine-fold (7.1 MFLOP per
-// position for both layers and directions), so both get kernels of their own.
+// position for both layers and directions), so both get tensor-core kernels of their own.  The fp32 twins
+// (rl_lstm_fp32, gemm_fp32_kernel) serve both sizes.
 constexpr int RL_H3 = 384;
 constexpr int RL_G43 = 4 * RL_H3;                  // 1536 gate rows per direction
 
@@ -838,6 +712,12 @@ constexpr int L3_OFF_H = 3 * L3_WLO_WG;
 constexpr int L3_OFF_X = L3_OFF_H + 4 * L3_HPLANE;
 constexpr int L3_OFF_BAR = L3_OFF_X + 3 * L3_XCH_WG;
 constexpr int L3_SMEM = L3_OFF_BAR + 16;                     // 210 KiB
+// element (direction d, gate row r, column k) of W_hh's lo plane in the tiles above: per (direction, cluster rank,
+// warpgroup) [k-group][row m = 16 gate + unit within the warpgroup][8 halfs]
+inline size_t l3_lo_index(int d, int r, int k) {
+    const int gate = r / RL_H3, j = r % RL_H3, rank = j / L3_UNITS, wg = (j % L3_UNITS) / 16, m = gate * 16 + j % 16;
+    return (((size_t)(d * L3_CL + rank) * 3 + wg) * (RL_H3 / 8) + k / 8) * (64 * 8) + m * 8 + k % 8;
+}
 
 __global__ void __cluster_dims__(L3_CL, 1, 1) __launch_bounds__(L3_THREADS, 1)
     rl_lstm384_tc_kernel(const float *__restrict__ gi, const __half *__restrict__ w_hi, const uint8_t *__restrict__ w_lo_tiles,
@@ -958,60 +838,6 @@ __global__ void __cluster_dims__(L3_CL, 1, 1) __launch_bounds__(L3_THREADS, 1)
     }
 }
 
-// ---------------------------------------------------------------------------------------------- fp32 twins at 384
-// The recurrence on the CUDA cores (validation path): one CTA = 8 windows of one direction, thread = hidden unit j with
-// all four gates, W_hh^T [k][4H] read from global memory (2.36 MB per direction, L2-resident), h in shared memory.
-constexpr int R3_NB = 8;
-__global__ void __launch_bounds__(RL_H3) rl_lstm384_kernel(const float *__restrict__ gi, const float *__restrict__ wt,
-                                                           float *__restrict__ out, int64_t B, int64_t P) {
-    __shared__ __align__(16) float hs[R3_NB][RL_H3];
-    const int j = threadIdx.x;
-    const int dir = blockIdx.y;
-    const int64_t b0 = (int64_t)blockIdx.x * R3_NB;
-    const int nb = (int)min((int64_t)R3_NB, B - b0);
-    const float *w = wt + (size_t)dir * RL_H3 * RL_G43 + j;
-#pragma unroll
-    for (int n = 0; n < R3_NB; ++n) hs[n][j] = 0.f;
-    float c_state[R3_NB];
-#pragma unroll
-    for (int n = 0; n < R3_NB; ++n) c_state[n] = 0.f;
-    __syncthreads();
-    for (int64_t step = 0; step < P; ++step) {
-        const int64_t t = dir ? (P - 1 - step) : step;
-        float a[4][R3_NB];
-#pragma unroll
-        for (int n = 0; n < R3_NB; ++n) {
-            const bool ok = n < nb;
-            const float *row = gi + (((b0 + (ok ? n : 0)) * P + t) * 2 + dir) * RL_G43 + j;
-#pragma unroll
-            for (int g = 0; g < 4; ++g) a[g][n] = ok ? __ldg(row + g * RL_H3) : 0.f;
-        }
-#pragma unroll 4
-        for (int k = 0; k < RL_H3; ++k) {
-            float wv[4];
-#pragma unroll
-            for (int g = 0; g < 4; ++g) wv[g] = __ldg(w + (size_t)k * RL_G43 + g * RL_H3);
-#pragma unroll
-            for (int n = 0; n < R3_NB; ++n) {
-                const float hk = hs[n][k];
-#pragma unroll
-                for (int g = 0; g < 4; ++g) a[g][n] = fmaf(wv[g], hk, a[g][n]);
-            }
-        }
-        __syncthreads();                                     // every thread has read h of the previous step
-#pragma unroll
-        for (int n = 0; n < R3_NB; ++n) {
-            const float ig = rl_sigmoid(a[0][n]), fg = rl_sigmoid(a[1][n]), gg = tanhf(a[2][n]), og = rl_sigmoid(a[3][n]);
-            const float c = fg * c_state[n] + ig * gg;
-            c_state[n] = c;
-            const float h = og * tanhf(c);
-            hs[n][j] = h;
-            if (n < nb) out[((b0 + n) * P + t) * (2 * RL_H3) + dir * RL_H3 + j] = h;
-        }
-        __syncthreads();
-    }
-}
-
 // Linear(2H = 768 -> 5) + softmax + argmax: one warp per position, 24 inputs per lane, the weights in shared memory.
 // labels (may be NULL): argmax of the five probabilities as written, first maximum wins (np.argmax, labels.py:1063)
 __global__ void __launch_bounds__(256) rl_head768_kernel(const float *__restrict__ h1, const float *__restrict__ lin_w,
@@ -1068,12 +894,12 @@ __global__ void __launch_bounds__(256) rl_head768_kernel(const float *__restrict
 
 // ---------------------------------------------------------------------------------------------- engine
 struct RlLstmLayer {
-    __half *w_hi = nullptr;     // [2][4H][H] fp16 hi plane of W_hh (tensor-core kernel: -> registers)
-    uint8_t *w_lo = nullptr;    // [2][4 gates][k-group 16][row 128][8 halfs] lo plane as shared-memory A operand tiles
     float *w_ih = nullptr;      // [2 dirs * 4H][in]   (both directions stacked: one GEMM)
     float *bias = nullptr;      // [2 * 4H]  b_ih + b_hh
-    float *w3t = nullptr;       // H = 128: [2][H][3H];   H = 384: W_hh^T [2][H k][4H] (fp32 recurrence)
-    float *wo = nullptr;        // [2][H][H]  (H = 128)
+    float *w_t = nullptr;       // [2][H k][4H]  W_hh^T (fp32 recurrence)
+    __half *w_hi = nullptr;     // [2][4H][H] fp16 hi plane of W_hh, row-major (tensor-core recurrences: -> registers)
+    uint8_t *w_lo = nullptr;    // fp16 lo plane of W_hh as the tensor-core recurrence's shared-memory A operand tiles
+                                // (lt_lo_index at H = 128, l3_lo_index at 384)
     uint8_t *w_ih_tc = nullptr; // H = 384: W_ih as rl_proj_tc_kernel's A tiles [row block 24][K chunk][hi | lo][8][128][8]
 };
 
@@ -1179,36 +1005,44 @@ int rl_upload_raw(mdk_rl_engine *e, const std::vector<T> &v, T **out) {
     return MDK_OK;
 }
 
-// LSTM weights at H = 384: fp32 copies for the CUDA-core twins, fp16 hi / lo operand tiles for the tensor-core kernels
-int rl_prepare_lstm384(mdk_rl_engine *e) {
-    constexpr int H3 = RL_H3, G4 = RL_G43;
+// LSTM weights of both layers at either size: W_ih of both directions stacked for one projection, b_ih + b_hh, W_hh^T for
+// the fp32 recurrence, W_hh as fp16 hi (row-major) and lo (the tensor-core recurrence's operand tiles) planes, and at
+// H = 384 W_ih as rl_proj_tc_kernel's operand tiles
+int rl_prepare_lstm(mdk_rl_engine *e) {
+    const int HH = e->H, G4 = 4 * HH;
     int rc;
     for (int l = 0; l < 2; ++l) {
-        const int in = l == 0 ? H3 : 2 * H3;
-        const int nchunks = in / PJ_KC;
-        std::vector<float> w_ih((size_t)2 * G4 * in), bias((size_t)2 * G4), wt((size_t)2 * H3 * G4);
-        std::vector<__half> hi((size_t)2 * G4 * H3), lo_t((size_t)2 * G4 * H3), ih_t((size_t)2 * G4 * in * 2);
+        const int in = l == 0 ? HH : 2 * HH;
+        std::vector<float> w_ih((size_t)2 * G4 * in), bias((size_t)2 * G4), w_t((size_t)2 * HH * G4);
+        std::vector<__half> hi((size_t)2 * G4 * HH), lo((size_t)2 * G4 * HH);
         for (int d = 0; d < 2; ++d) {
             const std::string sfx = "_l" + std::to_string(l) + (d ? "_reverse" : "");
             const std::vector<float> *wih = rl_get(e, "lstm.weight_ih" + sfx, (size_t)G4 * in);
-            const std::vector<float> *whh = rl_get(e, "lstm.weight_hh" + sfx, (size_t)G4 * H3);
+            const std::vector<float> *whh = rl_get(e, "lstm.weight_hh" + sfx, (size_t)G4 * HH);
             const std::vector<float> *bih = rl_get(e, "lstm.bias_ih" + sfx, G4);
             const std::vector<float> *bhh = rl_get(e, "lstm.bias_hh" + sfx, G4);
             if (!wih || !whh || !bih || !bhh) return MDK_ERR_STATE;
             std::copy(wih->begin(), wih->end(), w_ih.begin() + (size_t)d * G4 * in);
             for (int r = 0; r < G4; ++r) bias[(size_t)d * G4 + r] = (*bih)[r] + (*bhh)[r];
             for (int r = 0; r < G4; ++r)
-                for (int k = 0; k < H3; ++k) {
-                    const float v = (*whh)[(size_t)r * H3 + k];
-                    wt[((size_t)d * H3 + k) * G4 + r] = v;
+                for (int k = 0; k < HH; ++k) {
+                    const float v = (*whh)[(size_t)r * HH + k];
+                    w_t[((size_t)d * HH + k) * G4 + r] = v;
                     const __half h16 = __float2half_rn(v), l16 = __float2half_rn(v - __half2float(h16));
-                    hi[((size_t)d * G4 + r) * H3 + k] = h16;
-                    // lo tiles per (direction, cluster rank, warpgroup): row m = 16 gate + unit within the warpgroup
-                    const int gate = r / H3, j = r % H3, rank = j / L3_UNITS, wg = (j % L3_UNITS) / 16, m = gate * 16 + j % 16;
-                    lo_t[(((size_t)(d * L3_CL + rank) * 3 + wg) * (H3 / 8) + k / 8) * (64 * 8) + m * 8 + k % 8] = l16;
+                    hi[((size_t)d * G4 + r) * HH + k] = h16;
+                    lo[HH == RL_H3 ? l3_lo_index(d, r, k) : lt_lo_index(d, r, k)] = l16;
                 }
         }
+        RlLstmLayer &L = e->lstm[l];
+        __half *p = nullptr;
+        if ((rc = rl_upload(e, w_ih, &L.w_ih)) || (rc = rl_upload(e, bias, &L.bias)) || (rc = rl_upload(e, w_t, &L.w_t)) ||
+            (rc = rl_upload_raw(e, hi, &L.w_hi)) || (rc = rl_upload_raw(e, lo, &p)))
+            return rc;
+        L.w_lo = reinterpret_cast<uint8_t *>(p);
+        if (HH != RL_H3) continue;
         // W_ih of both directions as one [3072][in] matrix, tiled per (128-row block, 64-wide K chunk)
+        const int nchunks = in / PJ_KC;
+        std::vector<__half> ih_t((size_t)2 * G4 * in * 2);
         for (int r = 0; r < 2 * G4; ++r)
             for (int k = 0; k < in; ++k) {
                 const float v = w_ih[(size_t)r * in + k];
@@ -1218,14 +1052,8 @@ int rl_prepare_lstm384(mdk_rl_engine *e) {
                 ih_t[chunk + off] = h16;
                 ih_t[chunk + PJ_WPLANE / 2 + off] = l16;
             }
-        if ((rc = rl_upload(e, w_ih, &e->lstm[l].w_ih)) || (rc = rl_upload(e, bias, &e->lstm[l].bias)) ||
-            (rc = rl_upload(e, wt, &e->lstm[l].w3t)) || (rc = rl_upload_raw(e, hi, &e->lstm[l].w_hi)))
-            return rc;
-        __half *p = nullptr;
-        if ((rc = rl_upload_raw(e, lo_t, &p))) return rc;
-        e->lstm[l].w_lo = reinterpret_cast<uint8_t *>(p);
         if ((rc = rl_upload_raw(e, ih_t, &p))) return rc;
-        e->lstm[l].w_ih_tc = reinterpret_cast<uint8_t *>(p);
+        L.w_ih_tc = reinterpret_cast<uint8_t *>(p);
     }
     return MDK_OK;
 }
@@ -1323,11 +1151,9 @@ int rl_prepare(mdk_rl_engine *e) {
                     tc[((size_t)t * 2 + 0) * RL_C * RL_C + off] = hi;
                     tc[((size_t)t * 2 + 1) * RL_C * RL_C + off] = lo;
                 }
-        void *p = nullptr;
-        MDK_CUDA(cudaMalloc(&p, tc.size() * sizeof(__half)));
-        e->allocs.push_back(p);
-        MDK_CUDA(cudaMemcpy(p, tc.data(), tc.size() * sizeof(__half), cudaMemcpyHostToDevice));
-        e->c17_tc = static_cast<uint8_t *>(p);
+        __half *p = nullptr;
+        if ((rc = rl_upload_raw(e, tc, &p))) return rc;
+        e->c17_tc = reinterpret_cast<uint8_t *>(p);
     }
     // BatchNorm (inference): mean, 1 / sqrt(var + eps), weight, bias
     for (int l = 0; l < 2; ++l) {
@@ -1343,59 +1169,8 @@ int rl_prepare(mdk_rl_engine *e) {
             (rc = rl_upload(e, *b, &dst[3])))
             return rc;
     }
-    if (HH == RL_H3) {
-        if ((rc = rl_prepare_lstm384(e))) return rc;
-        e->prepared = true;
-        return MDK_OK;
-    }
-    for (int l = 0; l < 2; ++l) {
-        const int in = l == 0 ? RL_H : 2 * RL_H;
-        std::vector<float> w_ih((size_t)2 * RL_G4 * in), bias((size_t)2 * RL_G4), w3t((size_t)2 * RL_H * 3 * RL_H),
-            wo((size_t)2 * RL_H * RL_H);
-        for (int d = 0; d < 2; ++d) {
-            const std::string sfx = "_l" + std::to_string(l) + (d ? "_reverse" : "");
-            RL_NEED(wih, "lstm.weight_ih" + sfx, RL_G4 * in)
-            RL_NEED(whh, "lstm.weight_hh" + sfx, RL_G4 * RL_H)
-            RL_NEED(bih, "lstm.bias_ih" + sfx, RL_G4)
-            RL_NEED(bhh, "lstm.bias_hh" + sfx, RL_G4)
-            std::copy(wih->begin(), wih->end(), w_ih.begin() + (size_t)d * RL_G4 * in);
-            for (int r = 0; r < RL_G4; ++r) bias[(size_t)d * RL_G4 + r] = (*bih)[r] + (*bhh)[r];
-            for (int gate = 0; gate < 3; ++gate)
-                for (int jj = 0; jj < RL_H; ++jj)
-                    for (int k = 0; k < RL_H; ++k)
-                        w3t[((size_t)d * RL_H + k) * 3 * RL_H + gate * RL_H + jj] = (*whh)[((size_t)gate * RL_H + jj) * RL_H + k];
-            for (int jj = 0; jj < RL_H; ++jj)
-                for (int k = 0; k < RL_H; ++k) wo[((size_t)d * RL_H + jj) * RL_H + k] = (*whh)[((size_t)3 * RL_H + jj) * RL_H + k];
-        }
-        if ((rc = rl_upload(e, w_ih, &e->lstm[l].w_ih)) || (rc = rl_upload(e, bias, &e->lstm[l].bias)) ||
-            (rc = rl_upload(e, w3t, &e->lstm[l].w3t)) || (rc = rl_upload(e, wo, &e->lstm[l].wo)))
-            return rc;
-        // tensor-core operands: hi plane row-major (torch's [4H][H] as it is), lo plane as K-major tiles per gate
-        std::vector<__half> hi((size_t)2 * RL_G4 * RL_H), lo_t((size_t)2 * RL_G4 * RL_H);
-        for (int d = 0; d < 2; ++d) {
-            const std::string sfx = "_l" + std::to_string(l) + (d ? "_reverse" : "");
-            const std::vector<float> &whh = e->host["lstm.weight_hh" + sfx];
-            for (int r = 0; r < RL_G4; ++r)
-                for (int k = 0; k < RL_H; ++k) {
-                    const float v = whh[(size_t)r * RL_H + k];
-                    const __half h16 = __float2half_rn(v);
-                    hi[((size_t)d * RL_G4 + r) * RL_H + k] = h16;
-                    const int g = r / RL_H, jj = r % RL_H;
-                    const __half l16 = __float2half_rn(v - __half2float(h16));
-                    lo_t[(size_t)d * RL_G4 * RL_H + (((size_t)g * (RL_H / 8) + k / 8) * RL_H + jj) * 8 + (k % 8)] = l16;
-                }
-        }
-        void *p1 = nullptr, *p2 = nullptr;
-        MDK_CUDA(cudaMalloc(&p1, hi.size() * sizeof(__half)));
-        e->allocs.push_back(p1);
-        MDK_CUDA(cudaMalloc(&p2, lo_t.size() * sizeof(__half)));
-        e->allocs.push_back(p2);
-        MDK_CUDA(cudaMemcpy(p1, hi.data(), hi.size() * sizeof(__half), cudaMemcpyHostToDevice));
-        MDK_CUDA(cudaMemcpy(p2, lo_t.data(), lo_t.size() * sizeof(__half), cudaMemcpyHostToDevice));
-        e->lstm[l].w_hi = static_cast<__half *>(p1);
-        e->lstm[l].w_lo = static_cast<uint8_t *>(p2);
-    }
 #undef RL_NEED
+    if ((rc = rl_prepare_lstm(e))) return rc;
     e->prepared = true;
     return MDK_OK;
 }
@@ -1514,44 +1289,34 @@ int rl_launch(mdk_rl_engine *e) {
     const float *layer_in = e->z;
     float *layer_out[2] = {e->h0, e->h1};
     float *d_gi = e->gi;
-    if (e->H == RL_H3) {
-        for (int l = 0; l < 2; ++l) {
-            const int in = l == 0 ? RL_H3 : 2 * RL_H3;
-            if (e->lstm_tc) {
-                MDK_CUDA(cudaFuncSetAttribute(rl_proj_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PJ_SMEM));
-                rl_proj_tc_kernel<<<dim3((unsigned)((BP + PJ_N - 1) / PJ_N), 2 * RL_G43 / PJ_M), 256, PJ_SMEM, s>>>(
-                    layer_in, e->lstm[l].w_ih_tc, e->lstm[l].bias, d_gi, BP, in, 2 * RL_G43);
-                rl_mark(e, 2 + 2 * l);
-                rl_lstm384_tc_kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N * L3_CL), 2), L3_THREADS, L3_SMEM, s>>>(
-                    d_gi, e->lstm[l].w_hi, e->lstm[l].w_lo, layer_out[l], B, P);
-            } else {
-                rl_gemm_kernel<<<dim3((unsigned)((BP + 127) / 128), 2 * RL_G43 / 128), 256, 0, s>>>(
-                    layer_in, e->lstm[l].w_ih, e->lstm[l].bias, d_gi, BP, in, 2 * RL_G43);
-                rl_mark(e, 2 + 2 * l);
-                rl_lstm384_kernel<<<dim3((unsigned)((B + R3_NB - 1) / R3_NB), 2), RL_H3, 0, s>>>(d_gi, e->lstm[l].w3t,
-                                                                                               layer_out[l], B, P);
-            }
-            rl_mark(e, 3 + 2 * l);
-            layer_in = layer_out[l];
+    const bool h384 = e->H == RL_H3;
+    const int G8 = 8 * e->H;                          // gate rows of both directions
+    const dim3 grid_fp32((unsigned)((B + LF_NB - 1) / LF_NB), 2);
+    for (int l = 0; l < 2; ++l) {
+        const RlLstmLayer &L = e->lstm[l];
+        const int in = l == 0 ? e->H : 2 * e->H;
+        if (h384 && e->lstm_tc) {
+            MDK_CUDA(cudaFuncSetAttribute(rl_proj_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PJ_SMEM));
+            rl_proj_tc_kernel<<<dim3((unsigned)((BP + PJ_N - 1) / PJ_N), G8 / PJ_M), 256, PJ_SMEM, s>>>(layer_in, L.w_ih_tc, L.bias,
+                                                                                                     d_gi, BP, in, G8);
+        } else {
+            MDK_CUDA(launch_gemm_fp32(layer_in, L.w_ih, L.bias, d_gi, BP, in, G8, s));
         }
-    } else {
-        MDK_CUDA(cudaFuncSetAttribute(rl_lstm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RL_LSTM_SMEM));
-        for (int l = 0; l < 2; ++l) {
-            const int in = l == 0 ? RL_H : 2 * RL_H;
-            rl_gemm_kernel<<<dim3((unsigned)((BP + 127) / 128), 2 * RL_G4 / 128), 256, 0, s>>>(layer_in, e->lstm[l].w_ih, e->lstm[l].bias,
-                                                                                           d_gi, BP, in, 2 * RL_G4);
-            rl_mark(e, 2 + 2 * l);
-            if (e->lstm_tc) {
-                MDK_CUDA(cudaFuncSetAttribute(rl_lstm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LT_SMEM));
-                rl_lstm_tc_kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N), 2), LT_THREADS, LT_SMEM, s>>>(d_gi, e->lstm[l].w_hi, e->lstm[l].w_lo,
-                                                                                                layer_out[l], B, P);
-            } else {
-                rl_lstm_kernel<<<dim3((unsigned)((B + RL_NB - 1) / RL_NB), 2), 256, RL_LSTM_SMEM, s>>>(d_gi, e->lstm[l].w3t, e->lstm[l].wo,
-                                                                                                    layer_out[l], B, P);
-            }
-            rl_mark(e, 3 + 2 * l);
-            layer_in = layer_out[l];
+        rl_mark(e, 2 + 2 * l);
+        if (h384 && e->lstm_tc) {
+            rl_lstm384_tc_kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N * L3_CL), 2), L3_THREADS, L3_SMEM, s>>>(
+                d_gi, L.w_hi, L.w_lo, layer_out[l], B, P);
+        } else if (e->lstm_tc) {
+            MDK_CUDA(cudaFuncSetAttribute(rl_lstm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LT_SMEM));
+            rl_lstm_tc_kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N), 2), LT_THREADS, LT_SMEM, s>>>(d_gi, L.w_hi, L.w_lo,
+                                                                                                  layer_out[l], B, P);
+        } else if (h384) {
+            rl_lstm_fp32<RL_H3><<<grid_fp32, RL_H3, 0, s>>>(d_gi, L.w_t, layer_out[l], B, P);
+        } else {
+            rl_lstm_fp32<RL_H><<<grid_fp32, RL_H, 0, s>>>(d_gi, L.w_t, layer_out[l], B, P);
         }
+        rl_mark(e, 3 + 2 * l);
+        layer_in = layer_out[l];
     }
     MDK_CUDA(cudaGetLastError());
     // the previous group's results must have left probs / labels before the head rewrites them
@@ -1649,10 +1414,6 @@ int mdk_rl_create(int device, int32_t lstm_size, int32_t cnn_size, int32_t use_d
     e->use_dwells = use_dwells ? 1 : 0;
     e->H = lstm_size;
     e->sm_count = sms;
-    {
-        const char *v = getenv("MDK_RL_CONV");      // "fp32": CUDA-core convolution (validation)
-        if (v && v[0] == 'f') { e->conv_tc = 0; e->lstm_tc = 0; }
-    }
     cudaError_t err = cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking);
     if (err == cudaSuccess) err = cudaStreamCreateWithFlags(&e->copy_in, cudaStreamNonBlocking);
     if (err == cudaSuccess) err = cudaStreamCreateWithFlags(&e->copy_out, cudaStreamNonBlocking);

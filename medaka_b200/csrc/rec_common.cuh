@@ -1,4 +1,5 @@
-// Device helpers of the recurrent tensor-core kernel (gru_wg.cu): approximate activations, tile geometry.
+// Device helpers of the recurrent tensor-core kernels (gru_wg.cu; the activations also readlevel.cu): approximate
+// activations, tile geometry.
 #pragma once
 #include "common.cuh"
 #include "ptx.cuh"
