@@ -5,7 +5,6 @@
 #include <cstdlib>
 #include <cstring>
 #include <new>
-#include <vector>
 
 #include "common.cuh"
 
@@ -119,7 +118,7 @@ static int ensure_io(mdk_engine *e, mdk_lane &ln, int64_t B, int64_t T) {
     if (P <= ln.cap_io && feats <= ln.cap_feats) return MDK_OK;
     MDK_CUDA(cudaStreamSynchronize(ln.ws->stream));
     MDK_CUDA(cudaStreamSynchronize(e->copy_in));
-    MDK_CUDA(cudaStreamSynchronize(e->copy_out));
+    MDK_CUDA(cudaStreamSynchronize(e->copy_out.stream));
     ln.cap_io = 0; ln.cap_feats = 0;
     dev_free(ln.d_feats); dev_free(ln.d_probs); dev_free(ln.d_logits); dev_free(ln.d_labels);
     int rc;
@@ -212,102 +211,61 @@ static int acquire_lane(mdk_engine *e, int64_t P, int *out) {
     return MDK_OK;
 }
 
-// Seal the open group: one forward over all of its windows, then the results back to each call's buffers (host or
-// device: cudaMemcpyDefault).
-static int launch_group(mdk_engine *e) {
-    if (e->open_lane < 0) return MDK_OK;
-    mdk_lane &ln = e->lane[e->open_lane];
-    e->open_lane = -1;
-    ln.open = false;
-    if (ln.items.empty()) return MDK_OK;
-    int rc;
-    cudaStream_t s = ln.ws->stream;
-    e->ev = e->evr[e->fwd_count % mdk_engine::EV_RING];
-    e->fwd_count++;
-    MDK_CUDA(cudaEventRecord(e->ev[0], s));
-    MDK_CUDA(cudaEventRecord(ln.ev_in, e->copy_in));      // every feature copy of the group was queued on copy_in
-    MDK_CUDA(cudaStreamWaitEvent(s, ln.ev_in, 0));
-    if ((rc = run_forward(e, *ln.ws, ln.d_feats, ln.gB, ln.gT, ln.d_probs, ln.want_logits ? ln.d_logits : nullptr,
-                          ln.want_labels ? ln.d_labels : nullptr)))
-        return rc;
-    MDK_CUDA(cudaEventRecord(ln.ev_done, s));
-    MDK_CUDA(cudaEventRecord(e->ev[7], s));
-    MDK_CUDA(cudaStreamWaitEvent(e->copy_out, ln.ev_done, 0));
-    int64_t w0 = 0;
-    for (const mdk_lane::Item &it : ln.items) {
-        const size_t P = (size_t)it.B * ln.gT, off = (size_t)w0 * ln.gT;
-        MDK_CUDA(cudaMemcpyAsync(it.probs, ln.d_probs + off * NCLS, P * NCLS * sizeof(float), cudaMemcpyDefault, e->copy_out));
-        if (it.logits)
-            MDK_CUDA(cudaMemcpyAsync(it.logits, ln.d_logits + off * NCLS, P * NCLS * sizeof(float), cudaMemcpyDefault, e->copy_out));
-        if (it.labels) MDK_CUDA(cudaMemcpyAsync(it.labels, ln.d_labels + off, P, cudaMemcpyDefault, e->copy_out));
-        w0 += it.B;
+// The engine's side of the packing core (packing.h) for one call of B windows of T columns, features at feats (host or
+// device memory).  Launching alone (flush, sync, waits) needs no call.
+struct GruCall {
+    mdk_engine *e;
+    const float *feats = nullptr;
+    int64_t B = 0, T = 0;
+
+    int open(int64_t windows) {
+        // size class of the CALL: the tail piece of a split call stays with the big lanes
+        const int rc = acquire_lane(e, B * T, &e->open_lane);
+        // the staging grows to this call (at most one group of it); a reserved lane is already larger and keeps
+        // collecting further calls up to its size
+        return rc ? rc : ensure_io(e, e->lane[e->open_lane], windows, T);
     }
-    MDK_CUDA(cudaEventRecord(ln.ev_out, e->copy_out));
-    ln.busy = true;
-    return MDK_OK;
-}
+    int64_t capacity(int64_t len) {
+        const mdk_lane &ln = e->lane[e->open_lane];
+        return std::min(ln.cap_io / len, ln.cap_feats / (len * e->desc.num_features));
+    }
+    // copy-in stream: features into the staging (asynchronous for device and page-locked host memory), behind the
+    // group's earlier pieces
+    int stage(int64_t first, int64_t n, int64_t at) {
+        const size_t w = (size_t)T * e->desc.num_features;
+        MDK_CUDA(cudaMemcpyAsync(e->lane[e->open_lane].d_feats + at * w, feats + first * w, n * w * sizeof(float),
+                                 cudaMemcpyDefault, e->copy_in));
+        return MDK_OK;
+    }
+    // the sealed group on its lane: one forward over all of its windows, then the results back to each call's buffers
+    int launch() {
+        mdk_lane &ln = e->lane[e->open_lane];
+        const Packing &pk = e->pk;
+        bool logits = false, labels = false;      // whether any call wants them
+        for (const Packing::Piece &p : pk.pieces) { logits = logits || p.logits; labels = labels || p.labels; }
+        int rc;
+        cudaStream_t s = ln.ws->stream;
+        e->ev = e->evr[e->fwd_count % mdk_engine::EV_RING];
+        e->fwd_count++;
+        MDK_CUDA(cudaEventRecord(e->ev[0], s));
+        MDK_CUDA(cudaEventRecord(ln.ev_in, e->copy_in));      // every feature copy of the group was queued on copy_in
+        MDK_CUDA(cudaStreamWaitEvent(s, ln.ev_in, 0));
+        if ((rc = run_forward(e, *ln.ws, ln.d_feats, pk.windows, pk.len, ln.d_probs, logits ? ln.d_logits : nullptr,
+                              labels ? ln.d_labels : nullptr)))
+            return rc;
+        MDK_CUDA(cudaEventRecord(e->ev[7], s));
+        if ((rc = copy_back(e->copy_out, pk, s, ln.d_probs, ln.d_logits, ln.d_labels))) return rc;
+        MDK_CUDA(cudaEventRecord(ln.ev_out, e->copy_out.stream));
+        ln.busy = true;
+        return MDK_OK;
+    }
+};
+
+static int launch_group(mdk_engine *e) { return e->pk.launch(GruCall{e}); }
 
 // Most windows one group collects: one wave unless mdk_engine_set_group_windows says otherwise.
 static int64_t group_limit(mdk_engine *e) {
     return e->group_windows > 0 ? e->group_windows : mdk_engine_preferred_windows(e);
-}
-
-// One call's windows into the open group, window by window: a call that does not fit what is left of the group is split
-// (windows are independent, medaka/prediction.py:40-52 treats every row of a batch separately), so every group of a long
-// run holds gmax windows however the caller sized its calls.  Features are copied into the group's staging as they
-// arrive; results go back to each piece's own range of the call's buffers when the group completes.  Host and device
-// buffers take the same path (cudaMemcpyDefault).  ticket (may be NULL) follows the call's last piece.
-static int enqueue(mdk_engine *e, const float *feats, int64_t B, int64_t T, float *probs, float *logits,
-                   uint8_t *labels, int64_t gmax, int64_t *ticket) {
-    int rc;
-    const int64_t F = e->desc.num_features;
-    if (e->open_lane >= 0 && e->lane[e->open_lane].gT != T && (rc = launch_group(e))) return rc;
-    int64_t done = 0;
-    while (done < B) {
-        if (e->open_lane < 0) {
-            int li;
-            if ((rc = acquire_lane(e, B * T, &li))) return rc;      // size class of the CALL: the tail piece of a split
-                                                                    // call stays with the big lanes
-            mdk_lane &ln = e->lane[li];
-            // the staging grows to this call (at most one group of it); a reserved lane is already larger and keeps
-            // collecting further calls up to its size
-            if ((rc = ensure_io(e, ln, std::min<int64_t>(B - done, gmax), T))) return rc;
-            ln.items.clear();
-            ln.gB = 0; ln.gT = T;
-            ln.want_logits = false; ln.want_labels = false;
-            ln.open = true;
-            ln.group++;
-            e->open_lane = li;
-        }
-        mdk_lane &ln = e->lane[e->open_lane];
-        // windows the open group can still take: gmax, and what the lane's staging reaches
-        int64_t room = std::min(gmax, std::min(ln.cap_io / T, ln.cap_feats / (T * F))) - ln.gB;
-        if (ln.gB == 0 && room < 1) room = 1;        // (ensure_io above sized the staging for at least one window)
-        if (room < 1) {
-            if ((rc = launch_group(e))) return rc;
-            continue;
-        }
-        const int64_t n = std::min(room, B - done);
-        // copy-in stream: features into the staging (asynchronous for device and page-locked host memory), behind the
-        // group's earlier pieces
-        MDK_CUDA(cudaMemcpyAsync(ln.d_feats + (size_t)ln.gB * T * F, feats + (size_t)done * T * F,
-                                 (size_t)n * T * F * sizeof(float), cudaMemcpyDefault, e->copy_in));
-        ln.items.push_back(mdk_lane::Item{feats + (size_t)done * T * F, probs + (size_t)done * T * NCLS,
-                                          logits ? logits + (size_t)done * T * NCLS : nullptr,
-                                          labels ? labels + (size_t)done * T : nullptr, n});
-        ln.gB += n;
-        ln.want_logits = ln.want_logits || logits != nullptr;
-        ln.want_labels = ln.want_labels || labels != nullptr;
-        done += n;
-        if (done == B && ticket) {
-            const int64_t tk = e->submit_count++;
-            e->ticket_lane[tk % mdk_engine::TICKET_RING] = (int16_t)e->open_lane;
-            e->ticket_group[tk % mdk_engine::TICKET_RING] = ln.group;
-            *ticket = tk;
-        }
-        if (n == room && (rc = launch_group(e))) return rc;      // full: launch right away
-    }
-    return MDK_OK;
 }
 
 static float ev_ms(cudaEvent_t a, cudaEvent_t b) {
@@ -422,15 +380,15 @@ int mdk_engine_create(int device, const mdk_model_desc *desc, mdk_engine **out) 
         ln.ws = i < mdk_engine::BIG_LANES ? &e->ws[i % mdk_engine::BIG_WS]
                                           : &e->ws[mdk_engine::BIG_WS + (i - mdk_engine::BIG_LANES)];
         cudaEventCreateWithFlags(&ln.ev_in, cudaEventDisableTiming);
-        cudaEventCreateWithFlags(&ln.ev_done, cudaEventDisableTiming);
         cudaEventCreateWithFlags(&ln.ev_out, cudaEventDisableTiming);
     }
     e->stream = e->ws[0].stream;
     for (auto &set : e->evr) for (auto &ev : set) cudaEventCreate(&ev);
     cudaStreamCreateWithFlags(&e->copy_in, cudaStreamNonBlocking);
-    cudaStreamCreateWithFlags(&e->copy_out, cudaStreamNonBlocking);
     for (auto &ev : e->ev_timer) cudaEventCreate(&ev);
     cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming);
+    cudaError_t err = create_copy_out(e->copy_out);
+    if (err != cudaSuccess) { mdk_engine_destroy(e); return cuda_fail(err, "create_copy_out", __FILE__, __LINE__); }
     *out = e;
     return MDK_OK;
 }
@@ -439,7 +397,7 @@ int mdk_engine_destroy(mdk_engine *e) {
     if (!e) return MDK_OK;
     cudaSetDevice(e->device);
     for (auto &ws : e->ws) if (ws.stream) cudaStreamSynchronize(ws.stream);
-    if (e->copy_out) cudaStreamSynchronize(e->copy_out);
+    destroy_copy_out(e->copy_out);
     for (int l = 0; l < 2; ++l) {
         LayerWeights &lw = e->layer[l];
         for (int d = 0; d < NDIR; ++d) { dev_free(lw.w_ih[d]); dev_free(lw.w_hh[d]); dev_free(lw.b_ih[d]); dev_free(lw.b_hh[d]); }
@@ -456,11 +414,9 @@ int mdk_engine_destroy(mdk_engine *e) {
     for (auto &ln : e->lane) {
         dev_free(ln.d_feats); dev_free(ln.d_probs); dev_free(ln.d_logits); dev_free(ln.d_labels);
         if (ln.ev_in) cudaEventDestroy(ln.ev_in);
-        if (ln.ev_done) cudaEventDestroy(ln.ev_done);
         if (ln.ev_out) cudaEventDestroy(ln.ev_out);
     }
     if (e->copy_in) cudaStreamDestroy(e->copy_in);
-    if (e->copy_out) cudaStreamDestroy(e->copy_out);
     for (auto &set : e->evr) for (auto &ev : set) if (ev) cudaEventDestroy(ev);
     for (auto &ev : e->ev_timer) if (ev) cudaEventDestroy(ev);
     if (e->ev_join) cudaEventDestroy(e->ev_join);
@@ -565,19 +521,16 @@ int mdk_engine_forward_dev(mdk_engine *e, const float *feats_dev, int64_t B, int
         if ((rc = launch_group(e))) return rc;
         gmax = B;
     }
-    return enqueue(e, feats_dev, B, T, probs_dev, logits_dev, labels_dev, gmax, nullptr);
+    return e->pk.enqueue(GruCall{e, feats_dev, B, T}, B, T, probs_dev, logits_dev, labels_dev, gmax, nullptr);
 }
 
-// Submitted batches are packed into groups window by window (enqueue), so every group of a long run is exactly one wave
-// however the caller sized its batches.  The ticket follows the batch's last piece; groups complete in submission order
-// per lane and the pieces of one batch sit in consecutive groups.
 int mdk_engine_submit(mdk_engine *e, const float *feats_host, int64_t B, int64_t T, float *probs_host,
                       float *logits_host, uint8_t *labels_host, int64_t *ticket) {
     int rc;
     if ((rc = check_shapes(e, feats_host, B, T, probs_host))) return rc;
     MDK_REQUIRE(ticket, MDK_ERR_ARG, "submit: ticket is NULL");
     MDK_CUDA(cudaSetDevice(e->device));
-    return enqueue(e, feats_host, B, T, probs_host, logits_host, labels_host, group_limit(e), ticket);
+    return e->pk.enqueue(GruCall{e, feats_host, B, T}, B, T, probs_host, logits_host, labels_host, group_limit(e), ticket);
 }
 
 int mdk_engine_flush(mdk_engine *e) {
@@ -588,22 +541,9 @@ int mdk_engine_flush(mdk_engine *e) {
 
 int mdk_engine_wait(mdk_engine *e, int64_t ticket) {
     MDK_REQUIRE(e, MDK_ERR_ARG, "engine is NULL");
-    MDK_REQUIRE(ticket >= 0 && ticket < e->submit_count, MDK_ERR_ARG, "wait: unknown ticket");
-    if (ticket < e->submit_count - mdk_engine::TICKET_RING) return MDK_OK;   // its lane has been reused many times since
+    MDK_REQUIRE(ticket >= 0 && ticket < e->pk.tickets, MDK_ERR_ARG, "wait: unknown ticket");
     MDK_CUDA(cudaSetDevice(e->device));
-    const int li = e->ticket_lane[ticket % mdk_engine::TICKET_RING];
-    const int64_t grp = e->ticket_group[ticket % mdk_engine::TICKET_RING];
-    mdk_lane &ln = e->lane[li];
-    if (ln.group != grp) return MDK_OK;        // a later group runs on the lane: this one was waited for when it was reused
-    if (ln.open) {
-        int rc = launch_group(e);              // still collecting: the caller wants the result now
-        if (rc) return rc;
-    }
-    if (ln.busy) {
-        MDK_CUDA(cudaEventSynchronize(ln.ev_out));
-        ln.busy = false;
-    }
-    return MDK_OK;
+    return wait_ticket(e->copy_out, e->pk, GruCall{e}, ticket);
 }
 
 int mdk_engine_forward(mdk_engine *e, const float *feats_host, int64_t B, int64_t T, float *probs_host,
@@ -621,7 +561,7 @@ int mdk_engine_sync(mdk_engine *e) {
     if (rc) return rc;
     MDK_CUDA(cudaStreamSynchronize(e->copy_in));
     for (auto &ws : e->ws) MDK_CUDA(cudaStreamSynchronize(ws.stream));
-    MDK_CUDA(cudaStreamSynchronize(e->copy_out));
+    MDK_CUDA(cudaStreamSynchronize(e->copy_out.stream));
     for (auto &ln : e->lane) ln.busy = false;
     return MDK_OK;
 }
@@ -704,7 +644,7 @@ int mdk_engine_timer_stop(mdk_engine *e, float *elapsed_ms) {
         MDK_CUDA(cudaEventRecord(e->ev_join, e->ws[i].stream));
         MDK_CUDA(cudaStreamWaitEvent(e->stream, e->ev_join, 0));
     }
-    MDK_CUDA(cudaEventRecord(e->ev_join, e->copy_out));     // the end event must follow every copy-out still in flight
+    MDK_CUDA(cudaEventRecord(e->ev_join, e->copy_out.stream));     // the end event must follow every copy-out still in flight
     MDK_CUDA(cudaStreamWaitEvent(e->stream, e->ev_join, 0));
     MDK_CUDA(cudaEventRecord(e->ev_timer[1], e->stream));
     MDK_CUDA(cudaEventSynchronize(e->ev_timer[1]));

@@ -6,9 +6,9 @@
 #include <cstdint>
 #include <cstdio>
 #include <string>
-#include <vector>
 
 #include "../../include/medaka_b200.h"
+#include "packing.h"
 
 namespace mdk {
 
@@ -93,15 +93,70 @@ struct LayerWeights {
                                     // gemm_tc shared-memory A operand
 };
 
+// The copy-out side of packing.h in both engines: one copy-out stream per engine, so groups' results reach their calls'
+// buffers in serial order; ev[g % RING] marks those of group g until group g + RING reuses it.  RING is above the groups
+// a caller keeps in flight (run_prediction's look-ahead keeps at most 64 calls; in the remainder phase 14 calls of
+// distinct lengths, each sealing a group of its own), so a wait is on its own group's event and the small lanes' groups
+// keep running side by side.
+struct CopyOut {
+    static constexpr int RING = 128;
+    cudaStream_t stream = nullptr;
+    cudaEvent_t done = nullptr;    // compute stream -> copy-out stream
+    cudaEvent_t ev[RING] = {};
+};
+inline cudaError_t create_copy_out(CopyOut &co) {
+    cudaError_t err = cudaStreamCreateWithFlags(&co.stream, cudaStreamNonBlocking);
+    if (err == cudaSuccess) err = cudaEventCreateWithFlags(&co.done, cudaEventDisableTiming);
+    for (int i = 0; i < CopyOut::RING && err == cudaSuccess; ++i)
+        err = cudaEventCreateWithFlags(&co.ev[i], cudaEventDisableTiming);
+    return err;
+}
+
+inline void destroy_copy_out(CopyOut &co) {
+    if (co.stream) { cudaStreamSynchronize(co.stream); cudaStreamDestroy(co.stream); }
+    if (co.done) cudaEventDestroy(co.done);
+    for (cudaEvent_t ev : co.ev) if (ev) cudaEventDestroy(ev);
+}
+
+// Once the work queued on `compute` is done, per piece of the group being launched: the probabilities, and the logits
+// and labels where the piece has them, from the group's buffers to the call's (host or device); then ev[pk.serial].
+inline int copy_back(CopyOut &co, const Packing &pk, cudaStream_t compute, const float *probs, const float *logits,
+                     const uint8_t *labels) {
+    MDK_CUDA(cudaEventRecord(co.done, compute));
+    MDK_CUDA(cudaStreamWaitEvent(co.stream, co.done, 0));
+    int64_t w0 = 0;
+    for (const Packing::Piece &p : pk.pieces) {
+        const size_t n = (size_t)p.n * pk.len, dst = (size_t)p.first * pk.len, src = (size_t)w0 * pk.len;
+        const size_t bytes = n * NCLS * sizeof(float);
+        MDK_CUDA(cudaMemcpyAsync(p.probs + dst * NCLS, probs + src * NCLS, bytes, cudaMemcpyDefault, co.stream));
+        if (p.logits) MDK_CUDA(cudaMemcpyAsync(p.logits + dst * NCLS, logits + src * NCLS, bytes, cudaMemcpyDefault, co.stream));
+        if (p.labels) MDK_CUDA(cudaMemcpyAsync(p.labels + dst, labels + src, n, cudaMemcpyDefault, co.stream));
+        w0 += p.n;
+    }
+    MDK_CUDA(cudaEventRecord(co.ev[pk.serial % CopyOut::RING], co.stream));
+    return MDK_OK;
+}
+
+// Wait for ticket's group g (Packing::settle) on ev[g % RING]: it was last recorded for g or, once reused, for a later
+// group, whose copies leave the copy-out stream after g's.
+template <class Eng>
+int wait_ticket(CopyOut &co, Packing &pk, Eng &&eng, int64_t ticket) {
+    int64_t g = 0;
+    const int rc = pk.settle(eng, ticket, &g);
+    if (rc) return rc;
+    MDK_CUDA(cudaEventSynchronize(co.ev[g % CopyOut::RING]));
+    return MDK_OK;
+}
+
 }  // namespace mdk
 
-// The engine runs GROUPS of windows.  A workspace (mdk_ws) is a compute stream plus the intermediates of one forward; a
-// lane (mdk_lane) is the device-side staging of one group of calls - submitted host batches and device-resident
-// forward_dev calls alike (features in, probabilities / labels out) - and is bound to one workspace.  There are more
-// big lanes than big workspaces: while one group computes, others are receiving their features or draining their
-// results, so the copies never hold the workspace (43 GB for a 1056 x 10 000 group, 4 KiB per position) idle.  One big workspace: a one-wave group (one 16-window tile per CTA and
-// direction) already fills every SM, and a second 43 GB workspace would not fit beside it in 80 GB.  Small forwards (the
-// B = 1 remainder regions of medaka/prediction.py:196-209) spread over the small lanes, each with a workspace of its own.
+// The engine runs GROUPS of windows (packing.h).  A workspace (mdk_ws) is a compute stream plus the intermediates of one
+// forward; a lane (mdk_lane) is the device-side staging of one group of calls - submitted host batches and forward_dev
+// calls alike (features in, probabilities / labels out) - bound to one workspace.  There are more big lanes than big
+// workspaces: while one group computes, others receive their features or drain their results, so the copies never hold
+// the workspace (43 GB for a 1056 x 10 000 group, 4 KiB per position) idle.  One big workspace: a one-wave group already
+// fills every SM, and a second 43 GB workspace would not fit beside it in 80 GB.  Small forwards (the B = 1 remainder
+// regions of medaka/prediction.py:196-209) spread over the small lanes, each with a workspace of its own.
 struct mdk_ws {
     cudaStream_t stream = nullptr;
     int64_t cap_pos = 0;       // capacity in positions (rounded up to XT_ROWS)
@@ -123,19 +178,8 @@ struct mdk_lane {
     int64_t cap_feats = 0;     // floats
     float *d_feats = nullptr, *d_probs = nullptr, *d_logits = nullptr;
     uint8_t *d_labels = nullptr;
-    cudaEvent_t ev_in = nullptr, ev_done = nullptr, ev_out = nullptr;
-    // the group being collected (open) or in flight (busy)
-    struct Item {
-        const float *feats;
-        float *probs, *logits;
-        uint8_t *labels;
-        int64_t B;
-    };
-    std::vector<Item> items;
-    int64_t gB = 0, gT = 0;
-    bool want_logits = false, want_labels = false;
-    bool open = false, busy = false;
-    int64_t group = -1;        // serial number of the lane's current (open / in-flight / last finished) group
+    cudaEvent_t ev_in = nullptr, ev_out = nullptr;
+    bool busy = false;         // ev_out marks a group the lane has not been reclaimed from
 };
 
 struct mdk_engine {
@@ -150,7 +194,8 @@ struct mdk_engine {
     mdk_ws ws[N_WS];              // [0, BIG_WS): big groups; then one per small lane
     mdk_lane lane[N_LANES];       // big lane j computes on ws[j % BIG_WS], small lane i on ws[BIG_WS + i]
     int next_big = 0, next_small = 0;
-    int open_lane = -1;           // lane whose group is still collecting batches (at most one), -1 = none
+    mdk::Packing pk;
+    int open_lane = -1;           // lane of the open (or last launched) group
     int last_ws = 0;              // workspace of the most recent forward
     int64_t group_windows = 0;    // most windows coalesced into one group (0 = one wave, mdk_engine_preferred_windows)
     cudaStream_t stream = nullptr;       // == ws[0].stream: weight preparation, timers
@@ -165,12 +210,8 @@ struct mdk_engine {
     bool lin_loaded = false;
     bool keep_act = false;        // debugging: keep h1 (layer-1 output) in HBM, i.e. run the unfused head
     bool prepared = false;
-    cudaStream_t copy_in = nullptr, copy_out = nullptr;
-    // tickets: ticket -> (lane, group) for the last TICKET_RING submits; older ones have completed (their lane was reused)
-    static constexpr int TICKET_RING = 4096;
-    int16_t ticket_lane[TICKET_RING] = {};
-    int64_t ticket_group[TICKET_RING] = {};
-    int64_t submit_count = 0;
+    cudaStream_t copy_in = nullptr;
+    mdk::CopyOut copy_out;
     mdk_timings last{};
     int64_t launches = 0;
 };

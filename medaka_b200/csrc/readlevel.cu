@@ -907,13 +907,10 @@ struct RlLstmLayer {
 
 using namespace mdk;
 
-// Submitted calls are packed into GROUPS (DESIGN §4).  Each call's convolution runs when it is submitted, in slices of
-// windows bounded by RL_CONV_BUDGET, and writes z (the pooled pre_pool_expansion_layer output) for its windows into the
-// open group's z at their window offset; the projections, both recurrences and the head run once per group over all of
-// its windows.  One set of group buffers, one compute stream: the convolutions of the next group queue behind the
-// group in flight; only the feature copies (copy_in) and the result copies (copy_out) run beside the compute.
-// (The ticket bookkeeping is the counts engine's idea without its lanes: one group buffer set here, so a ticket maps to
-// a group serial number alone.)
+// Calls are packed into GROUPS (packing.h, DESIGN §4).  Staging a piece is its convolution, in slices of windows bounded
+// by RL_CONV_BUDGET, into the open group's z (pooled pre_pool_expansion_layer output) at the piece's window offset; the
+// projections, recurrences and head run once per group.  One set of group buffers, one compute stream: the next group's
+// convolutions queue behind the group in flight; only copy_in and copy_out run beside the compute.
 constexpr size_t RL_CONV_BUDGET = (size_t)2 << 30;     // feature staging + convolution scratch of one slice, bytes
 constexpr size_t RL_GROUP_BUDGET = (size_t)24 << 30;   // z, gi, h0, h1, probs, labels of one group, bytes
 constexpr int64_t RL_PREFERRED_P = 10000;              // window length mdk_rl_preferred_windows sizes for (chunk_len)
@@ -940,7 +937,8 @@ struct mdk_rl_engine {
     float *lin_w = nullptr, *lin_b = nullptr;
     std::vector<void *> allocs;
     cudaStream_t stream = nullptr;                   // compute: convolutions, then each group's LSTM and head
-    cudaStream_t copy_in = nullptr, copy_out = nullptr;
+    cudaStream_t copy_in = nullptr;
+    CopyOut copy_out;
     // convolution of one slice: features in two staging slots (the copy of the next slice runs under this one's
     // convolution), then mask | y1 (fp32 path only) | partial sums on the compute stream
     int8_t *xbuf[2] = {nullptr, nullptr};
@@ -953,23 +951,7 @@ struct mdk_rl_engine {
     int64_t cap_pos = 0;
     float *z = nullptr, *gi = nullptr, *h0 = nullptr, *h1 = nullptr, *probs = nullptr;
     uint8_t *labels = nullptr;
-    // the open group: its calls' output buffers (host), its windows so far and its window length
-    struct Item {
-        float *probs;
-        uint8_t *labels;
-        int64_t B;
-    };
-    std::vector<Item> items;
-    bool open = false;
-    int64_t gB = 0, gP = 0;
-    int64_t group = -1;                              // serial number of the open or last launched group
-    int64_t launched = -1;                           // serial number of the last launched group
-    static constexpr int OUT_RING = 8;
-    cudaEvent_t ev_done = nullptr;                   // compute -> copy_out
-    cudaEvent_t ev_out[OUT_RING] = {};               // results of group g in its callers' buffers: ev_out[g % OUT_RING]
-    static constexpr int TICKET_RING = 4096;
-    int64_t ticket_group[TICKET_RING] = {};
-    int64_t submit_count = 0;
+    Packing pk;
     int64_t last_B = 0, last_P = 0;                  // the last completed mdk_rl_forward (mdk_rl_debug_read), 0 = none
 };
 
@@ -1196,7 +1178,7 @@ int rl_grow(T **p, size_t *cap, size_t need) {
 int rl_ensure_group(mdk_rl_engine *e, int64_t pos) {
     if (pos <= e->cap_pos) return MDK_OK;
     MDK_CUDA(cudaStreamSynchronize(e->stream));
-    MDK_CUDA(cudaStreamSynchronize(e->copy_out));
+    MDK_CUDA(cudaStreamSynchronize(e->copy_out.stream));
     e->last_B = e->last_P = 0;                       // the last mdk_rl_forward's stages go with the old buffers
     float **fb[5] = {&e->z, &e->gi, &e->h0, &e->h1, &e->probs};
     for (float **p : fb) { if (*p) cudaFree(*p); *p = nullptr; }
@@ -1212,7 +1194,7 @@ int rl_ensure_group(mdk_rl_engine *e, int64_t pos) {
 }
 
 void rl_mark(mdk_rl_engine *e, int i) {
-    if (e->timing) cudaEventRecord(e->ev[e->group & 1][i], e->stream);
+    if (e->timing) cudaEventRecord(e->ev[e->pk.serial & 1][i], e->stream);
 }
 
 // The convolution of n windows of one call (host features x [n][P][D][F]) into z of the open group at window woff:
@@ -1276,14 +1258,11 @@ int rl_conv(mdk_rl_engine *e, const int8_t *x, int64_t n, int64_t P, int64_t D, 
     return MDK_OK;
 }
 
-// Seal the open group: the projections, both recurrences and the head over all of its windows on the compute stream,
+// Run the sealed group: the projections, both recurrences and the head over all of its windows on the compute stream,
 // then each call's probabilities (and labels) from the group buffers to its own buffers on copy_out.
-int rl_launch(mdk_rl_engine *e) {
-    if (!e->open) return MDK_OK;
-    e->open = false;
-    if (e->items.empty()) return MDK_OK;
+int rl_run_group(mdk_rl_engine *e) {
     e->last_B = e->last_P = 0;                       // the group buffers are about to be overwritten
-    const int64_t B = e->gB, P = e->gP, BP = B * P;
+    const int64_t B = e->pk.windows, P = e->pk.len, BP = B * P;
     cudaStream_t s = e->stream;
     rl_mark(e, 1);
     const float *layer_in = e->z;
@@ -1320,7 +1299,7 @@ int rl_launch(mdk_rl_engine *e) {
     }
     MDK_CUDA(cudaGetLastError());
     // the previous group's results must have left probs / labels before the head rewrites them
-    if (e->launched >= 0) MDK_CUDA(cudaStreamWaitEvent(s, e->ev_out[e->launched % mdk_rl_engine::OUT_RING], 0));
+    if (e->pk.launched >= 0) MDK_CUDA(cudaStreamWaitEvent(s, e->copy_out.ev[e->pk.launched % CopyOut::RING], 0));
     if (e->H == RL_H3) {
         int64_t blocks = (BP + 7) / 8;
         if (blocks > 132 * 8) blocks = 132 * 8;
@@ -1330,58 +1309,28 @@ int rl_launch(mdk_rl_engine *e) {
         MDK_CUDA(launch_head(e->h1, e->lin_w, e->lin_b, B, P, 0, e->probs, nullptr, e->labels, s));
     }
     rl_mark(e, 6);
-    MDK_CUDA(cudaEventRecord(e->ev_done, s));
-    MDK_CUDA(cudaStreamWaitEvent(e->copy_out, e->ev_done, 0));
-    int64_t w0 = 0;
-    for (const mdk_rl_engine::Item &it : e->items) {
-        const size_t n = (size_t)it.B * P, off = (size_t)w0 * P;
-        MDK_CUDA(cudaMemcpyAsync(it.probs, e->probs + off * NCLS, n * NCLS * sizeof(float), cudaMemcpyDeviceToHost, e->copy_out));
-        if (it.labels) MDK_CUDA(cudaMemcpyAsync(it.labels, e->labels + off, n, cudaMemcpyDeviceToHost, e->copy_out));
-        w0 += it.B;
-    }
-    MDK_CUDA(cudaEventRecord(e->ev_out[e->group % mdk_rl_engine::OUT_RING], e->copy_out));
-    e->launched = e->group;
-    return MDK_OK;
+    return copy_back(e->copy_out, e->pk, s, e->probs, nullptr, e->labels);
 }
 
-// One call into the open group, window by window: a new P seals the open group, a call that does not fit what is left
-// of the group is split (windows are independent), a full group is launched at once.  The group buffers grow, when a
-// group opens, to this call's windows (at most gmax): without mdk_rl_reserve a group collects calls only as far as the
-// buffers reach.  ticket (may be NULL) follows the call's last piece.
-int rl_enqueue(mdk_rl_engine *e, const int8_t *x, int64_t B, int64_t P, int64_t D, int64_t F, float *probs,
-               uint8_t *labels, int64_t gmax, int64_t *ticket) {
-    int rc;
-    if (e->open && e->gP != P && (rc = rl_launch(e))) return rc;
-    int64_t done = 0;
-    while (done < B) {
-        if (!e->open) {
-            if ((rc = rl_ensure_group(e, std::min(B - done, gmax) * P))) return rc;
-            e->items.clear();
-            e->gB = 0;
-            e->gP = P;
-            e->open = true;
-            e->group++;
-            e->last_B = e->last_P = 0;               // this group's convolutions overwrite z of the last mdk_rl_forward
-        }
-        const int64_t room = std::min(gmax, e->cap_pos / P) - e->gB;
-        if (room < 1) {
-            if ((rc = rl_launch(e))) return rc;
-            continue;
-        }
-        const int64_t n = std::min(room, B - done);
-        if ((rc = rl_conv(e, x + (size_t)done * P * D * F, n, P, D, F, e->gB))) return rc;
-        e->items.push_back(mdk_rl_engine::Item{probs + (size_t)done * P * NCLS, labels ? labels + (size_t)done * P : nullptr, n});
-        e->gB += n;
-        done += n;
-        if (done == B && ticket) {
-            const int64_t tk = e->submit_count++;
-            e->ticket_group[tk % mdk_rl_engine::TICKET_RING] = e->group;
-            *ticket = tk;
-        }
-        if (n == room && (rc = rl_launch(e))) return rc;
+// The engine's side of the packing core (packing.h) for one call: x_host [B][P][D][F].  Launching alone (flush, waits)
+// needs no call.
+struct RlCall {
+    mdk_rl_engine *e;
+    const int8_t *x = nullptr;
+    int64_t P = 0, D = 0, F = 0;
+
+    // the group buffers grow, when a group opens, to this call's windows (at most one group of them): without
+    // mdk_rl_reserve a group collects calls only as far as the buffers reach
+    int open(int64_t windows) {
+        e->last_B = e->last_P = 0;                   // this group's convolutions overwrite z of the last mdk_rl_forward
+        return rl_ensure_group(e, windows * P);
     }
-    return MDK_OK;
-}
+    int64_t capacity(int64_t len) { return e->cap_pos / len; }
+    int stage(int64_t first, int64_t n, int64_t at) { return rl_conv(e, x + (size_t)first * P * D * F, n, P, D, F, at); }
+    int launch() { return rl_run_group(e); }
+};
+
+int rl_launch(mdk_rl_engine *e) { return e->pk.launch(RlCall{e}); }
 
 int rl_check(mdk_rl_engine *e, const int8_t *x, int64_t B, int64_t P, int64_t D, int64_t F, const float *probs,
              const char *who) {
@@ -1416,14 +1365,11 @@ int mdk_rl_create(int device, int32_t lstm_size, int32_t cnn_size, int32_t use_d
     e->sm_count = sms;
     cudaError_t err = cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking);
     if (err == cudaSuccess) err = cudaStreamCreateWithFlags(&e->copy_in, cudaStreamNonBlocking);
-    if (err == cudaSuccess) err = cudaStreamCreateWithFlags(&e->copy_out, cudaStreamNonBlocking);
+    if (err == cudaSuccess) err = create_copy_out(e->copy_out);
     for (int i = 0; i < 2 && err == cudaSuccess; ++i) {
         err = cudaEventCreateWithFlags(&e->ev_xin[i], cudaEventDisableTiming);
         if (err == cudaSuccess) err = cudaEventCreateWithFlags(&e->ev_xfree[i], cudaEventDisableTiming);
     }
-    if (err == cudaSuccess) err = cudaEventCreateWithFlags(&e->ev_done, cudaEventDisableTiming);
-    for (int i = 0; i < mdk_rl_engine::OUT_RING && err == cudaSuccess; ++i)
-        err = cudaEventCreateWithFlags(&e->ev_out[i], cudaEventDisableTiming);
     if (err != cudaSuccess) { mdk_rl_destroy(e); return cuda_fail(err, "rl_create: streams / events", __FILE__, __LINE__); }
     *out = e;
     return MDK_OK;
@@ -1432,14 +1378,13 @@ int mdk_rl_create(int device, int32_t lstm_size, int32_t cnn_size, int32_t use_d
 int mdk_rl_destroy(mdk_rl_engine *e) {
     if (!e) return MDK_OK;
     cudaSetDevice(e->device);
-    for (cudaStream_t s : {e->copy_in, e->stream, e->copy_out})
+    for (cudaStream_t s : {e->copy_in, e->stream})
         if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); }
+    destroy_copy_out(e->copy_out);
     for (auto &set : e->ev)
         for (cudaEvent_t ev : set)
             if (ev) cudaEventDestroy(ev);
-    for (cudaEvent_t ev : {e->ev_xin[0], e->ev_xin[1], e->ev_xfree[0], e->ev_xfree[1], e->ev_done})
-        if (ev) cudaEventDestroy(ev);
-    for (cudaEvent_t ev : e->ev_out)
+    for (cudaEvent_t ev : {e->ev_xin[0], e->ev_xin[1], e->ev_xfree[0], e->ev_xfree[1]})
         if (ev) cudaEventDestroy(ev);
     for (void *p : e->allocs) cudaFree(p);
     for (void *p : {(void *)e->xbuf[0], (void *)e->xbuf[1], (void *)e->conv, (void *)e->z, (void *)e->gi, (void *)e->h0,
@@ -1478,9 +1423,9 @@ int mdk_rl_set_timing(mdk_rl_engine *e, int on) {
 int mdk_rl_stage_ms(mdk_rl_engine *e, float *ms) {
     MDK_REQUIRE(e && ms, MDK_ERR_ARG, "rl_stage_ms: NULL argument");
     for (int i = 0; i < 6; ++i) ms[i] = 0.f;
-    if (e->launched < 0 || !e->ev[0][0]) return MDK_OK;
+    if (e->pk.launched < 0 || !e->ev[0][0]) return MDK_OK;
     MDK_CUDA(cudaSetDevice(e->device));
-    cudaEvent_t *ev = e->ev[e->launched & 1];
+    cudaEvent_t *ev = e->ev[e->pk.launched & 1];
     MDK_CUDA(cudaEventSynchronize(ev[6]));
     for (int i = 0; i < 6; ++i) MDK_CUDA(cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]));
     return MDK_OK;
@@ -1513,7 +1458,7 @@ int mdk_rl_submit(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P, 
     if ((rc = rl_prepare(e))) return rc;
     int64_t gmax = 0;
     if ((rc = rl_group_limit(e, P, &gmax))) return rc;
-    return rl_enqueue(e, x_host, B, P, D, F, probs_host, labels_host, gmax, ticket);
+    return e->pk.enqueue(RlCall{e, x_host, P, D, F}, B, P, probs_host, nullptr, labels_host, gmax, ticket);
 }
 
 int mdk_rl_flush(mdk_rl_engine *e) {
@@ -1524,21 +1469,9 @@ int mdk_rl_flush(mdk_rl_engine *e) {
 
 int mdk_rl_wait(mdk_rl_engine *e, int64_t ticket) {
     MDK_REQUIRE(e, MDK_ERR_ARG, "rl_wait: engine is NULL");
-    MDK_REQUIRE(ticket >= 0 && ticket < e->submit_count, MDK_ERR_ARG, "rl_wait: unknown ticket");
+    MDK_REQUIRE(ticket >= 0 && ticket < e->pk.tickets, MDK_ERR_ARG, "rl_wait: unknown ticket");
     MDK_CUDA(cudaSetDevice(e->device));
-    if (ticket < e->submit_count - mdk_rl_engine::TICKET_RING) {   // long done, or at least queued before all of copy_out
-        MDK_CUDA(cudaStreamSynchronize(e->copy_out));
-        return MDK_OK;
-    }
-    const int64_t g = e->ticket_group[ticket % mdk_rl_engine::TICKET_RING];
-    if (e->open && g == e->group) {                  // still collecting: the caller wants the result now
-        int rc = rl_launch(e);
-        if (rc) return rc;
-    }
-    // groups leave copy_out in order: a later group's event also covers g once g's own has been reused
-    if (g > e->launched - mdk_rl_engine::OUT_RING) MDK_CUDA(cudaEventSynchronize(e->ev_out[g % mdk_rl_engine::OUT_RING]));
-    else MDK_CUDA(cudaStreamSynchronize(e->copy_out));
-    return MDK_OK;
+    return wait_ticket(e->copy_out, e->pk, RlCall{e}, ticket);
 }
 
 // The one-call form: the open group is sealed, then this call runs as one group of its own (however many windows it
@@ -1551,7 +1484,8 @@ int mdk_rl_forward(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P,
     if ((rc = rl_launch(e))) return rc;
     int64_t gmax = 0, ticket = -1;
     if ((rc = rl_group_limit(e, P, &gmax))) return rc;
-    if ((rc = rl_enqueue(e, x_host, B, P, D, F, probs_host, nullptr, std::max(B, gmax), &ticket))) return rc;
+    if ((rc = e->pk.enqueue(RlCall{e, x_host, P, D, F}, B, P, probs_host, nullptr, nullptr, std::max(B, gmax), &ticket)))
+        return rc;
     if ((rc = mdk_rl_wait(e, ticket))) return rc;
     e->last_B = B;
     e->last_P = P;

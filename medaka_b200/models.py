@@ -67,6 +67,20 @@ def pinned_array(cache, key, shape, dtype):
     return cur.array[:need].reshape(shape)
 
 
+class AsyncResult(object):
+    """Handle of one asynchronous call: ``result()`` waits for it, then returns the probabilities as a CPU tensor and
+    leaves the argmax labels on ``.labels`` and on the model's ``last_labels`` (copies of the page-locked staging)."""
+
+    def __init__(self, model, wait, probs, labels):
+        self._model, self._wait, self._probs, self._labels = model, wait, probs, labels
+
+    def result(self):
+        import torch
+        self._wait()
+        self._model.last_labels = self.labels = self._labels.copy()
+        return torch.from_numpy(self._probs.copy())
+
+
 class GRUModel(object):
     """Bidirectional GRU consensus model (gru.py:10-72) executing on an H100.
 
@@ -253,7 +267,6 @@ class GRUModel(object):
         reference's default 200-window batches then run as 1056-window groups, one computing at a time, with the
         PCIe copies of the neighbouring groups under the compute.
         """
-        import torch
         x = _as_f32(self.get_model_input_features(batch))
         B, T, F = x.shape
         slot = getattr(self, "_async_n", 0) % max(int(slots), 1)
@@ -263,16 +276,7 @@ class GRUModel(object):
         probs = self.pinned("aprobs%d" % slot, (B, T, 5), np.float32)
         labels = self.pinned("alabels%d" % slot, (B, T), np.uint8)
         ticket = self.submit_arrays(xin, probs, labels)
-        model = self
-
-        class _Handle(object):
-            def result(self_inner):
-                model.wait(ticket)
-                model.last_labels = labels.copy()
-                self_inner.labels = model.last_labels
-                return torch.from_numpy(probs.copy())
-
-        return _Handle()
+        return AsyncResult(self, lambda: self.wait(ticket), probs, labels)
 
     def lookahead(self, batch_size, window_len=None):
         """How many ``predict_async`` calls of ``batch_size`` windows to keep in flight (four coalesced groups, one per

@@ -169,7 +169,7 @@ class LatentSpaceLSTM(object):
 
     def _submit(self, batch, key):
         """Submit the batch's features through the page-locked staging arrays named `key`; returns the handle."""
-        import torch
+        from medaka_b200 import models
         x = self.get_model_input_features(batch)
         x = x.detach().cpu().numpy() if hasattr(x, "detach") else np.asarray(x)
         if x.ndim != 4:
@@ -186,16 +186,7 @@ class LatentSpaceLSTM(object):
                                     ffi.cast("float *", ffi.from_buffer(probs)),
                                     ffi.cast("uint8_t *", ffi.from_buffer(labels)), ticket))
         ticket = int(ticket[0])
-        model = self
-
-        class _Handle(object):
-            def result(self_inner):
-                _lm.check(_lm.lib.mdk_rl_wait(model._engine, ticket))
-                model.last_labels = labels.copy()
-                self_inner.labels = model.last_labels
-                return torch.from_numpy(probs.copy())
-
-        return _Handle()
+        return models.AsyncResult(self, lambda: _lm.check(_lm.lib.mdk_rl_wait(self._engine, ticket)), probs, labels)
 
     def preferred_batch_size(self):
         """Windows one packed group holds at the reference's 10 000-position chunks (mdk_rl_preferred_windows: one
