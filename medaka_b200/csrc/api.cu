@@ -1,6 +1,7 @@
-// C ABI of libmedaka_b200 (include/medaka_b200.h): engine life-cycle, weight loading, the forward
-// pipeline, and the featuriser / decode entry points.  Host orchestration only - kernels live in
-// misc.cu, gru_fp32.cu and gru_wg.cu.
+// C ABI of libmedaka_b200 (include/medaka_b200.h): the consensus (GRU) engine - life-cycle, weight loading, the forward
+// pipeline - and the device utilities, error reporting and cached device blobs the other entry points share.  Host
+// orchestration only - the engine's kernels live in misc.cu, gru_fp32.cu and gru_wg.cu.  The featuriser entry points
+// are in pileup.cu, the decode entry points in decode.cu, the read-level engine in readlevel.cu.
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -23,6 +24,35 @@ int cuda_fail(cudaError_t err, const char *what, const char *file, int line) {
         return MDK_ERR_NOMEM;
     }
     return MDK_ERR_CUDA;
+}
+
+struct CachedBlob {
+    int device = -1;
+    uint8_t *buf = nullptr;
+    size_t cap = 0;
+    ~CachedBlob() {
+        if (buf) cudaFree(buf);
+    }
+};
+static thread_local CachedBlob g_blob[2];     // indexed by Blob
+
+cudaError_t cached_blob(Blob role, size_t bytes, uint8_t **out) {
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    CachedBlob &b = g_blob[(int)role];
+    if (b.device != dev || b.cap < bytes) {
+        if (b.buf) cudaFree(b.buf);
+        b.buf = nullptr;
+        b.cap = 0;
+        const size_t want = bytes + bytes / 4 + (1 << 20);
+        e = cudaMalloc(&b.buf, want);
+        if (e != cudaSuccess) return e;
+        b.cap = want;
+        b.device = dev;
+    }
+    *out = b.buf;
+    return cudaSuccess;
 }
 
 template <typename T>
@@ -705,233 +735,6 @@ int mdk_engine_keep_activations(mdk_engine *e, int keep) {
 int64_t mdk_engine_preferred_windows(mdk_engine *e) {
     const int sms = e ? e->sm_count : 132;
     return (int64_t)mdk::WT * (sms / mdk::NDIR);
-}
-
-// ---------------------------------------------------------------------------- featuriser seam
-int mdk_normalise_counts_dev(int device, const uint64_t *counts_dev, const int64_t *major_dev,
-                             const int64_t *minor_dev, int64_t n, int32_t num_dtypes, int32_t mode,
-                             int32_t sym_indels, float *feats_out_dev, int64_t *depth_out_dev) {
-    MDK_REQUIRE(n >= 0, MDK_ERR_ARG, "normalise_counts: n < 0");
-    MDK_REQUIRE(num_dtypes >= 1 && num_dtypes <= 4, MDK_ERR_UNSUPPORTED, "normalise_counts: 1..4 dtypes supported");
-    MDK_REQUIRE(mode >= MDK_NORM_TOTAL && mode <= MDK_NORM_NONE, MDK_ERR_ARG, "normalise_counts: unknown mode");
-    if (n == 0) return MDK_OK;
-    MDK_REQUIRE(counts_dev && major_dev && minor_dev && feats_out_dev, MDK_ERR_ARG, "normalise_counts: NULL pointer");
-    MDK_CUDA(cudaSetDevice(device));
-    MDK_CUDA(launch_normalise(counts_dev, major_dev, minor_dev, n, num_dtypes, mode, sym_indels, feats_out_dev,
-                              depth_out_dev, 0));
-    return MDK_OK;
-}
-
-int mdk_normalise_counts(int device, const uint64_t *counts, const int64_t *major, const int64_t *minor, int64_t n,
-                         int32_t num_dtypes, int32_t mode, int32_t sym_indels, float *feats_out,
-                         int64_t *depth_out) {
-    MDK_REQUIRE(n >= 0, MDK_ERR_ARG, "normalise_counts: n < 0");
-    MDK_REQUIRE(num_dtypes >= 1 && num_dtypes <= 4, MDK_ERR_UNSUPPORTED, "normalise_counts: 1..4 dtypes supported");
-    if (n == 0) return MDK_OK;
-    MDK_REQUIRE(counts && major && minor && feats_out, MDK_ERR_ARG, "normalise_counts: NULL pointer");
-    MDK_CUDA(cudaSetDevice(device));
-    const size_t F = 10 * (size_t)num_dtypes;
-    uint8_t *buf = nullptr;
-    const size_t b_counts = (size_t)n * F * 8, b_pos = (size_t)n * 8, b_feats = (size_t)n * F * 4;
-    MDK_CUDA(plp_scratch(b_counts + 3 * b_pos + b_feats + 64, &buf, 1));   // cached per host thread (the loader threads call this per region)
-    uint64_t *d_counts = reinterpret_cast<uint64_t *>(buf);
-    int64_t *d_major = reinterpret_cast<int64_t *>(buf + b_counts);
-    int64_t *d_minor = d_major + n;
-    int64_t *d_depth = d_minor + n;
-    float *d_feats = reinterpret_cast<float *>(buf + b_counts + 3 * b_pos);
-    cudaError_t err = cudaMemcpy(d_counts, counts, b_counts, cudaMemcpyHostToDevice);
-    if (err == cudaSuccess) err = cudaMemcpy(d_major, major, b_pos, cudaMemcpyHostToDevice);
-    if (err == cudaSuccess) err = cudaMemcpy(d_minor, minor, b_pos, cudaMemcpyHostToDevice);
-    if (err == cudaSuccess) err = launch_normalise(d_counts, d_major, d_minor, n, num_dtypes, mode, sym_indels, d_feats, d_depth, 0);
-    if (err == cudaSuccess) err = cudaMemcpy(feats_out, d_feats, b_feats, cudaMemcpyDeviceToHost);
-    if (err == cudaSuccess && depth_out) err = cudaMemcpy(depth_out, d_depth, b_pos, cudaMemcpyDeviceToHost);
-    if (err != cudaSuccess) return cuda_fail(err, "normalise_counts", __FILE__, __LINE__);
-    return MDK_OK;
-}
-
-int mdk_pileup_counts(int device, int64_t n_rec, const int32_t *pos, const uint16_t *flag, const uint8_t *mapq,
-                      const uint8_t *dtype, const uint32_t *cigar, const int64_t *cigar_off, const uint8_t *seq,
-                      const int64_t *seq_off, int32_t start, int32_t end, int32_t num_dtypes, int32_t min_mapq,
-                      int64_t max_cols, uint64_t *counts_out, int64_t *major_out, int64_t *minor_out,
-                      int64_t *n_cols_out) {
-    MDK_REQUIRE(n_cols_out, MDK_ERR_ARG, "pileup_counts: n_cols_out is NULL");
-    *n_cols_out = 0;
-    MDK_REQUIRE(n_rec >= 0 && end >= start && max_cols >= 0, MDK_ERR_ARG, "pileup_counts: bad sizes");
-    MDK_REQUIRE(num_dtypes >= 1 && num_dtypes <= 4, MDK_ERR_UNSUPPORTED, "pileup_counts: 1..4 dtypes supported");
-    if (n_rec == 0 || end == start) return MDK_OK;
-    MDK_REQUIRE(pos && flag && mapq && dtype && cigar && cigar_off && seq && seq_off, MDK_ERR_ARG,
-                "pileup_counts: NULL record array");
-    MDK_REQUIRE(max_cols == 0 || (counts_out && major_out && minor_out), MDK_ERR_ARG, "pileup_counts: NULL output");
-    MDK_CUDA(cudaSetDevice(device));
-    const int64_t n_ops = cigar_off[n_rec], n_seq = seq_off[n_rec];
-    const int F = 10 * num_dtypes;
-    // one device blob: records in, columns out
-    size_t off = 0;
-    auto take = [&off](size_t bytes) { size_t o = off; off += (bytes + 15) / 16 * 16; return o; };
-    const size_t o_pos = take((size_t)n_rec * 4), o_flag = take((size_t)n_rec * 2), o_mapq = take((size_t)n_rec),
-                 o_dt = take((size_t)n_rec), o_cig = take((size_t)n_ops * 4), o_coff = take((size_t)(n_rec + 1) * 8),
-                 o_seq = take((size_t)n_seq), o_soff = take((size_t)(n_rec + 1) * 8),
-                 o_cnt = take((size_t)max_cols * F * 8), o_maj = take((size_t)max_cols * 8),
-                 o_min = take((size_t)max_cols * 8);
-    uint8_t *buf = nullptr;
-    MDK_CUDA(plp_scratch(off + 16, &buf, 1));     // cached per host thread: no cudaMalloc / cudaFree per region
-    cudaStream_t s = 0;
-    cudaError_t err = cudaMemcpy(buf + o_pos, pos, (size_t)n_rec * 4, cudaMemcpyHostToDevice);
-    if (err == cudaSuccess) err = cudaMemcpy(buf + o_flag, flag, (size_t)n_rec * 2, cudaMemcpyHostToDevice);
-    if (err == cudaSuccess) err = cudaMemcpy(buf + o_mapq, mapq, (size_t)n_rec, cudaMemcpyHostToDevice);
-    if (err == cudaSuccess) err = cudaMemcpy(buf + o_dt, dtype, (size_t)n_rec, cudaMemcpyHostToDevice);
-    if (err == cudaSuccess && n_ops) err = cudaMemcpy(buf + o_cig, cigar, (size_t)n_ops * 4, cudaMemcpyHostToDevice);
-    if (err == cudaSuccess) err = cudaMemcpy(buf + o_coff, cigar_off, (size_t)(n_rec + 1) * 8, cudaMemcpyHostToDevice);
-    if (err == cudaSuccess && n_seq) err = cudaMemcpy(buf + o_seq, seq, (size_t)n_seq, cudaMemcpyHostToDevice);
-    if (err == cudaSuccess) err = cudaMemcpy(buf + o_soff, seq_off, (size_t)(n_rec + 1) * 8, cudaMemcpyHostToDevice);
-    int rc = MDK_OK;
-    if (err == cudaSuccess) {
-        rc = pileup_counts_dev(n_rec, (const int32_t *)(buf + o_pos), (const uint16_t *)(buf + o_flag), buf + o_mapq,
-                               buf + o_dt, (const uint32_t *)(buf + o_cig), (const int64_t *)(buf + o_coff), n_ops,
-                               buf + o_seq, (const int64_t *)(buf + o_soff), start, end, num_dtypes, min_mapq, max_cols,
-                               (uint64_t *)(buf + o_cnt), (int64_t *)(buf + o_maj), (int64_t *)(buf + o_min),
-                               n_cols_out, s);
-    }
-    if (rc == MDK_OK && err == cudaSuccess && *n_cols_out > max_cols) {
-        set_error("pileup_counts: output buffers too small (see *n_cols_out)");
-        rc = MDK_ERR_NOMEM;
-    } else if (rc == MDK_OK && err == cudaSuccess && *n_cols_out > 0) {
-        const int64_t n = *n_cols_out;
-        err = cudaMemcpy(counts_out, buf + o_cnt, (size_t)n * F * 8, cudaMemcpyDeviceToHost);
-        if (err == cudaSuccess) err = cudaMemcpy(major_out, buf + o_maj, (size_t)n * 8, cudaMemcpyDeviceToHost);
-        if (err == cudaSuccess) err = cudaMemcpy(minor_out, buf + o_min, (size_t)n * 8, cudaMemcpyDeviceToHost);
-    }
-    if (err != cudaSuccess) return cuda_fail(err, "pileup_counts", __FILE__, __LINE__);
-    return rc;
-}
-
-// Fused featuriser: records -> counts -> normalised features without the counts ever leaving the device (SURVEY.md 8f row
-// f3: "a1 -> a3 fused").  Same arguments as mdk_pileup_counts plus the normalisation switches of mdk_normalise_counts;
-// copies out 64 B per column (F = 10: features 40, depth 8, positions 16) instead of 96 B out, 96 B back in and 48 B out.
-int mdk_pileup_features(int device, int64_t n_rec, const int32_t *pos, const uint16_t *flag, const uint8_t *mapq,
-                        const uint8_t *dtype, const uint32_t *cigar, const int64_t *cigar_off, const uint8_t *seq,
-                        const int64_t *seq_off, int32_t start, int32_t end, int32_t num_dtypes, int32_t min_mapq,
-                        int32_t mode, int32_t sym_indels, int64_t max_cols, float *feats_out, int64_t *depth_out,
-                        int64_t *major_out, int64_t *minor_out, int64_t *n_cols_out) {
-    MDK_REQUIRE(n_cols_out, MDK_ERR_ARG, "pileup_features: n_cols_out is NULL");
-    *n_cols_out = 0;
-    MDK_REQUIRE(n_rec >= 0 && end >= start && max_cols >= 0, MDK_ERR_ARG, "pileup_features: bad sizes");
-    MDK_REQUIRE(num_dtypes >= 1 && num_dtypes <= 4, MDK_ERR_UNSUPPORTED, "pileup_features: 1..4 dtypes supported");
-    MDK_REQUIRE(mode >= MDK_NORM_TOTAL && mode <= MDK_NORM_NONE, MDK_ERR_ARG, "pileup_features: unknown mode");
-    if (n_rec == 0 || end == start) return MDK_OK;
-    MDK_REQUIRE(pos && flag && mapq && dtype && cigar && cigar_off && seq && seq_off, MDK_ERR_ARG,
-                "pileup_features: NULL record array");
-    MDK_REQUIRE(max_cols == 0 || (feats_out && major_out && minor_out), MDK_ERR_ARG, "pileup_features: NULL output");
-    MDK_CUDA(cudaSetDevice(device));
-    const int64_t n_ops = cigar_off[n_rec], n_seq = seq_off[n_rec];
-    const int F = 10 * num_dtypes;
-    size_t off = 0;
-    auto take = [&off](size_t bytes) { size_t o = off; off += (bytes + 15) / 16 * 16; return o; };
-    const size_t o_pos = take((size_t)n_rec * 4), o_flag = take((size_t)n_rec * 2), o_mapq = take((size_t)n_rec),
-                 o_dt = take((size_t)n_rec), o_cig = take((size_t)n_ops * 4), o_coff = take((size_t)(n_rec + 1) * 8),
-                 o_seq = take((size_t)n_seq), o_soff = take((size_t)(n_rec + 1) * 8),
-                 o_cnt = take((size_t)max_cols * F * 8), o_maj = take((size_t)max_cols * 8),
-                 o_min = take((size_t)max_cols * 8), o_feat = take((size_t)max_cols * F * 4),
-                 o_dep = take((size_t)max_cols * 8);
-    uint8_t *buf = nullptr;
-    MDK_CUDA(plp_scratch(off + 16, &buf, 1));
-    cudaError_t err = cudaSuccess;
-    auto up = [&](size_t o, const void *src, size_t bytes) {
-        if (err == cudaSuccess && bytes) err = cudaMemcpy(buf + o, src, bytes, cudaMemcpyHostToDevice);
-    };
-    up(o_pos, pos, (size_t)n_rec * 4); up(o_flag, flag, (size_t)n_rec * 2); up(o_mapq, mapq, (size_t)n_rec);
-    up(o_dt, dtype, (size_t)n_rec); up(o_cig, cigar, (size_t)n_ops * 4); up(o_coff, cigar_off, (size_t)(n_rec + 1) * 8);
-    up(o_seq, seq, (size_t)n_seq); up(o_soff, seq_off, (size_t)(n_rec + 1) * 8);
-    if (err != cudaSuccess) return cuda_fail(err, "pileup_features (copy in)", __FILE__, __LINE__);
-    int rc = pileup_counts_dev(n_rec, (const int32_t *)(buf + o_pos), (const uint16_t *)(buf + o_flag), buf + o_mapq,
-                               buf + o_dt, (const uint32_t *)(buf + o_cig), (const int64_t *)(buf + o_coff), n_ops,
-                               buf + o_seq, (const int64_t *)(buf + o_soff), start, end, num_dtypes, min_mapq, max_cols,
-                               (uint64_t *)(buf + o_cnt), (int64_t *)(buf + o_maj), (int64_t *)(buf + o_min), n_cols_out, 0);
-    if (rc) return rc;
-    const int64_t n = *n_cols_out;
-    if (n > max_cols) {
-        set_error("pileup_features: output buffers too small (see *n_cols_out)");
-        return MDK_ERR_NOMEM;
-    }
-    if (n == 0) return MDK_OK;
-    MDK_CUDA(launch_normalise((const uint64_t *)(buf + o_cnt), (const int64_t *)(buf + o_maj), (const int64_t *)(buf + o_min), n,
-                              num_dtypes, mode, sym_indels, (float *)(buf + o_feat), (int64_t *)(buf + o_dep), 0));
-    err = cudaMemcpy(feats_out, buf + o_feat, (size_t)n * F * 4, cudaMemcpyDeviceToHost);
-    if (err == cudaSuccess && depth_out) err = cudaMemcpy(depth_out, buf + o_dep, (size_t)n * 8, cudaMemcpyDeviceToHost);
-    if (err == cudaSuccess) err = cudaMemcpy(major_out, buf + o_maj, (size_t)n * 8, cudaMemcpyDeviceToHost);
-    if (err == cudaSuccess) err = cudaMemcpy(minor_out, buf + o_min, (size_t)n * 8, cudaMemcpyDeviceToHost);
-    if (err != cudaSuccess) return cuda_fail(err, "pileup_features (copy out)", __FILE__, __LINE__);
-    return MDK_OK;
-}
-
-// ---------------------------------------------------------------------------- decode seam
-int mdk_decode_consensus_dev(int device, const float *probs_dev, int64_t n, uint8_t *labels_out_dev,
-                             uint8_t *quals_out_dev) {
-    MDK_REQUIRE(n >= 0, MDK_ERR_ARG, "decode_consensus: n < 0");
-    if (n == 0) return MDK_OK;
-    MDK_REQUIRE(probs_dev && labels_out_dev, MDK_ERR_ARG, "decode_consensus: NULL pointer");
-    MDK_CUDA(cudaSetDevice(device));
-    MDK_CUDA(launch_decode(probs_dev, n, labels_out_dev, quals_out_dev, 0));
-    return MDK_OK;
-}
-
-int mdk_decode_consensus(int device, const float *probs, int64_t n, uint8_t *labels_out, uint8_t *quals_out) {
-    MDK_REQUIRE(n >= 0, MDK_ERR_ARG, "decode_consensus: n < 0");
-    if (n == 0) return MDK_OK;
-    MDK_REQUIRE(probs && labels_out, MDK_ERR_ARG, "decode_consensus: NULL pointer");
-    MDK_CUDA(cudaSetDevice(device));
-    uint8_t *buf = nullptr;
-    const size_t b_probs = (size_t)n * NCLS * 4;
-    MDK_CUDA(cudaMalloc(&buf, b_probs + 2 * (size_t)n));
-    float *d_probs = reinterpret_cast<float *>(buf);
-    uint8_t *d_labels = buf + b_probs, *d_quals = d_labels + n;
-    cudaError_t err = cudaMemcpy(d_probs, probs, b_probs, cudaMemcpyHostToDevice);
-    if (err == cudaSuccess) err = launch_decode(d_probs, n, d_labels, quals_out ? d_quals : nullptr, 0);
-    if (err == cudaSuccess) err = cudaMemcpy(labels_out, d_labels, (size_t)n, cudaMemcpyDeviceToHost);
-    if (err == cudaSuccess && quals_out) err = cudaMemcpy(quals_out, d_quals, (size_t)n, cudaMemcpyDeviceToHost);
-    cudaFree(buf);
-    if (err != cudaSuccess) return cuda_fail(err, "decode_consensus", __FILE__, __LINE__);
-    return MDK_OK;
-}
-
-int mdk_decode_consensus_f64(int device, const double *probs, int64_t n, uint8_t *labels_out, uint8_t *quals_out) {
-    MDK_REQUIRE(n >= 0, MDK_ERR_ARG, "decode_consensus: n < 0");
-    if (n == 0) return MDK_OK;
-    MDK_REQUIRE(probs && labels_out, MDK_ERR_ARG, "decode_consensus: NULL pointer");
-    MDK_CUDA(cudaSetDevice(device));
-    uint8_t *buf = nullptr;
-    const size_t b_probs = (size_t)n * NCLS * 8;
-    MDK_CUDA(cudaMalloc(&buf, b_probs + 2 * (size_t)n));
-    double *d_probs = reinterpret_cast<double *>(buf);
-    uint8_t *d_labels = buf + b_probs, *d_quals = d_labels + n;
-    cudaError_t err = cudaMemcpy(d_probs, probs, b_probs, cudaMemcpyHostToDevice);
-    if (err == cudaSuccess) err = launch_decode_f64(d_probs, n, d_labels, quals_out ? d_quals : nullptr, 0);
-    if (err == cudaSuccess) err = cudaMemcpy(labels_out, d_labels, (size_t)n, cudaMemcpyDeviceToHost);
-    if (err == cudaSuccess && quals_out) err = cudaMemcpy(quals_out, d_quals, (size_t)n, cudaMemcpyDeviceToHost);
-    cudaFree(buf);
-    if (err != cudaSuccess) return cuda_fail(err, "decode_consensus_f64", __FILE__, __LINE__);
-    return MDK_OK;
-}
-
-int mdk_variant_columns(int device, const int64_t *minor, const uint8_t *reference, const uint8_t *prediction,
-                        uint8_t *out, int64_t len) {
-    MDK_REQUIRE(len >= 0, MDK_ERR_ARG, "variant_columns: len < 0");
-    if (len == 0) return MDK_OK;
-    MDK_REQUIRE(minor && reference && prediction && out, MDK_ERR_ARG, "variant_columns: NULL pointer");
-    MDK_CUDA(cudaSetDevice(device));
-    uint8_t *buf = nullptr;
-    const size_t n = (size_t)len;
-    MDK_CUDA(cudaMalloc(&buf, n * 8 + 3 * n + 64));
-    int64_t *d_minor = reinterpret_cast<int64_t *>(buf);
-    uint8_t *d_ref = buf + n * 8, *d_pred = d_ref + n, *d_out = d_pred + n;
-    cudaError_t err = cudaMemcpy(d_minor, minor, n * 8, cudaMemcpyHostToDevice);
-    if (err == cudaSuccess) err = cudaMemcpy(d_ref, reference, n, cudaMemcpyHostToDevice);
-    if (err == cudaSuccess) err = cudaMemcpy(d_pred, prediction, n, cudaMemcpyHostToDevice);
-    if (err == cudaSuccess) err = launch_variant_columns(d_minor, d_ref, d_pred, len, d_out, 0);
-    if (err == cudaSuccess) err = cudaMemcpy(out, d_out, n, cudaMemcpyDeviceToHost);
-    cudaFree(buf);
-    if (err != cudaSuccess) return cuda_fail(err, "variant_columns", __FILE__, __LINE__);
-    return MDK_OK;
 }
 
 int mdk_selftest_umma(int device, const float *A, const float *B, float *D, int N, int K, int variant) {

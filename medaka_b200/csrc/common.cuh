@@ -6,6 +6,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <string>
+#include <vector>
 
 #include "../../include/medaka_b200.h"
 #include "packing.h"
@@ -21,6 +22,60 @@ constexpr int NCLS = 5;             // gru.py:53-55
 
 void set_error(const std::string &msg);
 int cuda_fail(cudaError_t err, const char *what, const char *file, int line);
+
+// Device memory of the featuriser and decode entry points, cached per host thread and grown on demand: the loader
+// threads call them concurrently, per region and per contig, and a cudaMalloc / cudaFree pair per call costs more than
+// their kernels.  One blob per role that can be live on a thread at once: STAGING holds a call's copies of the host
+// arrays and its results, SCRATCH the kernels' intermediates under it (the column plan, or the stitch scratch under
+// mdk_stitch_consensus's staging).
+enum class Blob { STAGING, SCRATCH };
+cudaError_t cached_blob(Blob role, size_t bytes, uint8_t **out);
+
+// One call's arrays in a cached blob.  in() and take() name them (with and without host data to copy in); alloc() lays
+// them out in that order, 256-byte aligned, points the named pointers at them and queues the copies of the host data on
+// the legacy stream, ahead of the call's kernels (from page-locked memory the transfer overlaps the staging of the next
+// array); out() copies results back synchronously, after everything queued before it.  The first CUDA error ends the
+// chain, and result() reports it under the entry point's name.
+class Staging {
+  public:
+    Staging(Blob role, const char *what) : role_(role), what_(what) {}
+    template <class T> void take(T **dev, size_t n) { add(dev, &point<T>, nullptr, n * sizeof(T)); }
+    template <class T> void in(const T **dev, const T *host, size_t n) { add(dev, &point<const T>, host, n * sizeof(T)); }
+    bool alloc() {
+        uint8_t *base = nullptr;
+        check(cached_blob(role_, size_, &base));
+        for (const Array &a : arrays_) {
+            if (!ok()) break;
+            a.point(a.dev, base + a.off);
+            if (a.host && a.bytes) check(cudaMemcpyAsync(base + a.off, a.host, a.bytes, cudaMemcpyHostToDevice, 0));
+        }
+        return ok();
+    }
+    template <class T> void out(T *host, const T *dev, size_t n) {
+        if (n) check(cudaMemcpy(host, dev, n * sizeof(T), cudaMemcpyDeviceToHost));
+    }
+    void check(cudaError_t err) { if (ok()) err_ = err; }
+    bool ok() const { return err_ == cudaSuccess; }
+    int result(int rc = MDK_OK) const { return ok() ? rc : cuda_fail(err_, what_, __FILE__, __LINE__); }
+
+  private:
+    struct Array {
+        void *dev;
+        void (*point)(void *dev, uint8_t *at);
+        const void *host;
+        size_t off, bytes;
+    };
+    template <class T> static void point(void *dev, uint8_t *at) { *static_cast<T **>(dev) = reinterpret_cast<T *>(at); }
+    void add(void *dev, void (*pt)(void *, uint8_t *), const void *host, size_t bytes) {
+        arrays_.push_back(Array{dev, pt, host, size_, bytes});
+        size_ += (bytes + 255) / 256 * 256;
+    }
+    Blob role_;
+    const char *what_;
+    cudaError_t err_ = cudaSuccess;
+    size_t size_ = 0;
+    std::vector<Array> arrays_;
+};
 
 #define MDK_CUDA(call)                                                        \
     do {                                                                      \
@@ -226,13 +281,6 @@ cudaError_t launch_inproj0(const float *feats, const float *w_packed, const floa
 cudaError_t launch_head(const float *h1, const float *lin_w, const float *lin_b, int64_t B, int64_t T, int tiled,
                         float *probs, float *logits, uint8_t *labels, cudaStream_t s);
 cudaError_t launch_untile_rows(const float *src_tiled, float *dst, int64_t B, int64_t T, cudaStream_t s);
-cudaError_t launch_normalise(const uint64_t *counts, const int64_t *major, const int64_t *minor, int64_t n,
-                             int num_dtypes, int mode, int sym_indels, float *feats, int64_t *depth,
-                             cudaStream_t s);
-cudaError_t launch_decode(const float *probs, int64_t n, uint8_t *labels, uint8_t *quals, cudaStream_t s);
-cudaError_t launch_decode_f64(const double *probs, int64_t n, uint8_t *labels, uint8_t *quals, cudaStream_t s);
-cudaError_t launch_variant_columns(const int64_t *minor, const uint8_t *ref, const uint8_t *pred, int64_t n,
-                                   uint8_t *out, cudaStream_t s);
 cudaError_t launch_prepare_layer(const LayerWeights &lw, int in_features, bool build_in_tc, cudaStream_t s);
 cudaError_t launch_unpack_h0(const void *h0_tiles, float *out, int64_t B, int64_t T, cudaStream_t s);
 // gru_fp32.cu
@@ -264,11 +312,7 @@ cudaError_t launch_gemm_tc(const void *x_tiles, const __half *w_in_tm, const flo
                            int sm_count, cudaStream_t s);
 int selftest_umma(int device, const float *A, const float *B, float *D, int N, int K, int variant);
 // pileup.cu
-cudaError_t plp_scratch(size_t bytes, uint8_t **out, int slot);   // per-host-thread cached device buffers (slot 0 / 1)
-int pileup_counts_dev(int64_t n_rec, const int32_t *pos, const uint16_t *flag, const uint8_t *mapq,
-                      const uint8_t *dtype, const uint32_t *cigar, const int64_t *cigar_off, int64_t n_ops,
-                      const uint8_t *seq, const int64_t *seq_off, int32_t start, int32_t end, int num_dtypes,
-                      int min_mapq, int64_t max_cols, uint64_t *counts, int64_t *major, int64_t *minor,
-                      int64_t *n_cols_host, cudaStream_t s);
+// exclusive scan of n per-block counts, in place, by one block: counts[i] = sum of counts[0, i), counts[n] = the total
+cudaError_t launch_scan_blocks(int64_t *counts, int64_t n, cudaStream_t s);
 
 }  // namespace mdk

@@ -24,6 +24,8 @@
 // NOT counted (the `continue` at :282 comes before the base loop; the max_ins loop at :259-263 does not look at it).
 // All of it is HBM-bound integer/byte work: no tensor cores.  The device scratch is cached per host thread (no
 // cudaMalloc on the steady-state path) and nothing synchronises with the host before the final copies.
+// Count normalisation (normalise_kernel) lives here too: behind the counts in mdk_pileup_features, on its own in
+// mdk_normalise_counts[_dev].
 #include <algorithm>
 #include <climits>
 #include <cstdint>
@@ -180,23 +182,49 @@ __global__ void __launch_bounds__(SC_THREADS) plp_sum_cov_kernel(int32_t L, cons
     if (threadIdx.x == 0) blk[blockIdx.x] = total;
 }
 
-// phase 2: exclusive scan of up to a few thousand block sums by one block; blk[n] = grand total
-__global__ void __launch_bounds__(SC_THREADS) plp_scan_blocks_kernel(int64_t n, int64_t *__restrict__ blk) {
+// phase 2, and the block counts of stitching and variant decoding (decode.cu): exclusive scan of up to a few ten
+// thousand block counts, in place, by one block of 1024 threads walking them in 1024-entry strips with the running
+// total; counts[n] = the grand total.  Signed: the coverage block sums are sums of a difference array.
+constexpr int SCAN_THREADS = 1024;
+__global__ void __launch_bounds__(SCAN_THREADS) scan_blocks_kernel(int64_t *__restrict__ counts, int64_t n) {
+    __shared__ int64_t warp_sum[32];
     __shared__ int64_t carry;
     if (threadIdx.x == 0) carry = 0;
     __syncthreads();
-    for (int64_t s = 0; s < n; s += SC_THREADS) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int64_t s = 0; s < n; s += SCAN_THREADS) {
         const int64_t i = s + threadIdx.x;
-        const int64_t v = i < n ? blk[i] : 0;
-        int64_t total;
-        const int64_t ex = block_exclusive_scan(v, &total);
-        const int64_t c = carry;
-        if (i < n) blk[i] = c + ex;
+        const int64_t v = i < n ? counts[i] : 0;
+        int64_t x = v;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int64_t y = __shfl_up_sync(0xffffffffu, x, o);
+            if (lane >= o) x += y;
+        }
+        if (lane == 31) warp_sum[warp] = x;
         __syncthreads();
-        if (threadIdx.x == 0) carry = c + total;
+        if (warp == 0) {
+            int64_t w = warp_sum[lane];
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const int64_t y = __shfl_up_sync(0xffffffffu, w, o);
+                if (lane >= o) w += y;
+            }
+            warp_sum[lane] = w;                                // inclusive over warps
+        }
+        __syncthreads();
+        const int64_t before = carry + (warp ? warp_sum[warp - 1] : 0) + (x - v);
+        if (i < n) counts[i] = before;
+        __syncthreads();
+        if (threadIdx.x == SCAN_THREADS - 1) carry = before + v;
         __syncthreads();
     }
-    if (threadIdx.x == 0) blk[n] = carry;
+    if (threadIdx.x == 0) counts[n] = carry;
+}
+
+cudaError_t launch_scan_blocks(int64_t *counts, int64_t n, cudaStream_t s) {
+    scan_blocks_kernel<<<1, SCAN_THREADS, 0, s>>>(counts, n);
+    return cudaGetLastError();
 }
 
 // phase 3: depth -> width (kept in `maxins`' array) -> per-block sum of width
@@ -367,86 +395,151 @@ __global__ void plp_widen_kernel(int64_t n, const uint32_t *__restrict__ src, ui
     if (i < n) dst[i] = src[i];
 }
 
-// per-host-thread device scratch (grown on demand, reused across calls)
-struct PlpScratch {
-    int device = -1;
-    uint8_t *buf = nullptr;
-    size_t cap = 0;
-    ~PlpScratch() {
-        if (buf) cudaFree(buf);
-    }
-};
-static thread_local PlpScratch g_plp_scratch[5];      // 0: kernel scratch, 1: staging of the host-buffer entry point,
-                                                       // 2 / 3: the stitch entry points (stitch.cu), 4: variant decode
+// =====================================================================================
+// Count normalisation  (CountsFeatureEncoder._post_process_pileup, medaka/features.py:871-935)
+// One thread per pileup column.  Algorithmic bytes per column (F=10): read 80 (counts) + 16
+// (major, minor), write 40 (features) + 8 (depth) = 144 B.
+// =====================================================================================
+// index helpers for the per-(dtype, strand) groups of medaka/features.py:647-687:
+// feature order per dtype is 'acgtACGTdD' (src/medaka_counts.h:19): reverse = {0,1,2,3,8}, forward = {4,5,6,7,9}
+__device__ __forceinline__ bool feat_is_rev(int f10) { return f10 < 4 || f10 == 8; }
 
-cudaError_t plp_scratch(size_t bytes, uint8_t **out, int slot) {
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    PlpScratch &s = g_plp_scratch[slot];
-    if (s.device != dev || s.cap < bytes) {
-        if (s.buf) cudaFree(s.buf);
-        s.buf = nullptr;
-        s.cap = 0;
-        const size_t want = bytes + bytes / 4 + (1 << 20);
-        e = cudaMalloc(&s.buf, want);
-        if (e != cudaSuccess) return e;
-        s.cap = want;
-        s.device = dev;
+__device__ __forceinline__ int64_t lower_bound_major(const int64_t *__restrict__ major, int64_t n, int64_t key) {
+    int64_t lo = 0, hi = n;
+    while (lo < hi) {
+        int64_t mid = (lo + hi) >> 1;
+        if (major[mid] < key) lo = mid + 1; else hi = mid;
     }
-    *out = s.buf;
-    return cudaSuccess;
+    return lo;
 }
 
-// ---------------------------------------------------------------------------------------------------------
-// Host driver (device pointers in, device pointers out).  Returns the number of columns through *n_cols_host;
-// if it exceeds max_cols the outputs are incomplete and the caller re-runs with a larger buffer (the reference's
-// enlarge_plp_data, medaka_counts.c:266-271).
-int pileup_counts_dev(int64_t n_rec, const int32_t *pos, const uint16_t *flag, const uint8_t *mapq,
-                      const uint8_t *dtype, const uint32_t *cigar, const int64_t *cigar_off, int64_t n_ops,
-                      const uint8_t *seq, const int64_t *seq_off, int32_t start, int32_t end, int num_dtypes,
-                      int min_mapq, int64_t max_cols, uint64_t *counts, int64_t *major, int64_t *minor,
-                      int64_t *n_cols_host, cudaStream_t s) {
-    const int32_t L = end - start;
-    *n_cols_host = 0;
-    if (L <= 0 || n_rec == 0 || n_ops == 0) return MDK_OK;
-    const int F = 10 * num_dtypes;
-    const int64_t n_blk = (L + SC_BLOCK - 1) / SC_BLOCK;
-    size_t off = 0;
-    auto take = [&off](size_t bytes) { size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
-    const size_t o_rec = take((size_t)n_ops * 4), o_ref = take((size_t)n_ops * 4), o_qry = take((size_t)n_ops * 4),
-                 o_ins = take((size_t)n_ops * 4), o_cov = take((size_t)(L + 1) * 4), o_w = take((size_t)L * 4),
-                 o_col = take((size_t)L * 8), o_bc = take((size_t)(n_blk + 1) * 8), o_bw = take((size_t)(n_blk + 1) * 8),
-                 o_cnt = take((size_t)max_cols * F * 4);
-    uint8_t *scratch = nullptr;
-    MDK_CUDA(plp_scratch(off, &scratch, 0));
-    int32_t *op_rec = (int32_t *)(scratch + o_rec), *op_ref = (int32_t *)(scratch + o_ref), *op_qry = (int32_t *)(scratch + o_qry);
-    uint32_t *op_ins = (uint32_t *)(scratch + o_ins);
-    int32_t *cov = (int32_t *)(scratch + o_cov), *width = (int32_t *)(scratch + o_w);
-    int64_t *col_off = (int64_t *)(scratch + o_col), *blk_cov = (int64_t *)(scratch + o_bc), *blk_w = (int64_t *)(scratch + o_bw);
-    uint32_t *cnt32 = (uint32_t *)(scratch + o_cnt);
-    // cov and width are adjacent: one memset
-    MDK_CUDA(cudaMemsetAsync(scratch + o_cov, 0, (o_w - o_cov) + (size_t)L * 4, s));
-    if (max_cols > 0) MDK_CUDA(cudaMemsetAsync(cnt32, 0, (size_t)max_cols * F * 4, s));
-    const unsigned wb = (unsigned)((n_rec * 32 + 255) / 256), ob = (unsigned)((n_ops + 255) / 256);
-    plp_op_rec_kernel<<<wb, 256, 0, s>>>(n_rec, cigar_off, op_rec);
-    plp_walk_kernel<<<wb, 256, 0, s>>>(n_rec, pos, flag, mapq, min_mapq, cigar, cigar_off, start, end, op_ref, op_qry, op_ins,
-                                       cov, width);
-    plp_sum_cov_kernel<<<(unsigned)n_blk, SC_THREADS, 0, s>>>(L, cov, blk_cov);
-    plp_scan_blocks_kernel<<<1, SC_THREADS, 0, s>>>(n_blk, blk_cov);
-    plp_width_kernel<<<(unsigned)n_blk, SC_THREADS, 0, s>>>(L, cov, blk_cov, width, blk_w);
-    plp_scan_blocks_kernel<<<1, SC_THREADS, 0, s>>>(n_blk, blk_w);
-    plp_columns_kernel<<<(unsigned)n_blk, SC_THREADS, 0, s>>>(L, start, width, blk_w, max_cols, col_off, major, minor);
-    if (max_cols > 0) {
-        plp_count_kernel<<<ob, 256, 0, s>>>(n_ops, op_rec, cigar, op_ref, op_qry, op_ins, flag, mapq, dtype, seq, seq_off, min_mapq,
-                                            start, end, num_dtypes, col_off, max_cols, cnt32);
-        const int64_t n_out = max_cols * F;
-        plp_widen_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, s>>>(n_out, cnt32, counts);
+template <int ND>
+__global__ void __launch_bounds__(256) normalise_kernel(const uint64_t *__restrict__ counts,
+                                                        const int64_t *__restrict__ major,
+                                                        const int64_t *__restrict__ minor, int64_t n, int mode,
+                                                        int sym_indels, float *__restrict__ feats,
+                                                        int64_t *__restrict__ depth_out) {
+    constexpr int F = 10 * ND;
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint64_t c[F];
+    {
+        const ulonglong2 *src = reinterpret_cast<const ulonglong2 *>(counts + i * F);
+#pragma unroll
+        for (int q = 0; q < F / 2; ++q) {
+            ulonglong2 v = src[q];
+            c[2 * q] = v.x;
+            c[2 * q + 1] = v.y;
+        }
     }
-    MDK_CUDA(cudaGetLastError());
-    MDK_CUDA(cudaMemcpyAsync(n_cols_host, blk_w + n_blk, 8, cudaMemcpyDeviceToHost, s));
-    MDK_CUDA(cudaStreamSynchronize(s));
-    return MDK_OK;
+    const int64_t mn = minor[i];
+    // group sums of this column: gs[dt][0] = reverse strand, gs[dt][1] = forward strand
+    uint64_t gs_i[ND][2];
+#pragma unroll
+    for (int dt = 0; dt < ND; ++dt) {
+        gs_i[dt][0] = c[dt * 10 + 0] + c[dt * 10 + 1] + c[dt * 10 + 2] + c[dt * 10 + 3] + c[dt * 10 + 8];
+        gs_i[dt][1] = c[dt * 10 + 4] + c[dt * 10 + 5] + c[dt * 10 + 6] + c[dt * 10 + 7] + c[dt * 10 + 9];
+    }
+    uint64_t gs_p[ND][2];      // group sums of the parent (major) column, ORIGINAL counts
+    uint64_t del_p[ND][2];     // parent's original deletion counts (needed only if the parent is a minor column)
+    int64_t parent_minor = 0;
+    if (mn > 0) {
+        // np.searchsorted(positions['major'], major, side='left'): first column with this major.  Columns of one
+        // major are contiguous with minors counting up from the first one, so the parent is normally mn columns back
+        // (two loads to confirm); anything else (a chunk cut inside an insertion run, repeated majors) takes the search.
+        const int64_t mj = major[i];
+        int64_t j = i - mn;
+        if (j < 0 || major[j] != mj || (j > 0 && major[j - 1] == mj)) j = lower_bound_major(major, n, mj);
+        parent_minor = minor[j];
+        const ulonglong2 *src = reinterpret_cast<const ulonglong2 *>(counts + j * F);
+        uint64_t p[F];
+#pragma unroll
+        for (int q = 0; q < F / 2; ++q) {
+            ulonglong2 v = src[q];
+            p[2 * q] = v.x;
+            p[2 * q + 1] = v.y;
+        }
+#pragma unroll
+        for (int dt = 0; dt < ND; ++dt) {
+            gs_p[dt][0] = p[dt * 10 + 0] + p[dt * 10 + 1] + p[dt * 10 + 2] + p[dt * 10 + 3] + p[dt * 10 + 8];
+            gs_p[dt][1] = p[dt * 10 + 4] + p[dt * 10 + 5] + p[dt * 10 + 6] + p[dt * 10 + 7] + p[dt * 10 + 9];
+            del_p[dt][0] = p[dt * 10 + 8];
+            del_p[dt][1] = p[dt * 10 + 9];
+        }
+    } else {
+#pragma unroll
+        for (int dt = 0; dt < ND; ++dt) {
+            gs_p[dt][0] = gs_i[dt][0];
+            gs_p[dt][1] = gs_i[dt][1];
+            del_p[dt][0] = c[dt * 10 + 8];
+            del_p[dt][1] = c[dt * 10 + 9];
+        }
+    }
+    // depth = row sum of the parent column's original counts (features.py:889-890)
+    uint64_t depth = 0;
+#pragma unroll
+    for (int dt = 0; dt < ND; ++dt) depth += gs_p[dt][0] + gs_p[dt][1];
+    if (depth_out) depth_out[i] = (int64_t)depth;
+
+    if (sym_indels && mn > 0) {
+        // features.py:892-908: reads spanning the insertion site without the insertion count as deletions
+#pragma unroll
+        for (int dt = 0; dt < ND; ++dt) {
+            c[dt * 10 + 8] = gs_p[dt][0] - gs_i[dt][0];   // uint64 wrap-around like numpy
+            c[dt * 10 + 9] = gs_p[dt][1] - gs_i[dt][1];
+        }
+    }
+    float out[F];
+    if (mode == MDK_NORM_TOTAL) {
+        const double d = (double)(depth > 1 ? depth : 1);
+#pragma unroll
+        for (int f = 0; f < F; ++f) out[f] = __double2float_rn((double)c[f] / d);   // f64 divide then cast (features.py:914,926)
+    } else if (mode == MDK_NORM_FWD_REV) {
+        // features.py:915-923: per (dtype, strand) depth, recomputed from the (possibly sym_indels-modified)
+        // counts; minor columns take their parent's group depth.
+#pragma unroll
+        for (int dt = 0; dt < ND; ++dt) {
+#pragma unroll
+            for (int st = 0; st < 2; ++st) {
+                uint64_t g;
+                if (mn > 0) {
+                    g = gs_p[dt][st];
+                    // parent itself a minor column (chunk cut inside an insertion run): its own deletion
+                    // slot was overwritten by the sym_indels fill (with gs_p - gs_p = 0)
+                    if (sym_indels && parent_minor > 0) g -= del_p[dt][st];
+                } else {
+                    g = gs_i[dt][st];
+                }
+                const double d = (double)(g > 1 ? g : 1);
+#pragma unroll
+                for (int b = 0; b < 10; ++b) {
+                    if (feat_is_rev(b) == (st == 0)) out[dt * 10 + b] = __double2float_rn((double)c[dt * 10 + b] / d);
+                }
+            }
+        }
+    } else {
+#pragma unroll
+        for (int f = 0; f < F; ++f) out[f] = (float)c[f];
+    }
+    float2 *dst = reinterpret_cast<float2 *>(feats + i * F);
+#pragma unroll
+    for (int q = 0; q < F / 2; ++q) dst[q] = make_float2(out[2 * q], out[2 * q + 1]);
+}
+
+static cudaError_t launch_normalise(const uint64_t *counts, const int64_t *major, const int64_t *minor, int64_t n,
+                             int num_dtypes, int mode, int sym_indels, float *feats, int64_t *depth,
+                             cudaStream_t s) {
+    if (n == 0) return cudaSuccess;
+    const int threads = 256;
+    const unsigned blocks = (unsigned)((n + threads - 1) / threads);
+    switch (num_dtypes) {
+        case 1: normalise_kernel<1><<<blocks, threads, 0, s>>>(counts, major, minor, n, mode, sym_indels, feats, depth); break;
+        case 2: normalise_kernel<2><<<blocks, threads, 0, s>>>(counts, major, minor, n, mode, sym_indels, feats, depth); break;
+        case 3: normalise_kernel<3><<<blocks, threads, 0, s>>>(counts, major, minor, n, mode, sym_indels, feats, depth); break;
+        case 4: normalise_kernel<4><<<blocks, threads, 0, s>>>(counts, major, minor, n, mode, sym_indels, feats, depth); break;
+        default: return cudaErrorInvalidValue;
+    }
+    return cudaGetLastError();
 }
 
 
@@ -603,67 +696,107 @@ __global__ void __launch_bounds__(256) plp_fill_kernel(int64_t n_ops, RmArgs a, 
     }
 }
 
-// Column structure of a region (shared with the counts featuriser): leaves op_rec / op_ref / op_qry / op_ins / width /
-// col_off in the slot-0 scratch and writes major / minor; *n_cols_host = number of columns.
+// The eight BAM record arrays of a featuriser call (host or device copies); cigar_off / seq_off hold n_rec + 1 offsets.
+struct Records {
+    const int32_t *pos;
+    const uint16_t *flag;
+    const uint8_t *mapq, *dtype;
+    const uint32_t *cigar;
+    const int64_t *cigar_off;
+    const uint8_t *seq;
+    const int64_t *seq_off;
+};
+
+// Column structure of a region, shared by the counts and the read-level featurisers and only enqueued on s: op_rec /
+// op_ref / op_qry / op_ins / width / col_off in the SCRATCH blob, major / minor written, the number of columns left on
+// the device at n_cols for the caller to read once its own kernels are queued.  tail_words more 32-bit words of the
+// scratch, zeroed, are the caller's (the counts' accumulator).
 struct ColumnPlan {
     int32_t *op_rec, *op_ref, *op_qry, *width;
-    uint32_t *op_ins;
+    uint32_t *op_ins, *tail;
     int64_t *col_off;
+    const int64_t *n_cols;
 };
-static int plan_columns(int64_t n_rec, const int32_t *pos, const uint16_t *flag, const uint8_t *mapq, const uint32_t *cigar,
-                        const int64_t *cigar_off, int64_t n_ops, int32_t start, int32_t end, int min_mapq, int64_t max_cols,
-                        int64_t *major, int64_t *minor, int64_t *n_cols_host, ColumnPlan *plan, cudaStream_t s) {
+static int plan_columns(int64_t n_rec, const Records &d, int64_t n_ops, int32_t start, int32_t end, int min_mapq,
+                        int64_t max_cols, int64_t *major, int64_t *minor, size_t tail_words, ColumnPlan *plan,
+                        cudaStream_t s) {
     const int32_t L = end - start;
     const int64_t n_blk = (L + SC_BLOCK - 1) / SC_BLOCK;
-    size_t off = 0;
-    auto take = [&off](size_t bytes) { size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
-    const size_t o_rec = take((size_t)n_ops * 4), o_ref = take((size_t)n_ops * 4), o_qry = take((size_t)n_ops * 4),
-                 o_ins = take((size_t)n_ops * 4), o_cov = take((size_t)(L + 1) * 4), o_w = take((size_t)L * 4),
-                 o_col = take((size_t)L * 8), o_bc = take((size_t)(n_blk + 1) * 8), o_bw = take((size_t)(n_blk + 1) * 8);
-    uint8_t *scratch = nullptr;
-    MDK_CUDA(plp_scratch(off, &scratch, 0));
-    plan->op_rec = (int32_t *)(scratch + o_rec);
-    plan->op_ref = (int32_t *)(scratch + o_ref);
-    plan->op_qry = (int32_t *)(scratch + o_qry);
-    plan->op_ins = (uint32_t *)(scratch + o_ins);
-    int32_t *cov = (int32_t *)(scratch + o_cov);
-    plan->width = (int32_t *)(scratch + o_w);
-    plan->col_off = (int64_t *)(scratch + o_col);
-    int64_t *blk_cov = (int64_t *)(scratch + o_bc), *blk_w = (int64_t *)(scratch + o_bw);
-    MDK_CUDA(cudaMemsetAsync(scratch + o_cov, 0, (o_w - o_cov) + (size_t)L * 4, s));
+    Staging sc(Blob::SCRATCH, "pileup column plan");
+    int32_t *cov;
+    int64_t *blk_cov, *blk_w;
+    sc.take(&plan->op_rec, n_ops);
+    sc.take(&plan->op_ref, n_ops);
+    sc.take(&plan->op_qry, n_ops);
+    sc.take(&plan->op_ins, n_ops);
+    sc.take(&cov, L + 1);
+    sc.take(&plan->width, L);
+    sc.take(&plan->col_off, L);
+    sc.take(&blk_cov, n_blk + 1);
+    sc.take(&blk_w, n_blk + 1);
+    sc.take(&plan->tail, tail_words);
+    if (!sc.alloc()) return sc.result();
+    // cov and width are adjacent: one memset
+    MDK_CUDA(cudaMemsetAsync(cov, 0, (size_t)((uint8_t *)(plan->width + L) - (uint8_t *)cov), s));
+    if (tail_words) MDK_CUDA(cudaMemsetAsync(plan->tail, 0, tail_words * 4, s));
     const unsigned wb = (unsigned)((n_rec * 32 + 255) / 256);
-    plp_op_rec_kernel<<<wb, 256, 0, s>>>(n_rec, cigar_off, plan->op_rec);
-    plp_walk_kernel<<<wb, 256, 0, s>>>(n_rec, pos, flag, mapq, min_mapq, cigar, cigar_off, start, end, plan->op_ref, plan->op_qry,
-                                       plan->op_ins, cov, plan->width);
+    plp_op_rec_kernel<<<wb, 256, 0, s>>>(n_rec, d.cigar_off, plan->op_rec);
+    plp_walk_kernel<<<wb, 256, 0, s>>>(n_rec, d.pos, d.flag, d.mapq, min_mapq, d.cigar, d.cigar_off, start, end,
+                                       plan->op_ref, plan->op_qry, plan->op_ins, cov, plan->width);
     plp_sum_cov_kernel<<<(unsigned)n_blk, SC_THREADS, 0, s>>>(L, cov, blk_cov);
-    plp_scan_blocks_kernel<<<1, SC_THREADS, 0, s>>>(n_blk, blk_cov);
+    MDK_CUDA(launch_scan_blocks(blk_cov, n_blk, s));
     plp_width_kernel<<<(unsigned)n_blk, SC_THREADS, 0, s>>>(L, cov, blk_cov, plan->width, blk_w);
-    plp_scan_blocks_kernel<<<1, SC_THREADS, 0, s>>>(n_blk, blk_w);
-    plp_columns_kernel<<<(unsigned)n_blk, SC_THREADS, 0, s>>>(L, start, plan->width, blk_w, max_cols, plan->col_off, major, minor);
+    MDK_CUDA(launch_scan_blocks(blk_w, n_blk, s));
+    plp_columns_kernel<<<(unsigned)n_blk, SC_THREADS, 0, s>>>(L, start, plan->width, blk_w, max_cols, plan->col_off,
+                                                              major, minor);
     MDK_CUDA(cudaGetLastError());
-    MDK_CUDA(cudaMemcpyAsync(n_cols_host, blk_w + n_blk, 8, cudaMemcpyDeviceToHost, s));
+    plan->n_cols = blk_w + n_blk;
+    return MDK_OK;
+}
+
+// Counts of a region (device pointers in, device pointers out).  Returns the number of columns through *n_cols_host;
+// if it exceeds max_cols the outputs are incomplete and the caller re-runs with a larger buffer (the reference's
+// enlarge_plp_data, medaka_counts.c:266-271).
+static int pileup_counts_dev(int64_t n_rec, const Records &d, int64_t n_ops, int32_t start, int32_t end, int num_dtypes,
+                             int min_mapq, int64_t max_cols, uint64_t *counts, int64_t *major, int64_t *minor,
+                             int64_t *n_cols_host, cudaStream_t s) {
+    *n_cols_host = 0;
+    if (end <= start || n_rec == 0 || n_ops == 0) return MDK_OK;
+    const int F = 10 * num_dtypes;
+    ColumnPlan plan;
+    int rc = plan_columns(n_rec, d, n_ops, start, end, min_mapq, max_cols, major, minor, (size_t)max_cols * F, &plan, s);
+    if (rc) return rc;
+    if (max_cols > 0) {
+        plp_count_kernel<<<(unsigned)((n_ops + 255) / 256), 256, 0, s>>>(
+            n_ops, plan.op_rec, d.cigar, plan.op_ref, plan.op_qry, plan.op_ins, d.flag, d.mapq, d.dtype, d.seq, d.seq_off,
+            min_mapq, start, end, num_dtypes, plan.col_off, max_cols, plan.tail);
+        const int64_t n_out = max_cols * F;
+        plp_widen_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, s>>>(n_out, plan.tail, counts);
+    }
+    MDK_CUDA(cudaGetLastError());
+    MDK_CUDA(cudaMemcpyAsync(n_cols_host, plan.n_cols, 8, cudaMemcpyDeviceToHost, s));
     MDK_CUDA(cudaStreamSynchronize(s));
     return MDK_OK;
 }
 
-int read_matrix_dev(int64_t n_rec, const int32_t *pos, const uint16_t *flag, const uint8_t *mapq, const uint8_t *dtype,
-                    const uint32_t *cigar, const int64_t *cigar_off, int64_t n_ops, const uint8_t *seq,
-                    const int64_t *seq_off, const uint8_t *qual, const int64_t *qual_off, const int8_t *dwell,
-                    const uint8_t *has_dwell, const uint8_t *hap, const int32_t *row, int32_t start, int32_t end,
-                    int min_mapq, int n_rows, int featlen, int f_dwell, int f_hap, int f_dtype, int64_t max_cols,
-                    int8_t *matrix, int64_t *major, int64_t *minor, int64_t *n_cols_host, cudaStream_t s) {
+static int read_matrix_dev(int64_t n_rec, const Records &d, int64_t n_ops, const uint8_t *qual, const int64_t *qual_off,
+                           const int8_t *dwell, const uint8_t *has_dwell, const uint8_t *hap, const int32_t *row,
+                           int32_t start, int32_t end, int min_mapq, int n_rows, int featlen, int f_dwell, int f_hap,
+                           int f_dtype, int64_t max_cols, int8_t *matrix, int64_t *major, int64_t *minor,
+                           int64_t *n_cols_host, cudaStream_t s) {
     *n_cols_host = 0;
     if (end <= start || n_rec == 0 || n_ops == 0) return MDK_OK;
     ColumnPlan plan;
-    int rc = plan_columns(n_rec, pos, flag, mapq, cigar, cigar_off, n_ops, start, end, min_mapq, max_cols, major, minor,
-                          n_cols_host, &plan, s);
+    int rc = plan_columns(n_rec, d, n_ops, start, end, min_mapq, max_cols, major, minor, 0, &plan, s);
     if (rc) return rc;
+    MDK_CUDA(cudaMemcpyAsync(n_cols_host, plan.n_cols, 8, cudaMemcpyDeviceToHost, s));
+    MDK_CUDA(cudaStreamSynchronize(s));
     if (*n_cols_host > max_cols || n_rows <= 0 || max_cols == 0) return MDK_OK;      // caller retries / nothing to fill
     MDK_CUDA(cudaMemsetAsync(matrix, 0, (size_t)(*n_cols_host) * n_rows * featlen, s));
     RmArgs a;
-    a.op_rec = plan.op_rec; a.op_ref = plan.op_ref; a.op_qry = plan.op_qry; a.cigar = cigar; a.op_ins = plan.op_ins;
-    a.cigar_off = cigar_off; a.flag = flag; a.mapq = mapq; a.dtype = dtype; a.seq = seq; a.qual = qual;
-    a.seq_off = seq_off; a.qual_off = qual_off; a.dwell = dwell; a.has_dwell = has_dwell; a.hap = hap; a.row = row;
+    a.op_rec = plan.op_rec; a.op_ref = plan.op_ref; a.op_qry = plan.op_qry; a.cigar = d.cigar; a.op_ins = plan.op_ins;
+    a.cigar_off = d.cigar_off; a.flag = d.flag; a.mapq = d.mapq; a.dtype = d.dtype; a.seq = d.seq; a.qual = qual;
+    a.seq_off = d.seq_off; a.qual_off = qual_off; a.dwell = dwell; a.has_dwell = has_dwell; a.hap = hap; a.row = row;
     a.width = plan.width; a.col_off = plan.col_off; a.start = start; a.end = end; a.n_rows = n_rows; a.featlen = featlen;
     a.f_dwell = f_dwell; a.f_hap = f_hap; a.f_dtype = f_dtype; a.max_cols = max_cols; a.matrix = matrix;
     plp_fill_kernel<<<(unsigned)((n_ops + 255) / 256), 256, 0, s>>>(n_ops, a, min_mapq);
@@ -766,11 +899,153 @@ static bool rm_dwells(const uint8_t *mv, char type, uint32_t mv_len, bool revers
     return true;
 }
 
+// The record arrays are laid out first, and their device copies named in *d; the caller's own arrays go behind them.
+static void stage_records(Staging &st, int64_t n_rec, const Records &h, Records *d) {
+    st.in(&d->pos, h.pos, n_rec);
+    st.in(&d->flag, h.flag, n_rec);
+    st.in(&d->mapq, h.mapq, n_rec);
+    st.in(&d->dtype, h.dtype, n_rec);
+    st.in(&d->cigar, h.cigar, h.cigar_off[n_rec]);
+    st.in(&d->cigar_off, h.cigar_off, n_rec + 1);
+    st.in(&d->seq, h.seq, h.seq_off[n_rec]);
+    st.in(&d->seq_off, h.seq_off, n_rec + 1);
+}
+
+// The normalisation switches of mdk_pileup_features / mdk_normalise_counts and where the features go
+struct Normalise {
+    int mode, sym_indels;
+    float *feats;
+    int64_t *depth;
+};
+
+// mdk_pileup_counts (norm == nullptr: the counts come back) and mdk_pileup_features (the counts are normalised on the
+// device and the features come back), once their arguments are checked.
+static int pileup_host(const char *what, int device, int64_t n_rec, const Records &h, int32_t start, int32_t end,
+                       int num_dtypes, int min_mapq, int64_t max_cols, uint64_t *counts_out, const Normalise *norm,
+                       int64_t *major_out, int64_t *minor_out, int64_t *n_cols_out) {
+    MDK_CUDA(cudaSetDevice(device));
+    const int F = 10 * num_dtypes;
+    Staging st(Blob::STAGING, what);
+    Records d;
+    stage_records(st, n_rec, h, &d);
+    uint64_t *d_counts;
+    int64_t *d_major, *d_minor, *d_depth = nullptr;
+    float *d_feats = nullptr;
+    st.take(&d_counts, max_cols * F);
+    st.take(&d_major, max_cols);
+    st.take(&d_minor, max_cols);
+    if (norm) {
+        st.take(&d_feats, max_cols * F);
+        st.take(&d_depth, max_cols);
+    }
+    if (!st.alloc()) return st.result();
+    int rc = pileup_counts_dev(n_rec, d, h.cigar_off[n_rec], start, end, num_dtypes, min_mapq, max_cols, d_counts, d_major,
+                               d_minor, n_cols_out, 0);
+    if (rc) return rc;
+    const int64_t n = *n_cols_out;
+    if (n > max_cols) {
+        set_error(std::string(what) + ": output buffers too small (see *n_cols_out)");
+        return MDK_ERR_NOMEM;
+    }
+    if (norm) {
+        st.check(launch_normalise(d_counts, d_major, d_minor, n, num_dtypes, norm->mode, norm->sym_indels, d_feats, d_depth,
+                                  0));
+        st.out(norm->feats, d_feats, n * F);
+        if (norm->depth) st.out(norm->depth, d_depth, n);
+    } else {
+        st.out(counts_out, d_counts, n * F);
+    }
+    st.out(major_out, d_major, n);
+    st.out(minor_out, d_minor, n);
+    return st.result();
+}
+
 }  // namespace mdk
 
 using namespace mdk;
 
-extern "C" int mdk_read_matrix(int device, int64_t n_rec, const int32_t *pos, const uint16_t *flag, const uint8_t *mapq,
+extern "C" {
+
+int mdk_normalise_counts_dev(int device, const uint64_t *counts_dev, const int64_t *major_dev,
+                             const int64_t *minor_dev, int64_t n, int32_t num_dtypes, int32_t mode,
+                             int32_t sym_indels, float *feats_out_dev, int64_t *depth_out_dev) {
+    MDK_REQUIRE(n >= 0, MDK_ERR_ARG, "normalise_counts: n < 0");
+    MDK_REQUIRE(num_dtypes >= 1 && num_dtypes <= 4, MDK_ERR_UNSUPPORTED, "normalise_counts: 1..4 dtypes supported");
+    MDK_REQUIRE(mode >= MDK_NORM_TOTAL && mode <= MDK_NORM_NONE, MDK_ERR_ARG, "normalise_counts: unknown mode");
+    if (n == 0) return MDK_OK;
+    MDK_REQUIRE(counts_dev && major_dev && minor_dev && feats_out_dev, MDK_ERR_ARG, "normalise_counts: NULL pointer");
+    MDK_CUDA(cudaSetDevice(device));
+    MDK_CUDA(launch_normalise(counts_dev, major_dev, minor_dev, n, num_dtypes, mode, sym_indels, feats_out_dev,
+                              depth_out_dev, 0));
+    return MDK_OK;
+}
+
+int mdk_normalise_counts(int device, const uint64_t *counts, const int64_t *major, const int64_t *minor, int64_t n,
+                         int32_t num_dtypes, int32_t mode, int32_t sym_indels, float *feats_out,
+                         int64_t *depth_out) {
+    MDK_REQUIRE(n >= 0, MDK_ERR_ARG, "normalise_counts: n < 0");
+    MDK_REQUIRE(num_dtypes >= 1 && num_dtypes <= 4, MDK_ERR_UNSUPPORTED, "normalise_counts: 1..4 dtypes supported");
+    if (n == 0) return MDK_OK;
+    MDK_REQUIRE(counts && major && minor && feats_out, MDK_ERR_ARG, "normalise_counts: NULL pointer");
+    MDK_CUDA(cudaSetDevice(device));
+    const size_t F = 10 * (size_t)num_dtypes;
+    Staging st(Blob::STAGING, "normalise_counts");
+    const uint64_t *d_counts;
+    const int64_t *d_major, *d_minor;
+    int64_t *d_depth;
+    float *d_feats;
+    st.in(&d_counts, counts, n * F);
+    st.in(&d_major, major, n);
+    st.in(&d_minor, minor, n);
+    st.take(&d_depth, n);
+    st.take(&d_feats, n * F);
+    if (!st.alloc()) return st.result();
+    st.check(launch_normalise(d_counts, d_major, d_minor, n, num_dtypes, mode, sym_indels, d_feats, d_depth, 0));
+    st.out(feats_out, d_feats, n * F);
+    if (depth_out) st.out(depth_out, d_depth, n);
+    return st.result();
+}
+
+int mdk_pileup_counts(int device, int64_t n_rec, const int32_t *pos, const uint16_t *flag, const uint8_t *mapq,
+                      const uint8_t *dtype, const uint32_t *cigar, const int64_t *cigar_off, const uint8_t *seq,
+                      const int64_t *seq_off, int32_t start, int32_t end, int32_t num_dtypes, int32_t min_mapq,
+                      int64_t max_cols, uint64_t *counts_out, int64_t *major_out, int64_t *minor_out,
+                      int64_t *n_cols_out) {
+    MDK_REQUIRE(n_cols_out, MDK_ERR_ARG, "pileup_counts: n_cols_out is NULL");
+    *n_cols_out = 0;
+    MDK_REQUIRE(n_rec >= 0 && end >= start && max_cols >= 0, MDK_ERR_ARG, "pileup_counts: bad sizes");
+    MDK_REQUIRE(num_dtypes >= 1 && num_dtypes <= 4, MDK_ERR_UNSUPPORTED, "pileup_counts: 1..4 dtypes supported");
+    if (n_rec == 0 || end == start) return MDK_OK;
+    MDK_REQUIRE(pos && flag && mapq && dtype && cigar && cigar_off && seq && seq_off, MDK_ERR_ARG,
+                "pileup_counts: NULL record array");
+    MDK_REQUIRE(max_cols == 0 || (counts_out && major_out && minor_out), MDK_ERR_ARG, "pileup_counts: NULL output");
+    return pileup_host("pileup_counts", device, n_rec, Records{pos, flag, mapq, dtype, cigar, cigar_off, seq, seq_off},
+                       start, end, num_dtypes, min_mapq, max_cols, counts_out, nullptr, major_out, minor_out, n_cols_out);
+}
+
+// Fused featuriser: records -> counts -> normalised features without the counts ever leaving the device (SURVEY.md 8f row
+// f3: "a1 -> a3 fused").  Same arguments as mdk_pileup_counts plus the normalisation switches of mdk_normalise_counts;
+// copies out 64 B per column (F = 10: features 40, depth 8, positions 16) instead of 96 B out, 96 B back in and 48 B out.
+int mdk_pileup_features(int device, int64_t n_rec, const int32_t *pos, const uint16_t *flag, const uint8_t *mapq,
+                        const uint8_t *dtype, const uint32_t *cigar, const int64_t *cigar_off, const uint8_t *seq,
+                        const int64_t *seq_off, int32_t start, int32_t end, int32_t num_dtypes, int32_t min_mapq,
+                        int32_t mode, int32_t sym_indels, int64_t max_cols, float *feats_out, int64_t *depth_out,
+                        int64_t *major_out, int64_t *minor_out, int64_t *n_cols_out) {
+    MDK_REQUIRE(n_cols_out, MDK_ERR_ARG, "pileup_features: n_cols_out is NULL");
+    *n_cols_out = 0;
+    MDK_REQUIRE(n_rec >= 0 && end >= start && max_cols >= 0, MDK_ERR_ARG, "pileup_features: bad sizes");
+    MDK_REQUIRE(num_dtypes >= 1 && num_dtypes <= 4, MDK_ERR_UNSUPPORTED, "pileup_features: 1..4 dtypes supported");
+    MDK_REQUIRE(mode >= MDK_NORM_TOTAL && mode <= MDK_NORM_NONE, MDK_ERR_ARG, "pileup_features: unknown mode");
+    if (n_rec == 0 || end == start) return MDK_OK;
+    MDK_REQUIRE(pos && flag && mapq && dtype && cigar && cigar_off && seq && seq_off, MDK_ERR_ARG,
+                "pileup_features: NULL record array");
+    MDK_REQUIRE(max_cols == 0 || (feats_out && major_out && minor_out), MDK_ERR_ARG, "pileup_features: NULL output");
+    const Normalise norm{mode, sym_indels, feats_out, depth_out};
+    return pileup_host("pileup_features", device, n_rec, Records{pos, flag, mapq, dtype, cigar, cigar_off, seq, seq_off},
+                       start, end, num_dtypes, min_mapq, max_cols, nullptr, &norm, major_out, minor_out, n_cols_out);
+}
+
+int mdk_read_matrix(int device, int64_t n_rec, const int32_t *pos, const uint16_t *flag, const uint8_t *mapq,
                                const uint8_t *dtype, const uint32_t *cigar, const int64_t *cigar_off, const uint8_t *seq,
                                const int64_t *seq_off, const uint8_t *qual, const int64_t *qual_off, const uint8_t *aux,
                                const int64_t *aux_off, const char *names, const int64_t *name_off, int32_t start,
@@ -902,7 +1177,7 @@ extern "C" int mdk_read_matrix(int device, int64_t n_rec, const int32_t *pos, co
         right_ids[(size_t)q] = slots[(size_t)q].ref_end >= final_pos ? slots[(size_t)q].read : -1;
     }
     // ---- dwell / haplotype channels from the aux fields
-    const int64_t n_ops = cigar_off[n_rec], n_seq = seq_off[n_rec], n_qual = qual_off[n_rec];
+    const int64_t n_ops = cigar_off[n_rec], n_qual = qual_off[n_rec];
     std::vector<int8_t> dwell;
     std::vector<uint8_t> has_dwell, hap;
     if (include_dwells) { dwell.assign((size_t)n_qual, 0); has_dwell.assign((size_t)n_rec, 0); }
@@ -920,40 +1195,35 @@ extern "C" int mdk_read_matrix(int device, int64_t n_rec, const int32_t *pos, co
     }
     // ---- device: records in, columns + matrix out
     MDK_CUDA(cudaSetDevice(device));
-    size_t off = 0;
-    auto take = [&off](size_t bytes) { size_t o = off; off += (bytes + 15) / 16 * 16; return o; };
     const int64_t cell_cap = std::min<int64_t>(max_cells, max_cols * std::max<int64_t>(n_reads, 1) * featlen);
-    const size_t o_pos = take((size_t)n_rec * 4), o_flag = take((size_t)n_rec * 2), o_mapq = take((size_t)n_rec),
-                 o_dt = take((size_t)n_rec), o_cig = take((size_t)n_ops * 4), o_coff = take((size_t)(n_rec + 1) * 8),
-                 o_seq = take((size_t)n_seq), o_soff = take((size_t)(n_rec + 1) * 8), o_qual = take((size_t)n_qual),
-                 o_qoff = take((size_t)(n_rec + 1) * 8), o_dw = take(include_dwells ? (size_t)n_qual : 0),
-                 o_hdw = take(include_dwells ? (size_t)n_rec : 0), o_hap = take(include_haplotype ? (size_t)n_rec : 0),
-                 o_row = take((size_t)n_rec * 4), o_maj = take((size_t)max_cols * 8), o_min = take((size_t)max_cols * 8),
-                 o_mat = take((size_t)cell_cap);
-    uint8_t *buf = nullptr;
-    MDK_CUDA(plp_scratch(off + 16, &buf, 1));
-    cudaError_t err = cudaSuccess;
-    auto up = [&](size_t o, const void *src, size_t bytes) {
-        if (err == cudaSuccess && bytes) err = cudaMemcpy(buf + o, src, bytes, cudaMemcpyHostToDevice);
-    };
-    up(o_pos, pos, (size_t)n_rec * 4); up(o_flag, flag, (size_t)n_rec * 2); up(o_mapq, mapq, (size_t)n_rec);
-    up(o_dt, dtype, (size_t)n_rec); up(o_cig, cigar, (size_t)n_ops * 4); up(o_coff, cigar_off, (size_t)(n_rec + 1) * 8);
-    up(o_seq, seq, (size_t)n_seq); up(o_soff, seq_off, (size_t)(n_rec + 1) * 8); up(o_qual, qual, (size_t)n_qual);
-    up(o_qoff, qual_off, (size_t)(n_rec + 1) * 8); up(o_row, row.data(), (size_t)n_rec * 4);
-    if (include_dwells) { up(o_dw, dwell.data(), (size_t)n_qual); up(o_hdw, has_dwell.data(), (size_t)n_rec); }
-    if (include_haplotype) up(o_hap, hap.data(), (size_t)n_rec);
-    if (err != cudaSuccess) return cuda_fail(err, "read_matrix (copy in)", __FILE__, __LINE__);
+    Staging st(Blob::STAGING, "read_matrix");
+    Records recs;
+    stage_records(st, n_rec, Records{pos, flag, mapq, dtype, cigar, cigar_off, seq, seq_off}, &recs);
+    const uint8_t *d_qual, *d_has_dwell = nullptr, *d_hap = nullptr;
+    const int64_t *d_qual_off;
+    const int8_t *d_dwell = nullptr;
+    const int32_t *d_row;
+    int64_t *d_major, *d_minor;
+    int8_t *d_matrix;
+    st.in(&d_qual, qual, n_qual);
+    st.in(&d_qual_off, qual_off, n_rec + 1);
+    if (include_dwells) {
+        st.in(&d_dwell, dwell.data(), n_qual);
+        st.in(&d_has_dwell, has_dwell.data(), n_rec);
+    }
+    if (include_haplotype) st.in(&d_hap, hap.data(), n_rec);
+    st.in(&d_row, row.data(), n_rec);
+    st.take(&d_major, max_cols);
+    st.take(&d_minor, max_cols);
+    st.take(&d_matrix, cell_cap);
+    if (!st.alloc()) return st.result();
     // the matrix is only filled when the caller's buffers hold it: columns are counted first
     const int64_t rows_dev = n_reads;
     int64_t fill_cols = max_cols;
     if (rows_dev > 0 && max_cols * rows_dev * featlen > cell_cap) fill_cols = 0;
-    int rc = read_matrix_dev(n_rec, (const int32_t *)(buf + o_pos), (const uint16_t *)(buf + o_flag), buf + o_mapq, buf + o_dt,
-                             (const uint32_t *)(buf + o_cig), (const int64_t *)(buf + o_coff), n_ops, buf + o_seq,
-                             (const int64_t *)(buf + o_soff), buf + o_qual, (const int64_t *)(buf + o_qoff),
-                             include_dwells ? (const int8_t *)(buf + o_dw) : nullptr, include_dwells ? buf + o_hdw : nullptr,
-                             include_haplotype ? buf + o_hap : nullptr, (const int32_t *)(buf + o_row), start, end, min_mapq,
-                             (int)rows_dev, featlen, f_dwell, f_hap, f_dtype, fill_cols, (int8_t *)(buf + o_mat),
-                             (int64_t *)(buf + o_maj), (int64_t *)(buf + o_min), n_cols_out, 0);
+    int rc = read_matrix_dev(n_rec, recs, n_ops, d_qual, d_qual_off, d_dwell, d_has_dwell, d_hap, d_row, start, end, min_mapq,
+                             (int)rows_dev, featlen, f_dwell, f_hap, f_dtype, fill_cols, d_matrix, d_major, d_minor,
+                             n_cols_out, 0);
     if (rc) return rc;
     const int64_t n_cols = *n_cols_out;
     if (n_cols > max_cols || n_cols * n_reads * featlen > max_cells || fill_cols == 0) {
@@ -963,15 +1233,16 @@ extern "C" int mdk_read_matrix(int device, int64_t n_rec, const int32_t *pos, co
     }
     if (n_cols > 0) {
         MDK_REQUIRE(major_out && minor_out && (matrix_out || n_reads == 0), MDK_ERR_ARG, "read_matrix: NULL output");
-        err = cudaMemcpy(major_out, buf + o_maj, (size_t)n_cols * 8, cudaMemcpyDeviceToHost);
-        if (err == cudaSuccess) err = cudaMemcpy(minor_out, buf + o_min, (size_t)n_cols * 8, cudaMemcpyDeviceToHost);
-        if (err == cudaSuccess && n_reads > 0)
-            err = cudaMemcpy(matrix_out, buf + o_mat, (size_t)(n_cols * n_reads * featlen), cudaMemcpyDeviceToHost);
+        st.out(major_out, d_major, n_cols);
+        st.out(minor_out, d_minor, n_cols);
+        st.out(matrix_out, d_matrix, n_cols * n_reads * featlen);
     }
-    if (err != cudaSuccess) return cuda_fail(err, "read_matrix (copy out)", __FILE__, __LINE__);
+    if (!st.ok()) return st.result();
     if (left_read_out && right_read_out && n_reads > 0) {
         memcpy(left_read_out, left_ids.data(), (size_t)n_reads * 4);
         memcpy(right_read_out, right_ids.data(), (size_t)n_reads * 4);
     }
     return MDK_OK;
 }
+
+}  // extern "C"

@@ -77,16 +77,33 @@ def pileup_counts(region, bam, dtype_prefixes=None, region_split=100000, workers
     return _split_on_gaps(counts, positions)
 
 
+def _record_args(batch):
+    """The eight record arrays of a ``RecordBatch`` as the featuriser entry points take them, in ABI order (pos, flag,
+    mapq, dtype, cigar, cigar_off, seq, seq_off).  Each is a typed cffi buffer that keeps its numpy array alive for as
+    long as the returned list is referenced, so hold the list until the call returns."""
+    ffi = _lm.ffi
+    return [ffi.from_buffer(ctype + "[]", np.ascontiguousarray(getattr(batch, name), dtype))
+            for name, ctype, dtype in (("pos", "int32_t", np.int32), ("flag", "uint16_t", np.uint16),
+                                       ("mapq", "uint8_t", np.uint8), ("dtype", "uint8_t", np.uint8),
+                                       ("cigar", "uint32_t", np.uint32), ("cigar_off", "int64_t", np.int64),
+                                       ("seq", "uint8_t", np.uint8), ("seq_off", "int64_t", np.int64))]
+
+
+def _positions(major, minor, n):
+    """The (major, minor) positions array of the first n columns."""
+    positions = np.empty(n, dtype=[('major', '<i8'), ('minor', '<i8')])
+    positions['major'] = major[:n]
+    positions['minor'] = minor[:n]
+    return positions
+
+
 def pileup_counts_from_batch(batch, start, end, num_dtypes=1, min_mapq=1, device=0):
     """Run the GPU pileup over a ``RecordBatch``; returns (counts, positions) for [start, end)."""
     lib, ffi = _lm.load(), _lm.ffi
     n_rec = len(batch.pos)
     F = 10 * num_dtypes
     max_cols = max(2 * (end - start), 16)          # the reference's initial guess (medaka_counts.c:245)
-    arrs = dict(pos=np.ascontiguousarray(batch.pos, np.int32), flag=np.ascontiguousarray(batch.flag, np.uint16),
-                mapq=np.ascontiguousarray(batch.mapq, np.uint8), dtype=np.ascontiguousarray(batch.dtype, np.uint8),
-                cigar=np.ascontiguousarray(batch.cigar, np.uint32), coff=np.ascontiguousarray(batch.cigar_off, np.int64),
-                seq=np.ascontiguousarray(batch.seq, np.uint8), soff=np.ascontiguousarray(batch.seq_off, np.int64))
+    records = _record_args(batch)
     n_cols = ffi.new("int64_t *")
     for _ in range(2):
         # (np.empty: untouched pages of the reference-style over-allocation cost nothing; the library writes n rows)
@@ -94,15 +111,7 @@ def pileup_counts_from_batch(batch, start, end, num_dtypes=1, min_mapq=1, device
         major = np.empty(max_cols, dtype=np.int64)
         minor = np.empty(max_cols, dtype=np.int64)
         rc = lib.mdk_pileup_counts(
-            device, n_rec, ffi.cast("const int32_t *", ffi.from_buffer(arrs["pos"])),
-            ffi.cast("const uint16_t *", ffi.from_buffer(arrs["flag"])),
-            ffi.cast("const uint8_t *", ffi.from_buffer(arrs["mapq"])),
-            ffi.cast("const uint8_t *", ffi.from_buffer(arrs["dtype"])),
-            ffi.cast("const uint32_t *", ffi.from_buffer(arrs["cigar"])),
-            ffi.cast("const int64_t *", ffi.from_buffer(arrs["coff"])),
-            ffi.cast("const uint8_t *", ffi.from_buffer(arrs["seq"])),
-            ffi.cast("const int64_t *", ffi.from_buffer(arrs["soff"])),
-            int(start), int(end), num_dtypes, int(min_mapq), max_cols,
+            device, n_rec, *records, int(start), int(end), num_dtypes, int(min_mapq), max_cols,
             ffi.cast("uint64_t *", ffi.from_buffer(counts)), ffi.cast("int64_t *", ffi.from_buffer(major)),
             ffi.cast("int64_t *", ffi.from_buffer(minor)), n_cols)
         if rc == lib.MDK_ERR_NOMEM and n_cols[0] > max_cols:
@@ -111,9 +120,7 @@ def pileup_counts_from_batch(batch, start, end, num_dtypes=1, min_mapq=1, device
         _lm.check(rc)
         break
     n = int(n_cols[0])
-    positions = np.empty(n, dtype=[('major', '<i8'), ('minor', '<i8')])
-    positions['major'] = major[:n]
-    positions['minor'] = minor[:n]
+    positions = _positions(major, minor, n)
     return counts[:n], positions
 
 
@@ -125,10 +132,7 @@ def pileup_features_from_batch(batch, start, end, num_dtypes=1, min_mapq=1, norm
     n_rec = len(batch.pos)
     F = 10 * num_dtypes
     max_cols = max(2 * (end - start), 16)
-    arrs = dict(pos=np.ascontiguousarray(batch.pos, np.int32), flag=np.ascontiguousarray(batch.flag, np.uint16),
-                mapq=np.ascontiguousarray(batch.mapq, np.uint8), dtype=np.ascontiguousarray(batch.dtype, np.uint8),
-                cigar=np.ascontiguousarray(batch.cigar, np.uint32), coff=np.ascontiguousarray(batch.cigar_off, np.int64),
-                seq=np.ascontiguousarray(batch.seq, np.uint8), soff=np.ascontiguousarray(batch.seq_off, np.int64))
+    records = _record_args(batch)
     n_cols = ffi.new("int64_t *")
     for _ in range(2):
         feats = np.empty((max_cols, F), dtype=np.float32)
@@ -136,15 +140,8 @@ def pileup_features_from_batch(batch, start, end, num_dtypes=1, min_mapq=1, norm
         major = np.empty(max_cols, dtype=np.int64)
         minor = np.empty(max_cols, dtype=np.int64)
         rc = lib.mdk_pileup_features(
-            device, n_rec, ffi.cast("const int32_t *", ffi.from_buffer(arrs["pos"])),
-            ffi.cast("const uint16_t *", ffi.from_buffer(arrs["flag"])),
-            ffi.cast("const uint8_t *", ffi.from_buffer(arrs["mapq"])),
-            ffi.cast("const uint8_t *", ffi.from_buffer(arrs["dtype"])),
-            ffi.cast("const uint32_t *", ffi.from_buffer(arrs["cigar"])),
-            ffi.cast("const int64_t *", ffi.from_buffer(arrs["coff"])),
-            ffi.cast("const uint8_t *", ffi.from_buffer(arrs["seq"])),
-            ffi.cast("const int64_t *", ffi.from_buffer(arrs["soff"])),
-            int(start), int(end), num_dtypes, int(min_mapq), _NORM_MODES[normalise], 1 if sym_indels else 0, max_cols,
+            device, n_rec, *records, int(start), int(end), num_dtypes, int(min_mapq), _NORM_MODES[normalise],
+            1 if sym_indels else 0, max_cols,
             ffi.cast("float *", ffi.from_buffer(feats)), ffi.cast("int64_t *", ffi.from_buffer(depth)),
             ffi.cast("int64_t *", ffi.from_buffer(major)), ffi.cast("int64_t *", ffi.from_buffer(minor)), n_cols)
         if rc == lib.MDK_ERR_NOMEM and n_cols[0] > max_cols:
@@ -153,9 +150,7 @@ def pileup_features_from_batch(batch, start, end, num_dtypes=1, min_mapq=1, norm
         _lm.check(rc)
         break
     n = int(n_cols[0])
-    positions = np.empty(n, dtype=[('major', '<i8'), ('minor', '<i8')])
-    positions['major'] = major[:n]
-    positions['minor'] = minor[:n]
+    positions = _positions(major, minor, n)
     return feats[:n], depth[:n], positions
 
 
@@ -316,11 +311,8 @@ def read_matrix_from_batch(batch, start, end, num_dtypes=1, min_mapq=1, row_per_
     qual = batch.qual if batch.qual is not None else np.full(int(qual_off[-1]), 0xFF, dtype=np.uint8)
     aux = batch.aux if batch.aux is not None else np.zeros(0, dtype=np.uint8)
     aux_off = batch.aux_off if batch.aux_off is not None else np.zeros(n_rec + 1, dtype=np.int64)
-    arrs = dict(pos=np.ascontiguousarray(batch.pos, np.int32), flag=np.ascontiguousarray(batch.flag, np.uint16),
-                mapq=np.ascontiguousarray(batch.mapq, np.uint8), dtype=np.ascontiguousarray(batch.dtype, np.uint8),
-                cigar=np.ascontiguousarray(batch.cigar, np.uint32), coff=np.ascontiguousarray(batch.cigar_off, np.int64),
-                seq=np.ascontiguousarray(batch.seq, np.uint8), soff=np.ascontiguousarray(batch.seq_off, np.int64),
-                qual=np.ascontiguousarray(qual, np.uint8), qoff=qual_off,
+    records = _record_args(batch)
+    arrs = dict(qual=np.ascontiguousarray(qual, np.uint8), qoff=qual_off,
                 aux=np.ascontiguousarray(aux, np.uint8) if len(aux) else np.zeros(1, dtype=np.uint8),
                 aoff=np.ascontiguousarray(aux_off, np.int64))
     n_cols, n_reads = ffi.new("int64_t *"), ffi.new("int32_t *")
@@ -333,14 +325,7 @@ def read_matrix_from_batch(batch, start, end, num_dtypes=1, min_mapq=1, row_per_
         left = np.full(max(max_reads_buf, 1), -2, dtype=np.int32)
         right = np.full(max(max_reads_buf, 1), -2, dtype=np.int32)
         rc = lib.mdk_read_matrix(
-            device, n_rec, ffi.cast("const int32_t *", ffi.from_buffer(arrs["pos"])),
-            ffi.cast("const uint16_t *", ffi.from_buffer(arrs["flag"])),
-            ffi.cast("const uint8_t *", ffi.from_buffer(arrs["mapq"])),
-            ffi.cast("const uint8_t *", ffi.from_buffer(arrs["dtype"])),
-            ffi.cast("const uint32_t *", ffi.from_buffer(arrs["cigar"])),
-            ffi.cast("const int64_t *", ffi.from_buffer(arrs["coff"])),
-            ffi.cast("const uint8_t *", ffi.from_buffer(arrs["seq"])),
-            ffi.cast("const int64_t *", ffi.from_buffer(arrs["soff"])),
+            device, n_rec, *records,
             ffi.cast("const uint8_t *", ffi.from_buffer(arrs["qual"])),
             ffi.cast("const int64_t *", ffi.from_buffer(arrs["qoff"])),
             ffi.cast("const uint8_t *", ffi.from_buffer(arrs["aux"])),
@@ -358,9 +343,7 @@ def read_matrix_from_batch(batch, start, end, num_dtypes=1, min_mapq=1, row_per_
         _lm.check(rc)
         break
     n, d = int(n_cols[0]), int(n_reads[0])
-    positions = np.empty(n, dtype=[('major', '<i8'), ('minor', '<i8')])
-    positions['major'] = major[:n]
-    positions['minor'] = minor[:n]
+    positions = _positions(major, minor, n)
     matrix = matrix[:n, :d]
 
     def ids(idx):

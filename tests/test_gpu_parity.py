@@ -299,10 +299,12 @@ def test_decode_consensus_bit_exact(golden_dir):
 
 def test_decode_large_matches_oracle():
     from medaka_b200 import labels as mlabels
+    from tests.test_stitch import PHRED_EDGE_P, phred_edge_rows
     rs = np.random.RandomState(3)
     logits = rs.normal(0, 5, (3000000, 5)).astype(np.float32)
     e = np.exp(logits - logits.max(-1, keepdims=True))
     p = (e / e.sum(-1, keepdims=True)).astype(np.float32)
+    p[:len(PHRED_EDGE_P)] = phred_edge_rows()
     lab, q = mlabels.decode_arrays(p)
     exp_lab, exp_q = labels_oracle.decode_arrays(p)
     assert np.array_equal(lab, exp_lab)

@@ -27,6 +27,20 @@ def _flatten(contigs):
             for c in contigs]
 
 
+# The winning class's probability at the phred edges: 1, either side of the clip at 1 - 1e-7, and where -10 log10(1 - p)
+# lands on an integer (the quality byte truncates it)
+PHRED_EDGE_P = np.array([1.0, np.nextafter(np.float32(1 - 1e-7), np.float32(0)), np.float32(1 - 1e-7),
+                         np.nextafter(np.float32(1 - 1e-7), np.float32(1)), 0.9, 0.99, 0.999, 0.9999, 0.99999],
+                        np.float32)
+
+
+def phred_edge_rows(cls=2):
+    """5-class probability rows whose class cls (one per row, or one for all) takes the PHRED_EDGE_P values."""
+    rows = np.repeat(((1 - PHRED_EDGE_P) / 4)[:, None], 5, axis=1).astype(np.float32)
+    rows[np.arange(len(rows)), cls] = PHRED_EDGE_P
+    return rows
+
+
 def _cpu_decode(samples, pieces):
     """What decode_pieces must return, from the oracle's decode on the planned rows."""
     seqs, quals = [], []
@@ -135,12 +149,14 @@ def test_gpu_stitch_matches_reference(golden_dir):
 @pytest.mark.parametrize("rows", [[1], [3], [4], [5], [1023], [1024], [1025], [7, 1, 1, 2050, 3, 1021],
                                   [4096, 4096], [100003]])
 def test_gpu_decode_pieces_shapes(rows):
-    """Block / vector-width boundaries, one-row ranges, many ranges in one 4-row group."""
+    """Block / vector-width boundaries, one-row ranges, many ranges in one 4-row group; phred edges first in each range."""
     rs = np.random.RandomState(sum(rows))
     samples, pieces = [], []
     for k, n in enumerate(rows):
         p = rs.dirichlet(np.ones(5) * 0.3, size=n + 6).astype(np.float32)
         p[rs.rand(n + 6) < 0.4] = np.array([0.9, 0.025, 0.025, 0.025, 0.025], np.float32)      # gap calls
+        m = min(n, len(PHRED_EDGE_P))
+        p[3:3 + m] = phred_edge_rows()[:m]
         samples.append(Sample('c', None, None, None, None, p, None))
         pieces.append(stitch.Piece(k, 3, 3 + n, False, False))
     seqs, quals = stitch.decode_pieces(samples, pieces)

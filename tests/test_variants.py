@@ -6,6 +6,7 @@ reference's src/medaka_rnn_variants.c), plus the reference's literal cases (meda
 """
 import ctypes
 import json
+import math
 import os
 
 import numpy as np
@@ -239,16 +240,24 @@ def test_gpu_decode_variants_large_matches_oracle():
     """Config-4 scale (one 0.7 M-column joined sample): the records equal the oracle's; every reported variant changes
     the draft; the runs partition exactly the variant columns."""
     from medaka_b200 import common, labels
+    from tests.test_stitch import PHRED_EDGE_P, phred_edge_rows
     d = synth.synth_variant_pileup(seed=77, n_major=600000, p_mut=0.01, n_frac=0.001)
     ls = labels.HaploidLabelScheme()
+    is_major = d['positions']['minor'] == 0
+    codes = np.zeros(len(is_major), dtype=np.uint8)
+    codes[is_major] = ls.encode_reference(d['ref_seq'], d['positions']['major'][is_major])
+    # calls of the reference base with the winning probability at the phred edges
+    edge = np.flatnonzero(is_major & (codes >= 1) & (codes <= 4))[:len(PHRED_EDGE_P)]
+    d['label_probs'][edge] = phred_edge_rows(codes[edge])
     s = common.Sample(d['ref_name'], None, None, None, d['positions'], d['label_probs'], None)
     vs = ls.decode_variants(s, d['ref_seq'])
     assert len(vs) > 1000 and all(v.ref != v.alt[0] for v in vs)
     exp = vo.decode_variants(d['positions'], d['label_probs'], d['ref_seq'])
     same_records(_records(vs), [dict(e, alt=[e['alt']]) for e in exp])
-    is_major = d['positions']['minor'] == 0
-    codes = np.zeros(len(is_major), dtype=np.uint8)
-    codes[is_major] = ls.encode_reference(d['ref_seq'], d['positions']['major'][is_major])
     arr = labels.decode_variant_arrays(d['label_probs'], d['positions']['minor'], codes)
+    # float32 phred with the correctly rounded log10
+    want = [min(np.float32(-10) * np.float32(math.log10(min(max(np.float32(1) - p, np.float32(1e-7)), np.float32(1)))),
+                np.float32(70)) for p in PHRED_EDGE_P]
+    assert np.array_equal(arr['pred_q'][edge], want) and np.array_equal(arr['ref_q'][edge], want)
     assert int(arr['run_len'].sum()) == int(arr['is_var'].sum())
     assert np.all(arr['run_start'][1:] > arr['run_start'][:-1] + arr['run_len'][:-1])   # runs are separated
