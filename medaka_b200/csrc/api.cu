@@ -1,13 +1,15 @@
-// C ABI of libmedaka_b200 (include/medaka_b200.h): the consensus (GRU) engine - life-cycle, weight loading, the forward
-// pipeline - and the device utilities, error reporting and cached device blobs the other entry points share.  Host
-// orchestration only - the engine's kernels live in misc.cu, gru_fp32.cu and gru_wg.cu.  The featuriser entry points
-// are in pileup.cu, the decode entry points in decode.cu, the read-level engine in readlevel.cu.
+// C ABI of libmedaka_b200 (include/medaka_b200.h): the consensus (GRU) engine - life-cycle, weight loading (host copies,
+// packed on the host by gru_pack.cuh and uploaded before the first forward after a load), the forward pipeline - and the
+// device utilities, error reporting and cached device blobs the other entry points share.  Host orchestration only - the
+// engine's kernels live in misc.cu, gru_fp32.cu and gru_wg.cu.  The featuriser entry points are in pileup.cu, the decode
+// entry points in decode.cu, the read-level engine in readlevel.cu.
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
 #include <new>
 
 #include "common.cuh"
+#include "gru_pack.cuh"
 
 namespace mdk {
 
@@ -66,46 +68,30 @@ static void dev_free(T *&p) {
     p = nullptr;
 }
 
-// Host -> device upload ordered on the ENGINE stream.  A plain cudaMemcpy from pageable memory returns once the
-// data is staged, possibly before the DMA lands, and the engine stream is non-blocking (it does not synchronise
-// with the legacy default stream): the packing kernels could then read stale weights (seen as run-to-run
-// 3e-6 differences in layer-0 outputs).  cudaMemcpyAsync + stream sync closes that window.
-static int upload(cudaStream_t stream, float **dst, const float *src, size_t n) {
-    if (!*dst) {
-        int rc = dev_alloc(dst, n);
-        if (rc) return rc;
-    }
-    MDK_CUDA(cudaMemcpyAsync(*dst, src, n * sizeof(float), cudaMemcpyHostToDevice, stream));
-    MDK_CUDA(cudaStreamSynchronize(stream));
-    return MDK_OK;
-}
-
 static int in_features(const mdk_engine *e, int layer) { return layer == 0 ? e->desc.num_features : H2; }
 
+// The weights as the kernels read them, packed on the host (gru_pack.cuh) and uploaded once after each load.
 static int prepare_weights(mdk_engine *e) {
     if (e->prepared) return MDK_OK;
     for (int l = 0; l < 2; ++l) {
-        MDK_REQUIRE(e->layer[l].loaded[0] && e->layer[l].loaded[1], MDK_ERR_STATE,
+        MDK_REQUIRE(!e->layer[l].w_ih[0].empty() && !e->layer[l].w_ih[1].empty(), MDK_ERR_STATE,
                     "engine: GRU weights not loaded for every (layer, direction)");
     }
-    MDK_REQUIRE(e->lin_loaded, MDK_ERR_STATE, "engine: linear head weights not loaded");
+    MDK_REQUIRE(!e->lin_w_host.empty(), MDK_ERR_STATE, "engine: linear head weights not loaded");
+    DeviceWeights &dw = e->weights;
+    int rc;
     for (int l = 0; l < 2; ++l) {
         LayerWeights &lw = e->layer[l];
-        const int in = in_features(e, l);
-        int rc;
-        if (!lw.w_in_packed && (rc = dev_alloc(&lw.w_in_packed, (size_t)GI_COLS * in))) return rc;
-        if (!lw.bias_gi && (rc = dev_alloc(&lw.bias_gi, (size_t)GI_COLS))) return rc;
-        if (!lw.b_hn && (rc = dev_alloc(&lw.b_hn, (size_t)NDIR * H))) return rc;
-        if (!lw.bias_gi_tc && (rc = dev_alloc(&lw.bias_gi_tc, (size_t)GI_COLS))) return rc;
-        if (!lw.b_hn_tc && (rc = dev_alloc(&lw.b_hn_tc, (size_t)NDIR * H))) return rc;
-        if (!lw.w_hh_t && (rc = dev_alloc(&lw.w_hh_t, (size_t)NDIR * H * G3))) return rc;
-        if (!lw.w_hh_tm && (rc = dev_alloc(&lw.w_hh_tm, (size_t)NDIR * 2 * G3 * H))) return rc;
-        if (l == 0 && in <= 16 && !lw.w_x_tm && (rc = dev_alloc(&lw.w_x_tm, (size_t)NDIR * 2 * G3 * 16))) return rc;
-        if (l == 1 && !lw.w_in_tc && (rc = dev_alloc(&lw.w_in_tc, (size_t)2 * GI_COLS * H2))) return rc;
-        MDK_CUDA(launch_prepare_layer(lw, in, l == 1, e->stream));
-        e->launches++;
+        const PackedLayer p = pack_layer(lw, in_features(e, l), l);
+        if ((rc = dw.upload(e->stream, &lw.w_in_packed, p.w_in_packed)) || (rc = dw.upload(e->stream, &lw.bias_gi, p.bias_gi)) ||
+            (rc = dw.upload(e->stream, &lw.b_hn, p.b_hn)) || (rc = dw.upload(e->stream, &lw.bias_gi_tc, p.bias_gi_tc)) ||
+            (rc = dw.upload(e->stream, &lw.b_hn_tc, p.b_hn_tc)) || (rc = dw.upload(e->stream, &lw.w_hh_t, p.w_hh_t)) ||
+            (rc = dw.upload(e->stream, &lw.w_hh_tm, p.w_hh_tm)) || (rc = dw.upload(e->stream, &lw.w_x_tm, p.w_x_tm)) ||
+            (rc = dw.upload(e->stream, &lw.w_in_tc, p.w_in_tc)))
+            return rc;
     }
-    MDK_CUDA(cudaStreamSynchronize(e->stream));
+    if ((rc = dw.upload(e->stream, &e->lin_w, e->lin_w_host)) || (rc = dw.upload(e->stream, &e->lin_b, e->lin_b_host)))
+        return rc;
     e->prepared = true;
     return MDK_OK;
 }
@@ -428,14 +414,6 @@ int mdk_engine_destroy(mdk_engine *e) {
     cudaSetDevice(e->device);
     for (auto &ws : e->ws) if (ws.stream) cudaStreamSynchronize(ws.stream);
     destroy_copy_out(e->copy_out);
-    for (int l = 0; l < 2; ++l) {
-        LayerWeights &lw = e->layer[l];
-        for (int d = 0; d < NDIR; ++d) { dev_free(lw.w_ih[d]); dev_free(lw.w_hh[d]); dev_free(lw.b_ih[d]); dev_free(lw.b_hh[d]); }
-        dev_free(lw.w_in_packed); dev_free(lw.bias_gi); dev_free(lw.b_hn); dev_free(lw.w_hh_t);
-        dev_free(lw.bias_gi_tc); dev_free(lw.b_hn_tc);
-        dev_free(lw.w_hh_tm); dev_free(lw.w_x_tm); dev_free(lw.w_in_tc);
-    }
-    dev_free(e->lin_w); dev_free(e->lin_b);
     for (auto &ws : e->ws) {
         dev_free(ws.gi); dev_free(ws.h1); dev_free(ws.plog);
         if (ws.h0) cudaFree(ws.h0);
@@ -450,12 +428,13 @@ int mdk_engine_destroy(mdk_engine *e) {
     for (auto &set : e->evr) for (auto &ev : set) if (ev) cudaEventDestroy(ev);
     for (auto &ev : e->ev_timer) if (ev) cudaEventDestroy(ev);
     if (e->ev_join) cudaEventDestroy(e->ev_join);
-    delete e;
+    delete e;     // and with it the weights (DeviceWeights)
     cudaGetLastError();
     return MDK_OK;
 }
 
-// weights are read by every lane: quiesce all of them before the packed copies are rebuilt
+// weights are read by every lane: quiesce all of them, so that the calls made before a load run with the weights they
+// were made with and no forward is in flight when prepare_weights rewrites the device copies
 static int quiesce(mdk_engine *e) {
     int rc = launch_group(e);
     if (rc) return rc;
@@ -471,13 +450,10 @@ int mdk_engine_load_gru(mdk_engine *e, int layer, int direction, const float *w_
     MDK_CUDA(cudaSetDevice(e->device));
     { int rcq = quiesce(e); if (rcq) return rcq; }
     LayerWeights &lw = e->layer[layer];
-    const int in = in_features(e, layer);
-    int rc;
-    if ((rc = upload(e->stream, &lw.w_ih[direction], w_ih, (size_t)G3 * in))) return rc;
-    if ((rc = upload(e->stream, &lw.w_hh[direction], w_hh, (size_t)G3 * H))) return rc;
-    if ((rc = upload(e->stream, &lw.b_ih[direction], b_ih, (size_t)G3))) return rc;
-    if ((rc = upload(e->stream, &lw.b_hh[direction], b_hh, (size_t)G3))) return rc;
-    lw.loaded[direction] = true;
+    lw.w_ih[direction].assign(w_ih, w_ih + (size_t)G3 * in_features(e, layer));
+    lw.w_hh[direction].assign(w_hh, w_hh + (size_t)G3 * H);
+    lw.b_ih[direction].assign(b_ih, b_ih + G3);
+    lw.b_hh[direction].assign(b_hh, b_hh + G3);
     e->prepared = false;
     return MDK_OK;
 }
@@ -486,11 +462,9 @@ int mdk_engine_load_linear(mdk_engine *e, const float *w, const float *b) {
     MDK_REQUIRE(e && w && b, MDK_ERR_ARG, "load_linear: NULL argument");
     MDK_CUDA(cudaSetDevice(e->device));
     { int rcq = quiesce(e); if (rcq) return rcq; }
-    int rc;
-    if ((rc = upload(e->stream, &e->lin_w, w, (size_t)NCLS * H2))) return rc;
+    e->lin_w_host.assign(w, w + NCLS * H2);
+    e->lin_b_host.assign(b, b + NCLS);
     e->prepared = false;
-    if ((rc = upload(e->stream, &e->lin_b, b, (size_t)NCLS))) return rc;
-    e->lin_loaded = true;
     return MDK_OK;
 }
 

@@ -91,6 +91,31 @@ class Staging {
         }                             \
     } while (0)
 
+// An engine's device weights, freed with the engine.  upload() allocates an array on its first upload and reuses it on a
+// reload (the model fixes its size); an empty source leaves it absent (nullptr).  The copy is queued on the engine's
+// compute stream, which is then synchronised: a plain cudaMemcpy from pageable memory can return before its DMA lands,
+// and the engines' streams are non-blocking (they do not wait for the legacy stream), so the first forward could read
+// stale weights (seen as run-to-run 3e-6 differences in the GRU's layer-0 outputs).
+struct DeviceWeights {
+    std::vector<void *> allocs;
+    template <class T> int upload(cudaStream_t s, T **dst, const std::vector<T> &src) {
+        const size_t bytes = src.size() * sizeof(T);
+        if (!bytes) return MDK_OK;
+        if (!*dst) {
+            void *p = nullptr;
+            MDK_CUDA(cudaMalloc(&p, bytes));
+            allocs.push_back(p);
+            *dst = static_cast<T *>(p);
+        }
+        MDK_CUDA(cudaMemcpyAsync(*dst, src.data(), bytes, cudaMemcpyHostToDevice, s));
+        MDK_CUDA(cudaStreamSynchronize(s));
+        return MDK_OK;
+    }
+    ~DeviceWeights() {
+        for (void *p : allocs) cudaFree(p);
+    }
+};
+
 // Geometry of the fp16 hi/lo operand tiles the wgmma kernels consume (K-major, no swizzle:
 // [k-group][row][8 halfs]; see ptx.cuh make_smem_desc).
 constexpr int XT_ROWS = 128;                       // positions per activation tile
@@ -126,13 +151,11 @@ constexpr float GATE_SCALE_N = 2.8853900817779268f;
 __host__ __device__ inline float gate_scale(int gate) { return gate < 2 ? GATE_SCALE_RZ : GATE_SCALE_N; }
 
 struct LayerWeights {
-    // fp32 originals (device), torch layout
-    float *w_ih[NDIR] = {nullptr, nullptr};  // [3H][in]
-    float *w_hh[NDIR] = {nullptr, nullptr};  // [3H][H]
-    float *b_ih[NDIR] = {nullptr, nullptr};
-    float *b_hh[NDIR] = {nullptr, nullptr};
-    bool loaded[NDIR] = {false, false};
-    // derived (built by prepare_weights)
+    // as loaded (host, torch layout; empty until mdk_engine_load_gru)
+    std::vector<float> w_ih[NDIR];  // [3H][in]
+    std::vector<float> w_hh[NDIR];  // [3H][H]
+    std::vector<float> b_ih[NDIR], b_hh[NDIR];
+    // device arrays the kernels read, packed on the host from the above (gru_pack.cuh) and uploaded by prepare_weights
     float *w_in_packed = nullptr;   // [768][in] fp32: rows = dir*384 + gate*128 + j
     float *bias_gi = nullptr;       // [768]: r,z: b_ih+b_hh ; n: b_ih
     float *b_hn = nullptr;          // [2][128]
@@ -253,7 +276,7 @@ struct mdk_engine {
     int open_lane = -1;           // lane of the open (or last launched) group
     int last_ws = 0;              // workspace of the most recent forward
     int64_t group_windows = 0;    // most windows coalesced into one group (0 = one wave, mdk_engine_preferred_windows)
-    cudaStream_t stream = nullptr;       // == ws[0].stream: weight preparation, timers
+    cudaStream_t stream = nullptr;       // == ws[0].stream: weight uploads, timers
     static constexpr int EV_RING = 32;   // per-group event sets kept for mdk_engine_mean_timings
     cudaEvent_t evr[EV_RING][8] = {};
     cudaEvent_t *ev = evr[0];            // event set of the group being launched
@@ -261,8 +284,9 @@ struct mdk_engine {
     cudaEvent_t ev_timer[2] = {};
     cudaEvent_t ev_join = nullptr;
     mdk::LayerWeights layer[2];
+    std::vector<float> lin_w_host, lin_b_host;     // as loaded: [5][256], [5]
     float *lin_w = nullptr, *lin_b = nullptr;
-    bool lin_loaded = false;
+    mdk::DeviceWeights weights;   // every device array of layer[] and lin_w / lin_b
     bool keep_act = false;        // debugging: keep h1 (layer-1 output) in HBM, i.e. run the unfused head
     bool prepared = false;
     cudaStream_t copy_in = nullptr;
@@ -281,7 +305,6 @@ cudaError_t launch_inproj0(const float *feats, const float *w_packed, const floa
 cudaError_t launch_head(const float *h1, const float *lin_w, const float *lin_b, int64_t B, int64_t T, int tiled,
                         float *probs, float *logits, uint8_t *labels, cudaStream_t s);
 cudaError_t launch_untile_rows(const float *src_tiled, float *dst, int64_t B, int64_t T, cudaStream_t s);
-cudaError_t launch_prepare_layer(const LayerWeights &lw, int in_features, bool build_in_tc, cudaStream_t s);
 cudaError_t launch_unpack_h0(const void *h0_tiles, float *out, int64_t B, int64_t T, cudaStream_t s);
 // gru_fp32.cu
 cudaError_t launch_rec_fp32(const float *gi, const float *w_hh_t, const float *b_hn, float *h_out, int64_t B,

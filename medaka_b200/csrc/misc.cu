@@ -1,5 +1,5 @@
-// The GRU path's small kernels: layer-0 input projection, linear head + softmax + argmax, weight packing, and the
-// debug unpacking of the tiled intermediates.  All are coalesced / vectorised streaming kernels; none is GEMM-shaped.
+// The GRU path's small kernels: layer-0 input projection, linear head + softmax + argmax, and the debug unpacking of
+// the tiled intermediates.  All are coalesced / vectorised streaming kernels; none is GEMM-shaped.
 #include "common.cuh"
 #include "ptx.cuh"
 
@@ -212,83 +212,6 @@ cudaError_t launch_head(const float *h1, const float *lin_w, const float *lin_b,
     int64_t blocks = (P + 31) / 32;            // 8 warps per block, 4 positions per warp per iteration
     if (blocks > 132 * 8) blocks = 132 * 8;    // persistent-ish grid: multiple of the SM count
     head_kernel<<<(unsigned)blocks, 256, 0, s>>>(h1, lin_w, lin_b, P, B, T, tiled, probs, logits, labels);
-    return cudaGetLastError();
-}
-
-// =====================================================================================
-// Weight packing (runs once per load_state_dict)
-// =====================================================================================
-__global__ void pack_layer_kernel(const float *w_ih0, const float *w_ih1, const float *w_hh0, const float *w_hh1,
-                                  const float *b_ih0, const float *b_ih1, const float *b_hh0, const float *b_hh1,
-                                  int in_features, float *w_in_packed, float *bias_gi, float *b_hn, float *w_hh_t,
-                                  __half *w_hh_tm, __half *w_x_tm, __half *w_in_tc, float *bias_gi_tc, float *b_hn_tc) {
-    const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    const float *w_ih[2] = {w_ih0, w_ih1}, *w_hh[2] = {w_hh0, w_hh1};
-    const float *b_ih[2] = {b_ih0, b_ih1}, *b_hh[2] = {b_hh0, b_hh1};
-    // input weights packed [768][in]
-    for (int64_t i = tid; i < (int64_t)GI_COLS * in_features; i += stride) {
-        const int row = (int)(i / in_features), k = (int)(i % in_features);
-        const int d = row / G3, r = row % G3;
-        w_in_packed[i] = w_ih[d][(int64_t)r * in_features + k];
-    }
-    for (int64_t i = tid; i < GI_COLS; i += stride) {
-        const int d = (int)i / G3, r = (int)i % G3;
-        bias_gi[i] = (r < 2 * H) ? (b_ih[d][r] + b_hh[d][r]) : b_ih[d][r];
-        bias_gi_tc[i] = bias_gi[i] * gate_scale(r / H);
-    }
-    for (int64_t i = tid; i < NDIR * H; i += stride) {
-        const int d = (int)i / H, j = (int)i % H;
-        b_hn[i] = b_hh[d][2 * H + j];
-        b_hn_tc[i] = b_hn[i] * GATE_SCALE_N;
-    }
-    // recurrent weights, transposed fp32 [d][k][384] and fp16 hi/lo blocks [d][part][gate][kg][row][8]
-    for (int64_t i = tid; i < (int64_t)NDIR * G3 * H; i += stride) {
-        const int d = (int)(i / (G3 * H));
-        const int rem = (int)(i % (G3 * H));
-        const int c = rem / H, k = rem % H;          // c = gate row, k = input unit
-        const float v = w_hh[d][c * H + k];
-        w_hh_t[((int64_t)d * H + k) * G3 + c] = v;
-        const int g = c / H, j = c % H;
-        __half hi, lo;
-        split_f16(v * gate_scale(g), hi, lo);
-        const int64_t blk_halfs = (int64_t)H * H;   // 128x128 block
-        w_hh_tm[(((int64_t)d * 2 + 0) * 3 + g) * blk_halfs + j * H + k] = hi;
-        w_hh_tm[(((int64_t)d * 2 + 1) * 3 + g) * blk_halfs + j * H + k] = lo;
-    }
-    if (w_x_tm) {   // layer 0, in_features <= 16: [d][part][gate][row j][16], K zero-padded
-        for (int64_t i = tid; i < (int64_t)NDIR * G3 * 16; i += stride) {
-            const int d = (int)(i / (G3 * 16));
-            const int rem = (int)(i % (G3 * 16));
-            const int c = rem / 16, k = rem % 16;
-            const float v = (k < in_features) ? w_ih[d][(int64_t)c * in_features + k] : 0.f;
-            const int g = c / H, j = c % H;
-            __half hi, lo;
-            split_f16(v * gate_scale(g), hi, lo);
-            w_x_tm[((((int64_t)d * 2 + 0) * 3 + g) * H + j) * 16 + k] = hi;
-            w_x_tm[((((int64_t)d * 2 + 1) * 3 + g) * H + j) * 16 + k] = lo;
-        }
-    }
-    if (w_in_tc) {   // layer 1: [blk = dir*3+gate][part][row j][k] row-major
-        for (int64_t i = tid; i < (int64_t)GI_COLS * H2; i += stride) {
-            const int row = (int)(i / H2), k = (int)(i % H2);
-            const int d = row / G3, r = row % G3;
-            const float v = w_ih[d][(int64_t)r * H2 + k];
-            __half hi, lo;
-            split_f16(v * gate_scale(r / H), hi, lo);
-            const int blk = row / H, j = row % H;
-            const int64_t plane = (int64_t)H * H2;   // 128 x 256 halfs
-            w_in_tc[((int64_t)blk * 2 + 0) * plane + (int64_t)j * H2 + k] = hi;
-            w_in_tc[((int64_t)blk * 2 + 1) * plane + (int64_t)j * H2 + k] = lo;
-        }
-    }
-}
-
-cudaError_t launch_prepare_layer(const LayerWeights &lw, int in_features, bool build_in_tc, cudaStream_t s) {
-    pack_layer_kernel<<<296, 256, 0, s>>>(lw.w_ih[0], lw.w_ih[1], lw.w_hh[0], lw.w_hh[1], lw.b_ih[0], lw.b_ih[1],
-                                          lw.b_hh[0], lw.b_hh[1], in_features, lw.w_in_packed, lw.bias_gi,
-                                          lw.b_hn, lw.w_hh_t, lw.w_hh_tm, lw.w_x_tm, build_in_tc ? lw.w_in_tc : nullptr,
-                                          lw.bias_gi_tc, lw.b_hn_tc);
     return cudaGetLastError();
 }
 

@@ -210,8 +210,8 @@ template <> struct Wgmma<128> {
 // ---------------------------------------------------------------- fp16 hi/lo split
 // v ~= hi + lo with hi = fp16(v), lo = fp16(v - hi): ~22 significant bits for |v| in [2^-14, 65504],
 // absolute error <= 2^-25 below that (fp16 subnormals).  Three fp16 MMAs (hi*hi + hi*lo + lo*hi) with
-// fp32 accumulation then reproduce an fp32 product to ~1e-7 relative.
-__device__ __forceinline__ void split_f16(float v, __half &hi, __half &lo) {
+// fp32 accumulation then reproduce an fp32 product to ~1e-7 relative.  The host weight packers use the same split.
+__host__ __device__ __forceinline__ void split_f16(float v, __half &hi, __half &lo) {
     hi = __float2half_rn(v);
     lo = __float2half_rn(v - __half2float(hi));
 }

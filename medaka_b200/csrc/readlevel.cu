@@ -898,9 +898,9 @@ struct RlLstmLayer {
     float *bias = nullptr;      // [2 * 4H]  b_ih + b_hh
     float *w_t = nullptr;       // [2][H k][4H]  W_hh^T (fp32 recurrence)
     __half *w_hi = nullptr;     // [2][4H][H] fp16 hi plane of W_hh, row-major (tensor-core recurrences: -> registers)
-    uint8_t *w_lo = nullptr;    // fp16 lo plane of W_hh as the tensor-core recurrence's shared-memory A operand tiles
+    __half *w_lo = nullptr;     // fp16 lo plane of W_hh as the tensor-core recurrence's shared-memory A operand tiles
                                 // (lt_lo_index at H = 128, l3_lo_index at 384)
-    uint8_t *w_ih_tc = nullptr; // H = 384: W_ih as rl_proj_tc_kernel's A tiles [row block 24][K chunk][hi | lo][8][128][8]
+    __half *w_ih_tc = nullptr;  // H = 384: W_ih as rl_proj_tc_kernel's A tiles [row block 24][K chunk][hi | lo][8][128][8]
 };
 
 }  // namespace mdk
@@ -925,17 +925,17 @@ struct mdk_rl_engine {
     cudaEvent_t ev[2][7] = {};     // stage events, by group parity: one group's may be read while the next collects
     std::unordered_map<std::string, std::vector<float>> host;     // state-dict tensors as loaded
     bool prepared = false;
-    // device parameters
+    // device parameters, built from `host` by rl_prepare
+    DeviceWeights weights;
     float *emb_base = nullptr, *emb_strand = nullptr;
     float *c1_w = nullptr, *c1_b = nullptr, *bn1[4] = {nullptr, nullptr, nullptr, nullptr};
     float *c17_wt = nullptr, *c17_b = nullptr, *bn2[4] = {nullptr, nullptr, nullptr, nullptr};
-    uint8_t *c17_tc = nullptr;     // [17 taps][hi | lo][k-group 16][co 128][8 halfs]: the tensor-core kernel's A operand tiles
+    __half *c17_tc = nullptr;      // [17 taps][hi | lo][k-group 16][co 128][8 halfs]: the tensor-core kernel's A operand tiles
     int conv_tc = 1;               // 1: k = 17 convolution on wgmma (default), 0: fp32 CUDA cores
     int lstm_tc = 1;               // 1: LSTM recurrence on wgmma (default), 0: fp32 CUDA cores
     float *pool_w = nullptr, *pool_b = nullptr;
     RlLstmLayer lstm[2];
     float *lin_w = nullptr, *lin_b = nullptr;
-    std::vector<void *> allocs;
     cudaStream_t stream = nullptr;                   // compute: convolutions, then each group's LSTM and head
     cudaStream_t copy_in = nullptr;
     CopyOut copy_out;
@@ -957,15 +957,6 @@ struct mdk_rl_engine {
 
 namespace {
 
-int rl_upload(mdk_rl_engine *e, const std::vector<float> &v, float **out) {
-    void *p = nullptr;
-    MDK_CUDA(cudaMalloc(&p, std::max<size_t>(v.size(), 1) * sizeof(float)));
-    e->allocs.push_back(p);
-    if (!v.empty()) MDK_CUDA(cudaMemcpy(p, v.data(), v.size() * sizeof(float), cudaMemcpyHostToDevice));
-    *out = static_cast<float *>(p);
-    return MDK_OK;
-}
-
 const std::vector<float> *rl_get(mdk_rl_engine *e, const std::string &name, size_t want) {
     auto it = e->host.find(name);
     if (it == e->host.end()) { set_error("read-level model: tensor '" + name + "' was not loaded"); return nullptr; }
@@ -977,21 +968,12 @@ const std::vector<float> *rl_get(mdk_rl_engine *e, const std::string &name, size
     return &it->second;
 }
 
-template <class T>
-int rl_upload_raw(mdk_rl_engine *e, const std::vector<T> &v, T **out) {
-    void *p = nullptr;
-    MDK_CUDA(cudaMalloc(&p, v.size() * sizeof(T)));
-    e->allocs.push_back(p);
-    MDK_CUDA(cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
-    *out = static_cast<T *>(p);
-    return MDK_OK;
-}
-
 // LSTM weights of both layers at either size: W_ih of both directions stacked for one projection, b_ih + b_hh, W_hh^T for
 // the fp32 recurrence, W_hh as fp16 hi (row-major) and lo (the tensor-core recurrence's operand tiles) planes, and at
 // H = 384 W_ih as rl_proj_tc_kernel's operand tiles
 int rl_prepare_lstm(mdk_rl_engine *e) {
     const int HH = e->H, G4 = 4 * HH;
+    const auto up = [e](auto **dst, const auto &src) { return e->weights.upload(e->stream, dst, src); };
     int rc;
     for (int l = 0; l < 2; ++l) {
         const int in = l == 0 ? HH : 2 * HH;
@@ -1010,32 +992,24 @@ int rl_prepare_lstm(mdk_rl_engine *e) {
                 for (int k = 0; k < HH; ++k) {
                     const float v = (*whh)[(size_t)r * HH + k];
                     w_t[((size_t)d * HH + k) * G4 + r] = v;
-                    const __half h16 = __float2half_rn(v), l16 = __float2half_rn(v - __half2float(h16));
-                    hi[((size_t)d * G4 + r) * HH + k] = h16;
-                    lo[HH == RL_H3 ? l3_lo_index(d, r, k) : lt_lo_index(d, r, k)] = l16;
+                    split_f16(v, hi[((size_t)d * G4 + r) * HH + k], lo[HH == RL_H3 ? l3_lo_index(d, r, k) : lt_lo_index(d, r, k)]);
                 }
         }
         RlLstmLayer &L = e->lstm[l];
-        __half *p = nullptr;
-        if ((rc = rl_upload(e, w_ih, &L.w_ih)) || (rc = rl_upload(e, bias, &L.bias)) || (rc = rl_upload(e, w_t, &L.w_t)) ||
-            (rc = rl_upload_raw(e, hi, &L.w_hi)) || (rc = rl_upload_raw(e, lo, &p)))
+        if ((rc = up(&L.w_ih, w_ih)) || (rc = up(&L.bias, bias)) || (rc = up(&L.w_t, w_t)) || (rc = up(&L.w_hi, hi)) ||
+            (rc = up(&L.w_lo, lo)))
             return rc;
-        L.w_lo = reinterpret_cast<uint8_t *>(p);
         if (HH != RL_H3) continue;
         // W_ih of both directions as one [3072][in] matrix, tiled per (128-row block, 64-wide K chunk)
         const int nchunks = in / PJ_KC;
         std::vector<__half> ih_t((size_t)2 * G4 * in * 2);
         for (int r = 0; r < 2 * G4; ++r)
             for (int k = 0; k < in; ++k) {
-                const float v = w_ih[(size_t)r * in + k];
-                const __half h16 = __float2half_rn(v), l16 = __float2half_rn(v - __half2float(h16));
                 const size_t chunk = ((size_t)(r / PJ_M) * nchunks + k / PJ_KC) * (PJ_WCHUNK / 2);
                 const size_t off = (size_t)((k % PJ_KC) / 8) * (PJ_M * 8) + (r % PJ_M) * 8 + k % 8;
-                ih_t[chunk + off] = h16;
-                ih_t[chunk + PJ_WPLANE / 2 + off] = l16;
+                split_f16(w_ih[(size_t)r * in + k], ih_t[chunk + off], ih_t[chunk + PJ_WPLANE / 2 + off]);
             }
-        if ((rc = rl_upload_raw(e, ih_t, &p))) return rc;
-        L.w_ih_tc = reinterpret_cast<uint8_t *>(p);
+        if ((rc = up(&L.w_ih_tc, ih_t))) return rc;
     }
     return MDK_OK;
 }
@@ -1088,6 +1062,7 @@ int rl_prepare(mdk_rl_engine *e) {
     if (e->prepared) return MDK_OK;
     const int nin = RL_EMB + 1 + (e->use_dwells ? 1 : 0);
     const int HH = e->H;
+    const auto up = [e](auto **dst, const auto &src) { return e->weights.upload(e->stream, dst, src); };
     int rc;
     {   // at 384: one 8-CTA cluster of the recurrence must fit the device
         int wave = 0;
@@ -1104,15 +1079,15 @@ int rl_prepare(mdk_rl_engine *e) {
     RL_NEED(pb, "pre_pool_expansion_layer.bias", HH)
     RL_NEED(lw, "linear.weight", NCLS * 2 * HH)
     RL_NEED(lb, "linear.bias", NCLS)
-    if ((rc = rl_upload(e, *eb, &e->emb_base)) || (rc = rl_upload(e, *es, &e->emb_strand)) || (rc = rl_upload(e, *c1w, &e->c1_w)) ||
-        (rc = rl_upload(e, *c1b, &e->c1_b)) || (rc = rl_upload(e, *c17b, &e->c17_b)) ||
-        (rc = rl_upload(e, *pb, &e->pool_b)) || (rc = rl_upload(e, *lw, &e->lin_w)) || (rc = rl_upload(e, *lb, &e->lin_b)))
+    if ((rc = up(&e->emb_base, *eb)) || (rc = up(&e->emb_strand, *es)) || (rc = up(&e->c1_w, *c1w)) ||
+        (rc = up(&e->c1_b, *c1b)) || (rc = up(&e->c17_b, *c17b)) || (rc = up(&e->pool_b, *pb)) ||
+        (rc = up(&e->lin_w, *lw)) || (rc = up(&e->lin_b, *lb)))
         return rc;
     {   // Linear(C -> H) weights transposed to [k][h]: coalesced across the output units
         std::vector<float> wt((size_t)RL_C * HH);
         for (int h = 0; h < HH; ++h)
             for (int k = 0; k < RL_C; ++k) wt[(size_t)k * HH + h] = (*pw)[(size_t)h * RL_C + k];
-        if ((rc = rl_upload(e, wt, &e->pool_w))) return rc;
+        if ((rc = up(&e->pool_w, wt))) return rc;
     }
     // conv k = 17 weights: torch [out][in][tap] -> [tap][in][out]
     {
@@ -1120,22 +1095,17 @@ int rl_prepare(mdk_rl_engine *e) {
         for (int o = 0; o < RL_C; ++o)
             for (int i = 0; i < RL_C; ++i)
                 for (int t = 0; t < RL_TAPS; ++t) wt[((size_t)t * RL_C + i) * RL_C + o] = (*c17w)[((size_t)o * RL_C + i) * RL_TAPS + t];
-        if ((rc = rl_upload(e, wt, &e->c17_wt))) return rc;
+        if ((rc = up(&e->c17_wt, wt))) return rc;
         // the same weights as K-major fp16 hi / lo operand tiles, one 64 KiB block per tap
         std::vector<__half> tc((size_t)RL_TAPS * 2 * RL_C * RL_C);
         for (int t = 0; t < RL_TAPS; ++t)
             for (int o = 0; o < RL_C; ++o)
                 for (int i = 0; i < RL_C; ++i) {
-                    const float v = (*c17w)[((size_t)o * RL_C + i) * RL_TAPS + t];
-                    const __half hi = __float2half_rn(v);
-                    const __half lo = __float2half_rn(v - __half2float(hi));
                     const size_t off = (size_t)(i / 8) * (RL_C * 8) + (size_t)o * 8 + (i % 8);
-                    tc[((size_t)t * 2 + 0) * RL_C * RL_C + off] = hi;
-                    tc[((size_t)t * 2 + 1) * RL_C * RL_C + off] = lo;
+                    split_f16((*c17w)[((size_t)o * RL_C + i) * RL_TAPS + t], tc[((size_t)t * 2 + 0) * RL_C * RL_C + off],
+                              tc[((size_t)t * 2 + 1) * RL_C * RL_C + off]);
                 }
-        __half *p = nullptr;
-        if ((rc = rl_upload_raw(e, tc, &p))) return rc;
-        e->c17_tc = reinterpret_cast<uint8_t *>(p);
+        if ((rc = up(&e->c17_tc, tc))) return rc;
     }
     // BatchNorm (inference): mean, 1 / sqrt(var + eps), weight, bias
     for (int l = 0; l < 2; ++l) {
@@ -1147,8 +1117,7 @@ int rl_prepare(mdk_rl_engine *e) {
         std::vector<float> invstd(RL_C);
         for (int c = 0; c < RL_C; ++c) invstd[c] = 1.0f / sqrtf((*var)[c] + 1e-5f);
         float **dst = l == 0 ? e->bn1 : e->bn2;
-        if ((rc = rl_upload(e, *mean, &dst[0])) || (rc = rl_upload(e, invstd, &dst[1])) || (rc = rl_upload(e, *w, &dst[2])) ||
-            (rc = rl_upload(e, *b, &dst[3])))
+        if ((rc = up(&dst[0], *mean)) || (rc = up(&dst[1], invstd)) || (rc = up(&dst[2], *w)) || (rc = up(&dst[3], *b)))
             return rc;
     }
 #undef RL_NEED
@@ -1238,7 +1207,7 @@ int rl_conv(mdk_rl_engine *e, const int8_t *x, int64_t n, int64_t P, int64_t D, 
         rl_mask_kernel<<<(unsigned)(B * D), 256, 0, s>>>(d_x, P, (int)D, (int)F, d_mask);
         if (e->conv_tc) {
             rl_conv17_tc_kernel<<<dim3((unsigned)((P + CT_NPOS - 1) / CT_NPOS), (unsigned)n_groups, (unsigned)B), 256, CT_SMEM, s>>>(
-                d_x, d_mask, c1, c17, e->c17_tc, P, (int)D, (int)F, e->use_dwells, dgroup, d_part);
+                d_x, d_mask, c1, c17, (const uint8_t *)e->c17_tc, P, (int)D, (int)F, e->use_dwells, dgroup, d_part);
         } else {
             rl_embed_conv1_kernel<<<dim3((unsigned)((P + 31) / 32), (unsigned)(B * D)), RL_C, 0, s>>>(d_x, d_mask, c1, P, (int)D, (int)F,
                                                                                                  e->use_dwells, d_y1);
@@ -1276,19 +1245,19 @@ int rl_run_group(mdk_rl_engine *e) {
         const int in = l == 0 ? e->H : 2 * e->H;
         if (h384 && e->lstm_tc) {
             MDK_CUDA(cudaFuncSetAttribute(rl_proj_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PJ_SMEM));
-            rl_proj_tc_kernel<<<dim3((unsigned)((BP + PJ_N - 1) / PJ_N), G8 / PJ_M), 256, PJ_SMEM, s>>>(layer_in, L.w_ih_tc, L.bias,
-                                                                                                     d_gi, BP, in, G8);
+            rl_proj_tc_kernel<<<dim3((unsigned)((BP + PJ_N - 1) / PJ_N), G8 / PJ_M), 256, PJ_SMEM, s>>>(
+                layer_in, (const uint8_t *)L.w_ih_tc, L.bias, d_gi, BP, in, G8);
         } else {
             MDK_CUDA(launch_gemm_fp32(layer_in, L.w_ih, L.bias, d_gi, BP, in, G8, s));
         }
         rl_mark(e, 2 + 2 * l);
         if (h384 && e->lstm_tc) {
             rl_lstm384_tc_kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N * L3_CL), 2), L3_THREADS, L3_SMEM, s>>>(
-                d_gi, L.w_hi, L.w_lo, layer_out[l], B, P);
+                d_gi, L.w_hi, (const uint8_t *)L.w_lo, layer_out[l], B, P);
         } else if (e->lstm_tc) {
             MDK_CUDA(cudaFuncSetAttribute(rl_lstm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LT_SMEM));
-            rl_lstm_tc_kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N), 2), LT_THREADS, LT_SMEM, s>>>(d_gi, L.w_hi, L.w_lo,
-                                                                                                  layer_out[l], B, P);
+            rl_lstm_tc_kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N), 2), LT_THREADS, LT_SMEM, s>>>(
+                d_gi, L.w_hi, (const uint8_t *)L.w_lo, layer_out[l], B, P);
         } else if (h384) {
             rl_lstm_fp32<RL_H3><<<grid_fp32, RL_H3, 0, s>>>(d_gi, L.w_t, layer_out[l], B, P);
         } else {
@@ -1386,11 +1355,10 @@ int mdk_rl_destroy(mdk_rl_engine *e) {
             if (ev) cudaEventDestroy(ev);
     for (cudaEvent_t ev : {e->ev_xin[0], e->ev_xin[1], e->ev_xfree[0], e->ev_xfree[1]})
         if (ev) cudaEventDestroy(ev);
-    for (void *p : e->allocs) cudaFree(p);
     for (void *p : {(void *)e->xbuf[0], (void *)e->xbuf[1], (void *)e->conv, (void *)e->z, (void *)e->gi, (void *)e->h0,
                     (void *)e->h1, (void *)e->probs, (void *)e->labels})
         if (p) cudaFree(p);
-    delete e;
+    delete e;     // and with it the weights (DeviceWeights)
     cudaGetLastError();
     return MDK_OK;
 }

@@ -168,6 +168,29 @@ def test_fused_and_unfused_head_agree():
     m.close()
 
 
+@pytest.mark.parametrize("precision", ["fp32", "tc"])
+@pytest.mark.parametrize("F", [10, 20])
+def test_weight_reload_matches_fresh_model(precision, F):
+    """Loading model B into an engine that has run model A rewrites every weight array the kernels read: its forward is
+    bit for bit a fresh model B's, activations included."""
+    sd_a, sd_b = synth.synth_state_dict(1, num_features=F), synth.synth_state_dict(2, num_features=F)
+    feats = synth.synth_features(37, 65, F, seed=9)
+
+    def forward_b(first):
+        m = _make_model(first, F, precision)
+        m.keep_activations(True)
+        if first is not sd_b:
+            m.forward_arrays(feats, want_logits=True)
+            m.load_state_dict(sd_b)
+        out = m.forward_arrays(feats, want_logits=True, want_labels=True)
+        res = (out.probs, out.logits, out.labels, m.read_activation(0), m.read_activation(1))
+        m.close()
+        return res
+
+    for reloaded, fresh in zip(forward_b(sd_a), forward_b(sd_b)):
+        assert np.array_equal(reloaded, fresh)
+
+
 def test_predict_on_batch_interface():
     """TorchModel.predict_on_batch contract (medaka/models.py:303-313): CPU float32 tensor [B,T,5]."""
     import torch
