@@ -166,6 +166,10 @@ int mdk_engine_timer_stop(mdk_engine *e, float *elapsed_ms);
 /* debugging / layer-wise parity: copy an internal activation of the last forward to host.
  * which: 0 = layer-0 output [B][T][2H] fp32, 1 = layer-1 output [B][T][2H] fp32 */
 int mdk_engine_read_activation(mdk_engine *e, int which, float *out_host, int64_t n_floats);
+/* the same for windows first .. first + count - 1 only: out_host is [count][T][2H] (a full 1056 x 10 000 group's layer
+ * output is 10.8 GB) */
+int mdk_engine_read_activation_windows(mdk_engine *e, int which, int64_t first, int64_t count, float *out_host,
+                                       int64_t n_floats);
 /* keep != 0: leave the layer-1 output in HBM (for mdk_engine_read_activation(e, 1, ...)) by running the 5-class head as
  * its own kernel; default 0: the tensor-core path fuses the head into the layer-1 recurrence */
 int mdk_engine_keep_activations(mdk_engine *e, int keep);

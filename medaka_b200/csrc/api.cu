@@ -657,25 +657,33 @@ int mdk_engine_timer_stop(mdk_engine *e, float *elapsed_ms) {
 }
 
 int mdk_engine_read_activation(mdk_engine *e, int which, float *out_host, int64_t n_floats) {
+    MDK_REQUIRE(e, MDK_ERR_ARG, "engine is NULL");
+    return mdk_engine_read_activation_windows(e, which, 0, e->ws[e->last_ws].last_B, out_host, n_floats);
+}
+
+int mdk_engine_read_activation_windows(mdk_engine *e, int which, int64_t first, int64_t count, float *out_host,
+                                       int64_t n_floats) {
     MDK_REQUIRE(e && out_host, MDK_ERR_ARG, "NULL argument");
     MDK_REQUIRE(which == 0 || which == 1, MDK_ERR_ARG, "read_activation: which must be 0 or 1");
     mdk_ws &ln = e->ws[e->last_ws];
-    const int64_t P = ln.last_B * ln.last_T;
-    MDK_REQUIRE(P > 0 && n_floats == P * H2, MDK_ERR_ARG, "read_activation: size must be B*T*256 of the last forward");
+    MDK_REQUIRE(ln.last_B > 0 && ln.last_T > 0, MDK_ERR_STATE, "read_activation: no forward recorded");
+    MDK_REQUIRE(first >= 0 && count > 0 && first + count <= ln.last_B, MDK_ERR_ARG,
+                "read_activation: windows first .. first + count - 1 must lie in the last forward's B windows");
+    MDK_REQUIRE(n_floats == count * ln.last_T * H2, MDK_ERR_ARG, "read_activation: size must be count*T*256");
     MDK_REQUIRE(!(which == 1 && ln.last_fused_head), MDK_ERR_STATE,
                 "read_activation(1): the last forward fused the head into layer 1 (h1 never reached HBM); call "
                 "mdk_engine_keep_activations(e, 1) before the forward");
     MDK_CUDA(cudaSetDevice(e->device));
     MDK_CUDA(cudaStreamSynchronize(ln.stream));
     if (ln.last_precision == MDK_PREC_FP32) {
-        MDK_CUDA(cudaMemcpy(out_host, which == 1 ? (const void *)ln.h1 : (const void *)ln.h0,
-                            (size_t)n_floats * sizeof(float), cudaMemcpyDeviceToHost));
+        const float *src = (which == 1 ? ln.h1 : reinterpret_cast<const float *>(ln.h0)) + first * ln.last_T * H2;
+        MDK_CUDA(cudaMemcpy(out_host, src, (size_t)n_floats * sizeof(float), cudaMemcpyDeviceToHost));
     } else {
         // tensor-core path: rows are tile-interleaved (and layer 0 is stored as fp16 hi/lo operand tiles)
         float *tmp = nullptr;
         MDK_CUDA(cudaMalloc(&tmp, (size_t)n_floats * sizeof(float)));
-        cudaError_t err = which == 0 ? launch_unpack_h0(ln.h0, tmp, ln.last_B, ln.last_T, ln.stream)
-                                     : launch_untile_rows(ln.h1, tmp, ln.last_B, ln.last_T, ln.stream);
+        cudaError_t err = which == 0 ? launch_unpack_h0(ln.h0, tmp, first, count, ln.last_T, ln.stream)
+                                     : launch_untile_rows(ln.h1, tmp, first, count, ln.last_T, ln.stream);
         if (err == cudaSuccess) err = cudaStreamSynchronize(ln.stream);
         if (err == cudaSuccess) err = cudaMemcpy(out_host, tmp, (size_t)n_floats * sizeof(float), cudaMemcpyDeviceToHost);
         cudaFree(tmp);

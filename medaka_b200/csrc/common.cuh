@@ -304,8 +304,8 @@ cudaError_t launch_inproj0(const float *feats, const float *w_packed, const floa
                            int64_t P, int F, int64_t T, int tiled, cudaStream_t s);
 cudaError_t launch_head(const float *h1, const float *lin_w, const float *lin_b, int64_t B, int64_t T, int tiled,
                         float *probs, float *logits, uint8_t *labels, cudaStream_t s);
-cudaError_t launch_untile_rows(const float *src_tiled, float *dst, int64_t B, int64_t T, cudaStream_t s);
-cudaError_t launch_unpack_h0(const void *h0_tiles, float *out, int64_t B, int64_t T, cudaStream_t s);
+cudaError_t launch_untile_rows(const float *src_tiled, float *dst, int64_t w0, int64_t nw, int64_t T, cudaStream_t s);
+cudaError_t launch_unpack_h0(const void *h0_tiles, float *out, int64_t w0, int64_t nw, int64_t T, cudaStream_t s);
 // gru_fp32.cu
 cudaError_t launch_rec_fp32(const float *gi, const float *w_hh_t, const float *b_hn, float *h_out, int64_t B,
                             int64_t T, cudaStream_t s);

@@ -260,11 +260,13 @@ cudaError_t launch_head_plog(const float *plog, const float *lin_b, int64_t B, i
     return cudaGetLastError();
 }
 
-// fp16 hi/lo activation tiles (tile-interleaved rows) -> fp32 [B*T][256] in position order (debug / layer-wise parity)
-__global__ void unpack_h0_kernel(const __half *__restrict__ tiles, float *__restrict__ out, int64_t B, int64_t T) {
+// fp16 hi/lo activation tiles (tile-interleaved rows) -> fp32 [nw*T][256] in position order: windows w0 .. w0 + nw - 1
+// (debug / layer-wise parity)
+__global__ void unpack_h0_kernel(const __half *__restrict__ tiles, float *__restrict__ out, int64_t w0, int64_t nw,
+                                 int64_t T) {
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (i >= B * T * H2) return;
-    const int64_t p = i / H2;
+    if (i >= nw * T * H2) return;
+    const int64_t p = w0 * T + i / H2;
     const int k = (int)(i % H2);
     const int64_t row = tiled_row(p / T, p % T, T);
     const int64_t tile = row / XT_ROWS;
@@ -274,25 +276,27 @@ __global__ void unpack_h0_kernel(const __half *__restrict__ tiles, float *__rest
     out[i] = __half2float(base[off]) + __half2float(base[XT_PLANE_BYTES / 2 + off]);
 }
 
-cudaError_t launch_unpack_h0(const void *h0_tiles, float *out, int64_t B, int64_t T, cudaStream_t s) {
-    const int64_t n = B * T * H2;
+cudaError_t launch_unpack_h0(const void *h0_tiles, float *out, int64_t w0, int64_t nw, int64_t T, cudaStream_t s) {
+    const int64_t n = nw * T * H2;
     if (n == 0) return cudaSuccess;
-    unpack_h0_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(reinterpret_cast<const __half *>(h0_tiles), out, B, T);
+    unpack_h0_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(reinterpret_cast<const __half *>(h0_tiles), out, w0, nw, T);
     return cudaGetLastError();
 }
 
-// fp32 [rows'][256] in tile-interleaved order -> [B*T][256] in position order (debug / layer-wise parity)
-__global__ void untile_rows_kernel(const float *__restrict__ src, float *__restrict__ dst, int64_t B, int64_t T) {
+// fp32 [rows'][256] in tile-interleaved order -> [nw*T][256] in position order: windows w0 .. w0 + nw - 1 (debug /
+// layer-wise parity)
+__global__ void untile_rows_kernel(const float *__restrict__ src, float *__restrict__ dst, int64_t w0, int64_t nw,
+                                   int64_t T) {
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (i >= B * T * H2) return;
-    const int64_t p = i / H2;
+    if (i >= nw * T * H2) return;
+    const int64_t p = w0 * T + i / H2;
     dst[i] = src[tiled_row(p / T, p % T, T) * H2 + (i % H2)];
 }
 
-cudaError_t launch_untile_rows(const float *src_tiled, float *dst, int64_t B, int64_t T, cudaStream_t s) {
-    const int64_t n = B * T * H2;
+cudaError_t launch_untile_rows(const float *src_tiled, float *dst, int64_t w0, int64_t nw, int64_t T, cudaStream_t s) {
+    const int64_t n = nw * T * H2;
     if (n == 0) return cudaSuccess;
-    untile_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(src_tiled, dst, B, T);
+    untile_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(src_tiled, dst, w0, nw, T);
     return cudaGetLastError();
 }
 

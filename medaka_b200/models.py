@@ -326,14 +326,26 @@ class GRUModel(object):
         return {k: getattr(t, k) for k in ("h2d_ms", "inproj0_ms", "rec0_ms", "inproj1_ms", "rec1_ms",
                                              "head_ms", "d2h_ms", "total_ms", "launches")}
 
-    def read_activation(self, which):
-        """Layer output [B,T,256] of the last forward (0 = layer 0, 1 = layer 1) for layer-wise parity."""
+    def read_activation(self, which, first=0, count=None):
+        """Layer output [count,T,256] of windows first .. first + count - 1 (default: all B) of the last forward (0 = layer
+        0, 1 = layer 1) for layer-wise parity."""
         t = self.last_timings()  # syncs
         del t
         shape = self._last_shape
-        out = np.empty((shape[0], shape[1], 2 * self.gru_size), dtype=np.float32)
-        _lm.check(_lm.lib.mdk_engine_read_activation(
-            self._engine, which, _lm.ffi.cast("float *", _lm.ffi.from_buffer(out)), out.size))
+        count = shape[0] - first if count is None else count
+        out = np.empty((count, shape[1], 2 * self.gru_size), dtype=np.float32)
+        _lm.check(_lm.lib.mdk_engine_read_activation_windows(
+            self._engine, which, first, count, _lm.ffi.cast("float *", _lm.ffi.from_buffer(out)), out.size))
+        return out
+
+    def read_plog(self):
+        """Partial logits of the last forward on the fused-head path, float32 [2 directions][tiles][T][5 classes][16
+        windows] (mdk_debug_read_plog): what the layer-1 recurrence writes in place of h1."""
+        t = self.last_timings()  # syncs
+        del t
+        B, T = self._last_shape
+        out = np.empty((2, (B + 15) // 16, T, 5, 16), dtype=np.float32)
+        _lm.check(_lm.lib.mdk_debug_read_plog(self._engine, _lm.ffi.cast("float *", _lm.ffi.from_buffer(out)), out.size))
         return out
 
     def launch_count(self):

@@ -139,6 +139,7 @@ def test_forward_pingpong_path(B, T, F, rec_mode):
     ref_probs, ref_logits = gru_oracle.predict_on_batch(gru_oracle.build(sd, num_features=F), feats)
     m = _make_model(sd, F, "tc")
     m.set_rec_mode(rec_mode)
+    m.set_group_windows(B)      # one forward of all B windows (the default group of 1056 would split them)
     out = m.forward_arrays(feats, want_logits=True)
     err = _scaled_err(out.logits, ref_logits)
     flips, tie_flips, ties = label_parity(out.labels, ref_probs)
