@@ -139,6 +139,15 @@ int mdk_engine_forward(mdk_engine *e, const float *feats_host, int64_t B, int64_
 int mdk_engine_submit(mdk_engine *e, const float *feats_host, int64_t B, int64_t T,
                       float *probs_host, float *logits_host, uint8_t *labels_host, int64_t *ticket);
 int mdk_engine_wait(mdk_engine *e, int64_t ticket);
+/* one-pass consensus: the same forward, but what leaves the engine is the decoded call per position instead of the
+ * probabilities - labels_out uint8 [B][T] (argmax, first max wins) and quals_out uint8 [B][T] (phred+33 byte of the
+ * winning probability, min(70, -10 log10(clip(1 - p_max, 1e-7, 1))), or NULL), 2 B instead of 20 B per position.  Both
+ * are computed by the engine's head from the fp32 probability it produces, and are bit-identical to
+ * mdk_decode_consensus on the probabilities mdk_engine_submit returns for the same features.  feats and the outputs
+ * may each be host or device memory.  Packed like mdk_engine_submit (decoded and ordinary calls share groups);
+ * complete after mdk_engine_wait(ticket) or mdk_engine_sync. */
+int mdk_engine_submit_decoded(mdk_engine *e, const float *feats, int64_t B, int64_t T,
+                              uint8_t *labels_out, uint8_t *quals_out, int64_t *ticket);
 /* launch the group that is still collecting batches (if any) without waiting for it */
 int mdk_engine_flush(mdk_engine *e);
 /* most windows coalesced into one group; 0 (default) = one wave, 1 = never coalesce */
@@ -372,6 +381,16 @@ int mdk_stitch_consensus(int device, const float *const *seg_probs, const int64_
                          uint8_t *seq_out, uint8_t *qual_out, int64_t *seg_out_off);
 int mdk_stitch_consensus_dev(int device, const float *probs_dev, int64_t n_rows, const int64_t *seg_base,
                              int64_t n_seg, uint8_t *seq_out_dev, uint8_t *qual_out_dev, int64_t *seg_out_off);
+/* The same stitch on decoded outputs already on the device (mdk_engine_submit_decoded): segment k is the rows
+ * [seg_start[k], seg_start[k] + seg_rows[k]) of labels_dev / quals_dev (quals_dev may be NULL), seg_rows[k] > 0; every
+ * row lies inside the allocations labels_dev and quals_dev point into.
+ * Segments may come in any order and overlap.  seg_start, seg_rows and seg_out_off are host arrays; seq_out / qual_out
+ * are host buffers of capacity sum(seg_rows) (qual_out may be NULL).  Runs on the legacy stream: the engine that wrote
+ * the arena must have been synchronised (mdk_engine_sync).  Equal byte for byte to mdk_stitch_consensus on the
+ * probabilities the labels / quals were derived from. */
+int mdk_stitch_labels_dev(int device, const uint8_t *labels_dev, const uint8_t *quals_dev,
+                          const int64_t *seg_start, const int64_t *seg_rows, int64_t n_seg,
+                          uint8_t *seq_out, uint8_t *qual_out, int64_t *seg_out_off);
 
 /* variant_columns (src/medaka_rnn_variants.h:26, called at medaka/labels.py:869-887): which pileup columns belong
  * to a variant run.  minor [len] pileup minor indices; reference / prediction [len] one byte per column (the

@@ -135,8 +135,8 @@ static int ensure_io(mdk_engine *e, mdk_lane &ln, int64_t B, int64_t T) {
     MDK_CUDA(cudaStreamSynchronize(ln.ws->stream));
     MDK_CUDA(cudaStreamSynchronize(e->copy_in));
     MDK_CUDA(cudaStreamSynchronize(e->copy_out.stream));
-    ln.cap_io = 0; ln.cap_feats = 0;
-    dev_free(ln.d_feats); dev_free(ln.d_probs); dev_free(ln.d_logits); dev_free(ln.d_labels);
+    ln.cap_io = 0; ln.cap_feats = 0; ln.cap_quals = 0;
+    dev_free(ln.d_feats); dev_free(ln.d_probs); dev_free(ln.d_logits); dev_free(ln.d_labels); dev_free(ln.d_quals);
     int rc;
     if ((rc = dev_alloc(&ln.d_feats, (size_t)feats))) return rc;
     if ((rc = dev_alloc(&ln.d_probs, (size_t)P * NCLS))) return rc;
@@ -146,9 +146,22 @@ static int ensure_io(mdk_engine *e, mdk_lane &ln, int64_t B, int64_t T) {
     return MDK_OK;
 }
 
+// d_quals (1 B / position) only exists on lanes that have run a decoded call (mdk_engine_submit_decoded): allocated
+// when the group being launched needs it.  The lane's previous group has left it (acquire_lane), and ensure_io, which
+// frees it on growth, synchronises first.
+static int ensure_quals(mdk_lane &ln) {
+    if (ln.cap_quals >= ln.cap_io && ln.d_quals) return MDK_OK;
+    dev_free(ln.d_quals);
+    ln.cap_quals = 0;
+    int rc;
+    if ((rc = dev_alloc(&ln.d_quals, (size_t)ln.cap_io))) return rc;
+    ln.cap_quals = ln.cap_io;
+    return MDK_OK;
+}
+
 // The forward pipeline on the workspace's stream.  ev[1..6] bracket the stages for mdk_timings.
 static int run_forward(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int64_t B, int64_t T, float *probs_dev,
-                       float *logits_dev, uint8_t *labels_dev) {
+                       float *logits_dev, uint8_t *labels_dev, uint8_t *quals_dev) {
     int rc;
     if ((rc = prepare_weights(e))) return rc;
     if ((rc = ensure_workspace(e, ws, B, T))) return rc;
@@ -195,8 +208,8 @@ static int run_forward(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int64_
     }
     launches++;
     MDK_CUDA(cudaEventRecord(e->ev[5], s));
-    if (fuse_head) MDK_CUDA(launch_head_plog(ws.plog, e->lin_b, B, T, probs_dev, logits_dev, labels_dev, s));
-    else MDK_CUDA(launch_head(ws.h1, e->lin_w, e->lin_b, B, T, tc ? 1 : 0, probs_dev, logits_dev, labels_dev, s));
+    if (fuse_head) MDK_CUDA(launch_head_plog(ws.plog, e->lin_b, B, T, probs_dev, logits_dev, labels_dev, s, quals_dev));
+    else MDK_CUDA(launch_head(ws.h1, e->lin_w, e->lin_b, B, T, tc ? 1 : 0, probs_dev, logits_dev, labels_dev, s, quals_dev));
     launches++;
     MDK_CUDA(cudaEventRecord(e->ev[6], s));
     e->launches += launches;
@@ -257,9 +270,12 @@ struct GruCall {
     int launch() {
         mdk_lane &ln = e->lane[e->open_lane];
         const Packing &pk = e->pk;
-        bool logits = false, labels = false;      // whether any call wants them
-        for (const Packing::Piece &p : pk.pieces) { logits = logits || p.logits; labels = labels || p.labels; }
+        bool logits = false, labels = false, quals = false;      // whether any call wants them
+        for (const Packing::Piece &p : pk.pieces) {
+            logits = logits || p.logits; labels = labels || p.labels; quals = quals || p.quals;
+        }
         int rc;
+        if (quals && (rc = ensure_quals(ln))) return rc;
         cudaStream_t s = ln.ws->stream;
         e->ev = e->evr[e->fwd_count % mdk_engine::EV_RING];
         e->fwd_count++;
@@ -267,10 +283,10 @@ struct GruCall {
         MDK_CUDA(cudaEventRecord(ln.ev_in, e->copy_in));      // every feature copy of the group was queued on copy_in
         MDK_CUDA(cudaStreamWaitEvent(s, ln.ev_in, 0));
         if ((rc = run_forward(e, *ln.ws, ln.d_feats, pk.windows, pk.len, ln.d_probs, logits ? ln.d_logits : nullptr,
-                              labels ? ln.d_labels : nullptr)))
+                              labels ? ln.d_labels : nullptr, quals ? ln.d_quals : nullptr)))
             return rc;
         MDK_CUDA(cudaEventRecord(e->ev[7], s));
-        if ((rc = copy_back(e->copy_out, pk, s, ln.d_probs, ln.d_logits, ln.d_labels))) return rc;
+        if ((rc = copy_back(e->copy_out, pk, s, ln.d_probs, ln.d_logits, ln.d_labels, ln.d_quals))) return rc;
         MDK_CUDA(cudaEventRecord(ln.ev_out, e->copy_out.stream));
         ln.busy = true;
         return MDK_OK;
@@ -420,7 +436,7 @@ int mdk_engine_destroy(mdk_engine *e) {
         if (ws.stream) cudaStreamDestroy(ws.stream);
     }
     for (auto &ln : e->lane) {
-        dev_free(ln.d_feats); dev_free(ln.d_probs); dev_free(ln.d_logits); dev_free(ln.d_labels);
+        dev_free(ln.d_feats); dev_free(ln.d_probs); dev_free(ln.d_logits); dev_free(ln.d_labels); dev_free(ln.d_quals);
         if (ln.ev_in) cudaEventDestroy(ln.ev_in);
         if (ln.ev_out) cudaEventDestroy(ln.ev_out);
     }
@@ -535,6 +551,17 @@ int mdk_engine_submit(mdk_engine *e, const float *feats_host, int64_t B, int64_t
     MDK_REQUIRE(ticket, MDK_ERR_ARG, "submit: ticket is NULL");
     MDK_CUDA(cudaSetDevice(e->device));
     return e->pk.enqueue(GruCall{e, feats_host, B, T}, B, T, probs_host, logits_host, labels_host, group_limit(e), ticket);
+}
+
+int mdk_engine_submit_decoded(mdk_engine *e, const float *feats, int64_t B, int64_t T, uint8_t *labels_out,
+                              uint8_t *quals_out, int64_t *ticket) {
+    MDK_REQUIRE(e != nullptr, MDK_ERR_ARG, "engine is NULL");
+    MDK_REQUIRE(feats != nullptr && labels_out != nullptr, MDK_ERR_ARG, "submit_decoded: feats/labels must not be NULL");
+    MDK_REQUIRE(B >= 1 && T >= 1, MDK_ERR_ARG, "submit_decoded: need B >= 1 and T >= 1");
+    MDK_REQUIRE(B * T < (int64_t)1 << 40, MDK_ERR_ARG, "submit_decoded: B*T too large");
+    MDK_REQUIRE(ticket, MDK_ERR_ARG, "submit_decoded: ticket is NULL");
+    MDK_CUDA(cudaSetDevice(e->device));
+    return e->pk.enqueue(GruCall{e, feats, B, T}, B, T, nullptr, nullptr, labels_out, group_limit(e), ticket, quals_out);
 }
 
 int mdk_engine_flush(mdk_engine *e) {

@@ -196,19 +196,20 @@ inline void destroy_copy_out(CopyOut &co) {
     for (cudaEvent_t ev : co.ev) if (ev) cudaEventDestroy(ev);
 }
 
-// Once the work queued on `compute` is done, per piece of the group being launched: the probabilities, and the logits
-// and labels where the piece has them, from the group's buffers to the call's (host or device); then ev[pk.serial].
+// Once the work queued on `compute` is done, per piece of the group being launched: the probabilities, logits, labels
+// and qualities the piece has, from the group's buffers to the call's (host or device); then ev[pk.serial].
 inline int copy_back(CopyOut &co, const Packing &pk, cudaStream_t compute, const float *probs, const float *logits,
-                     const uint8_t *labels) {
+                     const uint8_t *labels, const uint8_t *quals = nullptr) {
     MDK_CUDA(cudaEventRecord(co.done, compute));
     MDK_CUDA(cudaStreamWaitEvent(co.stream, co.done, 0));
     int64_t w0 = 0;
     for (const Packing::Piece &p : pk.pieces) {
         const size_t n = (size_t)p.n * pk.len, dst = (size_t)p.first * pk.len, src = (size_t)w0 * pk.len;
         const size_t bytes = n * NCLS * sizeof(float);
-        MDK_CUDA(cudaMemcpyAsync(p.probs + dst * NCLS, probs + src * NCLS, bytes, cudaMemcpyDefault, co.stream));
+        if (p.probs) MDK_CUDA(cudaMemcpyAsync(p.probs + dst * NCLS, probs + src * NCLS, bytes, cudaMemcpyDefault, co.stream));
         if (p.logits) MDK_CUDA(cudaMemcpyAsync(p.logits + dst * NCLS, logits + src * NCLS, bytes, cudaMemcpyDefault, co.stream));
         if (p.labels) MDK_CUDA(cudaMemcpyAsync(p.labels + dst, labels + src, n, cudaMemcpyDefault, co.stream));
+        if (p.quals) MDK_CUDA(cudaMemcpyAsync(p.quals + dst, quals + src, n, cudaMemcpyDefault, co.stream));
         w0 += p.n;
     }
     MDK_CUDA(cudaEventRecord(co.ev[pk.serial % CopyOut::RING], co.stream));
@@ -253,9 +254,10 @@ struct mdk_lane {
     mdk_ws *ws = nullptr;      // where the lane's groups compute (fixed at engine creation)
     // device staging of the group's calls (their buffers may be host or device memory)
     int64_t cap_io = 0;        // positions
+    int64_t cap_quals = 0;     // positions of d_quals (allocated for decoded calls only)
     int64_t cap_feats = 0;     // floats
     float *d_feats = nullptr, *d_probs = nullptr, *d_logits = nullptr;
-    uint8_t *d_labels = nullptr;
+    uint8_t *d_labels = nullptr, *d_quals = nullptr;
     cudaEvent_t ev_in = nullptr, ev_out = nullptr;
     bool busy = false;         // ev_out marks a group the lane has not been reclaimed from
 };
@@ -302,8 +304,9 @@ namespace mdk {
 // tiled != 0: gi rows are written / h1 rows are read in tile-interleaved order (T = window length)
 cudaError_t launch_inproj0(const float *feats, const float *w_packed, const float *bias, float *gi,
                            int64_t P, int F, int64_t T, int tiled, cudaStream_t s);
+// quals (may be null): phred bytes of the argmax class (phred.cuh), from the probability the head writes
 cudaError_t launch_head(const float *h1, const float *lin_w, const float *lin_b, int64_t B, int64_t T, int tiled,
-                        float *probs, float *logits, uint8_t *labels, cudaStream_t s);
+                        float *probs, float *logits, uint8_t *labels, cudaStream_t s, uint8_t *quals = nullptr);
 cudaError_t launch_untile_rows(const float *src_tiled, float *dst, int64_t w0, int64_t nw, int64_t T, cudaStream_t s);
 cudaError_t launch_unpack_h0(const void *h0_tiles, float *out, int64_t w0, int64_t nw, int64_t T, cudaStream_t s);
 // gru_fp32.cu
@@ -327,9 +330,10 @@ enum { OUT_TILES = 0, OUT_ROWS = 1, OUT_LOGITS = 2 };
 // projection (OUT_TILES only), or nullptr to read the pre-activations from gi.  out: h0 tiles, h1 rows or plog (out_kind).
 cudaError_t launch_rec_tc(const float *gi, const RecX *xin, const __half *w_hh_tm, const float *b_hn, int tiles_per_cta,
                           int out_kind, void *out, const float *lin_w, int64_t B, int64_t T, cudaStream_t s);
-// head on the partial logits of the fused path: sum of the two directions + bias -> softmax / argmax
+// head on the partial logits of the fused path: sum of the two directions + bias -> softmax / argmax (/ quals, as
+// launch_head)
 cudaError_t launch_head_plog(const float *plog, const float *lin_b, int64_t B, int64_t T, float *probs, float *logits,
-                             uint8_t *labels, cudaStream_t s);
+                             uint8_t *labels, cudaStream_t s, uint8_t *quals = nullptr);
 constexpr int PLOG_TS_FLOATS = NCLS * WT;     // 80 floats per (tile-step, direction)
 cudaError_t launch_gemm_tc(const void *x_tiles, const __half *w_in_tm, const float *bias, float *gi, int64_t P,
                            int sm_count, cudaStream_t s);

@@ -16,6 +16,8 @@
 //   stitch_scatter_kernel   stable compaction: survivors move to block_base + rank-in-block; the first row of every
 //                           range records where that range's output starts
 // HBM-bound byte work: 20 B read per row + 2 B scratch written, 2 B scratch read + <= 2 B written.
+// From the engine's decoded outputs (labels and quality bytes in device memory, mdk_stitch_labels_dev) the first launch
+// is stitch_gather_kernel instead: the ranges' rows are gathered from wherever they lie (2 B read per row).
 //
 // Variant decoding (medaka/labels.py:889-1014 `decode_variants`, per joined sample): argmax-decode the [n,5] label
 // probabilities keeping gaps, lay the draft out with '*' on insertion columns, mark the variant columns, cut them into
@@ -30,20 +32,13 @@
 //   vd_runs_kernel       the k-th run start walks its run: length and the two left-to-right float32 sums
 // HBM-bound byte work: 29 B read + 10 B written per column in the first kernel, ~12 B per column in the others.
 #include "common.cuh"
+#include "phred.cuh"
 
 #include <vector>
 
 namespace mdk {
 
 namespace {
-
-// labels.py:387-401 on float32: err = clip(1 - p, 1e-7, 1); q = min(-10 log10(err), 70), with the correctly rounded
-// float32 log10
-__device__ __forceinline__ float phred_f32(float p_class) {
-    const float err = fminf(fmaxf(1.0f - p_class, 1e-7f), 1.0f);
-    const float l = __double2float_rn(log10((double)err));
-    return fminf(-10.0f * l, 70.0f);
-}
 
 // src/medaka_rnn_variants.c:28-55: a major column is variant when it mismatches; the minor (insertion) columns that
 // follow it are variant when ANY column of the group - the major or one of its minors - mismatches.  The first column is
@@ -76,7 +71,7 @@ __global__ void __launch_bounds__(256) decode_kernel(const float *__restrict__ p
         if (v > best) { best = v; arg = c; }   // strict '>' : first maximum wins, as np.argmax
     }
     labels[i] = (uint8_t)arg;
-    if (quals) quals[i] = (uint8_t)((int)phred_f32(best) + 33);     // astype('u1') truncation, +33
+    if (quals) quals[i] = phred_char(best);
 }
 
 // float64 probabilities (what numpy computes when label_probs is a float64 array, e.g. the reference's own
@@ -128,6 +123,11 @@ constexpr int ST_THREADS = 256;
 constexpr int ST_ROWS_PER_THREAD = 4;
 constexpr int ST_BLOCK_ROWS = ST_THREADS * ST_ROWS_PER_THREAD;   // 1024 rows per block
 
+// '*ACGT' (labels.py:342); 0 marks a gap call so the byte doubles as the keep flag
+__device__ __forceinline__ uint8_t label_symbol(int label) {
+    return (uint8_t)((0x5447434100ull >> (8 * label)) & 0xff);
+}
+
 __device__ __forceinline__ void decode_row(const float *__restrict__ p, uint8_t &sym, uint8_t &qual) {
     float best = p[0];
     int arg = 0;
@@ -136,9 +136,51 @@ __device__ __forceinline__ void decode_row(const float *__restrict__ p, uint8_t 
         const float v = p[c];
         if (v > best) { best = v; arg = c; }                  // first maximum wins (np.argmax)
     }
-    qual = (uint8_t)((int)phred_f32(best) + 33);
-    // '*ACGT' (labels.py:342); 0 marks a gap call so the byte doubles as the keep flag
-    sym = (uint8_t)((0x5447434100ull >> (8 * arg)) & 0xff);
+    qual = phred_char(best);
+    sym = label_symbol(arg);
+}
+
+// Gather for mdk_stitch_labels_dev: concatenated row r of the call lies in segment k (seg_base[k] <= r < seg_base[k+1])
+// at arena row seg_start[k] + r - seg_base[k].  Writes what stitch_decode_kernel writes (symbol | 0, quality, per-block
+// survivor count), so that stitch_scatter_kernel compacts either.  Thread t owns rows [base + 4t, base + 4t + 4).
+__global__ void __launch_bounds__(ST_THREADS) stitch_gather_kernel(const uint8_t *__restrict__ labels,
+                                                                   const uint8_t *__restrict__ quals,
+                                                                   const int64_t *__restrict__ seg_start,
+                                                                   const int64_t *__restrict__ seg_base, int64_t n_seg,
+                                                                   int64_t n, uint8_t *__restrict__ sym,
+                                                                   uint8_t *__restrict__ qual,
+                                                                   int64_t *__restrict__ block_count) {
+    __shared__ uint32_t warp_cnt[ST_THREADS / 32];
+    const int64_t r0 = (int64_t)blockIdx.x * ST_BLOCK_ROWS + (int64_t)threadIdx.x * ST_ROWS_PER_THREAD;
+    uint32_t kept = 0;
+    if (r0 < n) {
+        int64_t lo = 0, hi = n_seg;     // last segment starting at or before r0
+        while (hi - lo > 1) {
+            const int64_t mid = (lo + hi) >> 1;
+            if (seg_base[mid] <= r0) lo = mid; else hi = mid;
+        }
+        int64_t k = lo;
+        for (int j = 0; j < ST_ROWS_PER_THREAD && r0 + j < n; ++j) {
+            const int64_t r = r0 + j;
+            while (k + 1 < n_seg && seg_base[k + 1] <= r) ++k;
+            const int64_t a = seg_start[k] + (r - seg_base[k]);
+            const uint8_t l = labels[a];
+            const uint8_t s = l < NCLS ? label_symbol(l) : 0;
+            sym[r] = s;
+            qual[r] = quals ? quals[a] : 0;
+            kept += (s != 0);
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) kept += __shfl_xor_sync(0xffffffffu, kept, o);
+    if ((threadIdx.x & 31) == 0) warp_cnt[threadIdx.x >> 5] = kept;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint32_t t = 0;
+#pragma unroll
+        for (int w = 0; w < ST_THREADS / 32; ++w) t += warp_cnt[w];
+        block_count[blockIdx.x] = t;
+    }
 }
 
 // Thread t of a block owns rows [base + 4t, base + 4t + 4): the four outputs are one 32-bit store.
@@ -476,6 +518,53 @@ int mdk_stitch_consensus(int device, const float *const *seg_probs, const int64_
     if (rc) return rc;
     st.out(seq_out, d_seq, seg_out_off[n_seg]);
     if (qual_out) st.out(qual_out, d_qual, seg_out_off[n_seg]);
+    return st.result();
+}
+
+// Segments are row ranges of the engine's decoded outputs (mdk_engine_submit_decoded) anywhere in device memory; they are
+// concatenated in call order, gathered into the stitch scratch and compacted by the kernels mdk_stitch_consensus runs.
+int mdk_stitch_labels_dev(int device, const uint8_t *labels_dev, const uint8_t *quals_dev, const int64_t *seg_start,
+                          const int64_t *seg_rows, int64_t n_seg, uint8_t *seq_out, uint8_t *qual_out,
+                          int64_t *seg_out_off) {
+    MDK_REQUIRE(n_seg >= 0, MDK_ERR_ARG, "stitch_labels: n_seg < 0");
+    MDK_REQUIRE(seg_out_off, MDK_ERR_ARG, "stitch_labels: NULL seg_out_off");
+    if (n_seg == 0) { seg_out_off[0] = 0; return MDK_OK; }
+    MDK_REQUIRE(labels_dev && seg_start && seg_rows && seq_out, MDK_ERR_ARG, "stitch_labels: NULL pointer");
+    std::vector<int64_t> base((size_t)n_seg);
+    int64_t n = 0;
+    for (int64_t k = 0; k < n_seg; ++k) {
+        MDK_REQUIRE(seg_rows[k] > 0, MDK_ERR_ARG, "stitch_labels: every segment needs rows > 0");
+        base[(size_t)k] = n;
+        n += seg_rows[k];
+    }
+    MDK_CUDA(cudaSetDevice(device));
+    const int64_t n_blocks = (n + ST_BLOCK_ROWS - 1) / ST_BLOCK_ROWS;
+    const int64_t n4 = (n + 3) & ~(int64_t)3;      // whole 32-bit loads of four rows in the scatter
+    Staging st(Blob::STAGING, "stitch_labels_dev");
+    const int64_t *d_start, *d_seg;
+    int64_t *d_off, *d_base;
+    uint8_t *d_sym, *d_qual, *d_seq, *d_qout = nullptr;
+    st.in(&d_start, seg_start, n_seg);
+    st.in(&d_seg, base.data(), n_seg);
+    st.take(&d_off, n_seg + 1);
+    st.take(&d_base, n_blocks + 1);
+    st.take(&d_sym, n4);
+    st.take(&d_qual, n4);
+    st.take(&d_seq, n);
+    if (qual_out) st.take(&d_qout, n);
+    if (!st.alloc()) return st.result();
+    stitch_gather_kernel<<<(unsigned)n_blocks, ST_THREADS, 0, 0>>>(labels_dev, quals_dev, d_start, d_seg, n_seg, n,
+                                                                   d_sym, d_qual, d_base);
+    st.check(cudaGetLastError());
+    st.check(launch_scan_blocks(d_base, n_blocks, 0));
+    stitch_scatter_kernel<<<(unsigned)n_blocks, ST_THREADS, 0, 0>>>(d_sym, d_qual, n, d_base, d_seg, n_seg, d_seq,
+                                                                    d_qout, d_off);
+    st.check(cudaGetLastError());
+    if (st.ok()) st.check(cudaMemcpyAsync(d_off + n_seg, d_base + n_blocks, sizeof(int64_t), cudaMemcpyDeviceToDevice, 0));
+    st.out(seg_out_off, d_off, n_seg + 1);
+    if (!st.ok()) return st.result();
+    st.out(seq_out, d_seq, seg_out_off[n_seg]);
+    if (qual_out) st.out(qual_out, d_qout, seg_out_off[n_seg]);
     return st.result();
 }
 

@@ -1,6 +1,7 @@
 // The GRU path's small kernels: layer-0 input projection, linear head + softmax + argmax, and the debug unpacking of
 // the tiled intermediates.  All are coalesced / vectorised streaming kernels; none is GEMM-shaped.
 #include "common.cuh"
+#include "phred.cuh"
 #include "ptx.cuh"
 
 namespace mdk {
@@ -88,11 +89,13 @@ cudaError_t launch_inproj0(const float *feats, const float *w_packed, const floa
 // tile-interleaved row(w, t).  Each warp handles 4 positions per iteration: 8 of the 256 inputs per lane, the
 // 4 x 5 (padded to 4 x 8) partial dot products are reduced with a transposing butterfly (31 shuffles for all 32
 // values instead of 5 per value), after which lane L owns logit (position L/8, class L%8) and the softmax / argmax
-// run across the 8-lane groups - one expf per lane instead of five per lane.
+// run across the 8-lane groups - one expf per lane instead of five per lane.  QUALS: also the phred byte of the winning
+// probability (decoded forwards); the instantiation without it is the kernel of the ordinary forward.
+template <bool QUALS>
 __global__ void __launch_bounds__(256) head_kernel(const float *__restrict__ h1, const float *__restrict__ lin_w,
                                                    const float *__restrict__ lin_b, int64_t P, int64_t B, int64_t T,
                                                    int tiled, float *__restrict__ probs, float *__restrict__ logits,
-                                                   uint8_t *__restrict__ labels) {
+                                                   uint8_t *__restrict__ labels, uint8_t *__restrict__ quals) {
     const int lane = threadIdx.x & 31;
     const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -201,25 +204,30 @@ __global__ void __launch_bounds__(256) head_kernel(const float *__restrict__ h1,
                 if (logits) logits[p * NCLS + cls] = logit;
             }
             if (labels && cls == 0) labels[p] = (uint8_t)arg;
+            if (QUALS && cls == 0) quals[p] = phred_char(best);
         }
     }
 }
 
 cudaError_t launch_head(const float *h1, const float *lin_w, const float *lin_b, int64_t B, int64_t T, int tiled,
-                        float *probs, float *logits, uint8_t *labels, cudaStream_t s) {
+                        float *probs, float *logits, uint8_t *labels, cudaStream_t s, uint8_t *quals) {
     const int64_t P = B * T;
     if (P == 0) return cudaSuccess;
     int64_t blocks = (P + 31) / 32;            // 8 warps per block, 4 positions per warp per iteration
     if (blocks > 132 * 8) blocks = 132 * 8;    // persistent-ish grid: multiple of the SM count
-    head_kernel<<<(unsigned)blocks, 256, 0, s>>>(h1, lin_w, lin_b, P, B, T, tiled, probs, logits, labels);
+    if (quals) head_kernel<true><<<(unsigned)blocks, 256, 0, s>>>(h1, lin_w, lin_b, P, B, T, tiled, probs, logits, labels, quals);
+    else head_kernel<false><<<(unsigned)blocks, 256, 0, s>>>(h1, lin_w, lin_b, P, B, T, tiled, probs, logits, labels, nullptr);
     return cudaGetLastError();
 }
 
 // Head of the fused path (gru.py:53-55,67-71): logits = fwd partial + rev partial + bias, softmax, first-max argmax.
 // One thread per (window of the tile, time step); blockIdx.y = window tile.  41 B written per position, 40 B read.
+// QUALS as in head_kernel.
+template <bool QUALS>
 __global__ void __launch_bounds__(256) head_plog_kernel(const float *__restrict__ plog, const float *__restrict__ lin_b,
                                                         int64_t B, int64_t T, int64_t n_ts, float *__restrict__ probs,
-                                                        float *__restrict__ logits, uint8_t *__restrict__ labels) {
+                                                        float *__restrict__ logits, uint8_t *__restrict__ labels,
+                                                        uint8_t *__restrict__ quals) {
     const int64_t wt = blockIdx.y;
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;   // t * 16 + w
     const int64_t t = i >> 4;
@@ -249,14 +257,16 @@ __global__ void __launch_bounds__(256) head_plog_kernel(const float *__restrict_
         if (pr > best) { best = pr; arg = c; }     // first maximum wins (np.argmax, labels.py:1063)
     }
     if (labels) labels[p] = (uint8_t)arg;
+    if (QUALS) quals[p] = phred_char(best);
 }
 
 cudaError_t launch_head_plog(const float *plog, const float *lin_b, int64_t B, int64_t T, float *probs, float *logits,
-                             uint8_t *labels, cudaStream_t s) {
+                             uint8_t *labels, cudaStream_t s, uint8_t *quals) {
     if (B == 0 || T == 0) return cudaSuccess;
     const int64_t tiles = (B + WT - 1) / WT;
     dim3 grid((unsigned)((T * WT + 255) / 256), (unsigned)tiles);
-    head_plog_kernel<<<grid, 256, 0, s>>>(plog, lin_b, B, T, tiles * T, probs, logits, labels);
+    if (quals) head_plog_kernel<true><<<grid, 256, 0, s>>>(plog, lin_b, B, T, tiles * T, probs, logits, labels, quals);
+    else head_plog_kernel<false><<<grid, 256, 0, s>>>(plog, lin_b, B, T, tiles * T, probs, logits, labels, nullptr);
     return cudaGetLastError();
 }
 

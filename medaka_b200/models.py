@@ -255,6 +255,32 @@ class GRUModel(object):
         self._last_shape = (B, T)
         return int(ticket[0])
 
+    def submit_decoded(self, feats_pinned, labels_out, quals_out=None):
+        """Queue one forward whose outputs are the decoded calls (mdk_engine_submit_decoded); returns a ticket.
+
+        ``labels_out`` / ``quals_out`` receive uint8 [B, T] argmax labels and phred+33 quality bytes: numpy arrays,
+        or device addresses (int) of B * T bytes.  ``quals_out`` may be None.  Everything must stay alive and untouched
+        until ``wait(ticket)`` (or ``sync``).
+        """
+        B, T, F = feats_pinned.shape
+        lib, ffi = _lm.lib, _lm.ffi
+
+        def u8(x):
+            if x is None:
+                return ffi.NULL
+            return ffi.cast("uint8_t *", x) if isinstance(x, int) else ffi.cast("uint8_t *", ffi.from_buffer(x))
+
+        ticket = ffi.new("int64_t *")
+        _lm.check(lib.mdk_engine_submit_decoded(
+            self._engine, ffi.cast("const float *", ffi.from_buffer(feats_pinned)), B, T, u8(labels_out), u8(quals_out),
+            ticket))
+        self._last_shape = (B, T)
+        return int(ticket[0])
+
+    def sync(self):
+        """Wait for every call queued on the engine (mdk_engine_sync)."""
+        _lm.check(_lm.lib.mdk_engine_sync(self._engine))
+
     def wait(self, ticket):
         _lm.check(_lm.lib.mdk_engine_wait(self._engine, ticket))
 

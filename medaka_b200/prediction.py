@@ -14,7 +14,9 @@ import queue
 import threading
 from timeit import default_timer as now
 
-from medaka_b200 import common, datastore, features, torch_ext
+import numpy as np
+
+from medaka_b200 import common, datastore, features, libmedaka as _lm, torch_ext
 
 
 def triage_regions(bam_regions, chunk_len, bam_chunk, chunk_ovlp):
@@ -215,3 +217,175 @@ def predict_regions(output, bam, bam_regions, model, feature_encoder, chunk_len=
             logger.warning("{} regions were not processed: {}.".format(
                 len(new_remainders), [x[0] for x in new_remainders]))
     logger.info("Finished processing all regions.")
+
+
+class _LabelArena(object):
+    """Device memory for the decoded calls of a one-pass run (``predict_consensus``): 2 B per computed column.
+
+    Slabs of ``2 * half`` bytes from mdk_dev_alloc hold labels in their first half and quality bytes at the same offset
+    in the second.  A row is (slab index, offset); every stitch call reads from one slab.
+    """
+
+    def __init__(self, device, half=1 << 28):
+        self.device, self.half = device, int(half)
+        self.slabs = []          # device addresses
+        self.used = self.half    # bytes taken from the newest slab's halves
+
+    def take(self, n):
+        """Room for n rows -> (slab index, offset of the first row)."""
+        if n > self.half:
+            raise ValueError("a batch of {} columns does not fit a {} B arena slab".format(n, self.half))
+        if self.used + n > self.half:
+            lib, ffi = _lm.load(), _lm.ffi
+            pp = ffi.new("void **")
+            _lm.check(lib.mdk_dev_alloc(self.device, 2 * self.half, pp))
+            self.slabs.append(int(ffi.cast("uintptr_t", pp[0])))
+            self.used = 0
+        at = self.used
+        self.used += n
+        return len(self.slabs) - 1, at
+
+    def labels(self, slab):
+        return self.slabs[slab]
+
+    def quals(self, slab):
+        return self.slabs[slab] + self.half
+
+    def free(self):
+        lib, ffi = _lm.load(), _lm.ffi
+        while self.slabs:
+            _lm.check(lib.mdk_dev_free(self.device, ffi.cast("void *", self.slabs.pop())))
+
+
+def _stitch_view(sample, min_depth):
+    """What the stitch plan reads of a window, in the smallest exact form: positions as (int32 major unless a major
+    needs more, unsigned minor of the width its largest value needs), and, only when the run filters on depth, depth
+    clipped to min_depth (``depth >= min_depth`` is unchanged).  About 5 B per column instead of the 24 B of the
+    window's int64 positions and depth."""
+    major, minor = sample.positions['major'], sample.positions['minor']
+    big = len(major) and int(major[-1]) >= np.iinfo(np.int32).max
+    pos = np.empty(len(major), dtype=[('major', np.int64 if big else np.int32),
+                                      ('minor', np.min_scalar_type(int(minor.max()) if len(minor) else 0))])
+    pos['major'], pos['minor'] = major, minor
+    depth = None
+    if min_depth:
+        depth = np.minimum(np.asarray(sample.depth), min_depth).astype(np.min_scalar_type(min_depth))
+    return common.Sample(ref_name=sample.ref_name, features=None, labels=None, ref_seq=None, positions=pos,
+                         label_probs=None, depth=depth)
+
+
+def _run_decoded(samples, arena, bam, regions, model, feature_encoder, chunk_len, chunk_ovlp, min_depth,
+                 batch_size=200, enable_chunking=True, bam_workers=2):
+    """``run_prediction`` for ``predict_consensus``: every batch's decoded calls go to the arena, and
+    ``samples[name] = (_stitch_view of the window, arena slab, row in the slab)`` is kept for each window (the first
+    window of a name wins, as in a store).  Returns the remainder regions."""
+    logger = common.get_named_logger('PWorker')
+    if batch_size == "auto":
+        batch_size = model.preferred_batch_size()
+    loader = DataLoader(
+        bam, regions, batch_size, batch_cache_size=8, bam_workers=bam_workers,
+        feature_encoder=feature_encoder, chunk_len=chunk_len, chunk_overlap=chunk_ovlp,
+        enable_chunking=enable_chunking)
+    logger.info("Running one-pass inference for {:.1f}M draft bases.".format(sum(r.size for r in regions) / 1e6))
+    pending = collections.deque()
+    depth = None
+    n_calls = 0
+    for data, batch in loader:
+        x = model.get_model_input_features(batch)
+        x = x.detach().cpu().numpy() if hasattr(x, "detach") else x
+        nb, nt, nf = x.shape
+        if depth is None:
+            depth = model.lookahead(batch_size, nt)
+            if enable_chunking and nb * nt > (1 << 18):
+                model.reserve(max(model.preferred_batch_size(), nb), nt)
+        while len(pending) >= depth:
+            model.wait(pending.popleft())
+        # the page-locked feature slot is reused once the call that last used it has been waited for
+        xin = model.pinned("dfeats%d" % (n_calls % (depth + 1)), (nb, nt, nf), np.float32)
+        np.copyto(xin, x, casting="same_kind")
+        n_calls += 1
+        slab, row = arena.take(nb * nt)
+        pending.append(model.submit_decoded(xin, arena.labels(slab) + row, arena.quals(slab) + row))
+        for i, s in enumerate(data):
+            if len(s.positions) != nt:
+                raise ValueError("sample {} has {} columns in a batch of {}".format(s.name, len(s.positions), nt))
+            name = s.name
+            if name not in samples:
+                samples[name] = (_stitch_view(s, min_depth), slab, row + i * nt)
+    while pending:
+        model.wait(pending.popleft())
+    return loader.remainders
+
+
+def predict_consensus(bam, bam_regions, model, feature_encoder, draft, output, chunk_len=10000, chunk_ovlp=1000,
+                      batch_size=200, bam_chunk=int(1e6), bam_workers=2, regions=None, min_depth=0, fillgaps=True,
+                      fill_char=None, qualities=True, world_size=1):
+    """`medaka inference` followed by `medaka sequence` in one pass: the FASTQ / FASTA (and gap bed) that
+    ``predict_regions`` + ``stitch.sequence`` write, without the probabilities ever leaving the GPU.
+
+    The engine decodes every window in its head (labels and quality bytes, ``GRUModel.submit_decoded``) into a
+    device arena; per window only its name, positions and (with ``min_depth``) depth stay on the host.  At the end the
+    windows are indexed,
+    trimmed and stitched exactly as ``stitch.sequence`` does (``stitch.write_consensus``), the kept rows compacted on
+    the device (``stitch.decode_label_pieces``).
+
+    The arena holds 2 B per computed column (every column of every window, overlaps included) until the output is
+    written, and is freed on return, also on error: about (draft bases) x (1 + insertion column share) x chunk_len /
+    (chunk_len - chunk_ovlp) x 2 B, e.g. an estimated 7-8 GB for a 3.1 Gb draft with ~15 % insertion columns and
+    10 000 / 1 000 windows.  On the host each window keeps its positions as int32 major and (usually) uint8 minor, and
+    with ``min_depth`` a clipped depth of (usually) 1 B: about 5-6 B per computed column, an estimated 20-25 GB for
+    the same draft.
+
+    :param draft: FASTA path or mapping name -> sequence.
+    :param regions: Regions or region strings to stitch (default: every draft contig); ``bam_regions`` are the regions
+        to run inference on, as in ``predict_regions``.
+    """
+    if not hasattr(model, "submit_decoded"):
+        raise NotImplementedError(
+            "predict_consensus runs consensus (GRUModel) models only; for {} use predict_regions followed by "
+            "stitch.sequence".format(type(model).__name__))
+    if world_size != 1:
+        raise NotImplementedError("predict_consensus runs on one GPU; for several, use predict_regions with one "
+                                  "store per rank, then stitch.sequence over the stores")
+    from medaka_b200 import stitch
+    logger = common.get_named_logger('Predict')
+    model.check_feature_encoder_compatibility(feature_encoder)
+    long_regions, remainder_regions = triage_regions(bam_regions, chunk_len, bam_chunk, chunk_ovlp)
+    arena = _LabelArena(model.device().index)
+    samples = collections.OrderedDict()
+    try:
+        if long_regions:
+            logger.info("Processing {} long region(s) with batching.".format(len(long_regions)))
+            rem = _run_decoded(samples, arena, bam, long_regions, model, feature_encoder, chunk_len, chunk_ovlp,
+                               min_depth, batch_size=batch_size, bam_workers=bam_workers)
+            remainder_regions.extend([r[0] for r in rem])
+        if remainder_regions:
+            logger.info("Processing {} short region(s).".format(len(remainder_regions)))
+            new_rem = _run_decoded(samples, arena, bam, remainder_regions, model, feature_encoder, chunk_len,
+                                   chunk_ovlp, min_depth, batch_size=1, enable_chunking=False)
+            if new_rem:
+                logger.warning("{} regions were not processed: {}.".format(len(new_rem), [x[0] for x in new_rem]))
+        model.sync()
+
+        def decode(views, pieces):
+            # one stitch call per arena slab the pieces lie in, results back in piece order
+            where = [samples[views[p.sample].name][1:] for p in pieces]
+            seqs, quals = [None] * len(pieces), [None] * len(pieces)
+            for slab in sorted({w[0] for w in where}):
+                ks = [k for k, w in enumerate(where) if w[0] == slab]
+                got = stitch.decode_label_pieces(arena.labels(slab), arena.quals(slab),
+                                                 [where[k][1] + pieces[k].lo for k in ks],
+                                                 [pieces[k].hi - pieces[k].lo for k in ks], device=arena.device)
+                for k, s, q in zip(ks, *got):
+                    seqs[k], quals[k] = s, q
+            return seqs, quals
+
+        stitch.write_consensus(stitch.sample_index(samples), lambda names: [samples[n][0] for n in names], draft, output, regions=regions,
+                               min_depth=min_depth, fillgaps=fillgaps, fill_char=fill_char, qualities=qualities,
+                               decode=decode, device=arena.device)
+    finally:
+        try:
+            model.sync()
+        finally:
+            arena.free()
+    logger.info("Finished one-pass consensus of {} windows.".format(len(samples)))

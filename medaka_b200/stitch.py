@@ -6,14 +6,22 @@ views ever changes a probability, so here the stream is reduced to a *plan*: a l
 ranges plus the contig breaks, computed from positions / depths only.  The ranges of a whole region then go to the
 GPU in one call (libmedaka_b200 `mdk_stitch_consensus`): only the kept rows are copied in, decoded (argmax + phred),
 gap calls are removed by a stable compaction, and the bytes that come back are the FASTA/FASTQ text.
+
+``sequence`` is `medaka sequence` (medaka/stitch.py:197-309) over this package's stores; ``write_consensus`` is its
+body, shared with the one-pass ``prediction.predict_consensus``, whose decoded calls never leave the device
+(``decode_label_pieces``, libmedaka_b200 `mdk_stitch_labels_dev`).
 """
 import collections
+import functools
 import itertools
 
 import numpy as np
 
 from medaka_b200 import libmedaka as _lm
-from medaka_b200.common import OverlapException, Relationship, Sample, get_named_logger
+from medaka_b200.common import OverlapException, Region, Relationship, Sample, get_named_logger
+
+# stitch regions are at most this long (medaka/stitch.py:219)
+MAX_REGION_SIZE = int(1e6)
 
 Piece = collections.namedtuple('Piece', 'sample lo hi last heuristic')
 Piece.__doc__ = "rows [lo, hi) of samples[sample]; `last` closes a contig; `heuristic` = junction search was used"
@@ -178,28 +186,62 @@ def decode_pieces(samples, pieces, device=0, with_qualities=True):
         ffi.cast("uint8_t *", ffi.from_buffer(seq)),
         ffi.cast("uint8_t *", ffi.from_buffer(qual)) if with_qualities else ffi.NULL,
         ffi.cast("int64_t *", ffi.from_buffer(off))))
+    return _split_text(seq, qual, off)
+
+
+def decode_label_pieces(labels_dev, quals_dev, seg_start, seg_rows, device=0):
+    """Gap-strip row ranges of decoded calls already on the device (mdk_stitch_labels_dev).
+
+    :param labels_dev, quals_dev: device addresses (int) of the uint8 labels and phred+33 bytes (quals_dev may be None).
+    :param seg_start, seg_rows: range k is rows [seg_start[k], seg_start[k] + seg_rows[k]) of both arrays.
+    :returns: (list of str, list of str or None), one per range.
+    """
+    n = len(seg_start)
+    if n == 0:
+        return [], ([] if quals_dev is not None else None)
+    lib, ffi = _lm.load(), _lm.ffi
+    starts = np.ascontiguousarray(seg_start, dtype=np.int64)
+    rows = np.ascontiguousarray(seg_rows, dtype=np.int64)
+    total = int(rows.sum())
+    seq = np.empty(total, dtype=np.uint8)
+    qual = np.empty(total, dtype=np.uint8) if quals_dev is not None else None
+    off = np.empty(n + 1, dtype=np.int64)
+    _lm.check(lib.mdk_stitch_labels_dev(
+        device, ffi.cast("const uint8_t *", labels_dev),
+        ffi.cast("const uint8_t *", quals_dev) if quals_dev is not None else ffi.NULL,
+        ffi.cast("const int64_t *", ffi.from_buffer(starts)), ffi.cast("const int64_t *", ffi.from_buffer(rows)), n,
+        ffi.cast("uint8_t *", ffi.from_buffer(seq)),
+        ffi.cast("uint8_t *", ffi.from_buffer(qual)) if qual is not None else ffi.NULL,
+        ffi.cast("int64_t *", ffi.from_buffer(off))))
+    return _split_text(seq, qual, off)
+
+
+def _split_text(seq, qual, off):
+    """The stitch's concatenated output -> one str per range (and the qualities, or None)."""
+    n = len(off) - 1
     seq_txt = seq[:off[-1]].tobytes().decode('ascii')
-    seqs = [seq_txt[off[k]:off[k + 1]] for k in range(len(pieces))]
+    seqs = [seq_txt[off[k]:off[k + 1]] for k in range(n)]
     quals = None
-    if with_qualities:
+    if qual is not None:
         qual_txt = qual[:off[-1]].tobytes().decode('ascii')
-        quals = [qual_txt[off[k]:off[k + 1]] for k in range(len(pieces))]
+        quals = [qual_txt[off[k]:off[k + 1]] for k in range(n)]
     return seqs, quals
 
 
-def stitch_samples(samples, label_scheme=None, region=None, min_depth=0, device=0):
+def stitch_samples(samples, label_scheme=None, region=None, min_depth=0, device=0, decode=None):
     """Drop-in for `medaka.stitch._stitch_samples` (stitch.py:33-85).
 
     :param samples: iterable of Sample with positions, label_probs (and depth when min_depth is used).
     :param label_scheme: accepted for signature compatibility (the haploid '*ACGT' decoding is what the library does).
     :param region: object with .start / .end (either may be None) or None.
+    :param decode: ``decode(samples, pieces) -> (seqs, quals)``; default ``decode_pieces`` on the samples' label_probs.
     :returns: list of ((ref_name, first major, last major), [sequence parts], [quality parts]).
     """
     samples = list(samples)
     start = getattr(region, 'start', None)
     end = getattr(region, 'end', None)
     pieces = plan_pieces(samples, start, end, min_depth)
-    seqs, quals = decode_pieces(samples, pieces, device=device)
+    seqs, quals = (decode or functools.partial(decode_pieces, device=device))(samples, pieces)
     logger = get_named_logger('Stitch')
     logger.debug("Used heuristic {} times for {}.".format(sum(p.heuristic for p in pieces), region))
     contigs = []
@@ -286,3 +328,132 @@ def read_fasta(path):
     if name is not None:
         seqs[name] = ''.join(parts)
     return seqs
+
+
+def sample_index(names):
+    """Sample names -> OrderedDict ref_name -> list of sample names in stitch order (medaka/datastore.py:453-485):
+    reference names sorted, a reference's samples by start (major, minor), then by descending end."""
+    by_ref = collections.defaultdict(list)
+    for name in names:
+        d = Sample.decode_sample_name(name)
+        if d is not None:
+            by_ref[d['ref_name']].append((name, d['start'], d['end']))
+
+    def major_minor(x):
+        return tuple(int(i) for i in x.split('.'))
+
+    def sorter(item):
+        return major_minor(item[1]) + tuple(-i for i in major_minor(item[2]))
+
+    return collections.OrderedDict((ref, [x[0] for x in sorted(by_ref[ref], key=sorter)]) for ref in sorted(by_ref))
+
+
+def select_samples(index, region):
+    """Names of the indexed samples overlapping ``region``, in index order (medaka/datastore.py:504-515): a sample
+    covers the draft positions [int(start major), int(end major) + 1)."""
+    out = []
+    for name in index.get(region.ref_name, ()):
+        d = Sample.decode_sample_name(name)
+        if Region(d['ref_name'], int(float(d['start'])), int(float(d['end'])) + 1).overlaps(region):
+            out.append(name)
+    return out
+
+
+def plan_regions(index, draft_lengths, regions=None):
+    """The stitch regions of a run (medaka/stitch.py:206-233) and the requested contigs without samples.
+
+    :param regions: Regions or region strings to stitch; default every draft contig.  A missing start / end means the
+        contig's start / end.
+    :returns: (list of Region of at most MAX_REGION_SIZE, in request order; list of contig names absent from the index).
+    """
+    if regions is None:
+        regions = [Region(name, None, None) for name in draft_lengths]
+    todo, missing = [], []
+    for r in regions:
+        ref, start, end = Region.from_string(r) if isinstance(r, str) else r
+        if ref not in index:
+            if ref not in missing:
+                missing.append(ref)
+            continue
+        start = 0 if start is None else start
+        end = draft_lengths[ref] if end is None else end
+        todo.extend(Region(ref, start, end).split(MAX_REGION_SIZE, overlap=0, fixed_size=False))
+    return todo, missing
+
+
+def write_bed(gaps, path):
+    """Gap intervals -> bed (medaka/common.py write_intervaltrees_to_bed): contigs sorted, intervals sorted."""
+    with open(path, 'w') as fh:
+        for ref in sorted(gaps):
+            for a, b in sorted(gaps[ref]):
+                fh.write("{}\t{}\t{}\n".format(ref, a, b))
+
+
+def write_consensus(index, load, draft, output, regions=None, min_depth=0, fillgaps=True, fill_char=None,
+                    qualities=True, decode=None, device=0):
+    """The serial body of `medaka sequence` (medaka/stitch.py:197-309) over any sample source.
+
+    :param index: ``sample_index`` of the available samples.
+    :param load: list of sample names -> list of Sample (positions, depth, and whatever ``decode`` reads).
+    :param draft: FASTA path or mapping name -> sequence.
+    :param decode: as in ``stitch_samples``.
+    Writes ``output`` (FASTQ, or FASTA without ``qualities``) and, with ``fillgaps``,
+    ``output + '.gaps_in_draft_coords.bed'``.
+    """
+    if isinstance(draft, str):
+        draft = read_fasta(draft)
+    todo, missing = plan_regions(index, {k: len(v) for k, v in draft.items()}, regions)
+    logger = get_named_logger('Stitcher')
+
+    def pieces():
+        for region in todo:
+            logger.debug("Stitching {}".format(region))
+            yield from stitch_samples(load(select_samples(index, region)), region=region, min_depth=min_depth,
+                                      device=device, decode=decode)
+
+    contigs = collapse_neighbours(pieces())
+    with open(output, 'w') as fh:
+        if fillgaps:
+            contigs, gaps = fill_gaps(contigs, draft, fill_char)
+            for (ref, _, _), seq_parts, qual_parts in contigs:
+                write_fastx_segment(fh, (ref, seq_parts, qual_parts), qualities=qualities)
+            # requested contigs without any sample are copied verbatim, as one gap each
+            for ref in missing:
+                logger.info("Copying contig '{}' verbatim from input.".format(ref))
+                seq = draft[ref]
+                write_fastx_segment(fh, (ref, [seq], ['!' * len(seq)]), qualities=qualities)
+                gaps[ref] = [(0, len(seq))]
+        else:
+            last, k = None, 0
+            for (ref, start, stop), seq_parts, qual_parts in contigs:
+                k = k + 1 if ref == last else 0
+                write_fastx_segment(fh, ("{}_{} {}-{}".format(ref, k, start, stop + 1), seq_parts, qual_parts),
+                                    qualities=qualities)
+                last = ref
+    if fillgaps:
+        write_bed(gaps, output + ".gaps_in_draft_coords.bed")
+
+
+def sequence(stores, draft, output, regions=None, min_depth=0, fillgaps=True, fill_char=None, qualities=True,
+             device=0):
+    """`medaka sequence` (medaka/stitch.py:197-309, serial path) over stores written by ``prediction.predict_regions``.
+
+    :param stores: one store path or several (a sample name found in more than one is read from the first).
+    :param draft: FASTA path or mapping name -> sequence.
+    :param regions: Regions or region strings to stitch (default: every draft contig).
+    """
+    from medaka_b200 import datastore
+    if isinstance(stores, str):
+        stores = [stores]
+    opened = [datastore.DataStore(path, 'r') for path in stores]
+    try:
+        owner = {}
+        for ds in opened:
+            for name in ds.sample_registry:
+                owner.setdefault(name, ds)
+        write_consensus(sample_index(owner), lambda names: [owner[n].load_sample(n) for n in names], draft, output,
+                        regions=regions, min_depth=min_depth, fillgaps=fillgaps, fill_char=fill_char,
+                        qualities=qualities, device=device)
+    finally:
+        for ds in opened:
+            ds.close()
