@@ -148,6 +148,18 @@ int mdk_engine_wait(mdk_engine *e, int64_t ticket);
  * complete after mdk_engine_wait(ticket) or mdk_engine_sync. */
 int mdk_engine_submit_decoded(mdk_engine *e, const float *feats, int64_t B, int64_t T,
                               uint8_t *labels_out, uint8_t *quals_out, int64_t *ticket);
+/* one-pass variant calling: the same forward, but what leaves the engine is what variant decoding needs per position,
+ * 9 B instead of 20 B.  ref_bytes uint8 [B][T] in: the draft's label code per position (0..4 = '*ACGT', 0 on insertion
+ * columns; 5 = 'N'; 6 = any other symbol) in the low 3 bits, 0x80 on insertion columns (minor != 0).  Out: calls_out
+ * uint8 [B][T] = argmax label (first max wins) in the low 3 bits | 0x40 when it differs from the ref code | the ref
+ * byte's 0x80; pred_q_out / ref_q_out float [B][T] = min(70, -10 log10(clip(1 - p, 1e-7, 1))) of the winning class's
+ * and of the reference class's probability (codes 5 and 6 are scored as class 0).  Bit-identical to what
+ * mdk_decode_variants computes from the probabilities mdk_engine_submit returns for the same features (pred, pred !=
+ * ref code, pred_q, ref_q).  feats, ref_bytes and the outputs may each be host or device memory.  Packed like
+ * mdk_engine_submit (ordinary, decoded and variant-decoded calls share groups); complete after mdk_engine_wait(ticket)
+ * or mdk_engine_sync. */
+int mdk_engine_submit_variant_decoded(mdk_engine *e, const float *feats, int64_t B, int64_t T, const uint8_t *ref_bytes,
+                                      uint8_t *calls_out, float *pred_q_out, float *ref_q_out, int64_t *ticket);
 /* launch the group that is still collecting batches (if any) without waiting for it */
 int mdk_engine_flush(mdk_engine *e);
 /* most windows coalesced into one group; 0 (default) = one wave, 1 = never coalesce */
@@ -391,6 +403,30 @@ int mdk_stitch_consensus_dev(int device, const float *probs_dev, int64_t n_rows,
 int mdk_stitch_labels_dev(int device, const uint8_t *labels_dev, const uint8_t *quals_dev,
                           const int64_t *seg_start, const int64_t *seg_rows, int64_t n_seg,
                           uint8_t *seq_out, uint8_t *qual_out, int64_t *seg_out_off);
+/* Join and decode on the outputs of mdk_engine_submit_variant_decoded already on the device.  A piece k is the rows
+ * [0, seg_rows[k]) at the device addresses seg_calls[k] (call bytes) and seg_pred_q[k] / seg_ref_q[k] (phreds);
+ * seg_rows[k] > 0.  The pointer tables and every other array are host memory.  Both run on the legacy stream: the engine
+ * that wrote the outputs must have been synchronised (mdk_engine_sync).
+ * mdk_variant_join_cuts: per trimmed piece, cut_out[k] = the index of its last insertion-free column whose call equals
+ * the draft, or -1 when no column has call == draft != '*' - what join_samples (medaka/variant.py:84-93) reads of the
+ * labels.
+ * mdk_decode_variants_dev: mdk_decode_variants over joined samples; joined sample s is the pieces
+ * [sample_seg[s], sample_seg[s + 1]) back to back (sample_seg[0] = 0, sample_seg[n_samples] = n_seg, none empty).
+ * Neither the variant-column rule nor a run crosses a joined sample's edge.  Per run (in sample, then column order):
+ * run_sample, run_start (column within its sample), run_len and the two float32 left-to-right sums.  run_pred receives
+ * the labels of all run columns back to back (run k's at the sum of the earlier runs' lengths), run_col_pred_q /
+ * run_col_ref_q (both or neither may be NULL) their phreds, ref_q_out (or NULL) the reference phred of every column of
+ * every sample, back to back.  When more than max_runs runs or max_run_cols run columns are found, returns
+ * MDK_ERR_NOMEM with *n_runs_out / *n_run_cols_out set (retry with larger buffers).  MDK_ERR_ARG when a joined sample
+ * starts on an insertion column (labels.py:909-911). */
+int mdk_variant_join_cuts(int device, const uint8_t *const *seg_calls, const int64_t *seg_rows, int64_t n_seg,
+                          int64_t *cut_out);
+int mdk_decode_variants_dev(int device, const uint8_t *const *seg_calls, const float *const *seg_pred_q,
+                            const float *const *seg_ref_q, const int64_t *seg_rows, int64_t n_seg,
+                            const int64_t *sample_seg, int64_t n_samples, int64_t max_runs, int64_t *run_sample,
+                            int64_t *run_start, int64_t *run_len, float *run_pred_q, float *run_ref_q,
+                            int64_t max_run_cols, uint8_t *run_pred, float *run_col_pred_q, float *run_col_ref_q,
+                            float *ref_q_out, int64_t *n_runs_out, int64_t *n_run_cols_out);
 
 /* variant_columns (src/medaka_rnn_variants.h:26, called at medaka/labels.py:869-887): which pileup columns belong
  * to a variant run.  minor [len] pileup minor indices; reference / prediction [len] one byte per column (the

@@ -135,8 +135,9 @@ static int ensure_io(mdk_engine *e, mdk_lane &ln, int64_t B, int64_t T) {
     MDK_CUDA(cudaStreamSynchronize(ln.ws->stream));
     MDK_CUDA(cudaStreamSynchronize(e->copy_in));
     MDK_CUDA(cudaStreamSynchronize(e->copy_out.stream));
-    ln.cap_io = 0; ln.cap_feats = 0; ln.cap_quals = 0;
+    ln.cap_io = 0; ln.cap_feats = 0; ln.cap_quals = 0; ln.cap_var = 0;
     dev_free(ln.d_feats); dev_free(ln.d_probs); dev_free(ln.d_logits); dev_free(ln.d_labels); dev_free(ln.d_quals);
+    dev_free(ln.d_ref); dev_free(ln.d_calls); dev_free(ln.d_pred_q); dev_free(ln.d_ref_q);
     int rc;
     if ((rc = dev_alloc(&ln.d_feats, (size_t)feats))) return rc;
     if ((rc = dev_alloc(&ln.d_probs, (size_t)P * NCLS))) return rc;
@@ -159,9 +160,26 @@ static int ensure_quals(mdk_lane &ln) {
     return MDK_OK;
 }
 
+// The variant-decoded calls' buffers (mdk_engine_submit_variant_decoded, 10 B / position): the reference bytes, staged
+// next to the features, and the call bytes and phreds the head writes.  Allocated like d_quals, but when the first
+// variant piece is staged (its reference bytes go in then): a lane never frees them while a group collects, because
+// ensure_io only runs when a group opens.
+static int ensure_var(mdk_lane &ln) {
+    if (ln.cap_var >= ln.cap_io && ln.d_ref) return MDK_OK;
+    dev_free(ln.d_ref); dev_free(ln.d_calls); dev_free(ln.d_pred_q); dev_free(ln.d_ref_q);
+    ln.cap_var = 0;
+    int rc;
+    if ((rc = dev_alloc(&ln.d_ref, (size_t)ln.cap_io))) return rc;
+    if ((rc = dev_alloc(&ln.d_calls, (size_t)ln.cap_io))) return rc;
+    if ((rc = dev_alloc(&ln.d_pred_q, (size_t)ln.cap_io))) return rc;
+    if ((rc = dev_alloc(&ln.d_ref_q, (size_t)ln.cap_io))) return rc;
+    ln.cap_var = ln.cap_io;
+    return MDK_OK;
+}
+
 // The forward pipeline on the workspace's stream.  ev[1..6] bracket the stages for mdk_timings.
 static int run_forward(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int64_t B, int64_t T, float *probs_dev,
-                       float *logits_dev, uint8_t *labels_dev, uint8_t *quals_dev) {
+                       float *logits_dev, uint8_t *labels_dev, uint8_t *quals_dev, const HeadVariant *var) {
     int rc;
     if ((rc = prepare_weights(e))) return rc;
     if ((rc = ensure_workspace(e, ws, B, T))) return rc;
@@ -208,8 +226,9 @@ static int run_forward(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int64_
     }
     launches++;
     MDK_CUDA(cudaEventRecord(e->ev[5], s));
-    if (fuse_head) MDK_CUDA(launch_head_plog(ws.plog, e->lin_b, B, T, probs_dev, logits_dev, labels_dev, s, quals_dev));
-    else MDK_CUDA(launch_head(ws.h1, e->lin_w, e->lin_b, B, T, tc ? 1 : 0, probs_dev, logits_dev, labels_dev, s, quals_dev));
+    if (fuse_head) MDK_CUDA(launch_head_plog(ws.plog, e->lin_b, B, T, probs_dev, logits_dev, labels_dev, s, quals_dev, var));
+    else MDK_CUDA(launch_head(ws.h1, e->lin_w, e->lin_b, B, T, tc ? 1 : 0, probs_dev, logits_dev, labels_dev, s, quals_dev,
+                              var));
     launches++;
     MDK_CUDA(cudaEventRecord(e->ev[6], s));
     e->launches += launches;
@@ -241,11 +260,13 @@ static int acquire_lane(mdk_engine *e, int64_t P, int *out) {
 }
 
 // The engine's side of the packing core (packing.h) for one call of B windows of T columns, features at feats (host or
-// device memory).  Launching alone (flush, sync, waits) needs no call.
+// device memory), and for a variant-decoded call its reference bytes at ref.  Launching alone (flush, sync, waits) needs
+// no call.
 struct GruCall {
     mdk_engine *e;
     const float *feats = nullptr;
     int64_t B = 0, T = 0;
+    const uint8_t *ref = nullptr;
 
     int open(int64_t windows) {
         // size class of the CALL: the tail piece of a split call stays with the big lanes
@@ -262,18 +283,26 @@ struct GruCall {
     // group's earlier pieces
     int stage(int64_t first, int64_t n, int64_t at) {
         const size_t w = (size_t)T * e->desc.num_features;
-        MDK_CUDA(cudaMemcpyAsync(e->lane[e->open_lane].d_feats + at * w, feats + first * w, n * w * sizeof(float),
-                                 cudaMemcpyDefault, e->copy_in));
+        mdk_lane &ln = e->lane[e->open_lane];
+        MDK_CUDA(cudaMemcpyAsync(ln.d_feats + at * w, feats + first * w, n * w * sizeof(float), cudaMemcpyDefault,
+                                 e->copy_in));
+        if (ref) {
+            int rc;
+            if ((rc = ensure_var(ln))) return rc;
+            MDK_CUDA(cudaMemcpyAsync(ln.d_ref + at * T, ref + first * T, n * T, cudaMemcpyDefault, e->copy_in));
+        }
         return MDK_OK;
     }
     // the sealed group on its lane: one forward over all of its windows, then the results back to each call's buffers
     int launch() {
         mdk_lane &ln = e->lane[e->open_lane];
         const Packing &pk = e->pk;
-        bool logits = false, labels = false, quals = false;      // whether any call wants them
+        bool logits = false, labels = false, quals = false, var = false;      // whether any call wants them
         for (const Packing::Piece &p : pk.pieces) {
-            logits = logits || p.logits; labels = labels || p.labels; quals = quals || p.quals;
+            logits = logits || p.logits; labels = labels || (p.labels && !p.ref); quals = quals || p.quals;
+            var = var || p.ref;
         }
+        const HeadVariant hv{ln.d_ref, ln.d_calls, ln.d_pred_q, ln.d_ref_q};
         int rc;
         if (quals && (rc = ensure_quals(ln))) return rc;
         cudaStream_t s = ln.ws->stream;
@@ -283,10 +312,10 @@ struct GruCall {
         MDK_CUDA(cudaEventRecord(ln.ev_in, e->copy_in));      // every feature copy of the group was queued on copy_in
         MDK_CUDA(cudaStreamWaitEvent(s, ln.ev_in, 0));
         if ((rc = run_forward(e, *ln.ws, ln.d_feats, pk.windows, pk.len, ln.d_probs, logits ? ln.d_logits : nullptr,
-                              labels ? ln.d_labels : nullptr, quals ? ln.d_quals : nullptr)))
+                              labels ? ln.d_labels : nullptr, quals ? ln.d_quals : nullptr, var ? &hv : nullptr)))
             return rc;
         MDK_CUDA(cudaEventRecord(e->ev[7], s));
-        if ((rc = copy_back(e->copy_out, pk, s, ln.d_probs, ln.d_logits, ln.d_labels, ln.d_quals))) return rc;
+        if ((rc = copy_back(e->copy_out, pk, s, ln.d_probs, ln.d_logits, ln.d_labels, ln.d_quals, &hv))) return rc;
         MDK_CUDA(cudaEventRecord(ln.ev_out, e->copy_out.stream));
         ln.busy = true;
         return MDK_OK;
@@ -437,6 +466,7 @@ int mdk_engine_destroy(mdk_engine *e) {
     }
     for (auto &ln : e->lane) {
         dev_free(ln.d_feats); dev_free(ln.d_probs); dev_free(ln.d_logits); dev_free(ln.d_labels); dev_free(ln.d_quals);
+        dev_free(ln.d_ref); dev_free(ln.d_calls); dev_free(ln.d_pred_q); dev_free(ln.d_ref_q);
         if (ln.ev_in) cudaEventDestroy(ln.ev_in);
         if (ln.ev_out) cudaEventDestroy(ln.ev_out);
     }
@@ -562,6 +592,20 @@ int mdk_engine_submit_decoded(mdk_engine *e, const float *feats, int64_t B, int6
     MDK_REQUIRE(ticket, MDK_ERR_ARG, "submit_decoded: ticket is NULL");
     MDK_CUDA(cudaSetDevice(e->device));
     return e->pk.enqueue(GruCall{e, feats, B, T}, B, T, nullptr, nullptr, labels_out, group_limit(e), ticket, quals_out);
+}
+
+int mdk_engine_submit_variant_decoded(mdk_engine *e, const float *feats, int64_t B, int64_t T, const uint8_t *ref_bytes,
+                                      uint8_t *calls_out, float *pred_q_out, float *ref_q_out, int64_t *ticket) {
+    MDK_REQUIRE(e != nullptr, MDK_ERR_ARG, "engine is NULL");
+    MDK_REQUIRE(feats && ref_bytes && calls_out && pred_q_out && ref_q_out, MDK_ERR_ARG,
+                "submit_variant_decoded: NULL input or output");
+    MDK_REQUIRE(B >= 1 && T >= 1, MDK_ERR_ARG, "submit_variant_decoded: need B >= 1 and T >= 1");
+    MDK_REQUIRE(B * T < (int64_t)1 << 40, MDK_ERR_ARG, "submit_variant_decoded: B*T too large");
+    MDK_REQUIRE(ticket, MDK_ERR_ARG, "submit_variant_decoded: ticket is NULL");
+    MDK_CUDA(cudaSetDevice(e->device));
+    GruCall call{e, feats, B, T, ref_bytes};
+    return e->pk.enqueue(call, B, T, nullptr, nullptr, calls_out, group_limit(e), ticket, nullptr, ref_bytes,
+                         pred_q_out, ref_q_out);
 }
 
 int mdk_engine_flush(mdk_engine *e) {

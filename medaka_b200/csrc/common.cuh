@@ -196,10 +196,19 @@ inline void destroy_copy_out(CopyOut &co) {
     for (cudaEvent_t ev : co.ev) if (ev) cudaEventDestroy(ev);
 }
 
+// What a variant-decoded forward adds to the head (phred.cuh): per position p the reference byte ref[p] in, the call
+// byte calls[p] and the phreds of the winning and of the reference class out
+struct HeadVariant {
+    const uint8_t *ref;
+    uint8_t *calls;
+    float *pred_q, *ref_q;
+};
+
 // Once the work queued on `compute` is done, per piece of the group being launched: the probabilities, logits, labels
-// and qualities the piece has, from the group's buffers to the call's (host or device); then ev[pk.serial].
+// and qualities the piece has, from the group's buffers to the call's (host or device), and for a variant-decoded piece
+// the call bytes (into its labels) and phreds; then ev[pk.serial].
 inline int copy_back(CopyOut &co, const Packing &pk, cudaStream_t compute, const float *probs, const float *logits,
-                     const uint8_t *labels, const uint8_t *quals = nullptr) {
+                     const uint8_t *labels, const uint8_t *quals = nullptr, const HeadVariant *var = nullptr) {
     MDK_CUDA(cudaEventRecord(co.done, compute));
     MDK_CUDA(cudaStreamWaitEvent(co.stream, co.done, 0));
     int64_t w0 = 0;
@@ -208,8 +217,13 @@ inline int copy_back(CopyOut &co, const Packing &pk, cudaStream_t compute, const
         const size_t bytes = n * NCLS * sizeof(float);
         if (p.probs) MDK_CUDA(cudaMemcpyAsync(p.probs + dst * NCLS, probs + src * NCLS, bytes, cudaMemcpyDefault, co.stream));
         if (p.logits) MDK_CUDA(cudaMemcpyAsync(p.logits + dst * NCLS, logits + src * NCLS, bytes, cudaMemcpyDefault, co.stream));
-        if (p.labels) MDK_CUDA(cudaMemcpyAsync(p.labels + dst, labels + src, n, cudaMemcpyDefault, co.stream));
+        if (p.labels)
+            MDK_CUDA(cudaMemcpyAsync(p.labels + dst, (p.ref ? var->calls : labels) + src, n, cudaMemcpyDefault, co.stream));
         if (p.quals) MDK_CUDA(cudaMemcpyAsync(p.quals + dst, quals + src, n, cudaMemcpyDefault, co.stream));
+        if (p.ref) {
+            MDK_CUDA(cudaMemcpyAsync(p.pred_q + dst, var->pred_q + src, n * sizeof(float), cudaMemcpyDefault, co.stream));
+            MDK_CUDA(cudaMemcpyAsync(p.ref_q + dst, var->ref_q + src, n * sizeof(float), cudaMemcpyDefault, co.stream));
+        }
         w0 += p.n;
     }
     MDK_CUDA(cudaEventRecord(co.ev[pk.serial % CopyOut::RING], co.stream));
@@ -255,9 +269,12 @@ struct mdk_lane {
     // device staging of the group's calls (their buffers may be host or device memory)
     int64_t cap_io = 0;        // positions
     int64_t cap_quals = 0;     // positions of d_quals (allocated for decoded calls only)
+    int64_t cap_var = 0;       // positions of d_ref, d_calls, d_pred_q, d_ref_q (variant-decoded calls only)
     int64_t cap_feats = 0;     // floats
     float *d_feats = nullptr, *d_probs = nullptr, *d_logits = nullptr;
     uint8_t *d_labels = nullptr, *d_quals = nullptr;
+    uint8_t *d_ref = nullptr, *d_calls = nullptr;
+    float *d_pred_q = nullptr, *d_ref_q = nullptr;
     cudaEvent_t ev_in = nullptr, ev_out = nullptr;
     bool busy = false;         // ev_out marks a group the lane has not been reclaimed from
 };
@@ -304,9 +321,12 @@ namespace mdk {
 // tiled != 0: gi rows are written / h1 rows are read in tile-interleaved order (T = window length)
 cudaError_t launch_inproj0(const float *feats, const float *w_packed, const float *bias, float *gi,
                            int64_t P, int F, int64_t T, int tiled, cudaStream_t s);
-// quals (may be null): phred bytes of the argmax class (phred.cuh), from the probability the head writes
+enum { HEAD_PLAIN = 0, HEAD_QUALS = 1, HEAD_VARIANT = 2 };     // the heads' instantiations
+// quals (may be null): phred bytes of the argmax class (phred.cuh), from the probability the head writes; var (may be
+// null): the variant outputs, from the same probabilities
 cudaError_t launch_head(const float *h1, const float *lin_w, const float *lin_b, int64_t B, int64_t T, int tiled,
-                        float *probs, float *logits, uint8_t *labels, cudaStream_t s, uint8_t *quals = nullptr);
+                        float *probs, float *logits, uint8_t *labels, cudaStream_t s, uint8_t *quals = nullptr,
+                        const HeadVariant *var = nullptr);
 cudaError_t launch_untile_rows(const float *src_tiled, float *dst, int64_t w0, int64_t nw, int64_t T, cudaStream_t s);
 cudaError_t launch_unpack_h0(const void *h0_tiles, float *out, int64_t w0, int64_t nw, int64_t T, cudaStream_t s);
 // gru_fp32.cu
@@ -330,10 +350,11 @@ enum { OUT_TILES = 0, OUT_ROWS = 1, OUT_LOGITS = 2 };
 // projection (OUT_TILES only), or nullptr to read the pre-activations from gi.  out: h0 tiles, h1 rows or plog (out_kind).
 cudaError_t launch_rec_tc(const float *gi, const RecX *xin, const __half *w_hh_tm, const float *b_hn, int tiles_per_cta,
                           int out_kind, void *out, const float *lin_w, int64_t B, int64_t T, cudaStream_t s);
-// head on the partial logits of the fused path: sum of the two directions + bias -> softmax / argmax (/ quals, as
-// launch_head)
+// head on the partial logits of the fused path: sum of the two directions + bias -> softmax / argmax (/ quals / var,
+// as launch_head)
 cudaError_t launch_head_plog(const float *plog, const float *lin_b, int64_t B, int64_t T, float *probs, float *logits,
-                             uint8_t *labels, cudaStream_t s, uint8_t *quals = nullptr);
+                             uint8_t *labels, cudaStream_t s, uint8_t *quals = nullptr,
+                             const HeadVariant *var = nullptr);
 constexpr int PLOG_TS_FLOATS = NCLS * WT;     // 80 floats per (tile-step, direction)
 cudaError_t launch_gemm_tc(const void *x_tiles, const __half *w_in_tm, const float *bias, float *gi, int64_t P,
                            int sm_count, cudaStream_t s);

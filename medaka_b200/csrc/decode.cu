@@ -31,6 +31,14 @@
 //   scan_blocks_kernel   exclusive scan of the block counts (single block)
 //   vd_runs_kernel       the k-th run start walks its run: length and the two left-to-right float32 sums
 // HBM-bound byte work: 29 B read + 10 B written per column in the first kernel, ~12 B per column in the others.
+// From the engine's variant-decoded outputs (call bytes and the two phreds in device memory, phred.cuh):
+//   vd_join_cuts_kernel  per trimmed piece, the last insertion-free column whose call equals the draft - all that
+//                        join_samples (medaka/variant.py:30-119) reads of the labels (mdk_variant_join_cuts)
+//   vd_gather_kernel     the joined samples' pieces, from wherever they lie, into the columns vd_decode_kernel would
+//                        have written, one padding column (no mismatch, not an insertion) after every joined sample so
+//                        that neither the variant-column rule nor a run crosses into the next; then vd_group, vd_starts,
+//                        scan_blocks and vd_runs as above, and vd_run_cols_kernel compacts the run columns' labels (and
+//                        phreds) for the host (mdk_decode_variants_dev).  9 B read per column instead of 20 + 9.
 #include "common.cuh"
 #include "phred.cuh"
 
@@ -380,6 +388,90 @@ __global__ void __launch_bounds__(VD_THREADS) vd_runs_kernel(const uint8_t *__re
     run_ref_q[k] = sr;
 }
 
+// One block per piece k (rows [0, seg_rows[k]) at seg_calls[k]): cut[k] = the last column that is no insertion and whose
+// call equals the draft, or -1 when every column is "different" in join_samples' sense (call != draft, or both are
+// '*'; insertion columns always are), i.e. when no column has call == draft != '*'.
+__global__ void __launch_bounds__(VD_THREADS) vd_join_cuts_kernel(const uint8_t *const *__restrict__ seg_calls,
+                                                                  const int64_t *__restrict__ seg_rows,
+                                                                  int64_t *__restrict__ cut) {
+    __shared__ int64_t s_last[VD_THREADS / 32];
+    __shared__ int s_any[VD_THREADS / 32];
+    const uint8_t *c = seg_calls[blockIdx.x];
+    const int64_t n = seg_rows[blockIdx.x];
+    int64_t last = -1;
+    int any = 0;
+    for (int64_t i = threadIdx.x; i < n; i += VD_THREADS) {
+        const uint8_t v = c[i];
+        if (!(v & (VCALL_MISM | VCALL_INS))) {
+            last = i;                                   // rows grow with i: the thread's last match is its largest
+            any |= (v & VCALL_LABEL) != 0;
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        last = max(last, (int64_t)__shfl_xor_sync(0xffffffffu, (long long)last, o));
+        any |= __shfl_xor_sync(0xffffffffu, any, o);
+    }
+    if ((threadIdx.x & 31) == 0) { s_last[threadIdx.x >> 5] = last; s_any[threadIdx.x >> 5] = any; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < VD_THREADS / 32; ++w) { last = max(last, s_last[w]); any |= s_any[w]; }
+        cut[blockIdx.x] = any ? last : -1;
+    }
+}
+
+// Padded column r of the call: segment k (the last with pstart[k] <= r) holds rows [pstart[k], pstart[k] + seg_rows[k]);
+// the column just past a joined sample's last segment is its padding column.  Writes what vd_decode_kernel writes, and
+// the insertion flag as vd_group_kernel's minor.  bad: set when a joined sample starts on an insertion column.
+__global__ void __launch_bounds__(VD_THREADS) vd_gather_kernel(const uint8_t *const *__restrict__ seg_calls,
+                                                               const float *const *__restrict__ seg_pq,
+                                                               const float *__restrict__ const *seg_rq,
+                                                               const int64_t *__restrict__ pstart,
+                                                               const int64_t *__restrict__ seg_rows,
+                                                               const uint8_t *__restrict__ seg_first, int64_t n_seg,
+                                                               int64_t n, uint8_t *__restrict__ pred,
+                                                               uint8_t *__restrict__ mism, int64_t *__restrict__ minor,
+                                                               float *__restrict__ pred_q, float *__restrict__ ref_q,
+                                                               int *__restrict__ bad) {
+    const int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    int64_t lo = 0, hi = n_seg;
+    while (hi - lo > 1) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (pstart[mid] <= r) lo = mid; else hi = mid;
+    }
+    const int64_t j = r - pstart[lo];
+    if (j >= seg_rows[lo]) {                                      // padding
+        pred[r] = 0; mism[r] = 0; minor[r] = 0; pred_q[r] = 0.f; ref_q[r] = 0.f;
+        return;
+    }
+    const uint8_t v = seg_calls[lo][j];
+    pred[r] = v & VCALL_LABEL;
+    mism[r] = (v & VCALL_MISM) != 0;
+    minor[r] = (v & VCALL_INS) != 0;
+    pred_q[r] = seg_pq[lo][j];
+    ref_q[r] = seg_rq[lo][j];
+    if (j == 0 && seg_first[lo] && (v & VCALL_INS)) atomicOr(bad, 1);
+}
+
+// Run k's columns [run_start[k], run_start[k] + run_len[k]) to [off[k], off[k] + run_len[k]) of the compact outputs
+__global__ void __launch_bounds__(VD_THREADS) vd_run_cols_kernel(const uint8_t *__restrict__ pred,
+                                                                 const float *__restrict__ pred_q,
+                                                                 const float *__restrict__ ref_q,
+                                                                 const int64_t *__restrict__ run_start,
+                                                                 const int64_t *__restrict__ run_len,
+                                                                 const int64_t *__restrict__ off, int64_t n_runs,
+                                                                 uint8_t *__restrict__ cols_pred,
+                                                                 float *__restrict__ cols_pq, float *__restrict__ cols_rq) {
+    const int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (k >= n_runs) return;
+    const int64_t a = run_start[k], o = off[k];
+    for (int64_t j = 0; j < run_len[k]; ++j) {
+        cols_pred[o + j] = pred[a + j];
+        if (cols_pq) { cols_pq[o + j] = pred_q[a + j]; cols_rq[o + j] = ref_q[a + j]; }
+    }
+}
+
 // mdk_decode_consensus and mdk_decode_consensus_f64: the same staging for either probability type
 template <class P>
 int decode_host(const char *what, int device, const P *probs, int64_t n, uint8_t *labels_out, uint8_t *quals_out) {
@@ -627,6 +719,163 @@ int mdk_decode_variants(int device, const float *probs, const int64_t *minor, co
     st.out(run_len, d_rl, total);
     st.out(run_pred_q, d_rp, total);
     st.out(run_ref_q, d_rr, total);
+    return st.result();
+}
+
+// Pieces are row ranges of the engine's variant-decoded outputs anywhere in device memory; one block per piece.
+int mdk_variant_join_cuts(int device, const uint8_t *const *seg_calls, const int64_t *seg_rows, int64_t n_seg,
+                          int64_t *cut_out) {
+    MDK_REQUIRE(n_seg >= 0, MDK_ERR_ARG, "variant_join_cuts: n_seg < 0");
+    if (n_seg == 0) return MDK_OK;
+    MDK_REQUIRE(seg_calls && seg_rows && cut_out, MDK_ERR_ARG, "variant_join_cuts: NULL pointer");
+    MDK_REQUIRE(n_seg < ((int64_t)1 << 31), MDK_ERR_ARG, "variant_join_cuts: too many pieces");
+    for (int64_t k = 0; k < n_seg; ++k)
+        MDK_REQUIRE(seg_rows[k] > 0 && seg_calls[k], MDK_ERR_ARG, "variant_join_cuts: every piece needs rows > 0");
+    MDK_CUDA(cudaSetDevice(device));
+    Staging st(Blob::STAGING, "variant_join_cuts");
+    const uint8_t *const *d_calls;
+    const int64_t *d_rows;
+    int64_t *d_cut;
+    st.in(&d_calls, seg_calls, n_seg);
+    st.in(&d_rows, seg_rows, n_seg);
+    st.take(&d_cut, n_seg);
+    if (!st.alloc()) return st.result();
+    vd_join_cuts_kernel<<<(unsigned)n_seg, VD_THREADS, 0, 0>>>(d_calls, d_rows, d_cut);
+    st.check(cudaGetLastError());
+    st.out(cut_out, d_cut, n_seg);
+    return st.result();
+}
+
+// The joined samples' pieces are gathered into padded scratch (STAGING blob) by vd_gather_kernel and decoded by the
+// kernels of mdk_decode_variants; the run columns are compacted in the SCRATCH blob.
+int mdk_decode_variants_dev(int device, const uint8_t *const *seg_calls, const float *const *seg_pred_q,
+                            const float *const *seg_ref_q, const int64_t *seg_rows, int64_t n_seg,
+                            const int64_t *sample_seg, int64_t n_samples, int64_t max_runs, int64_t *run_sample,
+                            int64_t *run_start, int64_t *run_len, float *run_pred_q, float *run_ref_q,
+                            int64_t max_run_cols, uint8_t *run_pred, float *run_col_pred_q, float *run_col_ref_q,
+                            float *ref_q_out, int64_t *n_runs_out, int64_t *n_run_cols_out) {
+    MDK_REQUIRE(n_runs_out && n_run_cols_out, MDK_ERR_ARG, "decode_variants_dev: NULL count output");
+    *n_runs_out = 0;
+    *n_run_cols_out = 0;
+    MDK_REQUIRE(n_seg >= 0 && n_samples >= 0 && max_runs >= 0 && max_run_cols >= 0, MDK_ERR_ARG,
+                "decode_variants_dev: negative size");
+    if (n_samples == 0) return MDK_OK;
+    MDK_REQUIRE(seg_calls && seg_pred_q && seg_ref_q && seg_rows && sample_seg, MDK_ERR_ARG,
+                "decode_variants_dev: NULL pointer");
+    MDK_REQUIRE(max_runs == 0 || (run_sample && run_start && run_len && run_pred_q && run_ref_q), MDK_ERR_ARG,
+                "decode_variants_dev: NULL run output");
+    MDK_REQUIRE(max_run_cols == 0 || run_pred, MDK_ERR_ARG, "decode_variants_dev: NULL run column output");
+    MDK_REQUIRE((run_col_pred_q == nullptr) == (run_col_ref_q == nullptr), MDK_ERR_ARG,
+                "decode_variants_dev: give both run column phreds or neither");
+    MDK_REQUIRE(sample_seg[0] == 0 && sample_seg[n_samples] == n_seg, MDK_ERR_ARG,
+                "decode_variants_dev: sample_seg must run from 0 to n_seg");
+    // padded layout: joined sample s starts at its first row + s (one padding column after each sample)
+    std::vector<int64_t> pstart((size_t)n_seg), sample_pbase((size_t)n_samples + 1);
+    std::vector<uint8_t> first((size_t)n_seg, 0);
+    int64_t n = 0;
+    for (int64_t smp = 0; smp < n_samples; ++smp) {
+        MDK_REQUIRE(sample_seg[smp + 1] > sample_seg[smp], MDK_ERR_ARG, "decode_variants_dev: empty joined sample");
+        sample_pbase[(size_t)smp] = n;
+        first[(size_t)sample_seg[smp]] = 1;
+        for (int64_t k = sample_seg[smp]; k < sample_seg[smp + 1]; ++k) {
+            MDK_REQUIRE(seg_rows[k] > 0 && seg_calls[k] && seg_pred_q[k] && seg_ref_q[k], MDK_ERR_ARG,
+                        "decode_variants_dev: every piece needs rows > 0 and its three pointers");
+            pstart[(size_t)k] = n;
+            n += seg_rows[k];
+        }
+        n += 1;
+    }
+    sample_pbase[(size_t)n_samples] = n;
+    MDK_CUDA(cudaSetDevice(device));
+    const int64_t n_blocks = (n + VD_THREADS - 1) / VD_THREADS;
+    Staging st(Blob::STAGING, "decode_variants_dev");
+    const uint8_t *const *d_calls;
+    const float *const *d_spq, *const *d_srq;
+    const int64_t *d_pstart, *d_rows;
+    const uint8_t *d_first;
+    uint8_t *d_pred, *d_mism, *d_var;
+    int64_t *d_minor, *d_base, *d_rs, *d_rl, *d_tail;
+    float *d_pq, *d_rq, *d_rp, *d_rr;
+    st.in(&d_calls, seg_calls, n_seg);
+    st.in(&d_spq, seg_pred_q, n_seg);
+    st.in(&d_srq, seg_ref_q, n_seg);
+    st.in(&d_pstart, pstart.data(), n_seg);
+    st.in(&d_rows, seg_rows, n_seg);
+    st.in(&d_first, first.data(), n_seg);
+    st.take(&d_pred, n);
+    st.take(&d_mism, n);
+    st.take(&d_var, n);
+    st.take(&d_minor, n);
+    st.take(&d_pq, n);
+    st.take(&d_rq, n);
+    st.take(&d_base, n_blocks + 1);
+    st.take(&d_tail, 2);                 // total runs (copied from d_base[n_blocks]), the bad-start flag
+    st.take(&d_rs, max_runs);
+    st.take(&d_rl, max_runs);
+    st.take(&d_rp, max_runs);
+    st.take(&d_rr, max_runs);
+    if (!st.alloc()) return st.result();
+    const unsigned g = (unsigned)n_blocks;
+    st.check(cudaMemsetAsync(d_tail, 0, 2 * sizeof(int64_t), 0));
+    vd_gather_kernel<<<g, VD_THREADS, 0, 0>>>(d_calls, d_spq, d_srq, d_pstart, d_rows, d_first, n_seg, n, d_pred,
+                                              d_mism, d_minor, d_pq, d_rq, reinterpret_cast<int *>(d_tail + 1));
+    vd_group_kernel<<<g, VD_THREADS, 0, 0>>>(d_minor, d_mism, n, d_var);
+    vd_starts_kernel<<<g, VD_THREADS, 0, 0>>>(d_var, n, d_base);
+    st.check(launch_scan_blocks(d_base, n_blocks, 0));
+    vd_runs_kernel<<<g, VD_THREADS, 0, 0>>>(d_var, d_pq, d_rq, n, d_base, max_runs, d_rs, d_rl, d_rp, d_rr);
+    st.check(cudaGetLastError());
+    if (st.ok()) st.check(cudaMemcpyAsync(d_tail, d_base + n_blocks, sizeof(int64_t), cudaMemcpyDeviceToDevice, 0));
+    int64_t tail[2] = {0, 0};
+    st.out(tail, d_tail, 2);
+    if (!st.ok()) return st.result();
+    MDK_REQUIRE(tail[1] == 0, MDK_ERR_ARG,
+                "decode_variants_dev: the first position of a sample must not be an insertion (labels.py:909-911)");
+    const int64_t total = tail[0];
+    *n_runs_out = total;
+    if (total > max_runs) {
+        set_error("decode_variants_dev: run buffers too small (see *n_runs_out)");
+        return MDK_ERR_NOMEM;
+    }
+    st.out(run_start, d_rs, total);
+    st.out(run_len, d_rl, total);
+    st.out(run_pred_q, d_rp, total);
+    st.out(run_ref_q, d_rr, total);
+    if (!st.ok()) return st.result();
+    // padded -> per-sample positions; run columns' offsets
+    std::vector<int64_t> off((size_t)total + 1, 0);
+    for (int64_t k = 0, smp = 0; k < total; ++k) {
+        while (run_start[k] >= sample_pbase[(size_t)smp + 1]) ++smp;     // runs come in column order
+        run_sample[k] = smp;
+        off[(size_t)k + 1] = off[(size_t)k] + run_len[k];
+    }
+    const int64_t cols = off[(size_t)total];
+    *n_run_cols_out = cols;
+    if (cols > max_run_cols) {
+        set_error("decode_variants_dev: run column buffers too small (see *n_run_cols_out)");
+        return MDK_ERR_NOMEM;
+    }
+    if (ref_q_out)      // every real column's reference phred, padding dropped
+        for (int64_t smp = 0; smp < n_samples && st.ok(); ++smp)
+            st.out(ref_q_out + (sample_pbase[(size_t)smp] - smp), d_rq + sample_pbase[(size_t)smp],
+                   (size_t)(sample_pbase[(size_t)smp + 1] - sample_pbase[(size_t)smp] - 1));
+    if (total) {
+        const bool qs = run_col_pred_q != nullptr;
+        Staging sc(Blob::SCRATCH, "decode_variants_dev");
+        const int64_t *d_off;
+        uint8_t *d_cp;
+        float *d_cpq = nullptr, *d_crq = nullptr;
+        sc.in(&d_off, off.data(), total);
+        sc.take(&d_cp, cols);
+        if (qs) { sc.take(&d_cpq, cols); sc.take(&d_crq, cols); }
+        if (!sc.alloc()) return sc.result();
+        vd_run_cols_kernel<<<(unsigned)((total + VD_THREADS - 1) / VD_THREADS), VD_THREADS, 0, 0>>>(
+            d_pred, d_pq, d_rq, d_rs, d_rl, d_off, total, d_cp, d_cpq, d_crq);
+        sc.check(cudaGetLastError());
+        sc.out(run_pred, d_cp, cols);
+        if (qs) { sc.out(run_col_pred_q, d_cpq, cols); sc.out(run_col_ref_q, d_crq, cols); }
+        if (!sc.ok()) return sc.result();
+    }
+    for (int64_t k = 0; k < total; ++k) run_start[k] -= sample_pbase[(size_t)run_sample[k]];
     return st.result();
 }
 

@@ -89,13 +89,16 @@ cudaError_t launch_inproj0(const float *feats, const float *w_packed, const floa
 // tile-interleaved row(w, t).  Each warp handles 4 positions per iteration: 8 of the 256 inputs per lane, the
 // 4 x 5 (padded to 4 x 8) partial dot products are reduced with a transposing butterfly (31 shuffles for all 32
 // values instead of 5 per value), after which lane L owns logit (position L/8, class L%8) and the softmax / argmax
-// run across the 8-lane groups - one expf per lane instead of five per lane.  QUALS: also the phred byte of the winning
-// probability (decoded forwards); the instantiation without it is the kernel of the ordinary forward.
-template <bool QUALS>
+// run across the 8-lane groups - one expf per lane instead of five per lane.  HEAD_QUALS: also the phred byte of the
+// winning probability (consensus-decoded forwards); HEAD_VARIANT: also the call byte and the phreds of the winning and of
+// the reference class (variant-decoded forwards, phred.cuh), and the phred byte where quals is given.  HEAD_PLAIN is the
+// kernel of the ordinary forward.
+template <int MODE>
 __global__ void __launch_bounds__(256) head_kernel(const float *__restrict__ h1, const float *__restrict__ lin_w,
                                                    const float *__restrict__ lin_b, int64_t P, int64_t B, int64_t T,
                                                    int tiled, float *__restrict__ probs, float *__restrict__ logits,
-                                                   uint8_t *__restrict__ labels, uint8_t *__restrict__ quals) {
+                                                   uint8_t *__restrict__ labels, uint8_t *__restrict__ quals,
+                                                   HeadVariant var) {
     const int lane = threadIdx.x & 31;
     const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -198,36 +201,51 @@ __global__ void __launch_bounds__(256) head_kernel(const float *__restrict__ h1,
             p = rb + (lane >> 3);
             ok = p < P;
         }
+        uint8_t ref = 0;
+        float p_ref = 0.f;
+        if (MODE == HEAD_VARIANT) {             // the reference class's probability from its lane of the 8-lane group
+            if (ok) ref = var.ref[p];
+            p_ref = __shfl_sync(0xffffffffu, pr, (lane & 24) + ref_class(ref));
+        }
         if (ok) {
             if (cls < NCLS) {
                 probs[p * NCLS + cls] = pr;
                 if (logits) logits[p * NCLS + cls] = logit;
             }
             if (labels && cls == 0) labels[p] = (uint8_t)arg;
-            if (QUALS && cls == 0) quals[p] = phred_char(best);
+            if (MODE == HEAD_QUALS && cls == 0) quals[p] = phred_char(best);
+            if (MODE == HEAD_VARIANT && cls == 0) {
+                if (quals) quals[p] = phred_char(best);
+                var.calls[p] = variant_call(arg, ref);
+                var.pred_q[p] = phred_f32(best);
+                var.ref_q[p] = phred_f32(p_ref);
+            }
         }
     }
 }
 
 cudaError_t launch_head(const float *h1, const float *lin_w, const float *lin_b, int64_t B, int64_t T, int tiled,
-                        float *probs, float *logits, uint8_t *labels, cudaStream_t s, uint8_t *quals) {
+                        float *probs, float *logits, uint8_t *labels, cudaStream_t s, uint8_t *quals,
+                        const HeadVariant *var) {
     const int64_t P = B * T;
     if (P == 0) return cudaSuccess;
     int64_t blocks = (P + 31) / 32;            // 8 warps per block, 4 positions per warp per iteration
     if (blocks > 132 * 8) blocks = 132 * 8;    // persistent-ish grid: multiple of the SM count
-    if (quals) head_kernel<true><<<(unsigned)blocks, 256, 0, s>>>(h1, lin_w, lin_b, P, B, T, tiled, probs, logits, labels, quals);
-    else head_kernel<false><<<(unsigned)blocks, 256, 0, s>>>(h1, lin_w, lin_b, P, B, T, tiled, probs, logits, labels, nullptr);
+    const dim3 g((unsigned)blocks);
+    if (var) head_kernel<HEAD_VARIANT><<<g, 256, 0, s>>>(h1, lin_w, lin_b, P, B, T, tiled, probs, logits, labels, quals, *var);
+    else if (quals) head_kernel<HEAD_QUALS><<<g, 256, 0, s>>>(h1, lin_w, lin_b, P, B, T, tiled, probs, logits, labels, quals, {});
+    else head_kernel<HEAD_PLAIN><<<g, 256, 0, s>>>(h1, lin_w, lin_b, P, B, T, tiled, probs, logits, labels, nullptr, {});
     return cudaGetLastError();
 }
 
 // Head of the fused path (gru.py:53-55,67-71): logits = fwd partial + rev partial + bias, softmax, first-max argmax.
 // One thread per (window of the tile, time step); blockIdx.y = window tile.  41 B written per position, 40 B read.
-// QUALS as in head_kernel.
-template <bool QUALS>
+// MODE as in head_kernel.
+template <int MODE>
 __global__ void __launch_bounds__(256) head_plog_kernel(const float *__restrict__ plog, const float *__restrict__ lin_b,
                                                         int64_t B, int64_t T, int64_t n_ts, float *__restrict__ probs,
                                                         float *__restrict__ logits, uint8_t *__restrict__ labels,
-                                                        uint8_t *__restrict__ quals) {
+                                                        uint8_t *__restrict__ quals, HeadVariant var) {
     const int64_t wt = blockIdx.y;
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;   // t * 16 + w
     const int64_t t = i >> 4;
@@ -247,26 +265,37 @@ __global__ void __launch_bounds__(256) head_plog_kernel(const float *__restrict_
 #pragma unroll
     for (int c = 0; c < NCLS; ++c) { e[c] = expf(lg[c] - mx); sum += e[c]; }   // class order, like a sequential softmax
     const int64_t p = win * T + t;
-    float best = -1.f;
+    float best = -1.f, p_ref = 0.f;
     int arg = 0;
+    const uint8_t ref = MODE == HEAD_VARIANT ? var.ref[p] : 0;
+    const int rc = ref_class(ref);
 #pragma unroll
     for (int c = 0; c < NCLS; ++c) {
         const float pr = e[c] / sum;
         probs[p * NCLS + c] = pr;
         if (logits) logits[p * NCLS + c] = lg[c];
         if (pr > best) { best = pr; arg = c; }     // first maximum wins (np.argmax, labels.py:1063)
+        if (MODE == HEAD_VARIANT && c == rc) p_ref = pr;
     }
     if (labels) labels[p] = (uint8_t)arg;
-    if (QUALS) quals[p] = phred_char(best);
+    if (MODE == HEAD_QUALS) quals[p] = phred_char(best);
+    if (MODE == HEAD_VARIANT) {
+        if (quals) quals[p] = phred_char(best);
+        var.calls[p] = variant_call(arg, ref);
+        var.pred_q[p] = phred_f32(best);
+        var.ref_q[p] = phred_f32(p_ref);
+    }
 }
 
 cudaError_t launch_head_plog(const float *plog, const float *lin_b, int64_t B, int64_t T, float *probs, float *logits,
-                             uint8_t *labels, cudaStream_t s, uint8_t *quals) {
+                             uint8_t *labels, cudaStream_t s, uint8_t *quals, const HeadVariant *var) {
     if (B == 0 || T == 0) return cudaSuccess;
     const int64_t tiles = (B + WT - 1) / WT;
     dim3 grid((unsigned)((T * WT + 255) / 256), (unsigned)tiles);
-    if (quals) head_plog_kernel<true><<<grid, 256, 0, s>>>(plog, lin_b, B, T, tiles * T, probs, logits, labels, quals);
-    else head_plog_kernel<false><<<grid, 256, 0, s>>>(plog, lin_b, B, T, tiles * T, probs, logits, labels, nullptr);
+    const int64_t n_ts = tiles * T;
+    if (var) head_plog_kernel<HEAD_VARIANT><<<grid, 256, 0, s>>>(plog, lin_b, B, T, n_ts, probs, logits, labels, quals, *var);
+    else if (quals) head_plog_kernel<HEAD_QUALS><<<grid, 256, 0, s>>>(plog, lin_b, B, T, n_ts, probs, logits, labels, quals, {});
+    else head_plog_kernel<HEAD_PLAIN><<<grid, 256, 0, s>>>(plog, lin_b, B, T, n_ts, probs, logits, labels, nullptr, {});
     return cudaGetLastError();
 }
 

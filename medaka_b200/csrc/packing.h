@@ -21,6 +21,8 @@ struct Packing {
         int64_t first, n;          // first window in the call, windows
         uint8_t *quals;            // [B][len] phred bytes of the argmax class, or null (then probs may be null too:
                                    // a decoded call, mdk_engine_submit_decoded, wants labels and quals only)
+        const uint8_t *ref;        // a variant-decoded call (mdk_engine_submit_variant_decoded): its [B][len] reference
+        float *pred_q, *ref_q;     // bytes, and its phreds; `labels` then receives the call bytes.  Null otherwise.
     };
     std::vector<Piece> pieces;     // of the open group, or of the group last launched
     int64_t windows = 0, len = 0;  // the group's windows so far and its window length
@@ -44,7 +46,8 @@ struct Packing {
     // One call of B windows of length L, with at most gmax windows to a group; ticket may be null.
     template <class Eng>
     int enqueue(Eng &&eng, int64_t B, int64_t L, float *probs, float *logits, uint8_t *labels, int64_t gmax,
-                int64_t *ticket, uint8_t *quals = nullptr) {
+                int64_t *ticket, uint8_t *quals = nullptr, const uint8_t *ref = nullptr, float *pred_q = nullptr,
+                float *ref_q = nullptr) {
         int rc;
         if (open && len != L && (rc = launch(eng))) return rc;      // a new window length seals the open group
         for (int64_t done = 0; done < B;) {
@@ -63,7 +66,7 @@ struct Packing {
             }
             const int64_t n = std::min(room, B - done);
             if ((rc = eng.stage(done, n, windows))) return rc;
-            pieces.push_back(Piece{probs, logits, labels, done, n, quals});
+            pieces.push_back(Piece{probs, logits, labels, done, n, quals, ref, pred_q, ref_q});
             windows += n;
             done += n;
             if (done == B && ticket) {                                  // the piece that ends the call

@@ -106,6 +106,86 @@ def decode_variant_arrays(label_probs, minor, ref_codes, device=0, want_quals=Tr
                 run_pred_q=rp[:r], run_ref_q=rr[:r])
 
 
+def _run_index(run_start, run_len):
+    """Columns of the runs, back to back: run k's are run_start[k] .. run_start[k] + run_len[k] - 1."""
+    run_len = np.asarray(run_len, dtype=np.int64)
+    if len(run_len) == 0:
+        return np.zeros(0, dtype=np.int64)
+    off = np.cumsum(run_len) - run_len
+    return np.repeat(np.asarray(run_start, dtype=np.int64) - off, run_len) + np.arange(int(run_len.sum()))
+
+
+def variant_join_cuts(seg_calls, seg_rows, device=0):
+    """Per trimmed piece of variant-decoded calls on the device (libmedaka_b200 ``mdk_variant_join_cuts``): the index of
+    its last insertion-free column whose call equals the draft, or -1 when ``join_samples`` finds every column
+    different.
+
+    :param seg_calls: device addresses (int) of the pieces' first call bytes; :param seg_rows: their lengths.
+    :returns: int64 array.
+    """
+    n = len(seg_calls)
+    cut = np.empty(n, dtype=np.int64)
+    if n == 0:
+        return cut
+    lib, ffi = _lm.load(), _lm.ffi
+    ptrs = ffi.new("const uint8_t *[]", [ffi.cast("const uint8_t *", int(a)) for a in seg_calls])
+    rows = np.ascontiguousarray(seg_rows, dtype=np.int64)
+    _lm.check(lib.mdk_variant_join_cuts(device, ptrs, ffi.cast("const int64_t *", ffi.from_buffer(rows)), n,
+                                        ffi.cast("int64_t *", ffi.from_buffer(cut))))
+    return cut
+
+
+def decode_variant_segments(seg_calls, seg_pred_q, seg_ref_q, seg_rows, sample_seg, device=0, want_quals=False,
+                            want_ref_q=False):
+    """The array half of ``decode_variants`` for joined samples whose variant-decoded calls are already on the device
+    (libmedaka_b200 ``mdk_decode_variants_dev``).
+
+    :param seg_calls, seg_pred_q, seg_ref_q: device addresses (int) of each piece's first call byte and phreds.
+    :param seg_rows: the pieces' lengths.  :param sample_seg: joined sample s is pieces [sample_seg[s], sample_seg[s+1]).
+    :returns: dict(run_sample, run_start (column within its sample), run_len int64 [r], run_pred_q / run_ref_q float32
+        [r], run_pred uint8 [run columns], run_col_pred_q / run_col_ref_q float32 [run columns] (want_quals, else None),
+        ref_q float32 [all columns of all samples] (want_ref_q, else None)).
+    """
+    lib, ffi = _lm.load(), _lm.ffi
+    n_seg, n_samples = len(seg_calls), len(sample_seg) - 1
+    rows = np.ascontiguousarray(seg_rows, dtype=np.int64)
+    sseg = np.ascontiguousarray(sample_seg, dtype=np.int64)
+    n = int(rows.sum())
+
+    def table(ctype, addrs):
+        return ffi.new(ctype + "[]", [ffi.cast(ctype, int(a)) for a in addrs]) if n_seg else ffi.NULL
+
+    calls, pqs, rqs = (table("const uint8_t *", seg_calls), table("const float *", seg_pred_q),
+                       table("const float *", seg_ref_q))
+    ref_q = np.empty(n, dtype=np.float32) if want_ref_q else None
+    max_runs, max_cols = max(16, n // 64), max(64, n // 16)
+    n_runs, n_cols = ffi.new("int64_t *"), ffi.new("int64_t *")
+
+    def out(a, ctype):
+        return ffi.cast(ctype, ffi.from_buffer(a)) if a is not None else ffi.NULL
+
+    while True:
+        rsmp, rs, rl = (np.empty(max_runs, dtype=np.int64) for _ in range(3))
+        rp, rr = np.empty(max_runs, dtype=np.float32), np.empty(max_runs, dtype=np.float32)
+        cp = np.empty(max_cols, dtype=np.uint8)
+        cpq = np.empty(max_cols, dtype=np.float32) if want_quals else None
+        crq = np.empty(max_cols, dtype=np.float32) if want_quals else None
+        code = lib.mdk_decode_variants_dev(
+            device, calls, pqs, rqs, out(rows, "const int64_t *"), n_seg, out(sseg, "const int64_t *"), n_samples,
+            max_runs, out(rsmp, "int64_t *"), out(rs, "int64_t *"), out(rl, "int64_t *"), out(rp, "float *"),
+            out(rr, "float *"), max_cols, out(cp, "uint8_t *"), out(cpq, "float *"), out(crq, "float *"),
+            out(ref_q, "float *"), n_runs, n_cols)
+        if code == lib.MDK_ERR_NOMEM and (int(n_runs[0]) > max_runs or int(n_cols[0]) > max_cols):
+            max_runs, max_cols = max(max_runs, int(n_runs[0])), max(max_cols, int(n_cols[0]))   # enlarge and retry
+            continue
+        _lm.check(code)
+        break
+    r, c = int(n_runs[0]), int(n_cols[0])
+    return dict(run_sample=rsmp[:r], run_start=rs[:r], run_len=rl[:r], run_pred_q=rp[:r], run_ref_q=rr[:r],
+                run_pred=cp[:c], run_col_pred_q=cpq[:c] if want_quals else None,
+                run_col_ref_q=crq[:c] if want_quals else None, ref_q=ref_q)
+
+
 class HaploidLabelScheme(object):
     """The decode half of the reference's HaploidLabelScheme (labels.py:703-1085)."""
 
@@ -150,26 +230,51 @@ class HaploidLabelScheme(object):
         window = np.frombuffer(ref_seq[lo:hi].encode('ascii', 'replace'), dtype=np.uint8)
         return self._ref_table[window[majors - lo]]
 
+    def reference_codes(self, positions, ref_seq):
+        """The draft with '*' on insertion columns as label codes (labels.py:920): uint8 [n]."""
+        is_major = positions['minor'] == 0
+        ref_codes = np.zeros(len(positions), dtype=np.uint8)
+        ref_codes[is_major] = self.encode_reference(ref_seq, positions['major'][is_major])
+        return ref_codes
+
     def decode_variants(self, sample, ref_seq, ambig_ref=False, return_all=False):
         """Convert network output in sample to variant records (medaka/labels.py:889-1014).
 
         The consensus with gaps, the variant columns, the per-column qualities and the per-run sums come from the GPU
-        (``mdk_decode_variants``); the strings of the (few) variant runs, the ref == alt / ambiguous-draft filters and
-        the VCF normalisation are done here.  Returns a list of ``medaka_b200.variant.Variant``.
+        (``mdk_decode_variants``); the records are built by ``variant_records``.  Returns a list of
+        ``medaka_b200.variant.Variant``.
         """
-        from medaka_b200.variant import Variant
         pos = sample.positions
         if pos['minor'][0] != 0:
             raise ValueError("The first position of a sample must not be an insertion.")
-        is_major = pos['minor'] == 0
-        ref_codes = np.zeros(len(pos), dtype=np.uint8)            # '*' on insertion columns (labels.py:920)
-        ref_codes[is_major] = self.encode_reference(ref_seq, pos['major'][is_major])
+        ref_codes = self.reference_codes(pos, ref_seq)
         d = decode_variant_arrays(sample.label_probs, pos['minor'], ref_codes, self.device)
+        idx = _run_index(d['run_start'], d['run_len'])
+        return self.variant_records(
+            sample.ref_name, pos, ref_codes, ref_seq, d['run_start'], d['run_len'], d['run_pred_q'], d['run_ref_q'],
+            d['pred'][idx], d['pred_q'][idx] if self.verbose else None, d['ref_q'][idx] if self.verbose else None,
+            d['ref_q'][pos['minor'] == 0] if return_all else None, ambig_ref=ambig_ref, return_all=return_all)
+
+    def variant_records(self, ref_name, pos, ref_codes, ref_seq, run_start, run_len, run_pred_q, run_ref_q, run_pred,
+                        run_col_pred_q=None, run_col_ref_q=None, major_ref_q=None, ambig_ref=False, return_all=False):
+        """The host half of ``decode_variants`` (medaka/labels.py:927-1012): the decoded runs of one joined sample ->
+        list of ``medaka_b200.variant.Variant``.
+
+        :param pos, ref_codes: the sample's positions and ``reference_codes``.
+        :param run_start, run_len, run_pred_q, run_ref_q: the variant runs (columns of the sample) and their sums.
+        :param run_pred: the labels of all run columns back to back; ``run_col_pred_q`` / ``run_col_ref_q`` their
+            phreds (needed when ``self.verbose``).  :param major_ref_q: the reference phred of every major column
+            (needed with ``return_all``).
+        Covers string spelling, the ref == alt and ambiguous-draft filters, ``ambig_ref``, the verbose info, the gVCF
+        records and the VCF normalisation.
+        """
+        from medaka_b200.variant import Variant
         sym = np.frombuffer((self.symbols + 'N?').encode(), dtype=np.uint8)
-        major0 = int(pos['major'][0])
         variants = []
-        for rstart, rlen, spq, srq in zip(d['run_start'], d['run_len'], d['run_pred_q'], d['run_ref_q']):
-            rstart, rend = int(rstart), int(rstart + rlen)
+        o = 0
+        for rstart, rlen, spq, srq in zip(run_start, run_len, run_pred_q, run_ref_q):
+            rstart, rend, o0 = int(rstart), int(rstart + rlen), o
+            o += int(rlen)
             codes = ref_codes[rstart:rend]
             if np.any(codes == 6):
                 # spell the run's draft from the sequence itself (any IUPAC symbol)
@@ -177,7 +282,7 @@ class HaploidLabelScheme(object):
                                                                                      pos['minor'][rstart:rend]))
             else:
                 ref_g = sym[codes].tobytes().decode()
-            pred_g = sym[d['pred'][rstart:rend]].tobytes().decode()
+            pred_g = sym[run_pred[o0:o]].tobytes().decode()
             var_ref, var_pred = ref_g.replace('*', ''), pred_g.replace('*', '')
             if var_ref == var_pred:          # deletion followed by insertion of the same base (labels.py:942-944)
                 continue
@@ -186,32 +291,32 @@ class HaploidLabelScheme(object):
                     continue
                 if set(var_ref) - set(self.symbols) - {'N'}:
                     raise KeyError("draft symbol outside '*ACGTN' in a variant run at {}:{}".format(
-                        sample.ref_name, int(pos['major'][rstart])))
+                        ref_name, int(pos['major'][rstart])))
             qual = np.float32(spq) - np.float32(srq)          # log likelihood ratio (labels.py:974-975), float32
             info = {}
             if self.verbose:
                 info = {'ref_seq': ref_g, 'pred_seq': pred_g,
-                        'ref_qs': ','.join(self._pfmt(float(q)) for q in d['ref_q'][rstart:rend]),
-                        'pred_qs': ','.join(self._pfmt(float(q)) for q in d['pred_q'][rstart:rend]),
+                        'ref_qs': ','.join(self._pfmt(float(q)) for q in run_col_ref_q[o0:o]),
+                        'pred_qs': ','.join(self._pfmt(float(q)) for q in run_col_pred_q[o0:o]),
                         'ref_q': self._pfmt(float(srq)), 'pred_q': self._pfmt(float(spq)), 'n_cols': rend - rstart}
             genotype = {'GT': '1', 'GQ': self._pfmt(float(qual), 0)}
             var_pos = int(pos['major'][rstart])
             if pos['minor'][rstart] != 0:    # variant starts on an insertion column: prepend the draft base
                 var_ref = ref_seq[var_pos] + var_ref
                 var_pred = ref_seq[var_pos] + var_pred
-            v = Variant(sample.ref_name, var_pos, var_ref, alt=var_pred, filt='PASS', info=info,
+            v = Variant(ref_name, var_pos, var_ref, alt=var_pred, filt='PASS', info=info,
                         qual=self._pfmt(float(qual)), genotype_data=genotype)
             variants.append(v.normalize(reference=ref_seq))
         if return_all:
             # one record per reference position (labels.py:991-1012)
-            quals = d['ref_q'][is_major]
+            is_major = pos['minor'] == 0
+            quals = np.asarray(major_ref_q)
             qf, qi = np.char.mod("%.3f", quals), np.char.mod("%d", np.rint(quals))
             bases = [ref_seq[int(m)] for m in pos['major'][is_major]]
             for p_, base, f_, i_ in zip(pos['major'][is_major], bases, qf, qi):
-                variants.append(Variant(sample.ref_name, int(p_), base, alt='.', filt='.', info={}, qual=str(f_),
+                variants.append(Variant(ref_name, int(p_), base, alt='.', filt='.', info={}, qual=str(f_),
                                         genotype_data={'GT': '0', 'GQ': str(i_)}))
             variants.sort(key=lambda x: x.pos)
-        del major0
         return variants
 
     @property

@@ -277,6 +277,36 @@ class GRUModel(object):
         self._last_shape = (B, T)
         return int(ticket[0])
 
+    def submit_variant_decoded(self, feats, ref_bytes, calls_out, pred_q_out, ref_q_out):
+        """Queue one forward whose outputs are what variant decoding needs (mdk_engine_submit_variant_decoded); returns
+        a ticket.
+
+        ``feats`` float32 [B, T, F] and ``ref_bytes`` uint8 [B, T] (the draft's label code per column, 0x80 on insertion
+        columns) are numpy arrays (page-locked for an asynchronous copy) or CUDA tensors.  ``calls_out`` uint8 [B, T]
+        and ``pred_q_out`` / ``ref_q_out`` float32 [B, T] are numpy arrays or device addresses (int).  Everything must
+        stay alive and untouched until ``wait(ticket)`` (or ``sync``).
+        """
+        B, T, F = feats.shape
+        if tuple(ref_bytes.shape) != (B, T):
+            raise ValueError("ref_bytes must be [B, T] = [{}, {}], got {}".format(B, T, tuple(ref_bytes.shape)))
+        lib, ffi = _lm.lib, _lm.ffi
+
+        def ptr(x, ctype):
+            if isinstance(x, int):
+                return ffi.cast(ctype, x)
+            if hasattr(x, "data_ptr"):
+                if not x.is_contiguous():
+                    raise ValueError("tensors must be contiguous")
+                return ffi.cast(ctype, x.data_ptr())
+            return ffi.cast(ctype, ffi.from_buffer(x))
+
+        ticket = ffi.new("int64_t *")
+        _lm.check(lib.mdk_engine_submit_variant_decoded(
+            self._engine, ptr(feats, "const float *"), B, T, ptr(ref_bytes, "const uint8_t *"),
+            ptr(calls_out, "uint8_t *"), ptr(pred_q_out, "float *"), ptr(ref_q_out, "float *"), ticket))
+        self._last_shape = (B, T)
+        return int(ticket[0])
+
     def sync(self):
         """Wait for every call queued on the engine (mdk_engine_sync)."""
         _lm.check(_lm.lib.mdk_engine_sync(self._engine))

@@ -220,41 +220,52 @@ def predict_regions(output, bam, bam_regions, model, feature_encoder, chunk_len=
 
 
 class _LabelArena(object):
-    """Device memory for the decoded calls of a one-pass run (``predict_consensus``): 2 B per computed column.
+    """Device memory for the decoded outputs of a one-pass run: ``row_bytes[f]`` bytes of field f per computed column,
+    e.g. (1, 1) for the labels and quality bytes of ``predict_consensus``, (1, 4, 4) for the call bytes and the two
+    phreds of ``predict_variants``.
 
-    Slabs of ``2 * half`` bytes from mdk_dev_alloc hold labels in their first half and quality bytes at the same offset
-    in the second.  A row is (slab index, offset); every stitch call reads from one slab.
+    Slabs from mdk_dev_alloc hold ``half`` rows of every field, field after field.  A row is (slab index, offset); every
+    stitch call reads from one slab.  ``reset`` hands the slabs out again from the first (for a run in passes).
     """
 
-    def __init__(self, device, half=1 << 28):
+    def __init__(self, device, row_bytes, half=1 << 28):
         self.device, self.half = device, int(half)
+        self.row_bytes = tuple(int(b) for b in row_bytes)
+        self.field_at = [self.half * sum(self.row_bytes[:f]) for f in range(len(self.row_bytes))]
         self.slabs = []          # device addresses
-        self.used = self.half    # bytes taken from the newest slab's halves
+        self.cur = -1            # slab rows are taken from
+        self.used = self.half    # rows taken from it
+        self.peak = 0            # most slabs held at once, in bytes
 
     def take(self, n):
         """Room for n rows -> (slab index, offset of the first row)."""
         if n > self.half:
-            raise ValueError("a batch of {} columns does not fit a {} B arena slab".format(n, self.half))
+            raise ValueError("a batch of {} columns does not fit a {}-row arena slab".format(n, self.half))
         if self.used + n > self.half:
-            lib, ffi = _lm.load(), _lm.ffi
-            pp = ffi.new("void **")
-            _lm.check(lib.mdk_dev_alloc(self.device, 2 * self.half, pp))
-            self.slabs.append(int(ffi.cast("uintptr_t", pp[0])))
+            self.cur += 1
+            if self.cur == len(self.slabs):
+                lib, ffi = _lm.load(), _lm.ffi
+                pp = ffi.new("void **")
+                _lm.check(lib.mdk_dev_alloc(self.device, self.half * sum(self.row_bytes), pp))
+                self.slabs.append(int(ffi.cast("uintptr_t", pp[0])))
+                self.peak = max(self.peak, len(self.slabs) * self.half * sum(self.row_bytes))
             self.used = 0
         at = self.used
         self.used += n
-        return len(self.slabs) - 1, at
+        return self.cur, at
 
-    def labels(self, slab):
-        return self.slabs[slab]
+    def addr(self, slab, field, row=0):
+        """Device address of field ``field`` of row ``row`` of slab ``slab``."""
+        return self.slabs[slab] + self.field_at[field] + row * self.row_bytes[field]
 
-    def quals(self, slab):
-        return self.slabs[slab] + self.half
+    def reset(self):
+        self.cur, self.used = -1, self.half
 
     def free(self):
         lib, ffi = _lm.load(), _lm.ffi
         while self.slabs:
             _lm.check(lib.mdk_dev_free(self.device, ffi.cast("void *", self.slabs.pop())))
+        self.reset()
 
 
 def _stitch_view(sample, min_depth):
@@ -274,11 +285,12 @@ def _stitch_view(sample, min_depth):
                          label_probs=None, depth=depth)
 
 
-def _run_decoded(samples, arena, bam, regions, model, feature_encoder, chunk_len, chunk_ovlp, min_depth,
+def _run_decoded(samples, arena, bam, regions, model, feature_encoder, chunk_len, chunk_ovlp, view, submit,
                  batch_size=200, enable_chunking=True, bam_workers=2):
-    """``run_prediction`` for ``predict_consensus``: every batch's decoded calls go to the arena, and
-    ``samples[name] = (_stitch_view of the window, arena slab, row in the slab)`` is kept for each window (the first
-    window of a name wins, as in a store).  Returns the remainder regions."""
+    """``run_prediction`` for the one-pass runs: ``submit(features, data, slot, slab, row)`` queues every batch with its
+    decoded outputs going to the arena (``slot`` numbers the page-locked buffers it may reuse) and returns a ticket;
+    ``samples[name] = (view(window), arena slab, row in the slab)`` is kept for each window (the first window of a name
+    wins, as in a store).  Returns the remainder regions."""
     logger = common.get_named_logger('PWorker')
     if batch_size == "auto":
         batch_size = model.preferred_batch_size()
@@ -300,21 +312,43 @@ def _run_decoded(samples, arena, bam, regions, model, feature_encoder, chunk_len
                 model.reserve(max(model.preferred_batch_size(), nb), nt)
         while len(pending) >= depth:
             model.wait(pending.popleft())
-        # the page-locked feature slot is reused once the call that last used it has been waited for
-        xin = model.pinned("dfeats%d" % (n_calls % (depth + 1)), (nb, nt, nf), np.float32)
+        for s in data:
+            if len(s.positions) != nt:
+                raise ValueError("sample {} has {} columns in a batch of {}".format(s.name, len(s.positions), nt))
+        # the page-locked slots are reused once the call that last used them has been waited for
+        slot = n_calls % (depth + 1)
+        xin = model.pinned("dfeats%d" % slot, (nb, nt, nf), np.float32)
         np.copyto(xin, x, casting="same_kind")
         n_calls += 1
         slab, row = arena.take(nb * nt)
-        pending.append(model.submit_decoded(xin, arena.labels(slab) + row, arena.quals(slab) + row))
+        pending.append(submit(xin, data, slot, slab, row))
         for i, s in enumerate(data):
-            if len(s.positions) != nt:
-                raise ValueError("sample {} has {} columns in a batch of {}".format(s.name, len(s.positions), nt))
             name = s.name
             if name not in samples:
-                samples[name] = (_stitch_view(s, min_depth), slab, row + i * nt)
+                samples[name] = (view(s), slab, row + i * nt)
     while pending:
         model.wait(pending.popleft())
     return loader.remainders
+
+
+def _run_one_pass(samples, arena, bam, long_regions, remainder_regions, model, feature_encoder, chunk_len, chunk_ovlp,
+                  view, submit, batch_size, bam_workers):
+    """The long regions batched, then the remainder regions one window at a time (``predict_regions``), into the arena;
+    returns once the engine has finished."""
+    logger = common.get_named_logger('Predict')
+    remainder_regions = list(remainder_regions)
+    if long_regions:
+        logger.info("Processing {} long region(s) with batching.".format(len(long_regions)))
+        rem = _run_decoded(samples, arena, bam, long_regions, model, feature_encoder, chunk_len, chunk_ovlp, view,
+                           submit, batch_size=batch_size, bam_workers=bam_workers)
+        remainder_regions.extend([r[0] for r in rem])
+    if remainder_regions:
+        logger.info("Processing {} short region(s).".format(len(remainder_regions)))
+        new_rem = _run_decoded(samples, arena, bam, remainder_regions, model, feature_encoder, chunk_len, chunk_ovlp,
+                               view, submit, batch_size=1, enable_chunking=False)
+        if new_rem:
+            logger.warning("{} regions were not processed: {}.".format(len(new_rem), [x[0] for x in new_rem]))
+    model.sync()
 
 
 def predict_consensus(bam, bam_regions, model, feature_encoder, draft, output, chunk_len=10000, chunk_ovlp=1000,
@@ -351,21 +385,14 @@ def predict_consensus(bam, bam_regions, model, feature_encoder, draft, output, c
     logger = common.get_named_logger('Predict')
     model.check_feature_encoder_compatibility(feature_encoder)
     long_regions, remainder_regions = triage_regions(bam_regions, chunk_len, bam_chunk, chunk_ovlp)
-    arena = _LabelArena(model.device().index)
+    arena = _LabelArena(model.device().index, (1, 1))
     samples = collections.OrderedDict()
     try:
-        if long_regions:
-            logger.info("Processing {} long region(s) with batching.".format(len(long_regions)))
-            rem = _run_decoded(samples, arena, bam, long_regions, model, feature_encoder, chunk_len, chunk_ovlp,
-                               min_depth, batch_size=batch_size, bam_workers=bam_workers)
-            remainder_regions.extend([r[0] for r in rem])
-        if remainder_regions:
-            logger.info("Processing {} short region(s).".format(len(remainder_regions)))
-            new_rem = _run_decoded(samples, arena, bam, remainder_regions, model, feature_encoder, chunk_len,
-                                   chunk_ovlp, min_depth, batch_size=1, enable_chunking=False)
-            if new_rem:
-                logger.warning("{} regions were not processed: {}.".format(len(new_rem), [x[0] for x in new_rem]))
-        model.sync()
+        _run_one_pass(samples, arena, bam, long_regions, remainder_regions, model, feature_encoder, chunk_len,
+                      chunk_ovlp, lambda s: _stitch_view(s, min_depth),
+                      lambda x, data, slot, slab, row: model.submit_decoded(x, arena.addr(slab, 0, row),
+                                                                            arena.addr(slab, 1, row)),
+                      batch_size, bam_workers)
 
         def decode(views, pieces):
             # one stitch call per arena slab the pieces lie in, results back in piece order
@@ -373,7 +400,7 @@ def predict_consensus(bam, bam_regions, model, feature_encoder, draft, output, c
             seqs, quals = [None] * len(pieces), [None] * len(pieces)
             for slab in sorted({w[0] for w in where}):
                 ks = [k for k, w in enumerate(where) if w[0] == slab]
-                got = stitch.decode_label_pieces(arena.labels(slab), arena.quals(slab),
+                got = stitch.decode_label_pieces(arena.addr(slab, 0), arena.addr(slab, 1),
                                                  [where[k][1] + pieces[k].lo for k in ks],
                                                  [pieces[k].hi - pieces[k].lo for k in ks], device=arena.device)
                 for k, s, q in zip(ks, *got):
@@ -389,3 +416,176 @@ def predict_consensus(bam, bam_regions, model, feature_encoder, draft, output, c
         finally:
             arena.free()
     logger.info("Finished one-pass consensus of {} windows.".format(len(samples)))
+
+
+# bytes of arena per computed column of a variant run: the call byte and the two float32 phreds
+VARIANT_ROW_BYTES = (1, 4, 4)
+
+
+def estimated_columns(bases, chunk_len, chunk_ovlp, insertion_share=0.15):
+    """Computed columns (overlaps included) for ``bases`` draft bases: bases x (1 + insertion column share) x
+    chunk_len / (chunk_len - chunk_ovlp)."""
+    return int(bases * (1.0 + insertion_share) * chunk_len / max(chunk_len - chunk_ovlp, 1)) + 1
+
+
+def plan_passes(variant_regions, bam_regions, arena_bytes, chunk_len, chunk_ovlp, row_bytes=sum(VARIANT_ROW_BYTES)):
+    """Contigs of a ``predict_variants`` run grouped into passes whose estimated arena fits ``arena_bytes``.
+
+    Contigs come in the order the variant regions first name them, and only those with bam regions (the others have no
+    samples).  A pass never splits a contig; a contig whose estimate alone exceeds the budget gets a pass of its own.
+    The estimate is ``estimated_columns`` of the contig's bam region bases times ``row_bytes``.
+    :returns: list of lists of contig names.
+    """
+    bases = collections.OrderedDict()
+    for r in bam_regions:
+        bases[r.ref_name] = bases.get(r.ref_name, 0) + r.size
+    order = []
+    for r in variant_regions:
+        if r.ref_name in bases and r.ref_name not in order:
+            order.append(r.ref_name)
+    passes, cur, cur_bytes = [], [], 0
+    for name in order:
+        need = estimated_columns(bases[name], chunk_len, chunk_ovlp) * row_bytes
+        if cur and cur_bytes + need > arena_bytes:
+            passes.append(cur)
+            cur, cur_bytes = [], 0
+        cur.append(name)
+        cur_bytes += need
+    if cur:
+        passes.append(cur)
+    return passes
+
+
+def _variants_of_region(region, samples, index, arena, scheme, ref_seq, ambig_ref, return_all):
+    """``variant.variants`` for one region, on the calls in the arena: trimmed pieces (host, positions), join cuts and
+    decode (device), records (host)."""
+    from medaka_b200 import labels, stitch, variant
+    names = stitch.select_samples(index, region)
+    views = [samples[n][0] for n in names]
+    where = [samples[n][1:] for n in names]
+
+    def addr(field, k, lo):
+        slab, row = where[k]
+        return arena.addr(slab, field, row + lo)
+
+    pieces = stitch.plan_pieces(views)
+    inner = [p for p in pieces if not p.last]
+    cuts = np.full(len(pieces), -1, dtype=np.int64)
+    got = labels.variant_join_cuts([addr(0, p.sample, p.lo) for p in inner], [p.hi - p.lo for p in inner],
+                                   device=arena.device)
+    cuts[[k for k, p in enumerate(pieces) if not p.last]] = got
+    groups = list(variant.joined_pieces(views, pieces, cuts))
+    if not groups:
+        return []
+    segs, sample_seg, joined = [], [0], []
+    for g in groups:
+        parts = [common.Sample(ref_name=views[k].ref_name, features=None, labels=None, ref_seq=None,
+                               positions=views[k].positions[lo:hi], label_probs=None, depth=None) for k, lo, hi in g]
+        pos = common.Sample.from_samples(parts).positions
+        if pos['minor'][0] != 0:
+            raise ValueError("The first position of a sample must not be an insertion.")
+        joined.append(pos)
+        segs.extend((addr(0, k, lo), addr(1, k, lo), addr(2, k, lo), hi - lo) for k, lo, hi in g)
+        sample_seg.append(len(segs))
+    d = labels.decode_variant_segments([s[0] for s in segs], [s[1] for s in segs], [s[2] for s in segs],
+                                       [s[3] for s in segs], sample_seg, device=arena.device,
+                                       want_quals=scheme.verbose, want_ref_q=return_all)
+    run_edges = np.searchsorted(d['run_sample'], np.arange(len(joined) + 1), side='left')
+    col_edges = np.concatenate(([0], np.cumsum(d['run_len'])))
+    out, col0 = [], 0
+    for smp, pos in enumerate(joined):
+        r0, r1 = int(run_edges[smp]), int(run_edges[smp + 1])
+        c0, c1 = int(col_edges[r0]), int(col_edges[r1])
+        qs = (d['run_col_pred_q'][c0:c1], d['run_col_ref_q'][c0:c1]) if scheme.verbose else (None, None)
+        major_ref_q = d['ref_q'][col0:col0 + len(pos)][pos['minor'] == 0] if return_all else None
+        col0 += len(pos)
+        out.extend(variant.sort_records(scheme.variant_records(
+            region.ref_name, pos, scheme.reference_codes(pos, ref_seq), ref_seq, d['run_start'][r0:r1],
+            d['run_len'][r0:r1], d['run_pred_q'][r0:r1], d['run_ref_q'][r0:r1], d['run_pred'][c0:c1], *qs,
+            major_ref_q=major_ref_q, ambig_ref=ambig_ref, return_all=return_all)))
+    return out
+
+
+def predict_variants(bam, bam_regions, model, feature_encoder, draft, regions=None, ambig_ref=False, return_all=False,
+                     verbose=False, chunk_len=10000, chunk_ovlp=1000, batch_size=200, bam_chunk=int(1e6), bam_workers=2,
+                     arena_bytes=8 << 30, world_size=1):
+    """`medaka inference` followed by `medaka vcf` in one pass: the records ``predict_regions`` + ``variant.variants``
+    return, in the same order, without the probabilities ever leaving the GPU.
+
+    The engine decodes every window in its head (``GRUModel.submit_variant_decoded``: a call byte and the phreds of the
+    winning and of the draft's class, 9 B per column) into a device arena; per window only its name and positions stay
+    on the host.  The join cuts and the variant runs are computed on the device (``labels.variant_join_cuts``,
+    ``labels.decode_variant_segments``); only the runs come back.
+
+    The run goes in passes (``plan_passes``): contigs are grouped, in the order of the variant regions, so that a pass's
+    estimated arena fits ``arena_bytes``; each pass runs inference on its contigs' ``bam_regions``, then joins and decodes
+    its variant regions and hands the arena to the next.  A contig is never split; bam regions on contigs no variant
+    region asks for are skipped.  The arena is freed on return, also on error.
+
+    :param draft: FASTA path or mapping name -> sequence.
+    :param regions: Regions or region strings to call (default: every contig with samples, in index order).
+    """
+    if not hasattr(model, "submit_variant_decoded"):
+        raise NotImplementedError(
+            "predict_variants runs consensus (GRUModel) models only; for {} use predict_regions followed by "
+            "variant.variants".format(type(model).__name__))
+    from medaka_b200 import labels, stitch, variant
+    scheme_of_model = getattr(model, "label_scheme", None)
+    if scheme_of_model is not None and not isinstance(scheme_of_model, labels.HaploidLabelScheme):
+        raise NotImplementedError("predict_variants decodes haploid label schemes only; use predict_regions followed "
+                                  "by variant.variants")
+    if world_size != 1:
+        raise NotImplementedError("predict_variants runs on one GPU; for several, use predict_regions with one store "
+                                  "per rank, then variant.variants over the stores")
+    logger = common.get_named_logger('Predict')
+    model.check_feature_encoder_compatibility(feature_encoder)
+    if isinstance(draft, str):
+        draft = stitch.read_fasta(draft)
+    scheme = labels.HaploidLabelScheme(model.device().index)
+    scheme.verbose = verbose
+    # every contig with samples, in index order: the contigs of the bam regions, sorted (stitch.sample_index)
+    vregions = variant.variant_regions(sorted({r.ref_name for r in bam_regions}), regions)
+    passes = plan_passes(vregions, bam_regions, arena_bytes, chunk_len, chunk_ovlp)
+    ref_seqs = {}
+
+    def ref_seq(name):
+        if name not in ref_seqs:
+            ref_seqs[name] = draft[name].upper()
+        return ref_seqs[name]
+
+    arena = _LabelArena(model.device().index, VARIANT_ROW_BYTES)
+
+    def submit(x, data, slot, slab, row):
+        nb, nt = x.shape[:2]
+        ref = model.pinned("vref%d" % slot, (nb, nt), np.uint8)
+        for i, s in enumerate(data):
+            ins = s.positions['minor'] != 0
+            ref[i] = scheme.reference_codes(s.positions, ref_seq(s.ref_name)) | (ins.astype(np.uint8) << 7)
+        return model.submit_variant_decoded(x, ref, arena.addr(slab, 0, row), arena.addr(slab, 1, row),
+                                            arena.addr(slab, 2, row))
+
+    records = [None] * len(vregions)
+    n_windows = 0
+    try:
+        for k, contigs in enumerate(passes):
+            logger.info("Pass {} of {}: {} contig(s).".format(k + 1, len(passes), len(contigs)))
+            wanted = set(contigs)
+            long_regions, remainder_regions = triage_regions([r for r in bam_regions if r.ref_name in wanted],
+                                                             chunk_len, bam_chunk, chunk_ovlp)
+            samples = collections.OrderedDict()
+            arena.reset()
+            _run_one_pass(samples, arena, bam, long_regions, remainder_regions, model, feature_encoder, chunk_len,
+                          chunk_ovlp, lambda s: _stitch_view(s, 0), submit, batch_size, bam_workers)
+            n_windows += len(samples)
+            index = stitch.sample_index(samples)
+            for i, reg in enumerate(vregions):
+                if reg.ref_name in wanted:
+                    records[i] = _variants_of_region(reg, samples, index, arena, scheme, ref_seq(reg.ref_name),
+                                                     ambig_ref, return_all)
+    finally:
+        try:
+            model.sync()
+        finally:
+            arena.free()
+    logger.info("Finished one-pass variant calling of {} windows in {} pass(es).".format(n_windows, len(passes)))
+    return [v for recs in records if recs for v in recs]

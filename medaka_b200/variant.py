@@ -5,6 +5,10 @@ Stored samples of a region are trimmed at their overlaps (the plan of medaka_b20
 variant straddles a sample edge (``join_samples``), and every joined sample is decoded on the GPU
 (``HaploidLabelScheme.decode_variants`` -> libmedaka_b200 ``mdk_decode_variants``).  Writing VCF text is out of scope
 (SURVEY.md section 2); ``Variant`` carries what a VCF line needs.
+
+``variants`` is `medaka vcf` (the serial body of medaka/variant.py:180-244) over stores written by
+``prediction.predict_regions``; ``joined_pieces`` is ``join_samples`` replayed on positions and per-piece cuts, for the
+one-pass ``prediction.predict_variants``, whose calls never leave the device.
 """
 import collections
 
@@ -129,3 +133,92 @@ def variants_from_samples(samples, ref_seq, label_scheme=None, ambig_ref=False, 
     for joined in join_samples(trimmed_samples(samples), ref_seq, label_scheme):
         out.extend(label_scheme.decode_variants(joined, ref_seq, ambig_ref=ambig_ref, return_all=return_all))
     return out
+
+
+def sort_records(records):
+    """The order ``VCFWriter.write_variants(sort=True)`` writes one joined sample's records in (medaka/vcf.py:509-516):
+    a stable sort on 'chrom-pos' as loose versions, which for records of one contig is a stable sort on pos."""
+    return sorted(records, key=lambda v: v.pos)
+
+
+def joined_pieces(views, pieces, cuts):
+    """``join_samples`` on positions only: how the trimmed pieces are re-cut and grouped into joined samples.
+
+    :param views: list of Sample with positions (the pieces' samples); :param pieces: ``stitch.plan_pieces(views)``.
+    :param cuts: per piece, the index (within the piece) of its last insertion-free column whose call equals the draft,
+        or -1 when every column differs (``HaploidLabelScheme`` / ``mdk_variant_join_cuts``); ignored for pieces that
+        end a contig.
+    :yields: lists of (sample index, lo, hi) row ranges, one list per joined sample.
+    """
+    queue = []
+    p = None
+    for p, c in zip(pieces, cuts):
+        if p.last:
+            queue.append((p.sample, p.lo, p.hi))
+            yield queue
+            queue = []
+            continue
+        if c < 0:
+            queue.append((p.sample, p.lo, p.hi))
+            continue
+        major = views[p.sample].positions['major'][p.lo:p.hi]
+        cut = int(np.searchsorted(major, major[int(c)], side='left'))
+        to_yield = queue + ([(p.sample, p.lo, p.lo + cut)] if cut > 0 else [])
+        if to_yield:
+            yield to_yield
+        queue = [(p.sample, p.lo + cut, p.hi)]
+    if queue:
+        raise ValueError('Reached end of generator at {} without is_last_in_contig being True'.format(
+            views[p.sample].name))
+
+
+def _ref_seq(draft, ref_name):
+    return draft[ref_name].upper()
+
+
+def variants(stores, draft, regions=None, ambig_ref=False, return_all=False, verbose=False, device=0):
+    """`medaka vcf` (medaka/variant.py:180-244, serial path) over stores written by ``prediction.predict_regions``.
+
+    :param stores: one store path or several (a sample name found in more than one is read from the first).
+    :param draft: FASTA path or mapping name -> sequence.
+    :param regions: Regions or region strings (default: every indexed contig, in index order).  As in `medaka vcf`, a
+        region selects the samples overlapping it; their variants are not clipped to it.
+    :param ambig_ref: decode variants at ambiguous draft positions; :param return_all: also one record per draft
+        position (gVCF); :param verbose: per-run info fields.
+    :returns: list of Variant, in the order `medaka vcf` writes them: region by region, each joined sample's records
+        sorted by position.
+    """
+    from medaka_b200 import datastore, labels
+    if isinstance(stores, str):
+        stores = [stores]
+    if isinstance(draft, str):
+        draft = stitch.read_fasta(draft)
+    scheme = labels.HaploidLabelScheme(device)
+    scheme.verbose = verbose
+    opened = [datastore.DataStore(path, 'r') for path in stores]
+    out = []
+    try:
+        owner = {}
+        for ds in opened:
+            for name in ds.sample_registry:
+                owner.setdefault(name, ds)
+        index = stitch.sample_index(owner)
+        for reg in variant_regions(index, regions):
+            ref_seq = _ref_seq(draft, reg.ref_name)
+            samples = [owner[n].load_sample(n) for n in stitch.select_samples(index, reg)]
+            for joined in join_samples(trimmed_samples(samples), ref_seq, scheme):
+                out.extend(sort_records(scheme.decode_variants(joined, ref_seq, ambig_ref=ambig_ref,
+                                                               return_all=return_all)))
+    finally:
+        for ds in opened:
+            ds.close()
+    return out
+
+
+def variant_regions(index, regions=None):
+    """The regions of a `medaka vcf` run: as given (strings parsed), or every indexed contig in index order
+    (DataIndex.regions, medaka/datastore.py:446-451)."""
+    from medaka_b200.common import Region
+    if regions is None:
+        return [Region(name, None, None) for name in index]
+    return [Region.from_string(r) if isinstance(r, str) else r for r in regions]
