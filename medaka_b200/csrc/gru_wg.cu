@@ -450,94 +450,138 @@ cudaError_t launch_rec_tc(const float *gi, const RecX *xin, const __half *w_hh_t
 
 // =====================================================================================================
 // Layer-1 input projection on tensor cores:  gi[p][blk*128 + j] = sum_k W_ih[blk*128 + j][k] * x[p][k] + bias
-// Persistent: grid = 6 weight blocks x CT CTAs; each CTA keeps its 128x256 weight block (hi+lo, 128 KiB) resident in
-// shared memory and streams 128-position activation tiles (written by the layer-0 recurrent kernel directly in operand
-// layout) through a 2-stage ring of 64-wide K slices, filled by bulk async copies (TMA engine) behind an mbarrier.
-// Each warpgroup computes 64 gate rows x 128 positions with M64 N128 K16 wgmmas.
+// Persistent: grid = 6 weight blocks x CT CTAs; the six CTAs of one tile index walk the same tiles, so an activation
+// tile comes from HBM once and from L2 for the other five.  Warpgroup wg owns gate rows [64wg, 64wg + 64) of the CTA's
+// block and keeps their W hi and lo A fragments in REGISTERS for the whole kernel (the register form of wgmma: 2 planes
+// x 16 k-steps x 4 = 128 registers), so shared memory feeds only the activation operand.
+// 128-position activation tiles (written by the layer-0 recurrent kernel directly in operand layout) stream through a
+// ring of GW_NQ stages, one 64-wide K slice (hi + lo) each: slice q of every tile goes to stage q.  Thread 0 fills a
+// stage with bulk async copies behind its full mbarrier and refills it once all 8 warps have arrived on its empty
+// mbarrier.  A warp arrives when wgmma.wait_group 1 shows the group that read the stage complete, so one group of MMAs
+// stays in flight across slices and the next tile's slices load under this tile's MMAs.
+// At the end of a tile the accumulators (+ bias) go to a staging buffer laid out as gi's quad layout, and warp 0 writes
+// it out with one bulk store per lane (one window quad of one tile-step, 2 KiB contiguous in gi) while the next tile's
+// MMAs run.
+// Per element the sum runs in the order slice q, product (hi.hi, hi.lo, lo.hi), k-step.
 // =====================================================================================================
 constexpr int GW_THREADS = 256;
 constexpr int GW_QK = 8;                                        // k-groups per stage (K = 64)
 constexpr int GW_STAGE_PLANE = GW_QK * XT_ROWS * 16;            // 16 KiB
 constexpr int GW_STAGE = 2 * GW_STAGE_PLANE;                    // hi + lo
-constexpr int GW_NQ = XT_K / 8 / GW_QK;                         // stages per tile
-constexpr int GW_X_OFF = XT_TILE_BYTES;                         // behind the weight block
-constexpr int GW_BAR_OFF = GW_X_OFF + 2 * GW_STAGE;
-constexpr int GW_SMEM = GW_BAR_OFF + 16;
+constexpr int GW_NQ = XT_K / 8 / GW_QK;                         // slices per tile = stages of the ring
+constexpr int GW_KS = XT_K / 16;                                // k-steps per tile
+constexpr int GW_TS = XT_ROWS / WT;                             // gi tile-steps per tile
+constexpr int GW_QUAD = H * 4;                                  // floats of one (tile-step, block, window quad) piece of gi
+// staging: [tile-step 8][window quad 4] pieces, each padded by 16 floats so that the two window quads a warp's float2
+// stores reach in one instruction fall in opposite halves of the banks
+constexpr int GW_QUAD_PAD = GW_QUAD + 16;
+constexpr int GW_OUT_OFF = GW_NQ * GW_STAGE;
+constexpr int GW_BAR_OFF = GW_OUT_OFF + GW_TS * 4 * GW_QUAD_PAD * 4;    // full[GW_NQ], empty[GW_NQ]
+constexpr int GW_SMEM = GW_BAR_OFF + 2 * GW_NQ * 8;
+static_assert(GW_SMEM <= 227 * 1024, "smem budget");
+static_assert(GW_TS * 4 == 32, "one bulk store per lane of warp 0");
 
 __global__ void __launch_bounds__(GW_THREADS, 1)
 gemm_tc_kernel(const uint8_t *__restrict__ x_tiles, const __half *__restrict__ w_in_tm, const float *__restrict__ bias,
                float *__restrict__ gi, int64_t P, int64_t ntiles) {
     extern __shared__ __align__(128) uint8_t smem[];
-    uint64_t *full = reinterpret_cast<uint64_t *>(smem + GW_BAR_OFF);
+    uint64_t *full = reinterpret_cast<uint64_t *>(smem + GW_BAR_OFF), *empty = full + GW_NQ;
+    float *stg = reinterpret_cast<float *>(smem + GW_OUT_OFF);
     const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
     const int gq = lane >> 2, cq = lane & 3;
     const int blk = blockIdx.x;                 // weight block: dir*3 + gate
+    const int j0 = wg * 64 + warp * 16 + gq;    // this thread's gate rows: j0 and j0 + 8
     const uint32_t sbase = smem_u32(smem);
-    // weights (row-major fp16 [blk][plane][row j][k 256]) -> [plane][kg 32][row 128][8]
-    for (int i = tid; i < 2 * H * (H2 / 8); i += GW_THREADS) {
-        const int kg = i & 31, r = (i >> 5) & (H - 1), p = i >> 12;
-        const uint4 v = reinterpret_cast<const uint4 *>(w_in_tm + (((size_t)blk * 2 + p) * H + r) * H2)[kg];
-        *reinterpret_cast<uint4 *>(smem + p * XT_PLANE_BYTES + kg * (XT_ROWS * 16) + r * 16) = v;
-    }
-    if (tid == 0) {
-        mbar_init(&full[0], 1);
-        mbar_init(&full[1], 1);
-        fence_mbar_init();
-    }
-    fence_proxy_async_smem();   // the weight block's generic-proxy stores -> visible to wgmma reads
-    __syncthreads();
     const int64_t my_tiles = blockIdx.y < ntiles ? (ntiles - 1 - blockIdx.y) / gridDim.y + 1 : 0;
-    const int64_t nst = my_tiles * GW_NQ;
-    auto issue = [&](int64_t it) {
-        const int64_t tile = blockIdx.y + (it / GW_NQ) * gridDim.y;
-        const int q = (int)(it % GW_NQ), s = (int)(it & 1);
-        const uint8_t *src = x_tiles + tile * (int64_t)XT_TILE_BYTES + q * GW_STAGE_PLANE;
-        mbar_arrive_expect_tx(&full[s], GW_STAGE);
-        bulk_g2s(smem + GW_X_OFF + s * GW_STAGE, src, GW_STAGE_PLANE, &full[s]);
-        bulk_g2s(smem + GW_X_OFF + s * GW_STAGE + GW_STAGE_PLANE, src + XT_PLANE_BYTES, GW_STAGE_PLANE, &full[s]);
+    auto issue = [&](int64_t n, int q) {        // slice q of this CTA's n-th tile -> stage q
+        const uint8_t *src = x_tiles + (blockIdx.y + n * gridDim.y) * (int64_t)XT_TILE_BYTES + q * GW_STAGE_PLANE;
+        mbar_arrive_expect_tx(&full[q], GW_STAGE);
+        bulk_g2s(smem + q * GW_STAGE, src, GW_STAGE_PLANE, &full[q]);
+        bulk_g2s(smem + q * GW_STAGE + GW_STAGE_PLANE, src + XT_PLANE_BYTES, GW_STAGE_PLANE, &full[q]);
     };
     if (tid == 0) {
-        if (nst > 0) issue(0);
-        if (nst > 1) issue(1);
+        for (int q = 0; q < GW_NQ; ++q) {
+            mbar_init(&full[q], 1);
+            mbar_init(&empty[q], GW_THREADS / 32);
+        }
+        fence_mbar_init();
+        if (my_tiles > 0)
+            for (int q = 0; q < GW_NQ; ++q) issue(0, q);
     }
-    const float bj[2] = {bias[blk * H + wg * 64 + warp * 16 + gq], bias[blk * H + wg * 64 + warp * 16 + gq + 8]};
+    // W (row-major fp16 [blk][plane][row j][k 256]) hi and lo A fragments of rows j0, j0 + 8 (layout: ptx.cuh Wgmma)
+    uint32_t wa[2][GW_KS][4];
+#pragma unroll
+    for (int p = 0; p < 2; ++p)
+#pragma unroll
+        for (int ks = 0; ks < GW_KS; ++ks) {
+            const __half *w = w_in_tm + (((size_t)blk * 2 + p) * H + j0) * H2 + ks * 16 + 2 * cq;
+            wa[p][ks][0] = ld_u32(w);
+            wa[p][ks][1] = ld_u32(w + 8 * H2);
+            wa[p][ks][2] = ld_u32(w + 8);
+            wa[p][ks][3] = ld_u32(w + 8 * H2 + 8);
+        }
+    const float bj[2] = {bias[blk * H + j0], bias[blk * H + j0 + 8]};
+    const uint64_t policy = l2_evict_first_policy();
+    __syncthreads();                            // the mbarriers are initialised
+    // stage q has been read by this warp's MMAs of tile n: release it, and thread 0 refills it with tile n + 1
+    auto release = [&](int64_t n, int q) {
+        if (lane == 0) mbar_arrive(&empty[q]);
+        if (tid == 0 && n + 1 < my_tiles) {
+            mbar_wait(&empty[q], (uint32_t)(n & 1));
+            issue(n + 1, q);
+        }
+        __syncwarp();
+    };
     float acc[64];
 #pragma unroll 1
-    for (int64_t it = 0; it < nst; ++it) {
-        const int q = (int)(it % GW_NQ), s = (int)(it & 1);
-        mbar_wait(&full[s], (uint32_t)((it >> 1) & 1));
-        wg_fence();
+    for (int64_t n = 0; n < my_tiles; ++n) {
 #pragma unroll
-        for (int prod = 0; prod < 3; ++prod) {
-            const int pa = prod == 2, pb = prod == 1;   // W part hi, hi, lo ; x part hi, lo, hi
+        for (int q = 0; q < GW_NQ; ++q) {
+            mbar_wait(&full[q], (uint32_t)(n & 1));
+            wg_fence();
 #pragma unroll
-            for (int kk = 0; kk < GW_QK / 2; ++kk) {
-                const uint64_t a = make_smem_desc(sbase + pa * XT_PLANE_BYTES + (q * GW_QK + 2 * kk) * (XT_ROWS * 16) + wg * 64 * 16,
-                                                  XT_ROWS * 16, 128);
-                const uint64_t b = make_smem_desc(sbase + GW_X_OFF + s * GW_STAGE + pb * GW_STAGE_PLANE + 2 * kk * (XT_ROWS * 16),
-                                                  XT_ROWS * 16, 128);
-                Wgmma<128>::ss(acc, a, b, (q | prod | kk) ? 1u : 0u);
+            for (int prod = 0; prod < 3; ++prod) {
+                const int pa = prod == 2, pb = prod == 1;   // W part hi, hi, lo ; x part hi, lo, hi
+#pragma unroll
+                for (int kk = 0; kk < GW_QK / 2; ++kk) {
+                    const uint64_t b = make_smem_desc(sbase + q * GW_STAGE + pb * GW_STAGE_PLANE + 2 * kk * (XT_ROWS * 16),
+                                                      XT_ROWS * 16, 128);
+                    Wgmma<128>::rs(acc, wa[pa][q * (GW_QK / 2) + kk], b, (q | prod | kk) ? 1u : 0u);
+                }
+            }
+            wg_commit();
+            if (q > 0) {
+                wg_wait_1();
+                release(n, q - 1);
             }
         }
-        wg_commit();
         wg_wait_all();
         wg_hold(acc);
-        __syncthreads();                          // both warpgroups have read stage s
-        if (tid == 0 && it + 2 < nst) issue(it + 2);
-        if (q == GW_NQ - 1) {
-            // quad layout (common.cuh): position c of this tile = tile-step tile*8 + c/16, window c%16
-            const int64_t tile = blockIdx.y + (it / GW_NQ) * gridDim.y;
-            const int64_t prem = P - tile * XT_ROWS;   // rows of this tile that exist (a multiple of 16)
+        release(n, GW_NQ - 1);
+
+        // ---- epilogue: accumulators + bias -> staging (quad layout) -> bulk stores under the next tile's MMAs ----
+        const int64_t tile = blockIdx.y + n * gridDim.y;
+        const int64_t prem = P - tile * XT_ROWS;    // rows of this tile that exist (a multiple of 16)
+        if (tid < 32) bulk_wait_read_all();         // the previous tile's stores have read the staging buffer
+        __syncthreads();
 #pragma unroll
-            for (int k = 0; k < 64; k += 2) {
-                const int c = 8 * (k >> 2) + 2 * cq, hb = (k >> 1) & 1;
-                if (c >= prem) continue;
-                const int j = wg * 64 + warp * 16 + gq + 8 * hb;
-                float *o = gi + ((((tile * (XT_ROWS / WT) + (c >> 4)) * 6 + blk) * 4 + ((c & 15) >> 2)) * H + j) * 4 + (c & 3);
-                __stcs(reinterpret_cast<float2 *>(o), make_float2(acc[k] + bj[hb], acc[k + 1] + bj[hb]));
-            }
+        for (int k = 0; k < 64; k += 2) {
+            // position c = 8i + 2cq + e of the tile: tile-step i / 2, window quad 2 (i & 1) + cq / 2, w4 = 2 (cq & 1) + e
+            const int i = k >> 2, hb = (k >> 1) & 1;
+            float *o = stg + ((i >> 1) * 4 + 2 * (i & 1) + (cq >> 1)) * GW_QUAD_PAD + (j0 + 8 * hb) * 4 + 2 * (cq & 1);
+            *reinterpret_cast<float2 *>(o) = make_float2(acc[k] + bj[hb], acc[k + 1] + bj[hb]);
+        }
+        fence_proxy_async_smem();                   // staging writes -> visible to the bulk copies
+        __syncthreads();
+        if (tid < 32) {
+            const int ts = lane >> 2, cg = lane & 3;
+            if (ts * WT < prem)
+                bulk_s2g(gi + (((tile * GW_TS + ts) * 6 + blk) * 4 + cg) * GW_QUAD, stg + lane * GW_QUAD_PAD,
+                         GW_QUAD * 4, policy);
+            bulk_commit();
         }
     }
+    if (tid < 32) bulk_wait_all();
 }
 
 cudaError_t launch_gemm_tc(const void *x_tiles, const __half *w_in_tm, const float *bias, float *gi, int64_t P,
