@@ -37,7 +37,8 @@ namespace mdk {
 //   NT = 2: hi and lo planes of N = 32 rows each and three m64n32k16 MMAs (no registers left for accumulators twice as
 //           wide: 239-252 of 255).
 // FUSE_X (layer 0, F <= 16): the input projection W_ih . x_t is the same products per gate on an x tile laid out like
-// the h tile (K = 16), so layer 0 needs no gi buffer.  OUT: fp16 hi/lo operand tiles of the projection GEMM (layer 0),
+// the h tile (K = 16), so layer 0 needs no gi buffer.  OUT: fp16 hi/lo operand tiles of the projection GEMM (layer 0:
+// copied under the next step's MMAs from the h tile buffer, which already holds them in that layout, see store_h0),
 // fp32 rows, or (layer 1) partial logits: the 5-row linear head in fp32 on the CUDA cores, from the h values the threads
 // already hold, while the next step's MMAs run (see head_partials).
 // =====================================================================================================
@@ -144,7 +145,11 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
     float ar[NACC], az[NACC], an[NACC], axn[NX], hp[NA];
 #pragma unroll
     for (int k = 0; k < NA; ++k) hp[k] = 0.f;
-    // pre-activations of time t into the accumulators (gi in quad layout, common.cuh: the pair e = 0, 1 is contiguous)
+    // pre-activations of time t into the accumulators (gi in quad layout, common.cuh: the pair e = 0, 1 is contiguous).
+    // gi_thr: this thread's first element (tile wtile0, t = 0, its window quad and hidden unit j0); the rest of an address
+    // is t and compile-time offsets.
+    const float *gi_thr = FUSE_X ? nullptr
+                                 : gi + wtile0 * T * GI_TS_FLOATS + ((dir * 3 * 4 + (cq >> 1)) * H + j0) * 4 + 2 * (cq & 1);
     auto load_pre = [&](int64_t t) {
 #pragma unroll
         for (int i = 0; i < N / 8; ++i)
@@ -154,9 +159,8 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
                 if (FUSE_X) {
 #pragma unroll
                     for (int gate = 0; gate < 3; ++gate) v[gate] = make_float2(bx[gate][hb], bx[gate][hb]);
-                } else if (wtile0 + (i >> 1) < ntiles) {
-                    const float *p = gi + ((wtile0 + (i >> 1)) * T + t) * GI_TS_FLOATS +
-                                     (((dir * 3) * 4 + 2 * (i & 1) + (cq >> 1)) * H + j0 + 8 * hb) * 4 + 2 * (cq & 1);
+                } else if (i < 2 || wtile0 + (i >> 1) < ntiles) {     // (the grid has no CTA without a first tile)
+                    const float *p = gi_thr + ((i >> 1) * T + t) * GI_TS_FLOATS + (2 * (i & 1) * H + 8 * hb) * 4;
 #pragma unroll
                     for (int gate = 0; gate < 3; ++gate) v[gate] = __ldcs(reinterpret_cast<const float2 *>(p + gate * 16 * H));
                 }
@@ -200,7 +204,6 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
         for (int m = 0; m < NT; ++m) {
             if (xoff[m] < 0) continue;
             stage_x(0, m, xsrc[m] ? xsrc[m][t_first * xF] : 0.f);
-            if (xsrc[m] && T > 1) xreg[m] = xsrc[m][(dir ? T - 2 : 1) * xF];
         }
     }
     load_pre(t_first);
@@ -264,6 +267,24 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
         const int64_t wt = wtile0 + n / RT_N;
         if (wt < ntiles) plog[((dir * ntiles + wt) * T + t) * PLOG_TS_FLOATS + c * RT_N + (n & 15)] = s;
     };
+    // store_h0(b, t) (OUT_TILES): h_t from tile buffer b to the projection GEMM's operand tiles.  The 16 rows of one
+    // (window tile m, plane p, k-group kg) are 256 contiguous bytes in the buffer and in the operand tile (rows
+    // (wt T + t) 16 .. + 15 of a 128-row tile), so the CTA copies them as they are, one 16-byte row per thread and
+    // vector: vector q = tid + 256 r is row q & 15 of piece q >> 4 = (m * 2 + p) * 16 + kg.  Padding windows of a ragged
+    // tile go out too (never read back); tiles >= ntiles do not.
+    auto store_h0 = [&](int b, int64_t t) {
+#pragma unroll
+        for (int r = 0; r < NT * 512 / RW_THREADS; ++r) {
+            const int q = tid + RW_THREADS * r, row = q & 15, kg = (q >> 4) & 15, p = (q >> 8) & 1, m = q >> 9;
+            const int64_t wt = wtile0 + m;
+            if (wt >= ntiles) continue;
+            const int64_t orow = (wt * T + t) * RT_N + row;
+            const int4 v = *reinterpret_cast<const int4 *>(smem + L::h_off + b * L::PLANES * L::HPLANE + p * L::HLO + kg * L::KG +
+                                                           (m * RT_N + row) * 16);
+            *reinterpret_cast<int4 *>(reinterpret_cast<uint8_t *>(h_out) + (orow >> 7) * (int64_t)XT_TILE_BYTES +
+                                      p * XT_PLANE_BYTES + (dir * (H / 8) + kg) * (XT_ROWS * 16) + (orow & (XT_ROWS - 1)) * 16) = v;
+        }
+    };
 
 #pragma unroll 1
     for (int64_t step = 0; step < T; ++step) {
@@ -318,7 +339,17 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
             }
         }
         wg_commit();
-        // the next step's L2 prefetch and feature loads run under the MMAs
+        // FUSE_X: the next step's features load under the MMAs, so that their latency is not paid after the wait (the
+        // fence before the barrier waits for outstanding loads)
+        if (FUSE_X && step + 1 < T) {
+#pragma unroll
+            for (int m = 0; m < NT; ++m)
+                if (xsrc[m]) xreg[m] = xsrc[m][(dir ? t - 1 : t + 1) * xF];
+        }
+        // h of the previous step (published by the last barrier, and read by these MMAs) goes out to the h0 tiles; the
+        // buffer is rewritten only after the next barrier
+        if (OUT == OUT_TILES && step > 0) store_h0(buf, dir ? t + 1 : t - 1);
+        // the L2 prefetch of gi three steps ahead runs under the MMAs too
         if (!FUSE_X && tid == 0 && step + GI_PREFETCH_STEPS < T) {
             const int64_t tp = dir ? t - GI_PREFETCH_STEPS : t + GI_PREFETCH_STEPS;
 #pragma unroll
@@ -370,34 +401,25 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
             for (int m = 0; m < NT; ++m) {
                 if (xoff[m] < 0) continue;
                 stage_x(buf ^ 1, m, xreg[m]);
-                if (xsrc[m] && step + 2 < T) xreg[m] = xsrc[m][(dir ? t - 2 : t + 2) * xF];
             }
         }
-        // ---- outputs of this step ----
-        if (!LOGITS) {
+        // ---- outputs of this step (OUT_TILES: by store_h0, from the tile buffer) ----
+        if (OUT == OUT_ROWS) {
 #pragma unroll
             for (int k = 0; k < NA; ++k) {
                 const int i = k >> 2, n = 8 * i + 2 * cq + (k & 1);
                 const int64_t wt = wtile0 + (i >> 1);
                 if (wt >= ntiles) continue;
                 const int64_t orow = (wt * T + t) * RT_N + (n & 15);
-                const int kcol = dir * H + j0 + 8 * ((k >> 1) & 1);
-                if (OUT == OUT_TILES) {
-                    __half hi, lo;
-                    split_f16(hp[k], hi, lo);
-                    __half *o = reinterpret_cast<__half *>(reinterpret_cast<uint8_t *>(h_out) + (orow >> 7) * (int64_t)XT_TILE_BYTES +
-                                                           (kcol >> 3) * (XT_ROWS * 16) + (orow & (XT_ROWS - 1)) * 16) + (kcol & 7);
-                    o[0] = hi;
-                    o[XT_PLANE_BYTES / 2] = lo;
-                } else {
-                    reinterpret_cast<float *>(h_out)[orow * H2 + kcol] = hp[k];
-                }
+                reinterpret_cast<float *>(h_out)[orow * H2 + dir * H + j0 + 8 * ((k >> 1) & 1)] = hp[k];
             }
         }
-        if (step + 1 < T) load_pre(dir ? t - 1 : t + 1);
+        // (FUSE_X: biases, no loads; unconditional, so that the compiler moves them next to the MMAs that read them)
+        if (FUSE_X || step + 1 < T) load_pre(dir ? t - 1 : t + 1);
         fence_proxy_async_smem();     // h / x tile writes -> visible to the next step's wgmma operand reads
         __syncthreads();
     }
+    if (OUT == OUT_TILES) store_h0((int)(T & 1), dir ? 0 : T - 1);     // the last step's h
     if (LOGITS) {                     // the last two steps' logits: step T - 2 (partials in red), step T - 1 (in hp)
         if (T > 1) head_store((int)((T - 1) & 1), dir ? 1 : T - 2);
         head_partials((int)(T & 1));
