@@ -320,7 +320,26 @@ int mdk_rl_forward(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P,
  * mdk_rl_forward: windows never interact. */
 int mdk_rl_submit(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P, int64_t D, int64_t F,
                   float *probs_host, uint8_t *labels_host, int64_t *ticket);
+/* one-pass consensus with a read-level model: the same forward, but what leaves the engine is the decoded call per
+ * position instead of the probabilities - labels_out uint8 [B][P] (argmax, first max wins) and quals_out uint8 [B][P]
+ * (phred+33 byte of the winning probability, as mdk_engine_submit_decoded, or NULL).  Both are computed by the engine's
+ * head from the fp32 probability it produces, and are bit-identical to mdk_decode_consensus on the probabilities
+ * mdk_rl_submit returns for the same features.  x_host is host memory as for mdk_rl_submit; the outputs may be host or
+ * device memory.  Packed like mdk_rl_submit (ordinary and decoded calls share groups); complete after
+ * mdk_rl_wait(ticket) or mdk_rl_sync. */
+int mdk_rl_submit_decoded(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P, int64_t D, int64_t F,
+                          uint8_t *labels_out, uint8_t *quals_out, int64_t *ticket);
+/* one-pass variant calling with a read-level model: ref_bytes uint8 [B][P] in, calls_out uint8 [B][P] and pred_q_out /
+ * ref_q_out float [B][P] out, with the encodings of mdk_engine_submit_variant_decoded and bit-identical to what
+ * mdk_decode_variants computes from the probabilities mdk_rl_submit returns for the same features.  x_host is host
+ * memory; ref_bytes and the outputs may be host or device memory.  Packed like mdk_rl_submit (ordinary, decoded and
+ * variant-decoded calls share groups); complete after mdk_rl_wait(ticket) or mdk_rl_sync. */
+int mdk_rl_submit_variant_decoded(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P, int64_t D, int64_t F,
+                                  const uint8_t *ref_bytes, uint8_t *calls_out, float *pred_q_out, float *ref_q_out,
+                                  int64_t *ticket);
 int mdk_rl_wait(mdk_rl_engine *e, int64_t ticket);
+/* launch the open group (if any) and wait for everything queued on the engine */
+int mdk_rl_sync(mdk_rl_engine *e);
 /* launch the group that is still collecting calls (if any) without waiting for it */
 int mdk_rl_flush(mdk_rl_engine *e);
 /* size the group buffers for groups of up to min(windows, the group limit at P) windows of P positions (launches the

@@ -24,12 +24,14 @@
 //   LSTM recurrences      rl_lstm_tc_kernel (H = 128, one CTA per 16-window tile and direction), rl_lstm384_tc_kernel
 //                         (H = 384, one 8-CTA cluster per tile and direction); fp32 twin rl_lstm_fp32<H>
 //   head                  Linear(2H -> 5) + softmax + argmax: head_kernel (misc.cu, shared with the counts models) at
-//                         H = 128, rl_head768_kernel at H = 384
+//                         H = 128, rl_head768_kernel at H = 384; both also write the decoded outputs of
+//                         mdk_rl_submit_decoded / mdk_rl_submit_variant_decoded (HEAD_QUALS / HEAD_VARIANT)
 #include <string>
 #include <unordered_map>
 #include <vector>
 
 #include "common.cuh"
+#include "phred.cuh"
 #include "ptx.cuh"
 #include "rec_common.cuh"
 
@@ -839,10 +841,15 @@ __global__ void __cluster_dims__(L3_CL, 1, 1) __launch_bounds__(L3_THREADS, 1)
 }
 
 // Linear(2H = 768 -> 5) + softmax + argmax: one warp per position, 24 inputs per lane, the weights in shared memory.
-// labels (may be NULL): argmax of the five probabilities as written, first maximum wins (np.argmax, labels.py:1063)
+// labels (may be NULL for HEAD_PLAIN): argmax of the five probabilities as written, first maximum wins (np.argmax,
+// labels.py:1063).  MODE as head_kernel's (misc.cu): HEAD_QUALS also writes the phred byte of the winning probability,
+// HEAD_VARIANT the call byte and the phreds of the winning and of the reference class (and the phred byte where quals
+// is given), all from the fp32 probabilities the kernel stores (phred.cuh).  HEAD_PLAIN is the ordinary forward's.
+template <int MODE>
 __global__ void __launch_bounds__(256) rl_head768_kernel(const float *__restrict__ h1, const float *__restrict__ lin_w,
                                                          const float *__restrict__ lin_b, int64_t n_pos,
-                                                         float *__restrict__ probs, uint8_t *__restrict__ labels) {
+                                                         float *__restrict__ probs, uint8_t *__restrict__ labels,
+                                                         uint8_t *__restrict__ quals, HeadVariant var) {
     constexpr int W2 = 2 * RL_H3;
     __shared__ __align__(16) float ws[NCLS * W2];
     for (int i = threadIdx.x; i < NCLS * W2; i += blockDim.x) ws[i] = lin_w[i];
@@ -878,7 +885,7 @@ __global__ void __launch_bounds__(256) rl_head768_kernel(const float *__restrict
         for (int c = 1; c < NCLS; ++c) if (lane == c) v = s[c];
         const float pr = v / sum;                  // lane c < 5: probability of class c
         if (lane < NCLS) probs[p * NCLS + lane] = pr;
-        if (labels) {                              // argmax over lanes 0..4, first maximum wins
+        if (MODE != HEAD_PLAIN || labels) {        // argmax over lanes 0..4, first maximum wins
             float best = lane < NCLS ? pr : -1.f;
             int arg = lane;
 #pragma unroll
@@ -887,7 +894,25 @@ __global__ void __launch_bounds__(256) rl_head768_kernel(const float *__restrict
                 const int oa = __shfl_xor_sync(0xffffffffu, arg, m);
                 if (ob > best || (ob == best && oa < arg)) { best = ob; arg = oa; }
             }
-            if (lane == 0) labels[p] = (uint8_t)arg;
+            if (MODE == HEAD_PLAIN) {
+                if (lane == 0) labels[p] = (uint8_t)arg;
+            } else {
+                uint8_t ref = 0;
+                float p_ref = 0.f;
+                if (MODE == HEAD_VARIANT) {        // the reference class's probability from its lane
+                    ref = var.ref[p];
+                    p_ref = __shfl_sync(0xffffffffu, pr, ref_class(ref));
+                }
+                if (lane == 0) {
+                    if (labels) labels[p] = (uint8_t)arg;
+                    if (MODE == HEAD_QUALS || quals) quals[p] = phred_char(best);
+                    if (MODE == HEAD_VARIANT) {
+                        var.calls[p] = variant_call(arg, ref);
+                        var.pred_q[p] = phred_f32(best);
+                        var.ref_q[p] = phred_f32(p_ref);
+                    }
+                }
+            }
         }
     }
 }
@@ -951,6 +976,10 @@ struct mdk_rl_engine {
     int64_t cap_pos = 0;
     float *z = nullptr, *gi = nullptr, *h0 = nullptr, *h1 = nullptr, *probs = nullptr;
     uint8_t *labels = nullptr;
+    // decoded outputs (mdk_rl_submit_decoded / mdk_rl_submit_variant_decoded), 11 B per position for cap_pos positions:
+    // allocated when the first decoded call is staged, freed with the other group buffers when they regrow
+    uint8_t *quals = nullptr, *ref = nullptr, *calls = nullptr;
+    float *pred_q = nullptr, *ref_q = nullptr;
     Packing pk;
     int64_t last_B = 0, last_P = 0;                  // the last completed mdk_rl_forward (mdk_rl_debug_read), 0 = none
 };
@@ -1151,14 +1180,27 @@ int rl_ensure_group(mdk_rl_engine *e, int64_t pos) {
     e->last_B = e->last_P = 0;                       // the last mdk_rl_forward's stages go with the old buffers
     float **fb[5] = {&e->z, &e->gi, &e->h0, &e->h1, &e->probs};
     for (float **p : fb) { if (*p) cudaFree(*p); *p = nullptr; }
-    if (e->labels) cudaFree(e->labels);
-    e->labels = nullptr;
+    void **db[6] = {(void **)&e->labels, (void **)&e->quals, (void **)&e->ref, (void **)&e->calls, (void **)&e->pred_q,
+                    (void **)&e->ref_q};
+    for (void **p : db) { if (*p) cudaFree(*p); *p = nullptr; }
     e->cap_pos = 0;
     const size_t n = (size_t)pos, H = (size_t)e->H;
     const size_t floats[5] = {n * H, n * 8 * H, n * 2 * H, n * 2 * H, n * NCLS};
     for (int i = 0; i < 5; ++i) MDK_CUDA(cudaMalloc(fb[i], floats[i] * sizeof(float)));
     MDK_CUDA(cudaMalloc(&e->labels, n));
     e->cap_pos = pos;
+    return MDK_OK;
+}
+
+// The decoded outputs' group buffers (quals, ref, calls, pred_q, ref_q) for cap_pos positions, allocated when the first
+// decoded call is staged.  Nothing frees them while a group collects (rl_ensure_group only runs when one opens, after
+// draining the streams), so a group in flight never loses them.
+int rl_ensure_decoded(mdk_rl_engine *e) {
+    if (e->ref_q) return MDK_OK;                     // allocated last: all five are there
+    void **db[5] = {(void **)&e->quals, (void **)&e->ref, (void **)&e->calls, (void **)&e->pred_q, (void **)&e->ref_q};
+    const size_t n = (size_t)e->cap_pos, bytes[5] = {n, n, n, n * sizeof(float), n * sizeof(float)};
+    for (int i = 0; i < 5; ++i)
+        if (!*db[i]) MDK_CUDA(cudaMalloc(db[i], bytes[i]));
     return MDK_OK;
 }
 
@@ -1267,26 +1309,44 @@ int rl_run_group(mdk_rl_engine *e) {
         layer_in = layer_out[l];
     }
     MDK_CUDA(cudaGetLastError());
-    // the previous group's results must have left probs / labels before the head rewrites them
+    // the previous group's results must have left probs / labels (and the decoded outputs quals, calls, pred_q, ref_q,
+    // which copy_back moves on the same stream before recording this event) before the head rewrites them
     if (e->pk.launched >= 0) MDK_CUDA(cudaStreamWaitEvent(s, e->copy_out.ev[e->pk.launched % CopyOut::RING], 0));
+    // what the group's pieces want besides probabilities and labels, as GruCall::launch (api.cu)
+    bool quals = false, var = false;
+    for (const Packing::Piece &p : e->pk.pieces) {
+        quals = quals || p.quals;
+        var = var || p.ref;
+    }
+    const HeadVariant hv{e->ref, e->calls, e->pred_q, e->ref_q};
+    uint8_t *q = quals ? e->quals : nullptr;
     if (e->H == RL_H3) {
         int64_t blocks = (BP + 7) / 8;
         if (blocks > 132 * 8) blocks = 132 * 8;
-        rl_head768_kernel<<<(unsigned)blocks, 256, 0, s>>>(e->h1, e->lin_w, e->lin_b, BP, e->probs, e->labels);
+        const dim3 g((unsigned)blocks);
+        if (var)
+            rl_head768_kernel<HEAD_VARIANT><<<g, 256, 0, s>>>(e->h1, e->lin_w, e->lin_b, BP, e->probs, e->labels, q, hv);
+        else if (quals)
+            rl_head768_kernel<HEAD_QUALS><<<g, 256, 0, s>>>(e->h1, e->lin_w, e->lin_b, BP, e->probs, e->labels, q, {});
+        else
+            rl_head768_kernel<HEAD_PLAIN><<<g, 256, 0, s>>>(e->h1, e->lin_w, e->lin_b, BP, e->probs, e->labels, nullptr, {});
         MDK_CUDA(cudaGetLastError());
     } else {
-        MDK_CUDA(launch_head(e->h1, e->lin_w, e->lin_b, B, P, 0, e->probs, nullptr, e->labels, s));
+        MDK_CUDA(launch_head(e->h1, e->lin_w, e->lin_b, B, P, 0, e->probs, nullptr, e->labels, s, q, var ? &hv : nullptr));
     }
     rl_mark(e, 6);
-    return copy_back(e->copy_out, e->pk, s, e->probs, nullptr, e->labels);
+    return copy_back(e->copy_out, e->pk, s, e->probs, nullptr, e->labels, e->quals, &hv);
 }
 
-// The engine's side of the packing core (packing.h) for one call: x_host [B][P][D][F].  Launching alone (flush, waits)
-// needs no call.
+// The engine's side of the packing core (packing.h) for one call: x_host [B][P][D][F]; for a decoded call (quals or
+// variant outputs) `decoded`, and for a variant-decoded one its reference bytes ref [B][P].  Launching alone (flush,
+// sync, waits) needs no call.
 struct RlCall {
     mdk_rl_engine *e;
     const int8_t *x = nullptr;
     int64_t P = 0, D = 0, F = 0;
+    bool decoded = false;
+    const uint8_t *ref = nullptr;
 
     // the group buffers grow, when a group opens, to this call's windows (at most one group of them): without
     // mdk_rl_reserve a group collects calls only as far as the buffers reach
@@ -1295,16 +1355,26 @@ struct RlCall {
         return rl_ensure_group(e, windows * P);
     }
     int64_t capacity(int64_t len) { return e->cap_pos / len; }
-    int stage(int64_t first, int64_t n, int64_t at) { return rl_conv(e, x + (size_t)first * P * D * F, n, P, D, F, at); }
+    // The reference bytes go to the group's ref buffer on the COMPUTE stream, like the convolutions that fill z: the
+    // group in flight may not have reached its head yet, and a copy on copy_in could overwrite the bytes it reads.
+    int stage(int64_t first, int64_t n, int64_t at) {
+        int rc;
+        if (decoded && (rc = rl_ensure_decoded(e))) return rc;
+        if (ref)
+            MDK_CUDA(cudaMemcpyAsync(e->ref + (size_t)at * P, ref + (size_t)first * P, (size_t)n * P, cudaMemcpyDefault,
+                                     e->stream));
+        return rl_conv(e, x + (size_t)first * P * D * F, n, P, D, F, at);
+    }
     int launch() { return rl_run_group(e); }
 };
 
 int rl_launch(mdk_rl_engine *e) { return e->pk.launch(RlCall{e}); }
 
-int rl_check(mdk_rl_engine *e, const int8_t *x, int64_t B, int64_t P, int64_t D, int64_t F, const float *probs,
+// out: the output the call cannot do without (the probabilities, or a decoded call's labels / call bytes)
+int rl_check(mdk_rl_engine *e, const int8_t *x, int64_t B, int64_t P, int64_t D, int64_t F, const void *out,
              const char *who) {
     const std::string w(who);
-    MDK_REQUIRE(e && x && probs, MDK_ERR_ARG, w + ": NULL argument");
+    MDK_REQUIRE(e && x && out, MDK_ERR_ARG, w + ": NULL argument");
     MDK_REQUIRE(B >= 1 && P >= 1 && D >= 1, MDK_ERR_ARG, w + ": need B, P, D >= 1");
     MDK_REQUIRE(F == (e->use_dwells ? 5 : 4) || (!e->use_dwells && F >= 4), MDK_ERR_ARG,
                 w + ": feature vector length does not match the model (4, or 5 with dwells)");
@@ -1356,7 +1426,8 @@ int mdk_rl_destroy(mdk_rl_engine *e) {
     for (cudaEvent_t ev : {e->ev_xin[0], e->ev_xin[1], e->ev_xfree[0], e->ev_xfree[1]})
         if (ev) cudaEventDestroy(ev);
     for (void *p : {(void *)e->xbuf[0], (void *)e->xbuf[1], (void *)e->conv, (void *)e->z, (void *)e->gi, (void *)e->h0,
-                    (void *)e->h1, (void *)e->probs, (void *)e->labels})
+                    (void *)e->h1, (void *)e->probs, (void *)e->labels, (void *)e->quals, (void *)e->ref,
+                    (void *)e->calls, (void *)e->pred_q, (void *)e->ref_q})
         if (p) cudaFree(p);
     delete e;     // and with it the weights (DeviceWeights)
     cudaGetLastError();
@@ -1427,6 +1498,45 @@ int mdk_rl_submit(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P, 
     int64_t gmax = 0;
     if ((rc = rl_group_limit(e, P, &gmax))) return rc;
     return e->pk.enqueue(RlCall{e, x_host, P, D, F}, B, P, probs_host, nullptr, labels_host, gmax, ticket);
+}
+
+int mdk_rl_submit_decoded(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P, int64_t D, int64_t F,
+                          uint8_t *labels_out, uint8_t *quals_out, int64_t *ticket) {
+    int rc = rl_check(e, x_host, B, P, D, F, labels_out, "rl_submit_decoded");
+    if (rc) return rc;
+    MDK_REQUIRE(ticket, MDK_ERR_ARG, "rl_submit_decoded: ticket is NULL");
+    MDK_CUDA(cudaSetDevice(e->device));
+    if ((rc = rl_prepare(e))) return rc;
+    int64_t gmax = 0;
+    if ((rc = rl_group_limit(e, P, &gmax))) return rc;
+    return e->pk.enqueue(RlCall{e, x_host, P, D, F, quals_out != nullptr}, B, P, nullptr, nullptr, labels_out, gmax,
+                         ticket, quals_out);
+}
+
+int mdk_rl_submit_variant_decoded(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P, int64_t D, int64_t F,
+                                  const uint8_t *ref_bytes, uint8_t *calls_out, float *pred_q_out, float *ref_q_out,
+                                  int64_t *ticket) {
+    int rc = rl_check(e, x_host, B, P, D, F, calls_out, "rl_submit_variant_decoded");
+    if (rc) return rc;
+    MDK_REQUIRE(ref_bytes && pred_q_out && ref_q_out, MDK_ERR_ARG, "rl_submit_variant_decoded: NULL argument");
+    MDK_REQUIRE(ticket, MDK_ERR_ARG, "rl_submit_variant_decoded: ticket is NULL");
+    MDK_CUDA(cudaSetDevice(e->device));
+    if ((rc = rl_prepare(e))) return rc;
+    int64_t gmax = 0;
+    if ((rc = rl_group_limit(e, P, &gmax))) return rc;
+    return e->pk.enqueue(RlCall{e, x_host, P, D, F, true, ref_bytes}, B, P, nullptr, nullptr, calls_out, gmax, ticket,
+                         nullptr, ref_bytes, pred_q_out, ref_q_out);
+}
+
+int mdk_rl_sync(mdk_rl_engine *e) {
+    MDK_REQUIRE(e, MDK_ERR_ARG, "rl_sync: engine is NULL");
+    MDK_CUDA(cudaSetDevice(e->device));
+    int rc = rl_launch(e);
+    if (rc) return rc;
+    MDK_CUDA(cudaStreamSynchronize(e->copy_in));
+    MDK_CUDA(cudaStreamSynchronize(e->stream));
+    MDK_CUDA(cudaStreamSynchronize(e->copy_out.stream));
+    return MDK_OK;
 }
 
 int mdk_rl_flush(mdk_rl_engine *e) {

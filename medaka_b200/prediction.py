@@ -268,6 +268,13 @@ class _LabelArena(object):
         self.reset()
 
 
+def _device_index(model):
+    """CUDA device index of a model: ``GRUModel.device()`` is a torch.device, ``LatentSpaceLSTM.device()`` the string
+    "cuda:<index>"."""
+    dev = model.device()
+    return int(dev.rsplit(":", 1)[1]) if isinstance(dev, str) else dev.index
+
+
 def _stitch_view(sample, min_depth):
     """What the stitch plan reads of a window, in the smallest exact form: positions as (int32 major unless a major
     needs more, unsigned minor of the width its largest value needs), and, only when the run filters on depth, depth
@@ -305,7 +312,10 @@ def _run_decoded(samples, arena, bam, regions, model, feature_encoder, chunk_len
     for data, batch in loader:
         x = model.get_model_input_features(batch)
         x = x.detach().cpu().numpy() if hasattr(x, "detach") else x
-        nb, nt, nf = x.shape
+        # counts features float32 [nb, nt, F]; read-level features int8 [nb, nt, D, F], D the batch's deepest window
+        # (collated batches are uint8, cast like LatentSpaceLSTM's own submit)
+        nb, nt = x.shape[:2]
+        read_level = x.ndim == 4
         if depth is None:
             depth = model.lookahead(batch_size, nt)
             if enable_chunking and nb * nt > (1 << 18):
@@ -317,8 +327,8 @@ def _run_decoded(samples, arena, bam, regions, model, feature_encoder, chunk_len
                 raise ValueError("sample {} has {} columns in a batch of {}".format(s.name, len(s.positions), nt))
         # the page-locked slots are reused once the call that last used them has been waited for
         slot = n_calls % (depth + 1)
-        xin = model.pinned("dfeats%d" % slot, (nb, nt, nf), np.float32)
-        np.copyto(xin, x, casting="same_kind")
+        xin = model.pinned("dfeats%d" % slot, x.shape, np.int8 if read_level else np.float32)
+        np.copyto(xin, x, casting="unsafe" if read_level else "same_kind")
         n_calls += 1
         slab, row = arena.take(nb * nt)
         pending.append(submit(xin, data, slot, slab, row))
@@ -357,11 +367,10 @@ def predict_consensus(bam, bam_regions, model, feature_encoder, draft, output, c
     """`medaka inference` followed by `medaka sequence` in one pass: the FASTQ / FASTA (and gap bed) that
     ``predict_regions`` + ``stitch.sequence`` write, without the probabilities ever leaving the GPU.
 
-    The engine decodes every window in its head (labels and quality bytes, ``GRUModel.submit_decoded``) into a
-    device arena; per window only its name, positions and (with ``min_depth``) depth stay on the host.  At the end the
-    windows are indexed,
-    trimmed and stitched exactly as ``stitch.sequence`` does (``stitch.write_consensus``), the kept rows compacted on
-    the device (``stitch.decode_label_pieces``).
+    The engine decodes every window in its head (labels and quality bytes, ``submit_decoded`` of ``GRUModel`` or of the
+    read-level ``LatentSpaceLSTM``) into a device arena; per window only its name, positions and (with ``min_depth``)
+    depth stay on the host.  At the end the windows are indexed, trimmed and stitched exactly as ``stitch.sequence``
+    does (``stitch.write_consensus``), the kept rows compacted on the device (``stitch.decode_label_pieces``).
 
     The arena holds 2 B per computed column (every column of every window, overlaps included) until the output is
     written, and is freed on return, also on error: about (draft bases) x (1 + insertion column share) x chunk_len /
@@ -376,8 +385,8 @@ def predict_consensus(bam, bam_regions, model, feature_encoder, draft, output, c
     """
     if not hasattr(model, "submit_decoded"):
         raise NotImplementedError(
-            "predict_consensus runs consensus (GRUModel) models only; for {} use predict_regions followed by "
-            "stitch.sequence".format(type(model).__name__))
+            "predict_consensus runs models with decoded outputs (GRUModel, LatentSpaceLSTM) only; for {} use "
+            "predict_regions followed by stitch.sequence".format(type(model).__name__))
     if world_size != 1:
         raise NotImplementedError("predict_consensus runs on one GPU; for several, use predict_regions with one "
                                   "store per rank, then stitch.sequence over the stores")
@@ -385,7 +394,7 @@ def predict_consensus(bam, bam_regions, model, feature_encoder, draft, output, c
     logger = common.get_named_logger('Predict')
     model.check_feature_encoder_compatibility(feature_encoder)
     long_regions, remainder_regions = triage_regions(bam_regions, chunk_len, bam_chunk, chunk_ovlp)
-    arena = _LabelArena(model.device().index, (1, 1))
+    arena = _LabelArena(_device_index(model), (1, 1))
     samples = collections.OrderedDict()
     try:
         _run_one_pass(samples, arena, bam, long_regions, remainder_regions, model, feature_encoder, chunk_len,
@@ -512,9 +521,9 @@ def predict_variants(bam, bam_regions, model, feature_encoder, draft, regions=No
     """`medaka inference` followed by `medaka vcf` in one pass: the records ``predict_regions`` + ``variant.variants``
     return, in the same order, without the probabilities ever leaving the GPU.
 
-    The engine decodes every window in its head (``GRUModel.submit_variant_decoded``: a call byte and the phreds of the
-    winning and of the draft's class, 9 B per column) into a device arena; per window only its name and positions stay
-    on the host.  The join cuts and the variant runs are computed on the device (``labels.variant_join_cuts``,
+    The engine decodes every window in its head (``submit_variant_decoded`` of ``GRUModel`` or of the read-level
+    ``LatentSpaceLSTM``: a call byte and the phreds of the winning and of the draft's class, 9 B per column) into a
+    device arena; per window only its name and positions stay on the host.  The join cuts and the variant runs are computed on the device (``labels.variant_join_cuts``,
     ``labels.decode_variant_segments``); only the runs come back.
 
     The run goes in passes (``plan_passes``): contigs are grouped, in the order of the variant regions, so that a pass's
@@ -527,8 +536,8 @@ def predict_variants(bam, bam_regions, model, feature_encoder, draft, regions=No
     """
     if not hasattr(model, "submit_variant_decoded"):
         raise NotImplementedError(
-            "predict_variants runs consensus (GRUModel) models only; for {} use predict_regions followed by "
-            "variant.variants".format(type(model).__name__))
+            "predict_variants runs models with decoded outputs (GRUModel, LatentSpaceLSTM) only; for {} use "
+            "predict_regions followed by variant.variants".format(type(model).__name__))
     from medaka_b200 import labels, stitch, variant
     scheme_of_model = getattr(model, "label_scheme", None)
     if scheme_of_model is not None and not isinstance(scheme_of_model, labels.HaploidLabelScheme):
@@ -541,7 +550,7 @@ def predict_variants(bam, bam_regions, model, feature_encoder, draft, regions=No
     model.check_feature_encoder_compatibility(feature_encoder)
     if isinstance(draft, str):
         draft = stitch.read_fasta(draft)
-    scheme = labels.HaploidLabelScheme(model.device().index)
+    scheme = labels.HaploidLabelScheme(_device_index(model))
     scheme.verbose = verbose
     # every contig with samples, in index order: the contigs of the bam regions, sorted (stitch.sample_index)
     vregions = variant.variant_regions(sorted({r.ref_name for r in bam_regions}), regions)
@@ -553,7 +562,7 @@ def predict_variants(bam, bam_regions, model, feature_encoder, draft, regions=No
             ref_seqs[name] = draft[name].upper()
         return ref_seqs[name]
 
-    arena = _LabelArena(model.device().index, VARIANT_ROW_BYTES)
+    arena = _LabelArena(_device_index(model), VARIANT_ROW_BYTES)
 
     def submit(x, data, slot, slab, row):
         nb, nt = x.shape[:2]

@@ -188,6 +188,65 @@ class LatentSpaceLSTM(object):
         ticket = int(ticket[0])
         return models.AsyncResult(self, lambda: _lm.check(_lm.lib.mdk_rl_wait(self._engine, ticket)), probs, labels)
 
+    @staticmethod
+    def _ptr(x, ctype):
+        """cffi pointer to a numpy array or to a device address (int)."""
+        ffi = _lm.ffi
+        if x is None:
+            return ffi.NULL
+        return ffi.cast(ctype, x) if isinstance(x, int) else ffi.cast(ctype, ffi.from_buffer(x))
+
+    def _features(self, feats):
+        feats = np.asarray(feats)
+        if feats.ndim != 4 or feats.dtype != np.int8:
+            raise ValueError("expected int8 read-level features [batch, positions, reads, features], got {} {}".format(
+                feats.dtype, feats.shape))
+        if not feats.flags.c_contiguous:
+            raise ValueError("features must be contiguous")
+        self._last_call = None                               # the call's group overwrites the stages read_stage reads
+        return feats.shape
+
+    def submit_decoded(self, feats, labels_out, quals_out=None):
+        """Queue one forward whose outputs are the decoded calls (mdk_rl_submit_decoded); returns a ticket for ``wait``.
+
+        ``feats`` int8 [B, P, D, F] host array (page-locked, ``pinned``, for an asynchronous copy).  ``labels_out`` /
+        ``quals_out`` receive uint8 [B, P] argmax labels and phred+33 quality bytes: numpy arrays, or device addresses
+        (int) of B * P bytes.  ``quals_out`` may be None.  Everything must stay alive and untouched until
+        ``wait(ticket)`` (or ``sync``).
+        """
+        B, P, D, F = self._features(feats)
+        ticket = _lm.ffi.new("int64_t *")
+        _lm.check(_lm.lib.mdk_rl_submit_decoded(self._engine, self._ptr(feats, "const int8_t *"), B, P, D, F,
+                                                self._ptr(labels_out, "uint8_t *"), self._ptr(quals_out, "uint8_t *"),
+                                                ticket))
+        return int(ticket[0])
+
+    def submit_variant_decoded(self, feats, ref_bytes, calls_out, pred_q_out, ref_q_out):
+        """Queue one forward whose outputs are what variant decoding needs (mdk_rl_submit_variant_decoded); returns a
+        ticket.
+
+        ``feats`` int8 [B, P, D, F] host array; ``ref_bytes`` uint8 [B, P] (the draft's label code per column, 0x80 on
+        insertion columns) a numpy array or a device address.  ``calls_out`` uint8 [B, P] and ``pred_q_out`` /
+        ``ref_q_out`` float32 [B, P] are numpy arrays or device addresses (int).  Everything must stay alive and
+        untouched until ``wait(ticket)`` (or ``sync``).
+        """
+        B, P, D, F = self._features(feats)
+        if not isinstance(ref_bytes, int) and tuple(ref_bytes.shape) != (B, P):
+            raise ValueError("ref_bytes must be [B, P] = [{}, {}], got {}".format(B, P, tuple(ref_bytes.shape)))
+        ticket = _lm.ffi.new("int64_t *")
+        _lm.check(_lm.lib.mdk_rl_submit_variant_decoded(
+            self._engine, self._ptr(feats, "const int8_t *"), B, P, D, F, self._ptr(ref_bytes, "const uint8_t *"),
+            self._ptr(calls_out, "uint8_t *"), self._ptr(pred_q_out, "float *"), self._ptr(ref_q_out, "float *"), ticket))
+        return int(ticket[0])
+
+    def wait(self, ticket):
+        """Wait for a submitted call (mdk_rl_wait)."""
+        _lm.check(_lm.lib.mdk_rl_wait(self._engine, int(ticket)))
+
+    def sync(self):
+        """Launch the open group and wait for every call queued on the engine (mdk_rl_sync)."""
+        _lm.check(_lm.lib.mdk_rl_sync(self._engine))
+
     def preferred_batch_size(self):
         """Windows one packed group holds at the reference's 10 000-position chunks (mdk_rl_preferred_windows: one
         recurrence wave within the group buffers' memory budget, 112 at lstm_size 384 on an H100);
