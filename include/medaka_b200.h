@@ -45,7 +45,9 @@ extern "C" {
 #define MDK_PREC_FP32 1  /* CUDA-core fp32 FFMA path: validation / --full_precision */
 
 /* how many 16-window tiles each CTA of the tensor-core recurrences runs (mdk_engine_set_rec_mode) */
-#define MDK_REC_AUTO 0      /* two once the tiles of both directions outnumber the SMs (beyond one wave), else one */
+#define MDK_REC_AUTO 0      /* two whatever the batch size when F <= 16 (a group's layer-1 recurrence then runs on half the
+                               SMs beside the next group's layer 0); otherwise two once the tiles of both directions
+                               outnumber the SMs (beyond one wave), else one */
 #define MDK_REC_ONE_TILE 1  /* one tile per CTA, over several waves when the batch needs more CTAs than there are SMs */
 #define MDK_REC_PINGPONG 2  /* two tiles per CTA (one N = 32 MMA chain), whatever the batch size */
 

@@ -68,6 +68,12 @@ static void dev_free(T *&p) {
     p = nullptr;
 }
 
+// Both streams of a workspace: what its buffers are read or written by
+static cudaError_t ws_sync(mdk_ws &ws) {
+    cudaError_t err = cudaStreamSynchronize(ws.stream);
+    return err == cudaSuccess ? cudaStreamSynchronize(ws.l1_stream) : err;
+}
+
 static int in_features(const mdk_engine *e, int layer) { return layer == 0 ? e->desc.num_features : H2; }
 
 // The weights as the kernels read them, packed on the host (gru_pack.cuh) and uploaded once after each load.
@@ -101,7 +107,7 @@ static int ensure_workspace(mdk_engine *e, mdk_ws &ws, int64_t B, int64_t T) {
     const int64_t rows = tiled_rows(B, T);
     const int64_t need = ((rows + XT_ROWS - 1) / XT_ROWS) * XT_ROWS;
     if (need <= ws.cap_pos) return MDK_OK;
-    MDK_CUDA(cudaStreamSynchronize(ws.stream));
+    MDK_CUDA(ws_sync(ws));
     dev_free(ws.gi);
     if (ws.h0) { cudaFree(ws.h0); ws.h0 = nullptr; }
     dev_free(ws.h1);
@@ -119,7 +125,7 @@ static int ensure_workspace(mdk_engine *e, mdk_ws &ws, int64_t B, int64_t T) {
 // h1 (the layer-1 output, 1 KiB / position) only exists on the unfused-head paths: allocated on first use
 static int ensure_h1(mdk_ws &ws) {
     if (ws.cap_h1 >= ws.cap_pos && ws.h1) return MDK_OK;
-    MDK_CUDA(cudaStreamSynchronize(ws.stream));
+    MDK_CUDA(ws_sync(ws));
     dev_free(ws.h1);
     ws.cap_h1 = 0;
     int rc;
@@ -132,7 +138,7 @@ static int ensure_io(mdk_engine *e, mdk_lane &ln, int64_t B, int64_t T) {
     const int64_t P = B * T;
     const int64_t feats = P * e->desc.num_features;
     if (P <= ln.cap_io && feats <= ln.cap_feats) return MDK_OK;
-    MDK_CUDA(cudaStreamSynchronize(ln.ws->stream));
+    MDK_CUDA(ws_sync(*ln.ws));
     MDK_CUDA(cudaStreamSynchronize(e->copy_in));
     MDK_CUDA(cudaStreamSynchronize(e->copy_out.stream));
     ln.cap_io = 0; ln.cap_feats = 0; ln.cap_quals = 0; ln.cap_var = 0;
@@ -177,27 +183,36 @@ static int ensure_var(mdk_lane &ln) {
     return MDK_OK;
 }
 
-// The forward pipeline on the workspace's stream.  ev[1..6] bracket the stages for mdk_timings.
+// The forward pipeline on the workspace's two streams: [layer-0 input projection,] layer 0 and the layer-1 projection on
+// ws.stream, layer 1 and the head on ws.l1_stream.  ev[1..6] bracket the stages for mdk_timings; the wait for the previous
+// forward's layer 1 falls into h2d_ms (unfused layer 0) or rec0_ms (fused), and with the fused layer 0 the rec0_ms and
+// rec1_ms of consecutive forwards overlap in wall time.
 static int run_forward(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int64_t B, int64_t T, float *probs_dev,
                        float *logits_dev, uint8_t *labels_dev, uint8_t *quals_dev, const HeadVariant *var) {
     int rc;
     if ((rc = prepare_weights(e))) return rc;
     if ((rc = ensure_workspace(e, ws, B, T))) return rc;
     const int64_t P = B * T;
-    cudaStream_t s = ws.stream;
+    cudaStream_t s = ws.stream, s1 = ws.l1_stream;
     const bool tc = e->precision == MDK_PREC_TC;
     int launches = 0;
     const bool fuse_x = tc && e->layer[0].w_x_tm != nullptr;     // F <= 16
-    // Recurrent kernels of the tensor-core path.  One 16-window tile per CTA is a single dependent chain per SM; two tiles
-    // per CTA (one N = 32 MMA chain) need half as many CTAs, so AUTO takes two only once the tiles of both directions
-    // outnumber the SMs.  The linear head rides inside the layer-1 recurrence, fp32 on the CUDA cores (40 B/position of
-    // partial logits reach HBM instead of the 1 KiB/position h1 round trip), unless h1 is to be kept.
+    // Recurrent kernels of the tensor-core path.  With the fused layer-0 projection AUTO runs two tiles per CTA (one
+    // N = 32 MMA chain) for every forward: a group's layer 1 then takes half the SMs and the next group's layer 0 the
+    // other half, which does a group's two recurrences in less SM time than one tile per CTA on all of them in turn.
+    // It does not depend on B, so a window's outputs are the same whether it is packed into a group or runs alone.
+    // Otherwise layer 0 reads gi and cannot overlap the previous layer 1: one 16-window tile per CTA (a single dependent
+    // chain per SM) while the tiles of both directions fit the SMs, two beyond.  The linear head rides inside the layer-1
+    // recurrence, fp32 on the CUDA cores (40 B/position of partial logits reach HBM instead of the 1 KiB/position h1
+    // round trip), unless h1 is to be kept.
     const int64_t tiles = (B + WT - 1) / WT;
     const int tiles_per_cta = e->rec_mode == MDK_REC_PINGPONG ? 2
                             : e->rec_mode == MDK_REC_ONE_TILE ? 1
-                            : tiles * NDIR > (int64_t)e->sm_count ? 2 : 1;
+                            : fuse_x || tiles * NDIR > (int64_t)e->sm_count ? 2 : 1;
     const bool fuse_head = tc && !e->keep_act;
     if (!fuse_head && (rc = ensure_h1(ws))) return rc;
+    // gi is still read by the previous forward's layer 1: its first writer here waits for it
+    if (!fuse_x) MDK_CUDA(cudaStreamWaitEvent(s, ws.l1_done, 0));
     MDK_CUDA(cudaEventRecord(e->ev[1], s));
     if (!fuse_x) {
         MDK_CUDA(launch_inproj0(feats_dev, e->layer[0].w_in_packed, e->layer[0].bias_gi, ws.gi, P,
@@ -213,24 +228,28 @@ static int run_forward(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int64_
         MDK_CUDA(launch_rec_fp32(ws.gi, e->layer[0].w_hh_t, e->layer[0].b_hn, (float *)ws.h0, B, T, s));
     }
     launches++;
+    if (fuse_x) MDK_CUDA(cudaStreamWaitEvent(s, ws.l1_done, 0));
     MDK_CUDA(cudaEventRecord(e->ev[3], s));
     if (tc) MDK_CUDA(launch_gemm_tc(ws.h0, e->layer[1].w_in_tc, e->layer[1].bias_gi_tc, ws.gi, tiled_rows(B, T), e->sm_count, s));
     else MDK_CUDA(launch_gemm_fp32((const float *)ws.h0, e->layer[1].w_in_packed, e->layer[1].bias_gi, ws.gi, P, H2, GI_COLS, s));
     launches++;
     MDK_CUDA(cudaEventRecord(e->ev[4], s));
+    // layer 1 after the projection; the lane's features and reference bytes reached s before it (ev_in)
+    MDK_CUDA(cudaStreamWaitEvent(s1, e->ev[4], 0));
     if (tc) {
         MDK_CUDA(launch_rec_tc(ws.gi, nullptr, e->layer[1].w_hh_tm, e->layer[1].b_hn_tc, tiles_per_cta,
-                               fuse_head ? OUT_LOGITS : OUT_ROWS, fuse_head ? (void *)ws.plog : ws.h1, e->lin_w, B, T, s));
+                               fuse_head ? OUT_LOGITS : OUT_ROWS, fuse_head ? (void *)ws.plog : ws.h1, e->lin_w, B, T, s1));
     } else {
-        MDK_CUDA(launch_rec_fp32(ws.gi, e->layer[1].w_hh_t, e->layer[1].b_hn, ws.h1, B, T, s));
+        MDK_CUDA(launch_rec_fp32(ws.gi, e->layer[1].w_hh_t, e->layer[1].b_hn, ws.h1, B, T, s1));
     }
     launches++;
-    MDK_CUDA(cudaEventRecord(e->ev[5], s));
-    if (fuse_head) MDK_CUDA(launch_head_plog(ws.plog, e->lin_b, B, T, probs_dev, logits_dev, labels_dev, s, quals_dev, var));
-    else MDK_CUDA(launch_head(ws.h1, e->lin_w, e->lin_b, B, T, tc ? 1 : 0, probs_dev, logits_dev, labels_dev, s, quals_dev,
+    MDK_CUDA(cudaEventRecord(e->ev[5], s1));
+    MDK_CUDA(cudaEventRecord(ws.l1_done, s1));
+    if (fuse_head) MDK_CUDA(launch_head_plog(ws.plog, e->lin_b, B, T, probs_dev, logits_dev, labels_dev, s1, quals_dev, var));
+    else MDK_CUDA(launch_head(ws.h1, e->lin_w, e->lin_b, B, T, tc ? 1 : 0, probs_dev, logits_dev, labels_dev, s1, quals_dev,
                               var));
     launches++;
-    MDK_CUDA(cudaEventRecord(e->ev[6], s));
+    MDK_CUDA(cudaEventRecord(e->ev[6], s1));
     e->launches += launches;
     e->last.launches = launches;
     ws.last_fused_head = fuse_head;
@@ -314,8 +333,10 @@ struct GruCall {
         if ((rc = run_forward(e, *ln.ws, ln.d_feats, pk.windows, pk.len, ln.d_probs, logits ? ln.d_logits : nullptr,
                               labels ? ln.d_labels : nullptr, quals ? ln.d_quals : nullptr, var ? &hv : nullptr)))
             return rc;
-        MDK_CUDA(cudaEventRecord(e->ev[7], s));
-        if ((rc = copy_back(e->copy_out, pk, s, ln.d_probs, ln.d_logits, ln.d_labels, ln.d_quals, &hv))) return rc;
+        // the outputs are written by the head, on the layer-1 stream
+        MDK_CUDA(cudaEventRecord(e->ev[7], ln.ws->l1_stream));
+        if ((rc = copy_back(e->copy_out, pk, ln.ws->l1_stream, ln.d_probs, ln.d_logits, ln.d_labels, ln.d_quals, &hv)))
+            return rc;
         MDK_CUDA(cudaEventRecord(ln.ev_out, e->copy_out.stream));
         ln.busy = true;
         return MDK_OK;
@@ -434,6 +455,8 @@ int mdk_engine_create(int device, const mdk_model_desc *desc, mdk_engine **out) 
     e->sm_count = prop.multiProcessorCount;
     for (auto &ws : e->ws) {
         cudaError_t err = cudaStreamCreateWithFlags(&ws.stream, cudaStreamNonBlocking);
+        if (err == cudaSuccess) err = cudaStreamCreateWithFlags(&ws.l1_stream, cudaStreamNonBlocking);
+        if (err == cudaSuccess) err = cudaEventCreateWithFlags(&ws.l1_done, cudaEventDisableTiming);
         if (err != cudaSuccess) { mdk_engine_destroy(e); return cuda_fail(err, "cudaStreamCreate", __FILE__, __LINE__); }
     }
     for (int i = 0; i < mdk_engine::N_LANES; ++i) {
@@ -457,12 +480,17 @@ int mdk_engine_create(int device, const mdk_model_desc *desc, mdk_engine **out) 
 int mdk_engine_destroy(mdk_engine *e) {
     if (!e) return MDK_OK;
     cudaSetDevice(e->device);
-    for (auto &ws : e->ws) if (ws.stream) cudaStreamSynchronize(ws.stream);
+    for (auto &ws : e->ws) {
+        if (ws.stream) cudaStreamSynchronize(ws.stream);
+        if (ws.l1_stream) cudaStreamSynchronize(ws.l1_stream);
+    }
     destroy_copy_out(e->copy_out);
     for (auto &ws : e->ws) {
         dev_free(ws.gi); dev_free(ws.h1); dev_free(ws.plog);
         if (ws.h0) cudaFree(ws.h0);
         if (ws.stream) cudaStreamDestroy(ws.stream);
+        if (ws.l1_stream) cudaStreamDestroy(ws.l1_stream);
+        if (ws.l1_done) cudaEventDestroy(ws.l1_done);
     }
     for (auto &ln : e->lane) {
         dev_free(ln.d_feats); dev_free(ln.d_probs); dev_free(ln.d_logits); dev_free(ln.d_labels); dev_free(ln.d_quals);
@@ -484,7 +512,7 @@ int mdk_engine_destroy(mdk_engine *e) {
 static int quiesce(mdk_engine *e) {
     int rc = launch_group(e);
     if (rc) return rc;
-    for (auto &ws : e->ws) MDK_CUDA(cudaStreamSynchronize(ws.stream));
+    for (auto &ws : e->ws) MDK_CUDA(ws_sync(ws));
     return MDK_OK;
 }
 
@@ -635,7 +663,7 @@ int mdk_engine_sync(mdk_engine *e) {
     int rc = launch_group(e);
     if (rc) return rc;
     MDK_CUDA(cudaStreamSynchronize(e->copy_in));
-    for (auto &ws : e->ws) MDK_CUDA(cudaStreamSynchronize(ws.stream));
+    for (auto &ws : e->ws) MDK_CUDA(ws_sync(ws));
     MDK_CUDA(cudaStreamSynchronize(e->copy_out.stream));
     for (auto &ln : e->lane) ln.busy = false;
     return MDK_OK;
@@ -664,7 +692,7 @@ int mdk_engine_mean_timings(mdk_engine *e, int n_last, mdk_timings *out) {
     if (rc) return rc;
     MDK_REQUIRE(e->fwd_count >= 1, MDK_ERR_STATE, "mean_timings: no forward recorded");
     n_last = (int)std::min<int64_t>(n_last, e->fwd_count);
-    for (auto &ws : e->ws) MDK_CUDA(cudaStreamSynchronize(ws.stream));
+    for (auto &ws : e->ws) MDK_CUDA(ws_sync(ws));
     mdk_timings acc{};
     for (int i = 0; i < n_last; ++i) {
         mdk_timings t{};
@@ -689,7 +717,7 @@ int mdk_debug_timeline(mdk_engine *e, int n_last, float *out) {
     int rc = launch_group(e);
     if (rc) return rc;
     MDK_REQUIRE(n_last >= 1 && n_last <= mdk_engine::EV_RING && e->fwd_count >= n_last, MDK_ERR_ARG, "timeline: bad n_last");
-    for (auto &ws : e->ws) MDK_CUDA(cudaStreamSynchronize(ws.stream));
+    for (auto &ws : e->ws) MDK_CUDA(ws_sync(ws));
     for (int i = 0; i < n_last; ++i) {
         cudaEvent_t *ev = e->evr[(e->fwd_count - n_last + i) % mdk_engine::EV_RING];
         for (int k = 0; k < 8; ++k) MDK_CUDA(cudaEventElapsedTime(out + i * 8 + k, e->ev_timer[0], ev[k]));
@@ -698,7 +726,7 @@ int mdk_debug_timeline(mdk_engine *e, int n_last, float *out) {
 }
 
 // The timed region spans every lane: the start event goes on lane 0 after all lanes have drained, the stop event on
-// lane 0 after it has been made to wait for every other lane and for the copy-out stream.
+// lane 0 after it has been made to wait for every other stream of every workspace and for the copy-out stream.
 int mdk_engine_timer_start(mdk_engine *e) {
     MDK_REQUIRE(e, MDK_ERR_ARG, "engine is NULL");
     MDK_CUDA(cudaSetDevice(e->device));
@@ -706,7 +734,10 @@ int mdk_engine_timer_start(mdk_engine *e) {
     if (rc) return rc;
     MDK_CUDA(cudaEventRecord(e->ev_timer[0], e->stream));
     // work queued on the other lanes / copy streams after this point must not start before the start event
-    for (int i = 1; i < mdk_engine::N_WS; ++i) MDK_CUDA(cudaStreamWaitEvent(e->ws[i].stream, e->ev_timer[0], 0));
+    for (int i = 0; i < mdk_engine::N_WS; ++i) {
+        if (i) MDK_CUDA(cudaStreamWaitEvent(e->ws[i].stream, e->ev_timer[0], 0));
+        MDK_CUDA(cudaStreamWaitEvent(e->ws[i].l1_stream, e->ev_timer[0], 0));
+    }
     MDK_CUDA(cudaStreamWaitEvent(e->copy_in, e->ev_timer[0], 0));
     return MDK_OK;
 }
@@ -715,8 +746,13 @@ int mdk_engine_timer_stop(mdk_engine *e, float *elapsed_ms) {
     MDK_CUDA(cudaSetDevice(e->device));
     int rc = launch_group(e);
     if (rc) return rc;
-    for (int i = 1; i < mdk_engine::N_WS; ++i) {
-        MDK_CUDA(cudaEventRecord(e->ev_join, e->ws[i].stream));
+    // every layer-1 stream, ws[0]'s included: the last group's layer 1 and head run there after ws[0].stream is done
+    for (int i = 0; i < mdk_engine::N_WS; ++i) {
+        if (i) {
+            MDK_CUDA(cudaEventRecord(e->ev_join, e->ws[i].stream));
+            MDK_CUDA(cudaStreamWaitEvent(e->stream, e->ev_join, 0));
+        }
+        MDK_CUDA(cudaEventRecord(e->ev_join, e->ws[i].l1_stream));
         MDK_CUDA(cudaStreamWaitEvent(e->stream, e->ev_join, 0));
     }
     MDK_CUDA(cudaEventRecord(e->ev_join, e->copy_out.stream));     // the end event must follow every copy-out still in flight
@@ -745,7 +781,7 @@ int mdk_engine_read_activation_windows(mdk_engine *e, int which, int64_t first, 
                 "read_activation(1): the last forward fused the head into layer 1 (h1 never reached HBM); call "
                 "mdk_engine_keep_activations(e, 1) before the forward");
     MDK_CUDA(cudaSetDevice(e->device));
-    MDK_CUDA(cudaStreamSynchronize(ln.stream));
+    MDK_CUDA(ws_sync(ln));
     if (ln.last_precision == MDK_PREC_FP32) {
         const float *src = (which == 1 ? ln.h1 : reinterpret_cast<const float *>(ln.h0)) + first * ln.last_T * H2;
         MDK_CUDA(cudaMemcpy(out_host, src, (size_t)n_floats * sizeof(float), cudaMemcpyDeviceToHost));
@@ -772,7 +808,7 @@ int mdk_debug_read_plog(mdk_engine *e, float *out_host, int64_t n_floats) {
     const int64_t tiles = (ln.last_B + WT - 1) / WT;
     MDK_REQUIRE(n_floats == NDIR * tiles * ln.last_T * PLOG_TS_FLOATS, MDK_ERR_ARG, "read_plog: size must be 2*tiles*T*80");
     MDK_CUDA(cudaSetDevice(e->device));
-    MDK_CUDA(cudaStreamSynchronize(ln.stream));
+    MDK_CUDA(ws_sync(ln));
     MDK_CUDA(cudaMemcpy(out_host, ln.plog, (size_t)n_floats * sizeof(float), cudaMemcpyDeviceToHost));
     return MDK_OK;
 }

@@ -251,7 +251,12 @@ int wait_ticket(CopyOut &co, Packing &pk, Eng &&eng, int64_t ticket) {
 // fills every SM, and a second 43 GB workspace would not fit beside it in 80 GB.  Small forwards (the B = 1 remainder
 // regions of medaka/prediction.py:196-209) spread over the small lanes, each with a workspace of its own.
 struct mdk_ws {
-    cudaStream_t stream = nullptr;
+    cudaStream_t stream = nullptr;      // [layer-0 input projection,] layer-0 recurrence, layer-1 projection
+    // layer-1 recurrence and head: on a stream of their own, so that on the tensor-core path with the fused layer-0
+    // projection the next group's layer 0 (which writes only h0, already consumed by this group's projection) runs on
+    // the SMs beside this group's layer 1.  l1_done marks the last layer 1 queued: every writer of gi waits for it.
+    cudaStream_t l1_stream = nullptr;
+    cudaEvent_t l1_done = nullptr;
     int64_t cap_pos = 0;       // capacity in positions (rounded up to XT_ROWS)
     float *gi = nullptr;       // [cap_pos][768]
     void *h0 = nullptr;        // fp32 [cap_pos][256]  or  fp16 hi/lo tiles (same byte size)
@@ -295,7 +300,7 @@ struct mdk_engine {
     int open_lane = -1;           // lane of the open (or last launched) group
     int last_ws = 0;              // workspace of the most recent forward
     int64_t group_windows = 0;    // most windows coalesced into one group (0 = one wave, mdk_engine_preferred_windows)
-    cudaStream_t stream = nullptr;       // == ws[0].stream: weight uploads, timers
+    cudaStream_t stream = nullptr;       // == ws[0].stream: weight uploads, timers (waits for every other stream)
     static constexpr int EV_RING = 32;   // per-group event sets kept for mdk_engine_mean_timings
     cudaEvent_t evr[EV_RING][8] = {};
     cudaEvent_t *ev = evr[0];            // event set of the group being launched

@@ -350,7 +350,9 @@ class GRUModel(object):
         _lm.check(_lm.lib.mdk_engine_flush(self._engine))
 
     def set_rec_mode(self, mode):
-        """'auto' | 'one' | 'pp': tiles per CTA of the recurrent kernels (mdk_engine_set_rec_mode)."""
+        """'auto' | 'one' | 'pp': tiles per CTA of the recurrent kernels (mdk_engine_set_rec_mode).  'auto' runs two
+        tiles per CTA for every forward with at most 16 features, so that a group's layer 1 runs beside the next group's
+        layer 0, and otherwise one tile per CTA up to one wave of windows, two beyond."""
         code = {"auto": _lm.lib.MDK_REC_AUTO, "one": _lm.lib.MDK_REC_ONE_TILE, "pp": _lm.lib.MDK_REC_PINGPONG}[mode]
         _lm.check(_lm.lib.mdk_engine_set_rec_mode(self._engine, code))
 
