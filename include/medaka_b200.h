@@ -388,6 +388,33 @@ int mdk_bam_batch_arrays(mdk_bam_batch *x, const int32_t **pos, const uint16_t *
 int mdk_bam_batch_qual(mdk_bam_batch *x, const uint8_t **qual, const int64_t **qual_off);
 int mdk_bam_batch_free(mdk_bam_batch *x);
 
+/* ---- annotation seam: replaces the per-variant body of annotate_vcf_n_reads (medaka/vcf.py:1230-1302, `medaka tools
+ * annotate`) for one chunk of one contig.
+ *   records      as for mdk_pileup_counts, SORTED by position; the read-group filter is the caller's (the flag / min_mapq
+ *                filter of src/medaka_bamiter.c:19-21 runs on the device)
+ *   contig       bytes of the contig from contig_start, contig_n of them, covering every variant's padded window (may be
+ *                NULL when dpsp == 0); contig_len is the contig's full length (the windows are clipped to it)
+ *   variants     var_pos[n_var] 0-based, var_ref_len[n_var]; variant v's alleles (REF first, then the ALTs) are
+ *                hap_off[v] .. hap_off[v + 1] - 1, allele k's bytes alleles[allele_off[k] .. allele_off[k + 1])
+ *   score        int8 [16][16] substitution scores over htslib's 4-bit codes "=ACMGRSVTWYHKDBN" (read code, haplotype
+ *                code), each in [-8, 7]; haplotype bytes outside that alphabet score as N.  Gap of length k costs
+ *                gap_open + (k - 1) gap_extend (parasail's sw_trace_striped_32 convention), gap_open >= gap_extend.
+ * Out (host): dp_out [n_var][3] = DP, DPS fwd, DPS rev: the pileup counts (min_mapq, no depth cap) at the variant's major
+ * column, 0 without coverage.  With dpsp != 0 every read that spans the padded window [max(0, pos - pad),
+ * min(contig_len, pos + ref_len + pad)) is trimmed to it (trim_read, src/medaka_trimbam.c:101-246, partial = false; reads
+ * of trimmed length <= 1 dropped) and aligned (exact int32 affine Smith-Waterman) to every padded haplotype:
+ * sr_out [n_hap][2] reads whose first best haplotype it is, per strand (fwd, rev); sc_out [n_hap][2] their summed
+ * scores; ar_out [n_var][2] reads whose scores are all equal.  stats_out [2] (may be NULL) = alignment cells, pairs;
+ * kernel_ms (may be NULL) = device time of the call's kernels (CUDA events). */
+int mdk_annotate(int device, int64_t n_rec, const int32_t *pos, const uint16_t *flag, const uint8_t *mapq,
+                 const uint8_t *dtype, const uint32_t *cigar, const int64_t *cigar_off, const uint8_t *seq,
+                 const int64_t *seq_off, const uint8_t *contig, int32_t contig_start, int32_t contig_n,
+                 int32_t contig_len, int64_t n_var, const int32_t *var_pos, const int32_t *var_ref_len,
+                 const int64_t *hap_off, const int64_t *allele_off, const uint8_t *alleles, int32_t pad,
+                 int32_t min_mapq, int32_t dpsp, const int8_t *score, int32_t gap_open, int32_t gap_extend,
+                 int64_t *dp_out, int64_t *sr_out, int64_t *ar_out, int64_t *sc_out, int64_t *stats_out,
+                 float *kernel_ms);
+
 /* ---- decode seam: replaces the array part of HaploidLabelScheme.decode_consensus ------------
  * (medaka/labels.py:1053-1085 with _phred :387-401): labels = argmax (first max wins),
  * quals = uint8(min(70, -10*log10(clip(1-p_max, 1e-7, 1)))) + 33.  probs float32 [n][5].

@@ -367,5 +367,21 @@ int selftest_umma(int device, const float *A, const float *B, float *D, int N, i
 // pileup.cu
 // exclusive scan of n per-block counts, in place, by one block: counts[i] = sum of counts[0, i), counts[n] = the total
 cudaError_t launch_scan_blocks(int64_t *counts, int64_t n, cudaStream_t s);
+// The eight BAM record arrays of a featuriser call (host or device copies); cigar_off / seq_off hold n_rec + 1 offsets.
+struct Records {
+    const int32_t *pos;
+    const uint16_t *flag;
+    const uint8_t *mapq, *dtype;
+    const uint32_t *cigar;
+    const int64_t *cigar_off;
+    const uint8_t *seq;
+    const int64_t *seq_off;
+};
+// Counts of a region (device pointers in, device pointers out; the column plan lives in the SCRATCH blob until the call
+// returns).  Returns the number of columns through *n_cols_host; if it exceeds max_cols the outputs are incomplete and
+// the caller re-runs with a larger buffer.
+int pileup_counts_dev(int64_t n_rec, const Records &d, int64_t n_ops, int32_t start, int32_t end, int num_dtypes,
+                      int min_mapq, int64_t max_cols, uint64_t *counts, int64_t *major, int64_t *minor,
+                      int64_t *n_cols_host, cudaStream_t s);
 
 }  // namespace mdk

@@ -696,17 +696,6 @@ __global__ void __launch_bounds__(256) plp_fill_kernel(int64_t n_ops, RmArgs a, 
     }
 }
 
-// The eight BAM record arrays of a featuriser call (host or device copies); cigar_off / seq_off hold n_rec + 1 offsets.
-struct Records {
-    const int32_t *pos;
-    const uint16_t *flag;
-    const uint8_t *mapq, *dtype;
-    const uint32_t *cigar;
-    const int64_t *cigar_off;
-    const uint8_t *seq;
-    const int64_t *seq_off;
-};
-
 // Column structure of a region, shared by the counts and the read-level featurisers and only enqueued on s: op_rec /
 // op_ref / op_qry / op_ins / width / col_off in the SCRATCH blob, major / minor written, the number of columns left on
 // the device at n_cols for the caller to read once its own kernels are queued.  tail_words more 32-bit words of the
@@ -757,7 +746,7 @@ static int plan_columns(int64_t n_rec, const Records &d, int64_t n_ops, int32_t 
 // Counts of a region (device pointers in, device pointers out).  Returns the number of columns through *n_cols_host;
 // if it exceeds max_cols the outputs are incomplete and the caller re-runs with a larger buffer (the reference's
 // enlarge_plp_data, medaka_counts.c:266-271).
-static int pileup_counts_dev(int64_t n_rec, const Records &d, int64_t n_ops, int32_t start, int32_t end, int num_dtypes,
+int pileup_counts_dev(int64_t n_rec, const Records &d, int64_t n_ops, int32_t start, int32_t end, int num_dtypes,
                              int min_mapq, int64_t max_cols, uint64_t *counts, int64_t *major, int64_t *minor,
                              int64_t *n_cols_host, cudaStream_t s) {
     *n_cols_host = 0;
