@@ -179,15 +179,18 @@ def ablate(state_dict, which):
 def featuriser_like_features(B, T, F=10, seed=0, gaps=4):
     """Features float32 [B, T, F] as the counts featuriser makes them, which synth_features (Dirichlet rows) is not:
     raw counts from synth.synth_counts through features_oracle.post_process_pileup, cut into windows of T columns.
-    F = 10: one datatype, "total" normalisation; F = 20: two datatypes, "fwd_rev".  Major columns are one-hot-like (the
-    true base on both strands), insertion (minor) columns sparse and small, and each window of T >= 100 has `gaps` runs
-    of 5-60 columns without coverage (all-zero rows)."""
+    F = 10: one datatype, "total" normalisation; F = 20, 30, 40: two to four datatypes, "fwd_rev".  Major columns are
+    one-hot-like (the true base on both strands), insertion (minor) columns sparse and small, and each window of T >= 100
+    has `gaps` runs of 5-60 columns without coverage (all-zero rows)."""
     from oracle import features_oracle, synth
-    if F not in (10, 20):
-        raise ValueError("F must be 10 or 20")
+    if F not in (10, 20, 30, 40):
+        raise ValueError("F must be 10, 20, 30 or 40")
     ndt = F // 10
     n = B * T
-    counts, pos = synth.synth_counts(n, seed=seed, num_dtypes=ndt)
+    # 15 reads per datatype at three and four datatypes, as at two: strand groups of a few reads would make most
+    # normalised values quarters and halves, which fp16 holds exactly
+    depth = 30 if ndt <= 2 else 15 * ndt
+    counts, pos = synth.synth_counts(n, seed=seed, num_dtypes=ndt, mean_depth=depth, max_depth=4 * depth)
     rs = np.random.RandomState(seed + 1)
     for b in range(B):
         for _ in range(gaps if T >= 100 else 0):
@@ -199,5 +202,5 @@ def featuriser_like_features(B, T, F=10, seed=0, gaps=4):
     if ndt == 1:
         f, _ = features_oracle.post_process_pileup(counts, pos, "total")
     else:
-        f, _ = features_oracle.post_process_pileup(counts, pos, "fwd_rev", dtypes=("dt0", "dt1"))
+        f, _ = features_oracle.post_process_pileup(counts, pos, "fwd_rev", dtypes=tuple("dt%d" % k for k in range(ndt)))
     return np.ascontiguousarray(f.reshape(B, T, F), dtype=np.float32)
