@@ -32,10 +32,11 @@ namespace mdk {
 //   NT = 1: the h tile holds hi and lo as ONE operand of 32 rows (rows 0-15 h_hi of the 16 windows, 16-31 their h_lo).
 //           One RS m64n32k16 gives W_hi.h_hi in accumulator columns 0-15 and W_hi.h_lo in columns 16-31, one SS
 //           m64n16k16 adds W_lo.h_hi (the same descriptor at N = 16 reads rows 0-15) into columns 0-15 (d[0..7]); the
-//           pre-activation is d[k] + d[k + 8].  48 MMAs per warpgroup-step instead of 72, and r and z share one
-//           reciprocal (5 MUFU operations per value instead of 6).
+//           pre-activation is d[k] + d[k + 8].  48 MMAs per warpgroup-step instead of 72.
 //   NT = 2: hi and lo planes of N = 32 rows each and three m64n32k16 MMAs (no registers left for accumulators twice as
-//           wide: 239-252 of 255).
+//           wide: 241-253 of 255).
+// At both tile counts r and z share one reciprocal (5 MUFU operations per value instead of 6), and the new h goes into
+// the tile as fp16 hi / lo pairs by stmatrix (.trans: the accumulator fragment transposed is the K-major tile's layout).
 // FUSE_X (layer 0, F <= 16): the input projection W_ih . x_t is the same products per gate on an x tile laid out like
 // the h tile (K = 16), so layer 0 needs no gi buffer.  OUT: fp16 hi/lo operand tiles of the projection GEMM (layer 0:
 // copied under the next step's MMAs from the h tile buffer, which already holds them in that layout, see store_h0),
@@ -53,7 +54,8 @@ struct RwCfg {
     static constexpr int ROWS = HL ? 2 * N : N;     // rows of an activation operand
     static constexpr int PLANES = HL ? 1 : 2;       // operands per tile buffer
     static constexpr int KG = ROWS * 16 + 16;       // k-group stride of an activation tile (+16 B spreads the 2-byte
-                                                    // stores of one k-group over the banks)
+                                                    // x stores of one k-group over the banks; 16-B rows for stmatrix)
+    static_assert(KG % 16 == 0, "stmatrix rows are 16-byte aligned");
     static constexpr int HPLANE = (H / 8) * KG;
     static constexpr int XPLANE = 2 * KG;
     static constexpr int HLO = HL ? N * 16 : HPLANE;   // bytes from an h value's hi half to its lo half
@@ -139,6 +141,10 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
         }
     }
     const float bhn[2] = {b_hn[dir * H + j0], b_hn[dir * H + j0 + 8]};
+    // the h tile row this lane addresses in the step's stmatrix: row c = lane & 7 of matrix m = lane >> 3 (plane m / 2,
+    // hidden units of hb = m & 1) of window block 0, in tile buffer 0
+    const uint32_t hst_addr = sbase + L::h_off + (lane >> 4) * L::HLO + (wg * 8 + warp * 2 + ((lane >> 3) & 1)) * L::KG +
+                              (lane & 7) * 16;
 
     // Accumulator element k = 4i + 2hb + e: hidden unit j0 + 8hb, window n = 8i + 2cq + e of tile wtile0 + i/2
     // (HL: k >= NA is the lo part of window n - 16, element k - NA).
@@ -292,8 +298,9 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
         const int buf = (int)(step & 1);
         const uint32_t hb_addr = sbase + L::h_off + buf * L::PLANES * L::HPLANE;
         wg_fence();
+        // k-step outer, gate inner: consecutive MMAs go to different accumulators, so none waits for the one before it
+        // (each accumulator still sums its products in the order k-step, then hi.hi, hi.lo, lo.hi)
         if constexpr (L::HL) {
-            // k-step outer, gate inner: consecutive MMAs go to different accumulators
 #pragma unroll
             for (int ks = 0; ks < H / 16; ++ks) {
                 const uint64_t bh = make_smem_desc(hb_addr + ks * 2 * L::KG, L::KG, 128);
@@ -306,15 +313,17 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
             }
         } else {
 #pragma unroll
-            for (int gate = 0; gate < 3; ++gate) {
-                float(&acc)[NACC] = gate == 0 ? ar : (gate == 1 ? az : an);
+            for (int ks = 0; ks < H / 16; ++ks) {
+                const uint64_t bh = make_smem_desc(hb_addr + ks * 2 * L::KG, L::KG, 128);
+                const uint64_t bl = make_smem_desc(hb_addr + L::HPLANE + ks * 2 * L::KG, L::KG, 128);
 #pragma unroll
-                for (int ks = 0; ks < H / 16; ++ks) {
-                    const uint64_t bh = make_smem_desc(hb_addr + ks * 2 * L::KG, L::KG, 128);
-                    MMA::rs(acc, whi[gate][ks], bh, 1u);
-                    MMA::rs(acc, whi[gate][ks], make_smem_desc(hb_addr + L::HPLANE + ks * 2 * L::KG, L::KG, 128), 1u);
-                    MMA::ss(acc, make_smem_desc(sbase + L::wlo_off + (gate * 2 + wg) * RW_ABLK + ks * 2 * 1024, 1024, 128), bh, 1u);
-                }
+                for (int gate = 0; gate < 3; ++gate) MMA::rs(gate == 0 ? ar : (gate == 1 ? az : an), whi[gate][ks], bh, 1u);
+#pragma unroll
+                for (int gate = 0; gate < 3; ++gate) MMA::rs(gate == 0 ? ar : (gate == 1 ? az : an), whi[gate][ks], bl, 1u);
+#pragma unroll
+                for (int gate = 0; gate < 3; ++gate)
+                    MMA::ss(gate == 0 ? ar : (gate == 1 ? az : an),
+                            make_smem_desc(sbase + L::wlo_off + (gate * 2 + wg) * RW_ABLK + ks * 2 * 1024, 1024, 128), bh, 1u);
             }
         }
         if constexpr (FUSE_X) {
@@ -330,12 +339,13 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
             } else {
                 const uint64_t bl = make_smem_desc(xa + L::XPLANE, L::KG, 128);
 #pragma unroll
-                for (int gate = 0; gate < 3; ++gate) {
-                    float(&acc)[NACC] = gate == 0 ? ar : (gate == 1 ? az : axn);
-                    MMA::rs(acc, wxhi[gate], bh, 1u);
-                    MMA::rs(acc, wxhi[gate], bl, 1u);
-                    MMA::ss(acc, make_smem_desc(sbase + L::wxlo_off + (gate * 2 + wg) * RW_XBLK, 1024, 128), bh, 1u);
-                }
+                for (int gate = 0; gate < 3; ++gate) MMA::rs(gate == 0 ? ar : (gate == 1 ? az : axn), wxhi[gate], bh, 1u);
+#pragma unroll
+                for (int gate = 0; gate < 3; ++gate) MMA::rs(gate == 0 ? ar : (gate == 1 ? az : axn), wxhi[gate], bl, 1u);
+#pragma unroll
+                for (int gate = 0; gate < 3; ++gate)
+                    MMA::ss(gate == 0 ? ar : (gate == 1 ? az : axn),
+                            make_smem_desc(sbase + L::wxlo_off + (gate * 2 + wg) * RW_XBLK, 1024, 128), bh, 1u);
             }
         }
         wg_commit();
@@ -370,31 +380,31 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
         wg_hold(ar); wg_hold(az); wg_hold(an); wg_hold(axn);
 
         // ---- gate math (weights and biases carry the exp2 scale factors, common.cuh gate_scale) ----
-        uint8_t *hw = smem + L::h_off + (buf ^ 1) * L::PLANES * L::HPLANE;
 #pragma unroll
         for (int k = 0; k < NA; ++k) {
-            float pr = ar[k], pz = az[k], pn = an[k], px = axn[k], r, z;
+            float pr = ar[k], pz = az[k], pn = an[k], px = axn[k];
             if constexpr (L::HL) {
                 pr += ar[k + NA]; pz += az[k + NA]; pn += an[k + NA];
                 if constexpr (FUSE_X) px += axn[k + NA];
-                // one reciprocal for r and z: r = 1 / a = b / (a b), z = 1 / b = a / (a b); a, b <= 1 + 2^EXP_CLAMP, so
-                // the product stays finite
-                const float a = 1.f + ex2_approx(fminf(pr, EXP_CLAMP)), b = 1.f + ex2_approx(fminf(pz, EXP_CLAMP));
-                const float q = rcp_approx(a * b);
-                r = b * q;
-                z = a * q;
-            } else {
-                r = rcp_approx(1.f + ex2_approx(fminf(pr, EXP_CLAMP)));
-                z = rcp_approx(1.f + ex2_approx(fminf(pz, EXP_CLAMP)));
             }
+            // one reciprocal for r and z: r = 1 / a = b / (a b), z = 1 / b = a / (a b); a, b <= 1 + 2^EXP_CLAMP, so the
+            // product stays finite
+            const float a = 1.f + ex2_approx(fminf(pr, EXP_CLAMP)), b = 1.f + ex2_approx(fminf(pz, EXP_CLAMP));
+            const float q = rcp_approx(a * b);
+            const float r = b * q, z = a * q;
             const float en = ex2_approx(fminf(fmaf(r, pn, px), EXP_CLAMP));
             const float n = (en - 1.f) * rcp_approx(en + 1.f);
             hp[k] = fmaf(z, hp[k] - n, n);
-            const int j = j0 + 8 * ((k >> 1) & 1), col = 8 * (k >> 2) + 2 * cq + (k & 1);
-            __half hi, lo;
-            split_f16(hp[k], hi, lo);
-            *reinterpret_cast<__half *>(hw + (j >> 3) * L::KG + col * 16 + (j & 7) * 2) = hi;
-            *reinterpret_cast<__half *>(hw + L::HLO + (j >> 3) * L::KG + col * 16 + (j & 7) * 2) = lo;
+        }
+        // h as fp16 hi / lo into the other tile buffer, one stmatrix per 8 windows: the accumulator block (i, hb) is an
+        // 8 x 8 fragment (hidden units j0 - gq + 8 hb + 0..7 x windows 8i + 0..7), and transposed, its row c is the
+        // 16-byte row [k-group (j0 + 8 hb) / 8][window 8i + c] of the tile.  Matrices: hi hb 0, hi hb 1, lo hb 0, lo hb 1.
+#pragma unroll
+        for (int i = 0; i < N / 8; ++i) {
+            uint32_t hi[2], lo[2];
+#pragma unroll
+            for (int hb = 0; hb < 2; ++hb) split_f16x2(hp[4 * i + 2 * hb], hp[4 * i + 2 * hb + 1], hi[hb], lo[hb]);
+            stmatrix_x4_trans(hst_addr + (buf ^ 1) * L::PLANES * L::HPLANE + i * 128, hi[0], hi[1], lo[0], lo[1]);
         }
         if (FUSE_X && step + 1 < T) {
 #pragma unroll

@@ -245,6 +245,16 @@ template <> struct Wgmma<128> {
     }
 };
 
+// ---------------------------------------------------------------- stmatrix (sm_90)
+// Four 8x8 b16 matrices, each held in the mma fragment layout (lane l: row l/4, columns 2(l%4) and +1 in the low and
+// high half of its register r[m]), stored TRANSPOSED: the 16 bytes at the address from lane 8m + c (16-B aligned)
+// receive column c of matrix m, rows 0..7 in order.
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t smem_addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(smem_addr), "r"(r0),
+                 "r"(r1), "r"(r2), "r"(r3)
+                 : "memory");
+}
+
 // ---------------------------------------------------------------- fp16 hi/lo split
 // v ~= hi + lo with hi = fp16(v), lo = fp16(v - hi): ~22 significant bits for |v| in [2^-14, 65504],
 // absolute error <= 2^-25 below that (fp16 subnormals).  Three fp16 MMAs (hi*hi + hi*lo + lo*hi) with
@@ -252,6 +262,13 @@ template <> struct Wgmma<128> {
 __host__ __device__ __forceinline__ void split_f16(float v, __half &hi, __half &lo) {
     hi = __float2half_rn(v);
     lo = __float2half_rn(v - __half2float(hi));
+}
+// the same split of two values, packed as f16x2 (v0 in the low half): bit for bit what split_f16 gives for each
+__device__ __forceinline__ void split_f16x2(float v0, float v1, uint32_t &hi, uint32_t &lo) {
+    const __half2 h = __floats2half2_rn(v0, v1);
+    const __half2 l = __floats2half2_rn(v0 - __low2float(h), v1 - __high2float(h));
+    hi = *reinterpret_cast<const uint32_t *>(&h);
+    lo = *reinterpret_cast<const uint32_t *>(&l);
 }
 
 // ---------------------------------------------------------------- streaming global access
