@@ -63,7 +63,8 @@ typedef struct mdk_bam_batch mdk_bam_batch;  /* the records of one region, in BA
 /* GRUModel constructor arguments (medaka/architectures/gru.py:13-21). */
 typedef struct mdk_model_desc {
     int32_t num_features;   /* F = 10 * len(dtypes) */
-    int32_t gru_size;       /* H; this build supports 128 (every shipped counts-matrix model) */
+    int32_t gru_size;       /* H: 128 (every shipped counts-matrix model) or 256 (what `medaka train` builds by default,
+                               DEFAULT_MODEL_DICT); any other width fails with MDK_ERR_UNSUPPORTED */
     int32_t n_layers;       /* 2 */
     int32_t bidirectional;  /* 1 */
     int32_t num_classes;    /* linear head is hard-coded to 5 outputs (gru.py:53-55) */
@@ -118,10 +119,13 @@ int mdk_engine_load_linear(mdk_engine *e, const float *w, const float *b);
 /* TorchModel.half() / --full_precision (medaka/prediction.py:164-168): MDK_PREC_* */
 int mdk_engine_set_precision(mdk_engine *e, int mode);
 int mdk_engine_get_precision(mdk_engine *e, int *mode);
-/* MDK_REC_*: tiles per CTA of the recurrent kernels (A/B measurements; AUTO is the default) */
+/* MDK_REC_*: tiles per CTA of the recurrent kernels (A/B measurements; AUTO is the default).  At gru_size 256 the
+ * recurrence has one kernel (one 4-CTA cluster per 16-window tile and direction) and only MDK_REC_AUTO is accepted. */
 int mdk_engine_set_rec_mode(mdk_engine *e, int mode);
 /* pre-size the compute lanes (workspace + staging) for groups of up to B windows of T columns (otherwise grown on
- * demand, to the size of the batch that opens a group - i.e. without a reserve call nothing is coalesced) */
+ * demand, to the size of the batch that opens a group - i.e. without a reserve call nothing is coalesced).  At gru_size
+ * 256 B is capped at the group size (no group holds more) and the workspace (gi, h0, h1 in fp32: 10 KiB per position)
+ * has a budget of 48 GiB; a reserve beyond it fails with MDK_ERR_ARG. */
 int mdk_engine_reserve(mdk_engine *e, int64_t B, int64_t T);
 /* predict_on_batch with HOST buffers: H2D feats, forward, D2H probs (+logits, +labels when
  * non-NULL); returns when outputs are in host memory. */
@@ -172,7 +176,8 @@ int mdk_engine_set_group_windows(mdk_engine *e, int64_t windows);
  * T changes, or on flush / sync; results are copied from the staging into the call's own buffers (each output buffer is
  * written only by the pieces of its call).  So the tail of one call (say 55 windows) runs together with the head of
  * the next instead of as a forward that fills a few SMs for as long as a full one.  A call of more windows than a
- * group holds runs as one forward of its own.  feats_dev and the outputs must stay untouched until the sync; give
+ * group holds runs as one forward of its own (at gru_size 128; at 256 it is cut into groups, whose workspace is bounded).
+ * feats_dev and the outputs must stay untouched until the sync; give
  * calls that may be in flight together distinct output buffers. */
 int mdk_engine_forward_dev(mdk_engine *e, const float *feats_dev, int64_t B, int64_t T,
                            float *probs_dev, float *logits_dev, uint8_t *labels_dev);
@@ -194,14 +199,16 @@ int mdk_engine_read_activation(mdk_engine *e, int which, float *out_host, int64_
 int mdk_engine_read_activation_windows(mdk_engine *e, int which, int64_t first, int64_t count, float *out_host,
                                        int64_t n_floats);
 /* keep != 0: leave the layer-1 output in HBM (for mdk_engine_read_activation(e, 1, ...)) by running the 5-class head as
- * its own kernel; default 0: the tensor-core path fuses the head into the layer-1 recurrence */
+ * its own kernel; default 0: the tensor-core path fuses the head into the layer-1 recurrence (at gru_size 128 only: at
+ * 256 the head always runs as its own kernel and the layer-1 output is always kept) */
 int mdk_engine_keep_activations(mdk_engine *e, int keep);
 /* number of kernels launched by this engine since creation (bench.py "gpu_launches") */
 int64_t mdk_engine_launch_count(mdk_engine *e);
 /* Number of windows per predict_on_batch call that fills the device exactly once: the recurrent kernel runs one CTA per
  * (16-window tile, direction), so 16 * (SMs / 2) windows = 1056 on an H100 is one full wave (the reference's --batch_size
  * default, medaka/prediction.py:14 / medaka.py, is sized for its own GPUs' memory; a 200-window batch uses 26 of 132 SMs).
- * Callers that own the batching (run_prediction) should coalesce to this size. */
+ * At gru_size 256 it runs one 4-CTA cluster per (tile, direction): 16 windows per two clusters that are resident at once
+ * (240 on an H100 SXM).  Callers that own the batching (run_prediction) should coalesce to this size. */
 int64_t mdk_engine_preferred_windows(mdk_engine *e);
 
 /* ---- featuriser seam: replaces CountsFeatureEncoder._post_process_pileup --------------------

@@ -74,7 +74,14 @@ static cudaError_t ws_sync(mdk_ws &ws) {
     return err == cudaSuccess ? cudaStreamSynchronize(ws.l1_stream) : err;
 }
 
-static int in_features(const mdk_engine *e, int layer) { return layer == 0 ? e->desc.num_features : H2; }
+static int in_features(const mdk_engine *e, int layer) { return layer == 0 ? e->desc.num_features : 2 * e->desc.gru_size; }
+
+// At gru_size 256 the workspace holds gi, h0 and h1 as fp32 rows: 6H + 2H + 2H floats, 10 KiB per position (24.6 GB
+// for one wave of 240 windows x 10 000 columns on an H100 SXM).  Groups are cut to one wave and mdk_engine_reserve caps
+// its windows at a group, so only longer windows or a larger mdk_engine_set_group_windows can ask for more; beyond this
+// budget the forward fails instead of taking the whole card.
+constexpr int64_t WS256_BYTES_PER_POS = (int64_t)(GI256_COLS + 2 * H2_256) * sizeof(float);
+constexpr int64_t WS256_BUDGET = (int64_t)48 << 30;
 
 // The weights as the kernels read them, packed on the host (gru_pack.cuh) and uploaded once after each load.
 static int prepare_weights(mdk_engine *e) {
@@ -88,7 +95,7 @@ static int prepare_weights(mdk_engine *e) {
     int rc;
     for (int l = 0; l < 2; ++l) {
         LayerWeights &lw = e->layer[l];
-        const PackedLayer p = pack_layer(lw, in_features(e, l), l);
+        const PackedLayer p = pack_layer(lw, in_features(e, l), l, e->desc.gru_size);
         if ((rc = dw.upload(e->stream, &lw.w_in_packed, p.w_in_packed)) || (rc = dw.upload(e->stream, &lw.bias_gi, p.bias_gi)) ||
             (rc = dw.upload(e->stream, &lw.b_hn, p.b_hn)) || (rc = dw.upload(e->stream, &lw.bias_gi_tc, p.bias_gi_tc)) ||
             (rc = dw.upload(e->stream, &lw.b_hn_tc, p.b_hn_tc)) || (rc = dw.upload(e->stream, &lw.w_hh_t, p.w_hh_t)) ||
@@ -107,6 +114,10 @@ static int ensure_workspace(mdk_engine *e, mdk_ws &ws, int64_t B, int64_t T) {
     const int64_t rows = tiled_rows(B, T);
     const int64_t need = ((rows + XT_ROWS - 1) / XT_ROWS) * XT_ROWS;
     if (need <= ws.cap_pos) return MDK_OK;
+    const bool wide = e->desc.gru_size == H256;
+    MDK_REQUIRE(!wide || need * WS256_BYTES_PER_POS <= WS256_BUDGET, MDK_ERR_ARG,
+                "engine: at gru_size 256 a forward of this many positions exceeds the 48 GiB workspace budget (10 KiB "
+                "per position)");
     MDK_CUDA(ws_sync(ws));
     dev_free(ws.gi);
     if (ws.h0) { cudaFree(ws.h0); ws.h0 = nullptr; }
@@ -115,21 +126,22 @@ static int ensure_workspace(mdk_engine *e, mdk_ws &ws, int64_t B, int64_t T) {
     dev_free(ws.plog);
     ws.cap_pos = 0;
     int rc;
-    if ((rc = dev_alloc(&ws.gi, (size_t)need * GI_COLS))) return rc;
-    MDK_CUDA(cudaMalloc(&ws.h0, (size_t)need * H2 * sizeof(float)));
-    if ((rc = dev_alloc(&ws.plog, (size_t)NDIR * (need / WT) * PLOG_TS_FLOATS))) return rc;
+    if ((rc = dev_alloc(&ws.gi, (size_t)need * (wide ? GI256_COLS : GI_COLS)))) return rc;
+    MDK_CUDA(cudaMalloc(&ws.h0, (size_t)need * (wide ? H2_256 : H2) * sizeof(float)));
+    if (!wide && (rc = dev_alloc(&ws.plog, (size_t)NDIR * (need / WT) * PLOG_TS_FLOATS))) return rc;
     ws.cap_pos = need;
     return MDK_OK;
 }
 
-// h1 (the layer-1 output, 1 KiB / position) only exists on the unfused-head paths: allocated on first use
-static int ensure_h1(mdk_ws &ws) {
+// h1 (the layer-1 output, 1 KiB / position, 2 KiB at gru_size 256) only exists on the unfused-head paths: allocated on
+// first use
+static int ensure_h1(mdk_ws &ws, int width) {
     if (ws.cap_h1 >= ws.cap_pos && ws.h1) return MDK_OK;
     MDK_CUDA(ws_sync(ws));
     dev_free(ws.h1);
     ws.cap_h1 = 0;
     int rc;
-    if ((rc = dev_alloc(&ws.h1, (size_t)ws.cap_pos * H2))) return rc;
+    if ((rc = dev_alloc(&ws.h1, (size_t)ws.cap_pos * width))) return rc;
     ws.cap_h1 = ws.cap_pos;
     return MDK_OK;
 }
@@ -183,6 +195,45 @@ static int ensure_var(mdk_lane &ln) {
     return MDK_OK;
 }
 
+// The forward at gru_size 256, on the same streams and events as run_forward: the layer-0 input projection, the layer-0
+// recurrence and the layer-1 projection on ws.stream, the layer-1 recurrence and the head on ws.l1_stream.  Every
+// stage reads or writes gi, so each forward's first kernel waits for the previous forward's layer 1.
+static int run_forward256(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int64_t B, int64_t T, float *probs_dev,
+                          float *logits_dev, uint8_t *labels_dev, uint8_t *quals_dev, const HeadVariant *var) {
+    int rc;
+    if ((rc = ensure_h1(ws, H2_256))) return rc;
+    const int64_t P = B * T;
+    cudaStream_t s = ws.stream, s1 = ws.l1_stream;
+    const bool tc = e->precision == MDK_PREC_TC;
+    const LayerWeights &l0 = e->layer[0], &l1 = e->layer[1];
+    float *h0 = static_cast<float *>(ws.h0);
+    MDK_CUDA(cudaStreamWaitEvent(s, ws.l1_done, 0));
+    MDK_CUDA(cudaEventRecord(e->ev[1], s));
+    MDK_CUDA(launch_inproj0(feats_dev, l0.w_in_packed, l0.bias_gi, ws.gi, P, e->desc.num_features,
+                            T, tc ? 1 : 0, s, H256));
+    MDK_CUDA(cudaEventRecord(e->ev[2], s));
+    if (tc) MDK_CUDA(launch_rec256_tc(ws.gi, l0.w_hh_tm, l0.b_hn_tc, h0, B, T, s));
+    else MDK_CUDA(launch_rec_fp32(ws.gi, l0.w_hh_t, l0.b_hn, h0, B, T, s, H256));
+    MDK_CUDA(cudaEventRecord(e->ev[3], s));
+    if (tc) MDK_CUDA(launch_gemm256_tc(h0, l1.w_in_tc, l1.bias_gi_tc, ws.gi, tiled_rows(B, T), s));
+    else MDK_CUDA(launch_gemm_fp32(h0, l1.w_in_packed, l1.bias_gi, ws.gi, P, H2_256, GI256_COLS, s));
+    MDK_CUDA(cudaEventRecord(e->ev[4], s));
+    MDK_CUDA(cudaStreamWaitEvent(s1, e->ev[4], 0));
+    if (tc) MDK_CUDA(launch_rec256_tc(ws.gi, l1.w_hh_tm, l1.b_hn_tc, ws.h1, B, T, s1));
+    else MDK_CUDA(launch_rec_fp32(ws.gi, l1.w_hh_t, l1.b_hn, ws.h1, B, T, s1, H256));
+    MDK_CUDA(cudaEventRecord(e->ev[5], s1));
+    MDK_CUDA(cudaEventRecord(ws.l1_done, s1));
+    MDK_CUDA(launch_head(ws.h1, e->lin_w, e->lin_b, B, T, tc ? 1 : 0, probs_dev, logits_dev, labels_dev, s1, quals_dev,
+                         var, H2_256));
+    MDK_CUDA(cudaEventRecord(e->ev[6], s1));
+    e->launches += 5;
+    e->last.launches = 5;
+    ws.last_fused_head = false;
+    ws.last_B = B; ws.last_T = T; ws.last_precision = e->precision;
+    e->last_ws = (int)(&ws - e->ws);
+    return MDK_OK;
+}
+
 // The forward pipeline on the workspace's two streams: [layer-0 input projection,] layer 0 and the layer-1 projection on
 // ws.stream, layer 1 and the head on ws.l1_stream.  ev[1..6] bracket the stages for mdk_timings; the wait for the previous
 // forward's layer 1 falls into h2d_ms (unfused layer 0) or rec0_ms (fused), and with the fused layer 0 the rec0_ms and
@@ -192,6 +243,8 @@ static int run_forward(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int64_
     int rc;
     if ((rc = prepare_weights(e))) return rc;
     if ((rc = ensure_workspace(e, ws, B, T))) return rc;
+    if (e->desc.gru_size == H256)
+        return run_forward256(e, ws, feats_dev, B, T, probs_dev, logits_dev, labels_dev, quals_dev, var);
     const int64_t P = B * T;
     cudaStream_t s = ws.stream, s1 = ws.l1_stream;
     const bool tc = e->precision == MDK_PREC_TC;
@@ -210,7 +263,7 @@ static int run_forward(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int64_
                             : e->rec_mode == MDK_REC_ONE_TILE ? 1
                             : fuse_x || tiles * NDIR > (int64_t)e->sm_count ? 2 : 1;
     const bool fuse_head = tc && !e->keep_act;
-    if (!fuse_head && (rc = ensure_h1(ws))) return rc;
+    if (!fuse_head && (rc = ensure_h1(ws, H2))) return rc;
     // gi is still read by the previous forward's layer 1: its first writer here waits for it
     if (!fuse_x) MDK_CUDA(cudaStreamWaitEvent(s, ws.l1_done, 0));
     MDK_CUDA(cudaEventRecord(e->ev[1], s));
@@ -436,7 +489,8 @@ int mdk_device_synchronize(int device) {
 
 int mdk_engine_create(int device, const mdk_model_desc *desc, mdk_engine **out) {
     MDK_REQUIRE(desc && out, MDK_ERR_ARG, "engine_create: NULL argument");
-    MDK_REQUIRE(desc->gru_size == H, MDK_ERR_UNSUPPORTED, "engine_create: only gru_size == 128 is supported");
+    MDK_REQUIRE(desc->gru_size == H || desc->gru_size == H256, MDK_ERR_UNSUPPORTED,
+                "engine_create: gru_size must be 128 or 256");
     MDK_REQUIRE(desc->n_layers == 2 && desc->bidirectional == 1, MDK_ERR_UNSUPPORTED,
                 "engine_create: only the 2-layer bidirectional GRU is supported");
     MDK_REQUIRE(desc->num_features >= 1 && desc->num_features <= 1024, MDK_ERR_ARG, "engine_create: bad num_features");
@@ -453,6 +507,18 @@ int mdk_engine_create(int device, const mdk_model_desc *desc, mdk_engine **out) 
     e->device = device;
     e->desc = *desc;
     e->sm_count = prop.multiProcessorCount;
+    if (desc->gru_size == H256) {     // one wave of the cluster recurrence: one 4-CTA cluster per (tile, direction)
+        int clusters = 0;
+        cudaError_t err = rec256_max_clusters(&clusters);
+        if (err != cudaSuccess) { delete e; return cuda_fail(err, "rec256_max_clusters", __FILE__, __LINE__); }
+        if (clusters < 1) {
+            delete e;
+            set_error("engine_create: gru_size 256 needs a cluster of 4 CTAs with 150 KiB of shared memory each; none "
+                      "fits this device");
+            return MDK_ERR_UNSUPPORTED;
+        }
+        e->wave256 = (int64_t)WT * std::max(1, clusters / NDIR);
+    }
     for (auto &ws : e->ws) {
         cudaError_t err = cudaStreamCreateWithFlags(&ws.stream, cudaStreamNonBlocking);
         if (err == cudaSuccess) err = cudaStreamCreateWithFlags(&ws.l1_stream, cudaStreamNonBlocking);
@@ -524,10 +590,11 @@ int mdk_engine_load_gru(mdk_engine *e, int layer, int direction, const float *w_
     MDK_CUDA(cudaSetDevice(e->device));
     { int rcq = quiesce(e); if (rcq) return rcq; }
     LayerWeights &lw = e->layer[layer];
-    lw.w_ih[direction].assign(w_ih, w_ih + (size_t)G3 * in_features(e, layer));
-    lw.w_hh[direction].assign(w_hh, w_hh + (size_t)G3 * H);
-    lw.b_ih[direction].assign(b_ih, b_ih + G3);
-    lw.b_hh[direction].assign(b_hh, b_hh + G3);
+    const int g3 = 3 * e->desc.gru_size;
+    lw.w_ih[direction].assign(w_ih, w_ih + (size_t)g3 * in_features(e, layer));
+    lw.w_hh[direction].assign(w_hh, w_hh + (size_t)g3 * e->desc.gru_size);
+    lw.b_ih[direction].assign(b_ih, b_ih + g3);
+    lw.b_hh[direction].assign(b_hh, b_hh + g3);
     e->prepared = false;
     return MDK_OK;
 }
@@ -536,7 +603,7 @@ int mdk_engine_load_linear(mdk_engine *e, const float *w, const float *b) {
     MDK_REQUIRE(e && w && b, MDK_ERR_ARG, "load_linear: NULL argument");
     MDK_CUDA(cudaSetDevice(e->device));
     { int rcq = quiesce(e); if (rcq) return rcq; }
-    e->lin_w_host.assign(w, w + NCLS * H2);
+    e->lin_w_host.assign(w, w + NCLS * 2 * e->desc.gru_size);
     e->lin_b_host.assign(b, b + NCLS);
     e->prepared = false;
     return MDK_OK;
@@ -558,6 +625,8 @@ int mdk_engine_set_rec_mode(mdk_engine *e, int mode) {
     MDK_REQUIRE(e, MDK_ERR_ARG, "engine is NULL");
     MDK_REQUIRE(mode == MDK_REC_AUTO || mode == MDK_REC_ONE_TILE || mode == MDK_REC_PINGPONG, MDK_ERR_ARG,
                 "set_rec_mode: unknown mode");
+    MDK_REQUIRE(mode == MDK_REC_AUTO || e->desc.gru_size == H, MDK_ERR_UNSUPPORTED,
+                "set_rec_mode: at gru_size 256 the recurrence has one kernel; only MDK_REC_AUTO applies");
     e->rec_mode = mode;
     return MDK_OK;
 }
@@ -575,6 +644,7 @@ int mdk_engine_reserve(mdk_engine *e, int64_t B, int64_t T) {
     MDK_CUDA(cudaSetDevice(e->device));
     int rc;
     if ((rc = launch_group(e))) return rc;
+    if (e->desc.gru_size == H256) B = std::min(B, group_limit(e));   // no group at 256 holds more (forward_dev cuts too)
     const bool big = B * T > mdk_engine::SMALL_POS;
     const int l0 = big ? 0 : mdk_engine::BIG_LANES, l1 = big ? mdk_engine::BIG_LANES : mdk_engine::N_LANES;
     for (int i = l0; i < l1; ++i) {
@@ -594,8 +664,8 @@ int mdk_engine_forward_dev(mdk_engine *e, const float *feats_dev, int64_t B, int
     int64_t gmax = group_limit(e);
     // A call of more than one group's windows was sized by its caller (one full wave of the two-tile kernel is 2112
     // windows on an H100): it runs as one forward of its own instead of being cut into groups that each fill part of
-    // the device.
-    if (B > gmax) {
+    // the device.  At gru_size 256 a group is already a full wave and the workspace is bounded: the call is cut.
+    if (B > gmax && e->desc.gru_size == H) {
         if ((rc = launch_group(e))) return rc;
         gmax = B;
     }
@@ -776,21 +846,23 @@ int mdk_engine_read_activation_windows(mdk_engine *e, int which, int64_t first, 
     MDK_REQUIRE(ln.last_B > 0 && ln.last_T > 0, MDK_ERR_STATE, "read_activation: no forward recorded");
     MDK_REQUIRE(first >= 0 && count > 0 && first + count <= ln.last_B, MDK_ERR_ARG,
                 "read_activation: windows first .. first + count - 1 must lie in the last forward's B windows");
-    MDK_REQUIRE(n_floats == count * ln.last_T * H2, MDK_ERR_ARG, "read_activation: size must be count*T*256");
+    const int width = 2 * e->desc.gru_size;
+    MDK_REQUIRE(n_floats == count * ln.last_T * width, MDK_ERR_ARG, "read_activation: size must be count*T*2*gru_size");
     MDK_REQUIRE(!(which == 1 && ln.last_fused_head), MDK_ERR_STATE,
                 "read_activation(1): the last forward fused the head into layer 1 (h1 never reached HBM); call "
                 "mdk_engine_keep_activations(e, 1) before the forward");
     MDK_CUDA(cudaSetDevice(e->device));
     MDK_CUDA(ws_sync(ln));
     if (ln.last_precision == MDK_PREC_FP32) {
-        const float *src = (which == 1 ? ln.h1 : reinterpret_cast<const float *>(ln.h0)) + first * ln.last_T * H2;
+        const float *src = (which == 1 ? ln.h1 : reinterpret_cast<const float *>(ln.h0)) + first * ln.last_T * width;
         MDK_CUDA(cudaMemcpy(out_host, src, (size_t)n_floats * sizeof(float), cudaMemcpyDeviceToHost));
     } else {
-        // tensor-core path: rows are tile-interleaved (and layer 0 is stored as fp16 hi/lo operand tiles)
+        // tensor-core path: rows are tile-interleaved (and at gru_size 128 layer 0 is stored as fp16 hi/lo operand tiles)
         float *tmp = nullptr;
         MDK_CUDA(cudaMalloc(&tmp, (size_t)n_floats * sizeof(float)));
-        cudaError_t err = which == 0 ? launch_unpack_h0(ln.h0, tmp, first, count, ln.last_T, ln.stream)
-                                     : launch_untile_rows(ln.h1, tmp, first, count, ln.last_T, ln.stream);
+        const float *rows = which == 1 ? ln.h1 : static_cast<const float *>(ln.h0);
+        cudaError_t err = which == 0 && width == H2 ? launch_unpack_h0(ln.h0, tmp, first, count, ln.last_T, ln.stream)
+                                                    : launch_untile_rows(rows, tmp, first, count, ln.last_T, ln.stream, width);
         if (err == cudaSuccess) err = cudaStreamSynchronize(ln.stream);
         if (err == cudaSuccess) err = cudaMemcpy(out_host, tmp, (size_t)n_floats * sizeof(float), cudaMemcpyDeviceToHost);
         cudaFree(tmp);
@@ -822,6 +894,7 @@ int mdk_engine_keep_activations(mdk_engine *e, int keep) {
 }
 
 int64_t mdk_engine_preferred_windows(mdk_engine *e) {
+    if (e && e->desc.gru_size == H256) return e->wave256;
     const int sms = e ? e->sm_count : 132;
     return (int64_t)mdk::WT * (sms / mdk::NDIR);
 }

@@ -19,6 +19,11 @@ constexpr int NDIR = 2;
 constexpr int GI_COLS = NDIR * G3;  // 768: input-projection row [fwd r z n | rev r z n]
 constexpr int H2 = NDIR * H;        // 256: layer output width
 constexpr int NCLS = 5;             // gru.py:53-55
+// gru_size 256, the width `medaka train` builds by default (gru256.cu)
+constexpr int H256 = 256;
+constexpr int G3_256 = 3 * H256;
+constexpr int GI256_COLS = NDIR * G3_256;   // 1536
+constexpr int H2_256 = NDIR * H256;         // 512
 
 void set_error(const std::string &msg);
 int cuda_fail(cudaError_t err, const char *what, const char *file, int line);
@@ -290,6 +295,7 @@ struct mdk_engine {
     int precision = MDK_PREC_TC;
     int sm_count = 132;
     int rec_mode = MDK_REC_AUTO;  // tiles per CTA of the tensor-core recurrences (MDK_REC_*)
+    int64_t wave256 = 0;          // gru_size 256: windows of one wave of the cluster recurrence (16 per 2 clusters)
     static constexpr int BIG_WS = 1, BIG_LANES = 4, SMALL_LANES = 14;
     static constexpr int N_LANES = BIG_LANES + SMALL_LANES, N_WS = BIG_WS + SMALL_LANES;
     static constexpr int64_t SMALL_POS = 1 << 18;   // forwards up to this many positions run on the small lanes
@@ -324,19 +330,21 @@ namespace mdk {
 // ---- launchers (each returns cudaGetLastError() of its launch) -------------------------------
 // misc.cu
 // tiled != 0: gi rows are written / h1 rows are read in tile-interleaved order (T = window length)
+// hs: the GRU width (H or H256); gi has 6 hs columns
 cudaError_t launch_inproj0(const float *feats, const float *w_packed, const float *bias, float *gi,
-                           int64_t P, int F, int64_t T, int tiled, cudaStream_t s);
+                           int64_t P, int F, int64_t T, int tiled, cudaStream_t s, int hs = H);
 enum { HEAD_PLAIN = 0, HEAD_QUALS = 1, HEAD_VARIANT = 2 };     // the heads' instantiations
 // quals (may be null): phred bytes of the argmax class (phred.cuh), from the probability the head writes; var (may be
 // null): the variant outputs, from the same probabilities
 cudaError_t launch_head(const float *h1, const float *lin_w, const float *lin_b, int64_t B, int64_t T, int tiled,
                         float *probs, float *logits, uint8_t *labels, cudaStream_t s, uint8_t *quals = nullptr,
-                        const HeadVariant *var = nullptr);
-cudaError_t launch_untile_rows(const float *src_tiled, float *dst, int64_t w0, int64_t nw, int64_t T, cudaStream_t s);
+                        const HeadVariant *var = nullptr, int width = H2);     // width: h1 row width, H2 or H2_256
+cudaError_t launch_untile_rows(const float *src_tiled, float *dst, int64_t w0, int64_t nw, int64_t T, cudaStream_t s,
+                               int width = H2);
 cudaError_t launch_unpack_h0(const void *h0_tiles, float *out, int64_t w0, int64_t nw, int64_t T, cudaStream_t s);
 // gru_fp32.cu
 cudaError_t launch_rec_fp32(const float *gi, const float *w_hh_t, const float *b_hn, float *h_out, int64_t B,
-                            int64_t T, cudaStream_t s);
+                            int64_t T, cudaStream_t s, int hs = H);
 // C[M][N] = A[M][K] . W[N][K]^T + bias[N], fp32 (K % 16 == 0, N % 128 == 0)
 cudaError_t launch_gemm_fp32(const float *A, const float *W, const float *bias, float *C, int64_t M, int K, int N,
                              cudaStream_t s);
@@ -364,6 +372,15 @@ constexpr int PLOG_TS_FLOATS = NCLS * WT;     // 80 floats per (tile-step, direc
 cudaError_t launch_gemm_tc(const void *x_tiles, const __half *w_in_tm, const float *bias, float *gi, int64_t P,
                            int sm_count, cudaStream_t s);
 int selftest_umma(int device, const float *A, const float *B, float *D, int N, int K, int variant);
+// gru256.cu: the tensor-core path at gru_size 256.  gi [tiled rows][1536] and h [tiled rows][512] fp32 (gru256.cu).
+// One layer's recurrence, both directions, one 4-CTA cluster per (16-window tile, direction):
+cudaError_t launch_rec256_tc(const float *gi, const __half *w_hh_tm, const float *b_hn, float *h_out, int64_t B,
+                             int64_t T, cudaStream_t s);
+// clusters of the recurrence that are resident at once (one wave)
+cudaError_t rec256_max_clusters(int *clusters);
+// layer-1 input projection over M tiled rows (w_in_tm: LayerWeights::w_in_tc at 256)
+cudaError_t launch_gemm256_tc(const float *h0, const __half *w_in_tm, const float *bias, float *gi, int64_t M,
+                              cudaStream_t s);
 // pileup.cu
 // exclusive scan of n per-block counts, in place, by one block: counts[i] = sum of counts[0, i), counts[n] = the total
 cudaError_t launch_scan_blocks(int64_t *counts, int64_t n, cudaStream_t s);

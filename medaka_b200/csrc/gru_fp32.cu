@@ -11,46 +11,51 @@ namespace mdk {
 __device__ __forceinline__ float sigmoid_acc(float x) { return 1.0f / (1.0f + expf(-x)); }
 
 // -------------------------------------------------------------------------------------
-// Recurrent kernel.  One CTA = NB windows of one direction; 128 threads, thread j owns hidden
+// Recurrent kernel.  One CTA = NB windows of one direction; HS threads, thread j owns hidden
 // unit j: the r/z/n rows of W_hh for unit j stream from shared memory (W_hh^T resident for the
-// whole sequence, 192 KiB) while the NB h vectors are shared-memory broadcasts.
-// gi   [B*T][768]  (position p = b*T + t ; columns dir*384 + gate*128 + j)
-// h_out[B*T][256]  (columns dir*128 + j)
+// whole sequence, 192 KiB at HS = 128) or, at HS = 256 where W_hh^T takes 768 KiB, from L2, while
+// the NB h vectors are shared-memory broadcasts.
+// gi   [B*T][6 HS]  (position p = b*T + t ; columns dir*3HS + gate*HS + j)
+// h_out[B*T][2 HS]  (columns dir*HS + j)
 // -------------------------------------------------------------------------------------
 constexpr int REC_NB = 8;
 
-__global__ void __launch_bounds__(128, 1) rec_fp32_kernel(const float *__restrict__ gi,
-                                                          const float *__restrict__ w_hh_t,
-                                                          const float *__restrict__ b_hn,
-                                                          float *__restrict__ h_out, int64_t B, int64_t T) {
+template <int HS>
+__global__ void __launch_bounds__(HS, 1) rec_fp32_kernel(const float *__restrict__ gi,
+                                                         const float *__restrict__ w_hh_t,
+                                                         const float *__restrict__ b_hn,
+                                                         float *__restrict__ h_out, int64_t B, int64_t T) {
+    constexpr int G3S = 3 * HS, GIS = NDIR * G3S;
+    constexpr bool SMEM_W = HS == H;
     extern __shared__ __align__(16) float smem[];
-    float *wt = smem;                          // [128][384]
-    float *hs = smem + H * G3;                 // [2][NB][128]
+    float *hs = smem + (SMEM_W ? HS * G3S : 0);     // [2][NB][HS]
     const int j = threadIdx.x;
     const int dir = blockIdx.y;
     const int64_t b0 = (int64_t)blockIdx.x * REC_NB;
     const int nb = (int)min((int64_t)REC_NB, B - b0);
 
-    const float *wsrc = w_hh_t + (int64_t)dir * H * G3;
-    for (int i = j; i < H * G3 / 4; i += 128)
-        reinterpret_cast<float4 *>(wt)[i] = reinterpret_cast<const float4 *>(wsrc)[i];
-    for (int i = j; i < 2 * REC_NB * H; i += 128) hs[i] = 0.f;
-    const float bhn = b_hn[dir * H + j];
+    const float *wsrc = w_hh_t + (int64_t)dir * HS * G3S;
+    const float *wt = SMEM_W ? smem : wsrc;     // [HS][3 HS]
+    if (SMEM_W)
+        for (int i = j; i < HS * G3S / 4; i += HS)
+            reinterpret_cast<float4 *>(smem)[i] = reinterpret_cast<const float4 *>(wsrc)[i];
+    for (int i = j; i < 2 * REC_NB * HS; i += HS) hs[i] = 0.f;
+    const float bhn = b_hn[dir * HS + j];
     float hprev[REC_NB];
 #pragma unroll
     for (int n = 0; n < REC_NB; ++n) hprev[n] = 0.f;
     __syncthreads();
 
-    const int64_t col = (int64_t)dir * G3 + j;
+    const int64_t col = (int64_t)dir * G3S + j;
     float gnext[3][REC_NB];
     {
         const int64_t t = dir ? (T - 1) : 0;
 #pragma unroll
         for (int n = 0; n < REC_NB; ++n) {
             const bool ok = n < nb;
-            const float *row = gi + ((b0 + (ok ? n : 0)) * T + t) * GI_COLS + col;
+            const float *row = gi + ((b0 + (ok ? n : 0)) * T + t) * GIS + col;
 #pragma unroll
-            for (int g = 0; g < 3; ++g) gnext[g][n] = ok ? ldg_stream(row + g * H) : 0.f;
+            for (int g = 0; g < 3; ++g) gnext[g][n] = ok ? ldg_stream(row + g * HS) : 0.f;
         }
     }
     int cur = 0;
@@ -66,9 +71,9 @@ __global__ void __launch_bounds__(128, 1) rec_fp32_kernel(const float *__restric
 #pragma unroll
             for (int n = 0; n < REC_NB; ++n) {
                 const bool ok = n < nb;
-                const float *row = gi + ((b0 + (ok ? n : 0)) * T + tn) * GI_COLS + col;
+                const float *row = gi + ((b0 + (ok ? n : 0)) * T + tn) * GIS + col;
 #pragma unroll
-                for (int g = 0; g < 3; ++g) gnext[g][n] = ok ? ldg_stream(row + g * H) : 0.f;
+                for (int g = 0; g < 3; ++g) gnext[g][n] = ok ? ldg_stream(row + g * HS) : 0.f;
             }
         }
         float acc[3][REC_NB];
@@ -76,17 +81,17 @@ __global__ void __launch_bounds__(128, 1) rec_fp32_kernel(const float *__restric
         for (int g = 0; g < 3; ++g)
 #pragma unroll
             for (int n = 0; n < REC_NB; ++n) acc[g][n] = 0.f;
-        const float *hc = hs + cur * REC_NB * H;
+        const float *hc = hs + cur * REC_NB * HS;
 #pragma unroll 2
-        for (int k = 0; k < H; k += 4) {
+        for (int k = 0; k < HS; k += 4) {
             float4 hv[REC_NB];
 #pragma unroll
-            for (int n = 0; n < REC_NB; ++n) hv[n] = *reinterpret_cast<const float4 *>(hc + n * H + k);
+            for (int n = 0; n < REC_NB; ++n) hv[n] = *reinterpret_cast<const float4 *>(hc + n * HS + k);
 #pragma unroll
             for (int kk = 0; kk < 4; ++kk) {
-                const float wr = wt[(k + kk) * G3 + j];
-                const float wz = wt[(k + kk) * G3 + H + j];
-                const float wn = wt[(k + kk) * G3 + 2 * H + j];
+                const float wr = wt[(k + kk) * G3S + j];
+                const float wz = wt[(k + kk) * G3S + HS + j];
+                const float wn = wt[(k + kk) * G3S + 2 * HS + j];
 #pragma unroll
                 for (int n = 0; n < REC_NB; ++n) {
                     const float hvk = kk == 0 ? hv[n].x : kk == 1 ? hv[n].y : kk == 2 ? hv[n].z : hv[n].w;
@@ -96,7 +101,7 @@ __global__ void __launch_bounds__(128, 1) rec_fp32_kernel(const float *__restric
                 }
             }
         }
-        float *hn = hs + (cur ^ 1) * REC_NB * H;
+        float *hn = hs + (cur ^ 1) * REC_NB * HS;
 #pragma unroll
         for (int n = 0; n < REC_NB; ++n) {
             const float r = sigmoid_acc(gcur[0][n] + acc[0][n]);
@@ -104,29 +109,36 @@ __global__ void __launch_bounds__(128, 1) rec_fp32_kernel(const float *__restric
             const float nn = tanhf(gcur[2][n] + r * (acc[2][n] + bhn));
             const float h = (1.0f - z) * nn + z * hprev[n];
             hprev[n] = h;
-            hn[n * H + j] = h;
-            if (n < nb) h_out[((b0 + n) * T + t) * H2 + dir * H + j] = h;
+            hn[n * HS + j] = h;
+            if (n < nb) h_out[((b0 + n) * T + t) * (NDIR * HS) + dir * HS + j] = h;
         }
         __syncthreads();
         cur ^= 1;
     }
 }
 
-cudaError_t launch_rec_fp32(const float *gi, const float *w_hh_t, const float *b_hn, float *h_out, int64_t B,
-                            int64_t T, cudaStream_t s) {
-    if (B == 0 || T == 0) return cudaSuccess;
-    const size_t smem = (size_t)(H * G3 + 2 * REC_NB * H) * sizeof(float);
+template <int HS>
+static cudaError_t launch_rec_fp32_hs(const float *gi, const float *w_hh_t, const float *b_hn, float *h_out, int64_t B,
+                                      int64_t T, cudaStream_t s) {
+    const size_t smem = (size_t)((HS == H ? HS * 3 * HS : 0) + 2 * REC_NB * HS) * sizeof(float);
     // (the attribute is per device: set it on every launch, a process may drive several GPUs from several threads)
-    cudaError_t e = cudaFuncSetAttribute(rec_fp32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(rec_fp32_kernel<HS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     dim3 grid((unsigned)((B + REC_NB - 1) / REC_NB), NDIR);
-    rec_fp32_kernel<<<grid, 128, smem, s>>>(gi, w_hh_t, b_hn, h_out, B, T);
+    rec_fp32_kernel<HS><<<grid, HS, smem, s>>>(gi, w_hh_t, b_hn, h_out, B, T);
     return cudaGetLastError();
+}
+
+cudaError_t launch_rec_fp32(const float *gi, const float *w_hh_t, const float *b_hn, float *h_out, int64_t B,
+                            int64_t T, cudaStream_t s, int hs) {
+    if (B == 0 || T == 0) return cudaSuccess;
+    return hs == H256 ? launch_rec_fp32_hs<H256>(gi, w_hh_t, b_hn, h_out, B, T, s)
+                      : launch_rec_fp32_hs<H>(gi, w_hh_t, b_hn, h_out, B, T, s);
 }
 
 // -------------------------------------------------------------------------------------
 // Input projections, fp32: C[M][N] = A[M][K] . W[N][K]^T + bias[N];  K % 16 == 0, N % 128 == 0.
-// The GRU's layer 1 (K = 256, N = 768) and both layers of the read-level LSTM at either size.
+// The GRU's layer 1 (K = 256, N = 768; K = 512, N = 1536 at gru_size 256) and both layers of the read-level LSTM at either size.
 // Classic 128x128x16 shared-memory tiling, 256 threads, 8x8 register tile.
 // -------------------------------------------------------------------------------------
 constexpr int GM = 128, GN = 128, GK = 16;

@@ -7,23 +7,38 @@
 namespace mdk {
 
 // =====================================================================================
-// Layer-0 input projection: gi[p][c] = sum_f x[p][f] * W[c][f] + bias[c],  c in [0,768)
+// Layer-0 input projection: gi[p][c] = sum_f x[p][f] * W[c][f] + bias[c],  c in [0, 6 HS)
 // K = F (10 or 20) is far too thin for the tensor cores; the kernel is bound by the 3 KiB/position
-// write of gi.  256 threads, each owns 3 of the 768 columns with its weights in registers.
+// (6 KiB at HS = 256) write of gi.  256 threads, each owns 3 (6) of the 768 (1536) columns with its weights in registers.
 // =====================================================================================
-template <int F>
+// Column c of position p into gi: plain rows (fp32 path), or, on the tensor-core path, pre-scaled for the exp2-based gate
+// math (common.cuh gate_scale) in the quad layout (HS = 128, common.cuh) or as tile-interleaved rows (HS = 256, gru256.cu)
+template <int HS>
+__device__ __forceinline__ void store_gi(float *gi, int64_t p, int64_t T, int c, float a, int tiled) {
+    if (!tiled) {
+        gi[p * (6 * HS) + c] = a;
+        return;
+    }
+    const int64_t orow = tiled_row(p / T, p % T, T);
+    const float v = a * gate_scale((c % (3 * HS)) / HS);
+    if (HS == H) gi[gi_quad_index(orow, c)] = v;
+    else gi[orow * (6 * HS) + c] = v;
+}
+
+template <int F, int HS>
 __global__ void __launch_bounds__(256) inproj0_kernel(const float *__restrict__ feats, const float *__restrict__ w,
                                                       const float *__restrict__ bias, float *__restrict__ gi,
                                                       int64_t P, int64_t T, int tiled) {
     constexpr int PT = 64;   // positions per block
+    constexpr int NQ = 6 * HS / 256;   // columns per thread
     __shared__ float xs[PT * F];
     const int tid = threadIdx.x;
     const int64_t p0 = (int64_t)blockIdx.x * PT;
     const int np = (int)min((int64_t)PT, P - p0);
     for (int i = tid; i < np * F; i += 256) xs[i] = feats[p0 * F + i];
-    float wr[3][F], b[3];
+    float wr[NQ][F], b[NQ];
 #pragma unroll
-    for (int q = 0; q < 3; ++q) {
+    for (int q = 0; q < NQ; ++q) {
         const int c = tid + 256 * q;
         b[q] = bias[c];
 #pragma unroll
@@ -31,54 +46,51 @@ __global__ void __launch_bounds__(256) inproj0_kernel(const float *__restrict__ 
     }
     __syncthreads();
     for (int p = 0; p < np; ++p) {
-        float a0 = b[0], a1 = b[1], a2 = b[2];
+        float a[NQ];
+#pragma unroll
+        for (int q = 0; q < NQ; ++q) a[q] = b[q];
 #pragma unroll
         for (int f = 0; f < F; ++f) {
             const float x = xs[p * F + f];   // smem broadcast
-            a0 = fmaf(x, wr[0][f], a0);
-            a1 = fmaf(x, wr[1][f], a1);
-            a2 = fmaf(x, wr[2][f], a2);
+#pragma unroll
+            for (int q = 0; q < NQ; ++q) a[q] = fmaf(x, wr[q][f], a[q]);
         }
         const int64_t pp = p0 + p;
-        if (tiled) {   // tensor-core path: quad layout (common.cuh)
-            const int64_t orow = tiled_row(pp / T, pp % T, T);
-            // (pre-scaled for the exp2-based gate math of rec_tc_kernel, common.cuh gate_scale)
-            gi[gi_quad_index(orow, tid)] = a0 * gate_scale((tid % G3) / H);
-            gi[gi_quad_index(orow, tid + 256)] = a1 * gate_scale(((tid + 256) % G3) / H);
-            gi[gi_quad_index(orow, tid + 512)] = a2 * gate_scale(((tid + 512) % G3) / H);
-        } else {
-            float *row = gi + pp * GI_COLS;
-            row[tid] = a0;
-            row[tid + 256] = a1;
-            row[tid + 512] = a2;
-        }
+#pragma unroll
+        for (int q = 0; q < NQ; ++q) store_gi<HS>(gi, pp, T, tid + 256 * q, a[q], tiled);
     }
 }
 
 // generic F (weights streamed from L1/L2)
+template <int HS>
 __global__ void __launch_bounds__(256) inproj0_generic_kernel(const float *__restrict__ feats,
                                                               const float *__restrict__ w,
                                                               const float *__restrict__ bias, float *__restrict__ gi,
                                                               int64_t P, int F, int64_t T, int tiled) {
     const int64_t p = blockIdx.x;
     if (p >= P) return;
-    const int64_t orow = tiled ? tiled_row(p / T, p % T, T) : p;
-    for (int c = threadIdx.x; c < GI_COLS; c += 256) {
+    for (int c = threadIdx.x; c < 6 * HS; c += 256) {
         float a = bias[c];
         for (int f = 0; f < F; ++f) a = fmaf(feats[p * F + f], w[c * F + f], a);
-        if (tiled) gi[gi_quad_index(orow, c)] = a * gate_scale((c % G3) / H);
-        else gi[orow * GI_COLS + c] = a;
+        store_gi<HS>(gi, p, T, c, a, tiled);
     }
 }
 
-cudaError_t launch_inproj0(const float *feats, const float *w_packed, const float *bias, float *gi, int64_t P,
-                           int F, int64_t T, int tiled, cudaStream_t s) {
-    if (P == 0) return cudaSuccess;
+template <int HS>
+static cudaError_t launch_inproj0_hs(const float *feats, const float *w_packed, const float *bias, float *gi, int64_t P,
+                                     int F, int64_t T, int tiled, cudaStream_t s) {
     const unsigned blocks = (unsigned)((P + 63) / 64);
-    if (F == 10) inproj0_kernel<10><<<blocks, 256, 0, s>>>(feats, w_packed, bias, gi, P, T, tiled);
-    else if (F == 20) inproj0_kernel<20><<<blocks, 256, 0, s>>>(feats, w_packed, bias, gi, P, T, tiled);
-    else inproj0_generic_kernel<<<(unsigned)P, 256, 0, s>>>(feats, w_packed, bias, gi, P, F, T, tiled);
+    if (F == 10) inproj0_kernel<10, HS><<<blocks, 256, 0, s>>>(feats, w_packed, bias, gi, P, T, tiled);
+    else if (F == 20) inproj0_kernel<20, HS><<<blocks, 256, 0, s>>>(feats, w_packed, bias, gi, P, T, tiled);
+    else inproj0_generic_kernel<HS><<<(unsigned)P, 256, 0, s>>>(feats, w_packed, bias, gi, P, F, T, tiled);
     return cudaGetLastError();
+}
+
+cudaError_t launch_inproj0(const float *feats, const float *w_packed, const float *bias, float *gi, int64_t P,
+                           int F, int64_t T, int tiled, cudaStream_t s, int hs) {
+    if (P == 0) return cudaSuccess;
+    return hs == H256 ? launch_inproj0_hs<H256>(feats, w_packed, bias, gi, P, F, T, tiled, s)
+                      : launch_inproj0_hs<H>(feats, w_packed, bias, gi, P, F, T, tiled, s);
 }
 
 // =====================================================================================
@@ -93,7 +105,7 @@ cudaError_t launch_inproj0(const float *feats, const float *w_packed, const floa
 // winning probability (consensus-decoded forwards); HEAD_VARIANT: also the call byte and the phreds of the winning and of
 // the reference class (variant-decoded forwards, phred.cuh), and the phred byte where quals is given.  HEAD_PLAIN is the
 // kernel of the ordinary forward.
-template <int MODE>
+template <int MODE, int K>
 __global__ void __launch_bounds__(256) head_kernel(const float *__restrict__ h1, const float *__restrict__ lin_w,
                                                    const float *__restrict__ lin_b, int64_t P, int64_t B, int64_t T,
                                                    int tiled, float *__restrict__ probs, float *__restrict__ logits,
@@ -102,14 +114,15 @@ __global__ void __launch_bounds__(256) head_kernel(const float *__restrict__ h1,
     const int lane = threadIdx.x & 31;
     const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    float w[NCLS][8];
+    constexpr int NI = K / 32;                     // inputs per lane: 8 (H = 128) or 16 (H = 256)
+    float w[NCLS][NI];
 #pragma unroll
-    for (int c = 0; c < NCLS; ++c) {
-        const float4 a = *reinterpret_cast<const float4 *>(lin_w + c * H2 + lane * 8);
-        const float4 b = *reinterpret_cast<const float4 *>(lin_w + c * H2 + lane * 8 + 4);
-        w[c][0] = a.x; w[c][1] = a.y; w[c][2] = a.z; w[c][3] = a.w;
-        w[c][4] = b.x; w[c][5] = b.y; w[c][6] = b.z; w[c][7] = b.w;
-    }
+    for (int c = 0; c < NCLS; ++c)
+#pragma unroll
+        for (int v = 0; v < NI / 4; ++v) {
+            const float4 a = *reinterpret_cast<const float4 *>(lin_w + c * K + lane * NI + 4 * v);
+            w[c][4 * v] = a.x; w[c][4 * v + 1] = a.y; w[c][4 * v + 2] = a.z; w[c][4 * v + 3] = a.w;
+        }
     const int cls = lane & 7;                      // class owned by this lane after the reduction
     const float my_bias = cls < NCLS ? lin_b[cls] : 0.f;
     constexpr int PU = 4;
@@ -133,23 +146,27 @@ __global__ void __launch_bounds__(256) head_kernel(const float *__restrict__ h1,
     }
     for (int64_t q = q0; q < q1; ++q) {
         const int64_t rb = q * PU;                 // first row of the quad
-        float4 va[PU], vb[PU];
+        float4 va[PU][NI / 4];
 #pragma unroll
         for (int u = 0; u < PU; ++u) {
             const int64_t r = min(rb + u, rows - 1);
-            va[u] = ld_stream4(h1 + r * H2 + lane * 8);
-            vb[u] = ld_stream4(h1 + r * H2 + lane * 8 + 4);
+#pragma unroll
+            for (int v = 0; v < NI / 4; ++v) va[u][v] = ld_stream4(h1 + r * K + lane * NI + 4 * v);
         }
         float v[32];
 #pragma unroll
         for (int u = 0; u < PU; ++u) {
-            const float x[8] = {va[u].x, va[u].y, va[u].z, va[u].w, vb[u].x, vb[u].y, vb[u].z, vb[u].w};
+            float x[NI];
+#pragma unroll
+            for (int i = 0; i < NI / 4; ++i) {
+                x[4 * i] = va[u][i].x; x[4 * i + 1] = va[u][i].y; x[4 * i + 2] = va[u][i].z; x[4 * i + 3] = va[u][i].w;
+            }
 #pragma unroll
             for (int c = 0; c < 8; ++c) {
                 float s = 0.f;
                 if (c < NCLS) {
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) s = fmaf(x[i], w[c][i], s);
+                    for (int i = 0; i < NI; ++i) s = fmaf(x[i], w[c][i], s);
                 }
                 v[u * 8 + c] = s;
             }
@@ -224,18 +241,26 @@ __global__ void __launch_bounds__(256) head_kernel(const float *__restrict__ h1,
     }
 }
 
-cudaError_t launch_head(const float *h1, const float *lin_w, const float *lin_b, int64_t B, int64_t T, int tiled,
-                        float *probs, float *logits, uint8_t *labels, cudaStream_t s, uint8_t *quals,
-                        const HeadVariant *var) {
+template <int K>
+static cudaError_t launch_head_k(const float *h1, const float *lin_w, const float *lin_b, int64_t B, int64_t T, int tiled,
+                                 float *probs, float *logits, uint8_t *labels, cudaStream_t s, uint8_t *quals,
+                                 const HeadVariant *var) {
     const int64_t P = B * T;
-    if (P == 0) return cudaSuccess;
     int64_t blocks = (P + 31) / 32;            // 8 warps per block, 4 positions per warp per iteration
     if (blocks > 132 * 8) blocks = 132 * 8;    // persistent-ish grid: multiple of the SM count
     const dim3 g((unsigned)blocks);
-    if (var) head_kernel<HEAD_VARIANT><<<g, 256, 0, s>>>(h1, lin_w, lin_b, P, B, T, tiled, probs, logits, labels, quals, *var);
-    else if (quals) head_kernel<HEAD_QUALS><<<g, 256, 0, s>>>(h1, lin_w, lin_b, P, B, T, tiled, probs, logits, labels, quals, {});
-    else head_kernel<HEAD_PLAIN><<<g, 256, 0, s>>>(h1, lin_w, lin_b, P, B, T, tiled, probs, logits, labels, nullptr, {});
+    if (var) head_kernel<HEAD_VARIANT, K><<<g, 256, 0, s>>>(h1, lin_w, lin_b, P, B, T, tiled, probs, logits, labels, quals, *var);
+    else if (quals) head_kernel<HEAD_QUALS, K><<<g, 256, 0, s>>>(h1, lin_w, lin_b, P, B, T, tiled, probs, logits, labels, quals, {});
+    else head_kernel<HEAD_PLAIN, K><<<g, 256, 0, s>>>(h1, lin_w, lin_b, P, B, T, tiled, probs, logits, labels, nullptr, {});
     return cudaGetLastError();
+}
+
+cudaError_t launch_head(const float *h1, const float *lin_w, const float *lin_b, int64_t B, int64_t T, int tiled,
+                        float *probs, float *logits, uint8_t *labels, cudaStream_t s, uint8_t *quals,
+                        const HeadVariant *var, int width) {
+    if (B * T == 0) return cudaSuccess;
+    return width == H2_256 ? launch_head_k<H2_256>(h1, lin_w, lin_b, B, T, tiled, probs, logits, labels, s, quals, var)
+                           : launch_head_k<H2>(h1, lin_w, lin_b, B, T, tiled, probs, logits, labels, s, quals, var);
 }
 
 // Head of the fused path (gru.py:53-55,67-71): logits = fwd partial + rev partial + bias, softmax, first-max argmax.
@@ -322,20 +347,21 @@ cudaError_t launch_unpack_h0(const void *h0_tiles, float *out, int64_t w0, int64
     return cudaGetLastError();
 }
 
-// fp32 [rows'][256] in tile-interleaved order -> [nw*T][256] in position order: windows w0 .. w0 + nw - 1 (debug /
+// fp32 [rows'][width] in tile-interleaved order -> [nw*T][width] in position order: windows w0 .. w0 + nw - 1 (debug /
 // layer-wise parity)
 __global__ void untile_rows_kernel(const float *__restrict__ src, float *__restrict__ dst, int64_t w0, int64_t nw,
-                                   int64_t T) {
+                                   int64_t T, int width) {
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (i >= nw * T * H2) return;
-    const int64_t p = w0 * T + i / H2;
-    dst[i] = src[tiled_row(p / T, p % T, T) * H2 + (i % H2)];
+    if (i >= nw * T * width) return;
+    const int64_t p = w0 * T + i / width;
+    dst[i] = src[tiled_row(p / T, p % T, T) * width + (i % width)];
 }
 
-cudaError_t launch_untile_rows(const float *src_tiled, float *dst, int64_t w0, int64_t nw, int64_t T, cudaStream_t s) {
-    const int64_t n = nw * T * H2;
+cudaError_t launch_untile_rows(const float *src_tiled, float *dst, int64_t w0, int64_t nw, int64_t T, cudaStream_t s,
+                               int width) {
+    const int64_t n = nw * T * width;
     if (n == 0) return cudaSuccess;
-    untile_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(src_tiled, dst, w0, nw, T);
+    untile_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(src_tiled, dst, w0, nw, T, width);
     return cudaGetLastError();
 }
 

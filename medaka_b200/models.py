@@ -352,7 +352,8 @@ class GRUModel(object):
     def set_rec_mode(self, mode):
         """'auto' | 'one' | 'pp': tiles per CTA of the recurrent kernels (mdk_engine_set_rec_mode).  'auto' runs two
         tiles per CTA for every forward with at most 16 features, so that a group's layer 1 runs beside the next group's
-        layer 0, and otherwise one tile per CTA up to one wave of windows, two beyond."""
+        layer 0, and otherwise one tile per CTA up to one wave of windows, two beyond.  At gru_size 256 the recurrence
+        has one kernel and only 'auto' is accepted."""
         code = {"auto": _lm.lib.MDK_REC_AUTO, "one": _lm.lib.MDK_REC_ONE_TILE, "pp": _lm.lib.MDK_REC_PINGPONG}[mode]
         _lm.check(_lm.lib.mdk_engine_set_rec_mode(self._engine, code))
 
@@ -385,8 +386,8 @@ class GRUModel(object):
                                              "head_ms", "d2h_ms", "total_ms", "launches")}
 
     def read_activation(self, which, first=0, count=None):
-        """Layer output [count,T,256] of windows first .. first + count - 1 (default: all B) of the last forward (0 = layer
-        0, 1 = layer 1) for layer-wise parity."""
+        """Layer output [count,T,2*gru_size] of windows first .. first + count - 1 (default: all B) of the last forward
+        (0 = layer 0, 1 = layer 1) for layer-wise parity."""
         t = self.last_timings()  # syncs
         del t
         shape = self._last_shape
@@ -414,8 +415,8 @@ class GRUModel(object):
         _lm.check(_lm.lib.mdk_engine_keep_activations(self._engine, 1 if keep else 0))
 
     def preferred_batch_size(self):
-        """Windows per batch that fill the device in one wave (1056 on an H100); ``batch_size="auto"`` in
-        ``prediction.run_prediction`` / ``predict_regions`` resolves to this."""
+        """Windows per batch that fill the device in one wave (1056 on an H100 at gru_size 128, 240 at 256);
+        ``batch_size="auto"`` in ``prediction.run_prediction`` / ``predict_regions`` resolves to this."""
         return int(_lm.lib.mdk_engine_preferred_windows(self._engine))
 
     @property
