@@ -529,6 +529,69 @@ int mdk_debug_read_plog(mdk_engine *e, float *out_host, int64_t n_floats);
  * MDK_ERR_STATE before the first completed forward, MDK_ERR_ARG when n_floats is not the stage's size. */
 int mdk_rl_debug_read(mdk_rl_engine *e, int which, float *out_host, int64_t n_floats);
 
+/* ---- training seam: replaces the GRUModel forward / backward, CrossEntropyLoss, clip_grad_norm_ and the torch.optim
+ * step of medaka train (medaka/torch_ext.py run_epoch, medaka/models.py process_batch) for the consensus GRU of
+ * mdk_model_desc (2 layers, bidirectional, gru_size 128 or 256, 5 classes).  fp32 throughout, the arithmetic of
+ * MDK_PREC_FP32: the forward's logits and probabilities equal mdk_engine_forward's at MDK_PREC_FP32 bit for bit.
+ * An mdk_trainer is separate from any mdk_engine; it keeps fp32 master weights, their gradient and the optimizer state
+ * on the device.  Weights: the flat array of mdk_trainer_read_params is the state dict in torch order (per layer and
+ * direction weight_ih, weight_hh, bias_ih, bias_hh; then linear.weight, linear.bias), mdk_trainer_num_params floats. */
+typedef struct mdk_trainer mdk_trainer;
+
+#define MDK_OPT_RMSPROP 0   /* torch.optim.RMSprop (alpha, eps, weight_decay, momentum; not centered) */
+#define MDK_OPT_ADAM 1      /* torch.optim.Adam (beta1, beta2, eps, weight_decay; not amsgrad) */
+#define MDK_OPT_NADAM 2     /* torch.optim.NAdam (beta1, beta2, eps, weight_decay, momentum_decay) */
+#define MDK_OPT_SGD 3       /* torch.optim.SGD (momentum, dampening, weight_decay, nesterov) */
+
+typedef struct mdk_optim_desc {
+    int32_t kind;           /* MDK_OPT_* */
+    float alpha, beta1, beta2, eps, weight_decay, momentum, dampening, momentum_decay;
+    int32_t nesterov;
+} mdk_optim_desc;
+
+typedef struct mdk_train_stats {
+    double loss;            /* CrossEntropyLoss() of the batch: mean over the B*T positions */
+    int64_t n_correct;      /* positions whose argmax (first maximum) of the logits is the label */
+    int64_t n_positions;
+    float grad_norm;        /* L2 norm of all gradients before clipping (mdk_trainer_step only); NaN or inf when
+                               a gradient is not finite */
+    int32_t skipped;        /* the update was skipped (non-finite gradient): weights and optimizer state unchanged */
+} mdk_train_stats;
+
+int mdk_trainer_create(int device, const mdk_model_desc *desc, mdk_trainer **out);
+int mdk_trainer_destroy(mdk_trainer *tr);
+/* as mdk_engine_load_gru / mdk_engine_load_linear; a load resets the optimizer state and leaves the tensors it does not
+ * name at their current (trained) values */
+int mdk_trainer_load_gru(mdk_trainer *tr, int layer, int direction, const float *w_ih, const float *w_hh,
+                         const float *b_ih, const float *b_hh);
+int mdk_trainer_load_linear(mdk_trainer *tr, const float *w, const float *b);
+/* the optimizer and its hyper-parameters (the learning rate is per step); resets its state.  Default: RMSprop with
+ * the reference's arguments (alpha 0.9, eps 1e-7, momentum 0) */
+int mdk_trainer_set_optimizer(mdk_trainer *tr, const mdk_optim_desc *opt);
+/* One training step on B windows of T columns (host buffers: feats float32 [B][T][F], labels int32 [B][T] in [0, 5),
+ * MDK_ERR_ARG otherwise): forward, loss, backward, then - unless the gradient norm is not finite, which skips the
+ * update as GradScaler.step does - the gradients scaled by max_norm / (norm + 1e-6) when that is below 1
+ * (clip_grad_norm_; max_norm <= 0 means no clipping) and one optimizer step at learning rate lr.  Returns once the
+ * statistics are on the host.  The stored gradient (mdk_trainer_read_grads) is the unclipped one. */
+int mdk_trainer_step(mdk_trainer *tr, const float *feats, const int32_t *labels, int64_t B, int64_t T, float lr,
+                     float max_norm, mdk_train_stats *stats);
+/* forward and loss without a backward pass (validation).  labels may be NULL (no loss); probs / logits (host float32
+ * [B][T][5]) may be NULL. */
+int mdk_trainer_eval(mdk_trainer *tr, const float *feats, const int32_t *labels, int64_t B, int64_t T, float *probs,
+                     float *logits, mdk_train_stats *stats);
+int mdk_trainer_num_params(mdk_trainer *tr, int64_t *n);
+int mdk_trainer_read_params(mdk_trainer *tr, float *out_host, int64_t n);
+int mdk_trainer_read_grads(mdk_trainer *tr, float *out_host, int64_t n);
+/* device bytes a step of B windows x T columns needs (about 28 gru_size floats per position), and the budget above
+ * which a step fails with MDK_ERR_ARG (64 GiB) */
+int mdk_trainer_workspace_bytes(const mdk_model_desc *desc, int64_t B, int64_t T, size_t *bytes, size_t *budget);
+/* device times of the last step in ms (CUDA events): forward (with the feature and label copies), loss and head
+ * backward, BPTT recurrences, gradient reductions (and layer 1's dX), optimizer step (norm, update, weight repack) */
+int mdk_trainer_stage_ms(mdk_trainer *tr, float *ms);
+/* windows per CTA of the BPTT kernel: 1, 2, 4 or 8, or 0 (default) to choose from B (the fewest whose CTAs still fill
+ * no more than one wave).  For measurements. */
+int mdk_trainer_set_bptt_windows(mdk_trainer *tr, int nb);
+
 #ifdef __cplusplus
 }
 #endif

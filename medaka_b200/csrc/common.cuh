@@ -343,8 +343,9 @@ cudaError_t launch_untile_rows(const float *src_tiled, float *dst, int64_t w0, i
                                int width = H2);
 cudaError_t launch_unpack_h0(const void *h0_tiles, float *out, int64_t w0, int64_t nw, int64_t T, cudaStream_t s);
 // gru_fp32.cu
+// save (training): also r, z, n and W_hn.h_{t-1} + b_hn per position, direction and unit (gru_fp32.cu)
 cudaError_t launch_rec_fp32(const float *gi, const float *w_hh_t, const float *b_hn, float *h_out, int64_t B,
-                            int64_t T, cudaStream_t s, int hs = H);
+                            int64_t T, cudaStream_t s, int hs = H, float *save = nullptr);
 // C[M][N] = A[M][K] . W[N][K]^T + bias[N], fp32 (K % 16 == 0, N % 128 == 0)
 cudaError_t launch_gemm_fp32(const float *A, const float *W, const float *bias, float *C, int64_t M, int K, int N,
                              cudaStream_t s);

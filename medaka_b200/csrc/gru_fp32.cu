@@ -17,14 +17,17 @@ __device__ __forceinline__ float sigmoid_acc(float x) { return 1.0f / (1.0f + ex
 // the NB h vectors are shared-memory broadcasts.
 // gi   [B*T][6 HS]  (position p = b*T + t ; columns dir*3HS + gate*HS + j)
 // h_out[B*T][2 HS]  (columns dir*HS + j)
+// SAVE (training, gru_train.cu): also the activations backpropagation through time reads,
+// save[B*T][dir][4][HS] = r, z, n and W_hn.h_{t-1} + b_hn; the inference instantiation compiles as without it.
 // -------------------------------------------------------------------------------------
 constexpr int REC_NB = 8;
 
-template <int HS>
+template <int HS, bool SAVE>
 __global__ void __launch_bounds__(HS, 1) rec_fp32_kernel(const float *__restrict__ gi,
                                                          const float *__restrict__ w_hh_t,
                                                          const float *__restrict__ b_hn,
-                                                         float *__restrict__ h_out, int64_t B, int64_t T) {
+                                                         float *__restrict__ h_out, int64_t B, int64_t T,
+                                                         float *__restrict__ save) {
     constexpr int G3S = 3 * HS, GIS = NDIR * G3S;
     constexpr bool SMEM_W = HS == H;
     extern __shared__ __align__(16) float smem[];
@@ -106,34 +109,42 @@ __global__ void __launch_bounds__(HS, 1) rec_fp32_kernel(const float *__restrict
         for (int n = 0; n < REC_NB; ++n) {
             const float r = sigmoid_acc(gcur[0][n] + acc[0][n]);
             const float z = sigmoid_acc(gcur[1][n] + acc[1][n]);
-            const float nn = tanhf(gcur[2][n] + r * (acc[2][n] + bhn));
+            const float ghn = acc[2][n] + bhn;
+            const float nn = tanhf(gcur[2][n] + r * ghn);
             const float h = (1.0f - z) * nn + z * hprev[n];
             hprev[n] = h;
             hn[n * HS + j] = h;
             if (n < nb) h_out[((b0 + n) * T + t) * (NDIR * HS) + dir * HS + j] = h;
+            if (SAVE && n < nb) {
+                float *sv = save + (((b0 + n) * T + t) * NDIR + dir) * (4 * HS) + j;
+                sv[0] = r; sv[HS] = z; sv[2 * HS] = nn; sv[3 * HS] = ghn;
+            }
         }
         __syncthreads();
         cur ^= 1;
     }
 }
 
-template <int HS>
+template <int HS, bool SAVE>
 static cudaError_t launch_rec_fp32_hs(const float *gi, const float *w_hh_t, const float *b_hn, float *h_out, int64_t B,
-                                      int64_t T, cudaStream_t s) {
+                                      int64_t T, cudaStream_t s, float *save) {
     const size_t smem = (size_t)((HS == H ? HS * 3 * HS : 0) + 2 * REC_NB * HS) * sizeof(float);
     // (the attribute is per device: set it on every launch, a process may drive several GPUs from several threads)
-    cudaError_t e = cudaFuncSetAttribute(rec_fp32_kernel<HS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(rec_fp32_kernel<HS, SAVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     dim3 grid((unsigned)((B + REC_NB - 1) / REC_NB), NDIR);
-    rec_fp32_kernel<HS><<<grid, HS, smem, s>>>(gi, w_hh_t, b_hn, h_out, B, T);
+    rec_fp32_kernel<HS, SAVE><<<grid, HS, smem, s>>>(gi, w_hh_t, b_hn, h_out, B, T, save);
     return cudaGetLastError();
 }
 
 cudaError_t launch_rec_fp32(const float *gi, const float *w_hh_t, const float *b_hn, float *h_out, int64_t B,
-                            int64_t T, cudaStream_t s, int hs) {
+                            int64_t T, cudaStream_t s, int hs, float *save) {
     if (B == 0 || T == 0) return cudaSuccess;
-    return hs == H256 ? launch_rec_fp32_hs<H256>(gi, w_hh_t, b_hn, h_out, B, T, s)
-                      : launch_rec_fp32_hs<H>(gi, w_hh_t, b_hn, h_out, B, T, s);
+    if (save)
+        return hs == H256 ? launch_rec_fp32_hs<H256, true>(gi, w_hh_t, b_hn, h_out, B, T, s, save)
+                          : launch_rec_fp32_hs<H, true>(gi, w_hh_t, b_hn, h_out, B, T, s, save);
+    return hs == H256 ? launch_rec_fp32_hs<H256, false>(gi, w_hh_t, b_hn, h_out, B, T, s, nullptr)
+                      : launch_rec_fp32_hs<H, false>(gi, w_hh_t, b_hn, h_out, B, T, s, nullptr);
 }
 
 // -------------------------------------------------------------------------------------
