@@ -286,6 +286,19 @@ int mdk_read_matrix(int device, int64_t n_rec, const int32_t *pos, const uint16_
                     int8_t *matrix_out, int64_t *major_out, int64_t *minor_out, int64_t *n_cols_out,
                     int32_t *n_reads_out, int32_t *left_read_out, int32_t *right_read_out);
 
+/* ---- training labels: HaploidLabelScheme.encode joined to a sample's columns (medaka/labels.py:422-484,
+ * medaka/features.py:979-992) for one truth alignment.  The truth record in BAM's packed encodings: pos 0-based
+ * reference start, cigar[n_cigar] (len << 4 | op), seq 4-bit codes (two per byte, high nibble first) of l_seq bases,
+ * every one of them A, C, G or T, and the CIGAR's query length equal to l_seq.  [clip_start, clip_end) is the window
+ * the alignment was trimmed to.  labels_out[i] (int64, the dtype the reference stores) is the code ('*ACGT' -> 0..4) of
+ * the truth at (major[i], minor[i]): the base aligned to major[i] (minor 0; 0 on a deletion or skip), or the minor[i]-th
+ * base of the query-only run (I ops, a trailing soft clip) behind major[i]; 0 (the padding vector) where the truth has
+ * no such position or major[i] lies outside the window.  MDK_ERR_ARG for a non-ACGT base or a CIGAR that does not
+ * fit the sequence.  All pointers are HOST pointers. */
+int mdk_truth_labels(int device, int32_t pos, const uint32_t *cigar, int64_t n_cigar, const uint8_t *seq,
+                     int64_t l_seq, int32_t clip_start, int32_t clip_end, int64_t n_cols, const int64_t *major,
+                     const int64_t *minor, int64_t *labels_out);
+
 /* ---- read-level model seam: LatentSpaceLSTM (medaka/architectures/latent_space_lstm.py:34-207, the model class of the
  * `rl_` consensus models) behind TorchModel.predict_on_batch (medaka/models.py:303-313) with
  * ReadLevelFeaturesModel.get_model_input_features = batch.read_level_features (base_classes.py:29-36).

@@ -48,8 +48,9 @@ constexpr uint32_t INS_NOCOUNT = 0x80000000u;   // op_ins flag: the run hangs of
 __device__ __forceinline__ bool read_passes(uint16_t flag, uint8_t mapq, int min_mapq) {
     return !(flag & PLP_FILTER_FLAGS) && (int)mapq >= min_mapq;
 }
-__device__ __forceinline__ bool consumes_ref(int op) { return op == OP_M || op == OP_D || op == OP_N || op == OP_EQ || op == OP_X; }
-__device__ __forceinline__ bool is_match(int op) { return op == OP_M || op == OP_EQ || op == OP_X; }
+__host__ __device__ __forceinline__ bool consumes_ref(int op) { return op == OP_M || op == OP_D || op == OP_N || op == OP_EQ || op == OP_X; }
+__host__ __device__ __forceinline__ bool is_match(int op) { return op == OP_M || op == OP_EQ || op == OP_X; }
+__host__ __device__ __forceinline__ bool consumes_qry(int op) { return is_match(op) || op == OP_I || op == OP_S; }
 
 // State of the insertion-run scan after an op: kind of the last op that is neither I nor P (0 none yet, 1 consumes the
 // reference, 2 reference skip, 3 anything else) and the inserted bases seen since then.  Associative combine: a later
@@ -90,7 +91,7 @@ __global__ void __launch_bounds__(256) plp_walk_kernel(int64_t n_rec, const int3
         const int op = live ? (int)(c & 0xF) : OP_P;     // padding consumes nothing and breaks nothing
         const int32_t len = live ? (int32_t)(c >> 4) : 0;
         int32_t dx = consumes_ref(op) ? len : 0;
-        int32_t dy = (is_match(op) || op == OP_I || op == OP_S) ? len : 0;
+        int32_t dy = consumes_qry(op) ? len : 0;
         RunState st;
         st.kind = (op == OP_I || op == OP_P) ? 0u : (op == OP_N ? 2u : (consumes_ref(op) ? 1u : 3u));
         st.ins = op == OP_I ? (uint32_t)len : 0u;
@@ -393,6 +394,117 @@ __global__ void plp_op_rec_kernel(int64_t n_rec, const int64_t *__restrict__ cig
 __global__ void plp_widen_kernel(int64_t n, const uint32_t *__restrict__ src, uint64_t *__restrict__ dst) {
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (i < n) dst[i] = src[i];
+}
+
+// =====================================================================================
+// Truth labels of a pileup's columns (HaploidLabelScheme.encode joined to the sample positions, medaka/labels.py:422-484
+// and medaka/features.py:979-992) for one truth alignment, without the per-pair dictionary:
+//   1. truth_sum_kernel / launch_scan_blocks / truth_ops_kernel: exclusive scans of the reference bases, query bases and
+//      reference-consuming ops (length > 0) over the CIGAR, the latter compacting those ops into rstart[j] (reference
+//      position of op j's first base) and qstart[j] (query position there), with the end of the alignment as entry
+//      n_ref.  Only I and S consume the query between two reference-consuming ops (H and P yield no pairs), so the
+//      query-only run behind op j - the insertion columns of its last base - is qstart[j] + (match ? len : 0) ..
+//      qstart[j + 1]: a trailing soft clip is the last op's run, a leading one precedes every op and is never looked at.
+//   2. truth_label_kernel: one thread per column binary-searches the op holding its major and reads the base there.
+// Columns outside [clip_start, clip_end), not covered by the alignment, on a deletion or skip, or beyond their position's
+// run get 0, the '*' / padding code.
+// =====================================================================================
+struct TruthSums {
+    int64_t ref, qry, ops;
+};
+
+// a thread's SC_PER_THREAD consecutive ops (past the end: 0, an empty M) and their sums
+__device__ __forceinline__ TruthSums truth_thread_ops(int64_t i0, int64_t n_ops, const uint32_t *__restrict__ cigar,
+                                                      uint32_t (&c)[SC_PER_THREAD]) {
+    TruthSums s{0, 0, 0};
+#pragma unroll
+    for (int j = 0; j < SC_PER_THREAD; ++j) {
+        c[j] = i0 + j < n_ops ? cigar[i0 + j] : 0u;
+        const int op = (int)(c[j] & 0xF);
+        const int64_t len = c[j] >> 4;
+        if (consumes_ref(op)) {
+            s.ref += len;
+            s.ops += len > 0;
+        }
+        if (consumes_qry(op)) s.qry += len;
+    }
+    return s;
+}
+
+// per block of SC_BLOCK ops: blk[0][b], blk[1][b], blk[2][b] = reference bases, query bases, reference-consuming ops
+__global__ void __launch_bounds__(SC_THREADS) truth_sum_kernel(int64_t n_ops, const uint32_t *__restrict__ cigar,
+                                                               int64_t n_blk, int64_t *__restrict__ blk) {
+    uint32_t c[SC_PER_THREAD];
+    const TruthSums s = truth_thread_ops(blockIdx.x * (int64_t)SC_BLOCK + threadIdx.x * SC_PER_THREAD, n_ops, cigar, c);
+    int64_t tr, tq, tn;
+    block_exclusive_scan(s.ref, &tr);
+    block_exclusive_scan(s.qry, &tq);
+    block_exclusive_scan(s.ops, &tn);
+    if (threadIdx.x == 0) {
+        blk[blockIdx.x] = tr;
+        blk[(n_blk + 1) + blockIdx.x] = tq;
+        blk[2 * (n_blk + 1) + blockIdx.x] = tn;
+    }
+}
+
+// after the three block scans: the compacted reference-consuming ops and the end entry
+__global__ void __launch_bounds__(SC_THREADS) truth_ops_kernel(int64_t n_ops, const uint32_t *__restrict__ cigar, int32_t pos,
+                                                               int64_t n_blk, const int64_t *__restrict__ blk,
+                                                               int64_t *__restrict__ rstart, int64_t *__restrict__ qstart,
+                                                               uint8_t *__restrict__ match) {
+    const int64_t *blk_ref = blk, *blk_qry = blk + (n_blk + 1), *blk_ops = blk + 2 * (n_blk + 1);
+    uint32_t c[SC_PER_THREAD];
+    const TruthSums s = truth_thread_ops(blockIdx.x * (int64_t)SC_BLOCK + threadIdx.x * SC_PER_THREAD, n_ops, cigar, c);
+    int64_t r = pos + blk_ref[blockIdx.x] + block_exclusive_scan(s.ref, nullptr);
+    int64_t q = blk_qry[blockIdx.x] + block_exclusive_scan(s.qry, nullptr);
+    int64_t k = blk_ops[blockIdx.x] + block_exclusive_scan(s.ops, nullptr);
+#pragma unroll
+    for (int j = 0; j < SC_PER_THREAD; ++j) {
+        const int op = (int)(c[j] & 0xF);
+        const int64_t len = c[j] >> 4;
+        if (consumes_ref(op) && len > 0) {
+            rstart[k] = r;
+            qstart[k] = q;
+            match[k] = is_match(op) ? 1 : 0;
+            ++k;
+        }
+        if (consumes_ref(op)) r += len;
+        if (consumes_qry(op)) q += len;
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        rstart[blk_ops[n_blk]] = pos + blk_ref[n_blk];
+        qstart[blk_ops[n_blk]] = blk_qry[n_blk];
+    }
+}
+
+__global__ void __launch_bounds__(256) truth_label_kernel(int64_t n_cols, const int64_t *__restrict__ major,
+                                                          const int64_t *__restrict__ minor, const int64_t *__restrict__ n_ref_dev,
+                                                          const int64_t *__restrict__ rstart, const int64_t *__restrict__ qstart,
+                                                          const uint8_t *__restrict__ match, const uint8_t *__restrict__ seq,
+                                                          int32_t clip_start, int32_t clip_end, int64_t *__restrict__ labels) {
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (i >= n_cols) return;
+    const int64_t M = major[i], m = minor[i], n_ref = *n_ref_dev;
+    int64_t label = 0;
+    if (M >= clip_start && M < clip_end) {
+        int64_t lo = 0, hi = n_ref;                     // first op starting behind M
+        while (lo < hi) {
+            const int64_t mid = (lo + hi) >> 1;
+            if (rstart[mid] <= M) lo = mid + 1; else hi = mid;
+        }
+        const int64_t j = lo - 1;
+        if (j >= 0 && M < rstart[j + 1]) {
+            int64_t q = -1;
+            if (m == 0) {
+                if (match[j]) q = qstart[j] + (M - rstart[j]);
+            } else if (m > 0 && M == rstart[j + 1] - 1) {
+                const int64_t run = qstart[j] + (match[j] ? rstart[j + 1] - rstart[j] : 0);
+                if (m <= qstart[j + 1] - run) q = run + m - 1;
+            }
+            if (q >= 0) label = c_num2countbase[seq_code(seq, 0, (int32_t)q)] - 3;     // forward A C G T -> 4..7 -> 1..4
+        }
+    }
+    labels[i] = label;
 }
 
 // =====================================================================================
@@ -1232,6 +1344,57 @@ int mdk_read_matrix(int device, int64_t n_rec, const int32_t *pos, const uint16_
         memcpy(right_read_out, right_ids.data(), (size_t)n_reads * 4);
     }
     return MDK_OK;
+}
+
+int mdk_truth_labels(int device, int32_t pos, const uint32_t *cigar, int64_t n_cigar, const uint8_t *seq, int64_t l_seq,
+                     int32_t clip_start, int32_t clip_end, int64_t n_cols, const int64_t *major, const int64_t *minor,
+                     int64_t *labels_out) {
+    MDK_REQUIRE(n_cigar >= 0 && l_seq >= 0 && n_cols >= 0, MDK_ERR_ARG, "truth_labels: bad sizes");
+    if (n_cols == 0) return MDK_OK;
+    MDK_REQUIRE(major && minor && labels_out, MDK_ERR_ARG, "truth_labels: NULL column array");
+    MDK_REQUIRE((cigar || n_cigar == 0) && (seq || l_seq == 0), MDK_ERR_ARG, "truth_labels: NULL record array");
+    // the kernels read the bases the CIGAR names: its query length must be the sequence's, and every base a label
+    int64_t qlen = 0;
+    for (int64_t k = 0; k < n_cigar; ++k)
+        if (consumes_qry((int)(cigar[k] & 0xF))) qlen += cigar[k] >> 4;
+    MDK_REQUIRE(qlen == l_seq, MDK_ERR_ARG, "truth_labels: CIGAR query length differs from l_seq");
+    for (int64_t q = 0; q < l_seq; ++q) {
+        const int code = (q & 1) ? (seq[q >> 1] & 0xF) : (seq[q >> 1] >> 4);
+        MDK_REQUIRE(code == 1 || code == 2 || code == 4 || code == 8, MDK_ERR_ARG,
+                    "truth_labels: truth sequence has a base other than A, C, G, T");
+    }
+    if (n_cigar == 0) {
+        memset(labels_out, 0, (size_t)n_cols * sizeof(int64_t));
+        return MDK_OK;
+    }
+    MDK_CUDA(cudaSetDevice(device));
+    const int64_t n_blk = (n_cigar + SC_BLOCK - 1) / SC_BLOCK;
+    Staging st(Blob::STAGING, "truth_labels");
+    const uint32_t *d_cigar;
+    const uint8_t *d_seq;
+    const int64_t *d_major, *d_minor;
+    int64_t *d_labels, *d_blk, *d_rstart, *d_qstart;
+    uint8_t *d_match;
+    st.in(&d_cigar, cigar, n_cigar);
+    st.in(&d_seq, seq, (l_seq + 1) / 2);
+    st.in(&d_major, major, n_cols);
+    st.in(&d_minor, minor, n_cols);
+    st.take(&d_labels, n_cols);
+    st.take(&d_blk, 3 * (n_blk + 1));
+    st.take(&d_rstart, n_cigar + 1);
+    st.take(&d_qstart, n_cigar + 1);
+    st.take(&d_match, n_cigar);
+    if (!st.alloc()) return st.result();
+    truth_sum_kernel<<<(unsigned)n_blk, SC_THREADS, 0, 0>>>(n_cigar, d_cigar, n_blk, d_blk);
+    for (int k = 0; k < 3; ++k) st.check(launch_scan_blocks(d_blk + k * (n_blk + 1), n_blk, 0));
+    truth_ops_kernel<<<(unsigned)n_blk, SC_THREADS, 0, 0>>>(n_cigar, d_cigar, pos, n_blk, d_blk, d_rstart, d_qstart,
+                                                            d_match);
+    truth_label_kernel<<<(unsigned)((n_cols + 255) / 256), 256, 0, 0>>>(
+        n_cols, d_major, d_minor, d_blk + 3 * (n_blk + 1) - 1, d_rstart, d_qstart, d_match, d_seq, clip_start, clip_end,
+        d_labels);
+    st.check(cudaGetLastError());
+    st.out(labels_out, d_labels, n_cols);
+    return st.result();
 }
 
 }  // extern "C"

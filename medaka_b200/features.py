@@ -8,6 +8,9 @@ by src/medaka_counts.c; here it is pluggable (``pileup_source``) because no BAM 
 part of the reference tree; ``pileup_counts`` below is the GPU replacement (BAM inflate/parse on the
 host in medaka_b200/bam.py, per-base counting in csrc/pileup.cu), and a custom ``pileup_source`` can
 still be plugged in (the benchmark's synthetic source does).
+
+The training half (``bams_to_training_samples`` :937-994, the truth arguments of ``SampleGenerator``,
+``create_samples`` :1316-1414) labels the samples of both encoders from truth alignments (medaka_b200/labels.py).
 """
 import inspect
 from collections import defaultdict
@@ -288,6 +291,34 @@ class CountsFeatureEncoder(object):
             samples.append(self._post_process_pileup(counts, positions, region))
         return samples
 
+    def bams_to_training_samples(self, truth_bam, bam, region, label_scheme, truth_haplotag=None, min_length=1000):
+        """Labelled samples of a region (medaka/features.py:937-994): per filtered truth alignment, the samples of the
+        reads over its trimmed span, each column labelled from the truth on the GPU (0, the padding vector, where the
+        truth has no position; truth positions without a column are dropped).
+
+        :param truth_bam: BAM (path or ``bam.BamFile``) of the truth aligned to the draft.
+        :param bam: BAM of the reads.  :param label_scheme: a ``labels.HaploidLabelScheme``.
+        :param truth_haplotag: tag grouping the truth alignments by haplotype.
+        :param min_length: shortest truth alignment kept.
+        :returns: tuple of ``common.Sample`` with int64 labels.
+        """
+        from medaka_b200 import labels
+        if not isinstance(label_scheme, labels.HaploidLabelScheme):
+            raise NotImplementedError("training labels are implemented for the HaploidLabelScheme only")
+        alns = labels.TruthAlignment.bam_to_alignments(truth_bam, region, haplotag=truth_haplotag,
+                                                       min_length=min_length)
+        if len(alns) == 0:
+            self.logger.info("Filtering and grouping removed all alignments of truth to ref from {}.".format(region))
+        for aln in alns:
+            if len(aln) != label_scheme.n_elements:
+                raise ValueError('{} alignments were passed to {}, requires {}'.format(
+                    len(aln), type(label_scheme).__name__, label_scheme.n_elements))
+        samples = []
+        for aln in alns:
+            for sample in self.bam_to_sample(bam, common.Region(region.ref_name, aln[0].start, aln[0].end)):
+                samples.append(sample.amend(labels=label_scheme.label_columns(aln, sample.positions)))
+        return tuple(samples)
+
 
 # ---------------------------------------------------------------------------------------------------------
 # Read-level features (medaka/features.py:258-560, 1100-1205): one int8 vector per (pileup column, read row).
@@ -516,10 +547,12 @@ class ReadAlignmentFeatureEncoder(CountsFeatureEncoder):
 
 
 class SampleGenerator(object):
-    """Chunked inference samples for one region (medaka/features.py:1208-1313, inference half)."""
+    """Chunked inference or training samples for one region (medaka/features.py:1208-1313).  With ``truth_bam`` the
+    samples are labelled (``bams_to_training_samples`` of the encoder with ``label_scheme``, ``truth_haplotag`` and
+    ``min_truth_length``)."""
 
     def __init__(self, bam, region, feature_encoder, chunk_len=1000, chunk_overlap=200,
-                 enable_chunking=True):
+                 enable_chunking=True, truth_bam=None, label_scheme=None, truth_haplotag=None, min_truth_length=1000):
         self.logger = common.get_named_logger("Sampler")
         self.fencoder = feature_encoder
         self.bam = bam
@@ -527,13 +560,24 @@ class SampleGenerator(object):
         self.chunk_len = chunk_len
         self.chunk_overlap = chunk_overlap
         self.enable_chunking = enable_chunking
+        self.truth_bam = truth_bam
+        self.label_scheme = label_scheme
+        self.truth_haplotag = truth_haplotag
+        self.min_truth_length = min_truth_length
         self._source = None
         self._quarantined = list()     # (Region, pileup width) of sources narrower than chunk_len
+        if self.truth_bam is not None and self.label_scheme is None:
+            raise ValueError("A `LabelScheme` must be given to create training data.")
 
     def _fill_features(self):
         if self._source is None:
             t0 = now()
-            self._source = self.fencoder.bam_to_sample(self.bam, self.region)
+            if self.truth_bam is not None:
+                self._source = self.fencoder.bams_to_training_samples(
+                    self.truth_bam, self.bam, self.region, self.label_scheme, truth_haplotag=self.truth_haplotag,
+                    min_length=self.min_truth_length)
+            else:
+                self._source = self.fencoder.bam_to_sample(self.bam, self.region)
             self.logger.debug("Took {:.2f}s to make features.".format(now() - t0))
 
     @property
@@ -554,3 +598,78 @@ class SampleGenerator(object):
                 continue
             out.extend(source.chunks(chunk_len=self.chunk_len, overlap=self.chunk_overlap))
         return out
+
+
+def _bam_regions(bam, regions=None):
+    """The regions to process, with integer bounds clipped to the contigs (medaka/common.py:762-790): every contig of
+    the BAM, or the given ``Region``s / region strings.  KeyError for a contig the BAM does not have."""
+    from medaka_b200 import bam as mbam
+    bf = bam if isinstance(bam, mbam.BamFile) else mbam.BamFile(bam)
+    lengths = dict(bf.get_regions())
+    if regions is None:
+        return [common.Region(name, 0, length) for name, length in lengths.items()]
+    out = []
+    for r in regions:
+        r = common.Region.from_string(r) if isinstance(r, str) else r
+        if r.ref_name not in lengths:
+            raise KeyError('Contig {} is not one of the bam references.'.format(r.ref_name))
+        start = max(0, r.start) if r.start is not None else 0
+        end = min(r.end, lengths[r.ref_name]) if r.end is not None else lengths[r.ref_name]
+        out.append(common.Region(r.ref_name, start, end))
+    return out
+
+
+MAX_REGION_SIZE = 1000000     # regions are processed in pieces of this size (medaka/features.py:1390)
+
+
+def create_samples(bam, output, regions=None, truth=None, truth_haplotag=None, feature_encoder=None,
+                   label_scheme='HaploidLabelScheme', chunk_len=10000, chunk_ovlp=1000, min_region_size=0):
+    """`medaka features`: chunked samples of the regions, labelled from the truth alignments in ``truth`` when it is
+    given, written to a ``DataStore`` with ``feature_encoder`` and ``label_scheme`` meta (medaka/features.py:1316-1414).
+
+    :param bam: BAM of the reads.  :param output: the store to write (deleted again when no sample is written).
+    :param regions: ``Region``s or region strings (default: every contig of ``bam``); each is processed in 1 Mb
+        pieces (``Region.split``, whose last piece overlaps the one before; a sample already written is not written
+        again).  Regions shorter than ``min_region_size`` are skipped.
+    :param truth: BAM of the truth aligned to the draft, or None for unlabelled samples.
+    :param feature_encoder: a ``CountsFeatureEncoder`` or ``ReadAlignmentFeatureEncoder`` (default: counts, total
+        normalisation).  :param label_scheme: a ``labels.HaploidLabelScheme`` or its class name.
+    :param chunk_len, chunk_ovlp: sample length and overlap; sources shorter than ``chunk_len`` are not written.
+    :returns: the number of samples in the store.
+    """
+    import os
+    import shutil
+    from medaka_b200 import datastore, labels
+    logger = common.get_named_logger('Prepare')
+    if chunk_ovlp >= chunk_len:
+        raise ValueError('chunk_ovlp {} is not smaller than chunk_len {}'.format(chunk_ovlp, chunk_len))
+    if isinstance(label_scheme, str):
+        label_scheme = labels.from_name(label_scheme)
+    if feature_encoder is None:
+        feature_encoder = CountsFeatureEncoder()
+    pieces = []
+    for r in _bam_regions(bam, regions):
+        if r.size < min_region_size:
+            logger.warning("Region {} is smaller than min region size {}, skipping.".format(r, min_region_size))
+            continue
+        pieces.extend(r.split(MAX_REGION_SIZE))
+    if truth is None:
+        logger.warning('Running medaka features without a truth bam, unlabelled data will be produced.')
+    with datastore.DataStore(output, 'w') as ds:
+        ds.set_meta(feature_encoder, 'feature_encoder')
+        ds.set_meta(label_scheme, 'label_scheme')
+        for reg in pieces:
+            samples = SampleGenerator(bam, reg, feature_encoder, chunk_len=chunk_len, chunk_overlap=chunk_ovlp,
+                                      truth_bam=truth, label_scheme=label_scheme,
+                                      truth_haplotag=truth_haplotag).samples
+            logger.info("Writing {} samples for region {}".format(len(samples), reg))
+            for sample in samples:
+                ds.write_sample(sample)
+        n_samples = ds.n_samples
+    if n_samples == 0:
+        logger.critical("Warning: No training data was written to file, deleting output.")
+        if os.path.isdir(output):
+            shutil.rmtree(output)
+        elif os.path.exists(output):
+            os.remove(output)
+    return n_samples

@@ -1,11 +1,20 @@
-"""Decode seam: per-position label decode on the GPU.
+"""Decode seam: per-position label decode on the GPU; and the training-label half: truth alignments and their labels.
 
 Mirrors ``HaploidLabelScheme.decode_consensus`` (medaka/labels.py:1053-1085) and ``_phred``
 (:387-401).  The array work - argmax (first maximum wins), probability of the chosen class,
 ``uint8(min(70, -10*log10(clip(1-p, 1e-7, 1)))) + 33`` - runs in libmedaka_b200
 (mdk_decode_consensus); gap removal and string building, which are O(n) byte shuffles on
 the result, stay on the host.
+
+Training labels (medaka/labels.py:27-266, :422-567, :703-771): ``TruthAlignment`` selects and trims the truth
+alignments of a region (host bookkeeping over a handful of records); the label of every pileup column - the reference's
+per-pair dictionary joined to the sample positions - comes from the GPU (mdk_truth_labels).
 """
+import collections
+import copy
+import itertools
+import re
+
 import numpy as np
 
 from medaka_b200 import libmedaka as _lm
@@ -186,8 +195,225 @@ def decode_variant_segments(seg_calls, seg_pred_q, seg_ref_q, seg_rows, sample_s
                 run_col_ref_q=crq[:c] if want_quals else None, ref_q=ref_q)
 
 
+# ---------------------------------------------------------------------------------------------------------
+# Truth alignments
+_OP_REF = np.array([c in "MDN=X" for c in "MIDNSHP=X"] + [False] * 7)     # by BAM op code
+_OP_QRY = np.array([c in "MIS=X" for c in "MIDNSHP=X"] + [False] * 7)
+_OP_MATCH = np.array([c in "M=X" for c in "MIDNSHP=X"] + [False] * 7)
+_OP_D = 2
+_NT16 = np.frombuffer(b"=ACMGRSVTWYHKDBN", dtype=np.uint8)
+_NT16_LABEL = np.full(16, -1, dtype=np.int64)          # 4-bit base -> '*ACGT' code
+_NT16_LABEL[[1, 2, 4, 8]] = [1, 2, 3, 4]
+_MD_TOKEN = re.compile(r"(\d+)|(\^[A-Za-z]+)|([A-Za-z])")
+TRUTH_EXCLUDE_FLAGS = 0x4 | 0x100          # UNMAP | SECONDARY: supplementary truth alignments are kept
+
+
+class TruthRecord(object):
+    """One truth alignment in BAM's packed encodings (CIGAR ops, 4-bit sequence) with the ``pysam.AlignedSegment``
+    properties the truth filters read."""
+
+    def __init__(self, reference_name, pos, cigar, seq, l_seq, tags=None, flag=0, query_name=None):
+        self.reference_name = reference_name
+        self.reference_start = int(pos)
+        self.cigar = np.ascontiguousarray(cigar, dtype=np.uint32)
+        self.seq = np.ascontiguousarray(seq, dtype=np.uint8)
+        self.l_seq = int(l_seq)
+        self.tags = dict(tags or {})
+        self.flag = int(flag)
+        self.query_name = query_name
+        ops, lens = self.cigar & 0xF, (self.cigar >> 4).astype(np.int64)
+        self.reference_length = int(lens[_OP_REF[ops]].sum())
+        self.reference_end = self.reference_start + self.reference_length
+
+    @classmethod
+    def from_batch(cls, batch, reference_name):
+        """Records of a ``RecordBatch`` fetched with tags and names."""
+        return [cls(reference_name, batch.pos[i], batch.cigar[batch.cigar_off[i]:batch.cigar_off[i + 1]],
+                    batch.seq[batch.seq_off[i]:batch.seq_off[i + 1]], batch.l_seq[i],
+                    batch.tags[i] if batch.tags is not None else None, batch.flag[i],
+                    batch.names[i] if batch.names is not None else None) for i in range(len(batch.pos))]
+
+    def _nibbles(self):
+        nib = np.empty(2 * len(self.seq), dtype=np.uint8)
+        nib[0::2], nib[1::2] = self.seq >> 4, self.seq & 0xF
+        return nib[:self.l_seq]
+
+    @property
+    def query_sequence(self):
+        return _NT16[self._nibbles()].tobytes().decode()
+
+    def aligned_pairs(self):
+        """(query position, reference position) of every pair ``get_aligned_pairs`` yields, -1 for None: M, = and X
+        give both, I and S the query position, D and N the reference position, H and P nothing."""
+        ops, lens = self.cigar & 0xF, (self.cigar >> 4).astype(np.int64)
+        r0 = self.reference_start + np.concatenate([[0], np.cumsum(np.where(_OP_REF[ops], lens, 0))[:-1]])
+        q0 = np.concatenate([[0], np.cumsum(np.where(_OP_QRY[ops], lens, 0))[:-1]])
+        n = np.where(_OP_REF[ops] | _OP_QRY[ops], lens, 0)
+        op_of = np.repeat(np.arange(len(ops)), n)
+        k = np.arange(int(n.sum())) - np.repeat(np.cumsum(n) - n, n)
+        qpos = np.where(_OP_QRY[ops][op_of], q0[op_of] + k, -1)
+        rpos = np.where(_OP_REF[ops][op_of], r0[op_of] + k, -1)
+        return qpos, rpos
+
+    def get_reference_sequence(self):
+        """The reference under the alignment, rebuilt from the query and the MD tag like pysam's (upper case; skipped
+        reference has no bases in MD and none here).  ValueError when MD is absent or does not fit the CIGAR."""
+        md = self.tags.get("MD")
+        if md is None:
+            raise ValueError("MD tag not present")
+        ops, lens = self.cigar & 0xF, (self.cigar >> 4).astype(np.int64)
+        qpos, rpos = self.aligned_pairs()
+        op_of = np.repeat(np.arange(len(ops)), np.where(_OP_REF[ops] | _OP_QRY[ops], lens, 0))
+        aligned = (rpos >= 0) & (ops[op_of] != 3)               # M, =, X and D: the positions MD describes
+        is_del = ops[op_of][aligned] == _OP_D
+        ref = _NT16[self._nibbles()][np.where(is_del, 0, qpos[aligned])]
+        ref[is_del] = ord("-")
+        at = 0
+        for num, dele, mism in _MD_TOKEN.findall(md):
+            if num:
+                at += int(num)
+            else:
+                bases = (dele[1:] if dele else mism).upper().encode()
+                if at + len(bases) > len(ref) or bool(is_del[at:at + len(bases)].all()) != bool(dele):
+                    raise ValueError("MD tag {} does not fit the CIGAR of {}".format(md, self.query_name))
+                ref[at:at + len(bases)] = np.frombuffer(bases, dtype=np.uint8)
+                at += len(bases)
+        if at != len(ref):
+            raise ValueError("MD tag {} does not fit the CIGAR of {}".format(md, self.query_name))
+        return ref.tobytes().decode()
+
+
+class TruthAlignment(object):
+    """A truth alignment and the window [start, end) of it that is used (medaka/labels.py:27-266)."""
+
+    def __init__(self, alignment):
+        self.aln = alignment
+        self.start = alignment.reference_start
+        self.end = alignment.reference_end
+        self.is_kept = True
+
+    def _valid_symbols(self):
+        """Neither the query nor the reference under it has a symbol other than A, C, G, T."""
+        acgt = set("ACGT")
+        return set(self.aln.get_reference_sequence().upper()) <= acgt and set(self.aln.query_sequence.upper()) <= acgt
+
+    @staticmethod
+    def _filter_alignments(alignments, region, min_length=1000, length_ratio=2.0, overlap_fraction=0.5):
+        """The alignments suitable for training, trimmed to the region and sorted by start.
+
+        Alignments with an ambiguous symbol go first.  Then every overlapping pair (over the untrimmed alignment
+        spans) is resolved: of similar lengths (ratio < length_ratio), a large overlap (>= overlap_fraction of the
+        shorter) drops both and a small one trims both to abut; otherwise a large overlap drops the shorter and a small
+        one moves the start of the later one behind the overlap.  Last the region trim and ``min_length``.
+        """
+        kept = [copy.copy(a) for a in alignments if a._valid_symbols()]
+        for a, b in itertools.combinations(kept, 2):
+            first, second = sorted((a, b), key=lambda t: t.aln.reference_start)
+            ovl_start, ovl_end = second.aln.reference_start, first.aln.reference_end
+            if ovl_end <= ovl_start:
+                continue
+            shorter, longer = sorted((a, b), key=lambda t: t.aln.reference_length)
+            large = (ovl_end - ovl_start) / shorter.aln.reference_length >= overlap_fraction
+            if longer.aln.reference_length / shorter.aln.reference_length < length_ratio:
+                if large:
+                    a.is_kept = b.is_kept = False
+                else:
+                    first.end, second.start = ovl_start, ovl_end
+            elif large:
+                shorter.is_kept = False
+            else:
+                second.start = ovl_end
+        for al in kept:
+            if region.start is not None:
+                al.start = max(region.start, al.start)
+            if region.end is not None:
+                al.end = min(region.end, al.end)
+        kept = [al for al in kept if al.is_kept and al.end - al.start >= min_length]
+        kept.sort(key=lambda t: t.start)
+        return kept
+
+    @staticmethod
+    def _load_alignments(truth_bam, region, haplotag=None):
+        """{haplotype: [TruthAlignment]} of the mapped, primary or supplementary truth records overlapping the region,
+        sorted by start.  A record without the ``haplotag`` tag raises KeyError."""
+        from medaka_b200 import bam as mbam
+        bf = truth_bam if isinstance(truth_bam, mbam.BamFile) else mbam.BamFile(truth_bam)
+        batch = bf.fetch(region.ref_name, region.start, region.end, exclude_flags=TRUTH_EXCLUDE_FLAGS, min_mapq=0,
+                         with_tags=True, with_names=True)
+        alignments = collections.defaultdict(list)
+        for rec in TruthRecord.from_batch(batch, region.ref_name):
+            alignments[rec.tags[haplotag] if haplotag is not None else None].append(TruthAlignment(rec))
+        for algns in alignments.values():
+            algns.sort(key=lambda t: t.start)
+        return alignments
+
+    @staticmethod
+    def bam_to_alignments(truth_bam, region, haplotag=None, min_length=1000):
+        """Filtered truth alignments of a region, as tuples of one ``TruthAlignment`` per haplotype trimmed to a
+        common window."""
+        algns = TruthAlignment._load_alignments(truth_bam, region, haplotag)
+        algns = {h: TruthAlignment._filter_alignments(a, region=region, min_length=min_length)
+                 for h, a in algns.items()}
+        if not algns:
+            return []
+        return TruthAlignment._group_and_trim_by_haplotype(algns)
+
+    @staticmethod
+    def _group_and_trim_by_haplotype(alignments):
+        """{haplotype: [TruthAlignment]} -> tuples, one alignment per haplotype (in sorted haplotype order), trimmed to
+        their common window.  Each alignment of the first haplotype is taken in turn; in every other haplotype the
+        alignment overlapping the window built so far the most (the first of equals) joins it; an alignment that finds
+        no partner in some haplotype is skipped."""
+        haplotypes = sorted(alignments.keys())
+        if len(haplotypes) == 1:
+            return [(a,) for a in alignments[haplotypes[0]]]
+        grouped = []
+        for a in alignments[haplotypes[0]]:
+            group, lo, hi = [a], a.start, a.end
+            for h in haplotypes[1:]:
+                cands = [o for o in alignments[h] if o.start < o.end and o.start < hi and o.end > lo]
+                if not cands:
+                    break
+                best = max(cands, key=lambda o: min(hi, o.end) - max(lo, o.start))
+                lo, hi = max(lo, best.start), min(hi, best.end)
+                group.append(best)
+            if len(group) != len(haplotypes):
+                continue
+            for al in group:
+                al.start, al.end = lo, hi
+            grouped.append(tuple(group))
+        return grouped
+
+
+def truth_labels(truth, positions, device=0):
+    """Label codes (int64, '*ACGT' -> 0..4, 0 where the truth has no such position) of the pileup columns at
+    ``positions`` from one ``TruthAlignment``, on the GPU (mdk_truth_labels)."""
+    lib, ffi = _lm.load(), _lm.ffi
+    rec = truth.aln
+    major = np.ascontiguousarray(positions['major'], dtype=np.int64)
+    minor = np.ascontiguousarray(positions['minor'], dtype=np.int64)
+    out = np.empty(len(major), dtype=np.int64)
+
+    def ptr(ctype, a):
+        return ffi.cast(ctype, ffi.from_buffer(a)) if a.size else ffi.NULL
+    _lm.check(lib.mdk_truth_labels(
+        device, rec.reference_start, ptr("const uint32_t *", rec.cigar), len(rec.cigar), ptr("const uint8_t *", rec.seq),
+        rec.l_seq, int(truth.start), int(truth.end), len(major), ptr("const int64_t *", major),
+        ptr("const int64_t *", minor), ptr("int64_t *", out)))
+    return out
+
+
+def from_name(name):
+    """A label scheme by its class name; the diploid and run-length schemes are not implemented."""
+    if name == 'HaploidLabelScheme':
+        return HaploidLabelScheme()
+    if name in ('DiploidLabelScheme', 'DiploidZygosityLabelScheme', 'RLELabelScheme'):
+        raise NotImplementedError("label scheme {} is not implemented".format(name))
+    raise ValueError("unknown label scheme {}".format(name))
+
+
 class HaploidLabelScheme(object):
-    """The decode half of the reference's HaploidLabelScheme (labels.py:703-1085)."""
+    """The reference's HaploidLabelScheme (labels.py:703-1085): decoding, and the encoding of haploid truth labels."""
 
     symbols = '*ACGT'     # labels.py:342
     n_elements = 1
@@ -322,6 +548,60 @@ class HaploidLabelScheme(object):
     @property
     def num_classes(self):
         return len(self.symbols)
+
+    # ---- encoding (labels.py:422-567, :730-756)
+    @property
+    def _encoding(self):
+        """label tuple -> integer: ('*',) 0, ('A',) 1, ('C',) 2, ('G',) 3, ('T',) 4."""
+        return {(s,): i for i, s in enumerate(self.symbols)}
+
+    def _labels_to_encoded_labels(self, labels):
+        enc = self._encoding
+        return np.fromiter((enc[x] for x in labels), dtype=np.int64, count=len(labels))
+
+    @property
+    def padding_vector(self):
+        """The code of a column the truth has no base for: the gap's."""
+        return self._labels_to_encoded_labels([('*',)])[0]
+
+    def _check_truth(self, truth_alns):
+        if len(truth_alns) != self.n_elements:
+            raise ValueError('{} alignments were passed to {}, requires {}'.format(
+                len(truth_alns), type(self).__name__, self.n_elements))
+
+    def encode(self, truth_alns):
+        """Truth positions (structured major / minor) and their codes (int64) of a 1-tuple of ``TruthAlignment``.
+
+        The alignment's pairs are taken from the first one on a reference position >= start up to the first one on a
+        position >= end: a reference position gets (pos, 0) and the base or '*', each query-only pair behind it (pos,
+        k) for the k-th of its run - so a trailing soft clip becomes insertions, a leading one is dropped.
+        """
+        self._check_truth(truth_alns)
+        aln = truth_alns[0]
+        qpos, rpos = aln.aln.aligned_pairs()
+        inside = rpos >= aln.start
+        first = int(np.argmax(inside)) if inside.any() else len(rpos)
+        beyond = rpos >= aln.end
+        beyond[:first] = False
+        stop = int(np.argmax(beyond)) if beyond.any() else len(rpos)
+        qpos, rpos = qpos[first:stop], rpos[first:stop]
+        idx = np.arange(len(rpos))
+        last_ref = np.maximum.accumulate(np.where(rpos >= 0, idx, 0))
+        positions = np.empty(len(rpos), dtype=[('major', '<i8'), ('minor', '<i8')])
+        positions['major'] = rpos[last_ref]
+        positions['minor'] = idx - last_ref
+        codes = np.zeros(len(rpos), dtype=np.int64)
+        has_q = qpos >= 0
+        codes[has_q] = _NT16_LABEL[aln.aln._nibbles()[qpos[has_q]]]
+        if np.any(codes < 0):
+            raise KeyError("truth base outside 'ACGT' in {}".format(aln.aln.query_name))
+        return positions, codes
+
+    def label_columns(self, truth_alns, positions):
+        """Labels of a sample's columns from a 1-tuple of ``TruthAlignment``: ``encode`` joined to the sample's
+        positions, the padding vector where the truth has no position, computed on the GPU (mdk_truth_labels)."""
+        self._check_truth(truth_alns)
+        return truth_labels(truth_alns[0], positions, self.device)
 
     @staticmethod
     def _phred(err, cap=70.0):
