@@ -605,6 +605,44 @@ int mdk_trainer_stage_ms(mdk_trainer *tr, float *ms);
  * no more than one wave).  For measurements. */
 int mdk_trainer_set_bptt_windows(mdk_trainer *tr, int nb);
 
+/* ---- read-level training: medaka train for the LatentSpaceLSTM the read-level engine accepts (bidirectional, mean
+ * pooling, kernel sizes 1 and 17, cnn_size 128, lstm_size 128 or 384, 5 classes, with or without dwells), fp32.  The
+ * model is in training mode: both BatchNorm layers normalise with the batch's statistics over all B*D*P elements of the
+ * padded batch (empty and padding reads included) and update their running statistics (momentum 0.1, unbiased
+ * variance) at every step, a skipped one included.  Per-read activations live only in a bounded scratch: device
+ * memory grows with B*P and the int8 features, not with the read depth.
+ * Weights: the flat array of mdk_rl_trainer_read_params is named_parameters() in order (read_level_conv.
+ * expansion_layer included: the forward never uses it, so it gets no gradient and no update).  The BatchNorm running
+ * statistics and num_batches_tracked are kept apart (mdk_rl_trainer_read_buffers). */
+typedef struct mdk_rl_trainer mdk_rl_trainer;
+
+int mdk_rl_trainer_create(int device, int32_t lstm_size, int32_t cnn_size, int32_t use_dwells, int32_t num_classes,
+                          mdk_rl_trainer **out);
+int mdk_rl_trainer_destroy(mdk_rl_trainer *tr);
+/* one tensor by its torch state-dict name (parameters and buffers; num_batches_tracked as one float); resets the
+ * optimizer state, and the tensors it does not name keep their current values */
+int mdk_rl_trainer_load(mdk_rl_trainer *tr, const char *name, const float *data, int64_t n);
+int mdk_rl_trainer_set_optimizer(mdk_rl_trainer *tr, const mdk_optim_desc *opt);
+/* One training step on x int8 [B][P][D][F] (strand + 1 clamped to [0, 2], as the engine reads it) and labels int32
+ * [B][P] in [0, 5): as mdk_trainer_step.  F is 5 with dwells, 4 or more without (MDK_ERR_ARG otherwise). */
+int mdk_rl_trainer_step(mdk_rl_trainer *tr, const int8_t *x, const int32_t *labels, int64_t B, int64_t P, int64_t D,
+                        int64_t F, float lr, float max_norm, mdk_train_stats *stats);
+/* validation (model.eval()): the running statistics, the read-level engine's fp32 kernels (probabilities equal the
+ * engine's fp32 path bit for bit); labels, probs, logits may be NULL */
+int mdk_rl_trainer_eval(mdk_rl_trainer *tr, const int8_t *x, const int32_t *labels, int64_t B, int64_t P, int64_t D,
+                        int64_t F, float *probs, float *logits, mdk_train_stats *stats);
+int mdk_rl_trainer_num_params(mdk_rl_trainer *tr, int64_t *n);
+int mdk_rl_trainer_read_params(mdk_rl_trainer *tr, float *out_host, int64_t n);
+/* out: running_mean, running_var of convs.2, then of convs.5 (n = 4 cnn_size); num_batches_tracked[2] may be NULL */
+int mdk_rl_trainer_read_buffers(mdk_rl_trainer *tr, float *out_host, int64_t n, int64_t *num_batches_tracked);
+int mdk_rl_trainer_read_grads(mdk_rl_trainer *tr, float *out_host, int64_t n);
+/* device bytes a step on B x P x D x F needs, and the budget above which a step fails with MDK_ERR_ARG (64 GiB) */
+int mdk_rl_trainer_workspace_bytes(int32_t lstm_size, int64_t B, int64_t P, int64_t D, int64_t F, size_t *bytes,
+                                   size_t *budget);
+/* device times of the last step in ms: stats pass, forward pass (with the copies), LSTM forward, loss and head
+ * backward, BPTT, read backward pass, reductions, optimizer step */
+int mdk_rl_trainer_stage_ms(mdk_rl_trainer *tr, float *ms);
+
 #ifdef __cplusplus
 }
 #endif

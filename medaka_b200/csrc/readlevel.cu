@@ -34,14 +34,10 @@
 #include "phred.cuh"
 #include "ptx.cuh"
 #include "rec_common.cuh"
+#include "rl_common.cuh"
 
 namespace mdk {
 
-constexpr int RL_C = 128;        // cnn_size
-constexpr int RL_H = 128;        // lstm_size
-constexpr int RL_EMB = 6;        // bases_embedding_size
-constexpr int RL_TAPS = 17;
-constexpr int RL_PAD = 8;
 constexpr int RL_G4 = 4 * RL_H;
 
 __device__ __forceinline__ float rl_sigmoid(float x) { return 1.0f / (1.0f + expf(-x)); }
@@ -69,14 +65,6 @@ __global__ void __launch_bounds__(256) rl_mask_kernel(const int8_t *__restrict__
 }
 
 // ---------------------------------------------------------------------------------------------- embedding + conv k=1
-struct RlConv1 {
-    const float *emb_base;      // [6][6]
-    const float *emb_strand;    // [3][6]
-    const float *w;             // [C][in]   in = 7 (+1 dwell)
-    const float *b;             // [C]
-    const float *bn_mean, *bn_invstd, *bn_w, *bn_b;   // [C]
-};
-
 __global__ void __launch_bounds__(RL_C) rl_embed_conv1_kernel(const int8_t *__restrict__ x, const uint8_t *__restrict__ mask,
                                                               RlConv1 a, int64_t P, int D, int F, int use_dwells,
                                                               float *__restrict__ y1) {
@@ -114,11 +102,6 @@ __global__ void __launch_bounds__(RL_C) rl_embed_conv1_kernel(const int8_t *__re
 }
 
 // ---------------------------------------------------------------------------------------------- conv k=17 + pooling
-struct RlConv17 {
-    const float *w_t;           // [17][C in][C out]  (transposed from torch's [out][in][tap])
-    const float *b;             // [C]
-    const float *bn_mean, *bn_invstd, *bn_w, *bn_b;
-};
 constexpr int RL_PT = 64;                        // positions per CTA
 constexpr int RL_ROWS = RL_PT + 2 * RL_PAD;      // 80 staged input rows
 constexpr int RL_YS = RL_C + 4;                  // padded row stride of the staged input
@@ -410,11 +393,13 @@ __global__ void __launch_bounds__(RL_C) rl_pool_linear_kernel(const float *__res
 // w_t [dir][H k][4H]     W_hh^T
 // The recurrence on the CUDA cores (validation path, both sizes): one CTA = 8 windows of one direction, thread = hidden
 // unit j with all four gates, W_hh^T read from global memory (L2-resident: 0.26 MB per direction at H = 128, 2.36 MB at
-// 384), h in shared memory.
+// 384), h in shared memory.  SAVE (training) also keeps the gates i, f, g, o and the cell c of every position:
+// save [B*P][2 dirs][5H].
 constexpr int LF_NB = 8;
-template <int H>
+template <int H, bool SAVE>
 __global__ void __launch_bounds__(H) rl_lstm_fp32(const float *__restrict__ gi, const float *__restrict__ wt,
-                                                  float *__restrict__ out, int64_t B, int64_t P) {
+                                                  float *__restrict__ out, int64_t B, int64_t P,
+                                                  float *__restrict__ save) {
     __shared__ __align__(16) float hs[LF_NB][H];
     const int j = threadIdx.x;
     const int dir = blockIdx.y;
@@ -458,6 +443,10 @@ __global__ void __launch_bounds__(H) rl_lstm_fp32(const float *__restrict__ gi, 
             const float h = og * tanhf(c);
             hs[n][j] = h;
             if (n < nb) out[((b0 + n) * P + t) * (2 * H) + dir * H + j] = h;
+            if (SAVE && n < nb) {
+                float *sv = save + (((b0 + n) * P + t) * 2 + dir) * (5 * H) + j;
+                sv[0] = ig; sv[H] = fg; sv[2 * H] = gg; sv[3 * H] = og; sv[4 * H] = c;
+            }
         }
         __syncthreads();
     }
@@ -579,7 +568,6 @@ __global__ void __launch_bounds__(LT_THREADS, 1) rl_lstm_tc_kernel(const float *
 // direction (2.25 MiB as fp16 hi + lo, more than one SM holds) and the input projections grow nine-fold (7.1 MFLOP per
 // position for both layers and directions), so both get tensor-core kernels of their own.  The fp32 twins
 // (rl_lstm_fp32, gemm_fp32_kernel) serve both sizes.
-constexpr int RL_H3 = 384;
 constexpr int RL_G43 = 4 * RL_H3;                  // 1536 gate rows per direction
 
 // ---------------------------------------------------------------------------------------------- projections on wgmma
@@ -917,6 +905,55 @@ __global__ void __launch_bounds__(256) rl_head768_kernel(const float *__restrict
     }
 }
 
+// ---------------------------------------------------------------------------------------------- shared launchers
+// (rl_common.cuh): the fp32 kernels above as the trainer (rl_train.cu) runs them
+constexpr int RL_DGROUP = 4;      // reads per partial sum of the fp32 convolution
+
+cudaError_t rl_launch_mask(const int8_t *x, int64_t B, int64_t P, int D, int F, uint8_t *mask, cudaStream_t s) {
+    rl_mask_kernel<<<(unsigned)(B * D), 256, 0, s>>>(x, P, D, F, mask);
+    return cudaGetLastError();
+}
+
+cudaError_t rl_launch_conv_fp32(const int8_t *x, const uint8_t *mask, const RlConv1 &c1, const RlConv17 &c17,
+                                const float *pool_w_t, const float *pool_b, int64_t B, int64_t P, int D, int F,
+                                int use_dwells, int H, float *y1, float *part, float *z, cudaStream_t s) {
+    const int n_groups = (D + RL_DGROUP - 1) / RL_DGROUP;
+    cudaError_t e = cudaFuncSetAttribute(rl_conv17_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RL_CONV_SMEM);
+    if (e != cudaSuccess) return e;
+    rl_embed_conv1_kernel<<<dim3((unsigned)((P + 31) / 32), (unsigned)(B * D)), RL_C, 0, s>>>(x, mask, c1, P, D, F,
+                                                                                         use_dwells, y1);
+    rl_conv17_pool_kernel<<<dim3((unsigned)((P + RL_PT - 1) / RL_PT), (unsigned)n_groups, (unsigned)B), 256, RL_CONV_SMEM, s>>>(
+        y1, mask, c17, P, D, RL_DGROUP, part);
+    if (H == RL_H3)
+        rl_pool_linear_kernel<RL_H3><<<dim3((unsigned)((P + RL_PLT - 1) / RL_PLT), (unsigned)B), RL_C, 0, s>>>(
+            part, mask, pool_w_t, pool_b, P, D, n_groups, z);
+    else
+        rl_pool_linear_kernel<RL_H><<<dim3((unsigned)((P + RL_PLT - 1) / RL_PLT), (unsigned)B), RL_C, 0, s>>>(
+            part, mask, pool_w_t, pool_b, P, D, n_groups, z);
+    return cudaGetLastError();
+}
+
+cudaError_t rl_launch_lstm_fp32(const float *gi, const float *w_t, float *out, int64_t B, int64_t P, int H,
+                                cudaStream_t s, float *save) {
+    const dim3 grid((unsigned)((B + LF_NB - 1) / LF_NB), 2);
+    if (H == RL_H3) {
+        if (save) rl_lstm_fp32<RL_H3, true><<<grid, RL_H3, 0, s>>>(gi, w_t, out, B, P, save);
+        else rl_lstm_fp32<RL_H3, false><<<grid, RL_H3, 0, s>>>(gi, w_t, out, B, P, nullptr);
+    } else {
+        if (save) rl_lstm_fp32<RL_H, true><<<grid, RL_H, 0, s>>>(gi, w_t, out, B, P, save);
+        else rl_lstm_fp32<RL_H, false><<<grid, RL_H, 0, s>>>(gi, w_t, out, B, P, nullptr);
+    }
+    return cudaGetLastError();
+}
+
+cudaError_t rl_launch_head(const float *h1, const float *lin_w, const float *lin_b, int64_t n, int H, float *probs,
+                           float *logits, cudaStream_t s) {
+    if (H != RL_H3) return launch_head(h1, lin_w, lin_b, 1, n, 0, probs, logits, nullptr, s);
+    const int64_t blocks = std::min<int64_t>((n + 7) / 8, 132 * 8);
+    rl_head768_kernel<HEAD_PLAIN><<<(unsigned)blocks, 256, 0, s>>>(h1, lin_w, lin_b, n, probs, nullptr, nullptr, {});
+    return cudaGetLastError();
+}
+
 // ---------------------------------------------------------------------------------------------- engine
 struct RlLstmLayer {
     float *w_ih = nullptr;      // [2 dirs * 4H][in]   (both directions stacked: one GEMM)
@@ -1213,7 +1250,7 @@ void rl_mark(mdk_rl_engine *e, int i) {
 // least).  Each slice's features go to a staging slot on copy_in; a slot is refilled once the convolution that read it
 // is done.  Every window is its own grid slice of each kernel, so the slicing does not change any output bit.
 int rl_conv(mdk_rl_engine *e, const int8_t *x, int64_t n, int64_t P, int64_t D, int64_t F, int64_t woff) {
-    const int dgroup = 4;
+    const int dgroup = RL_DGROUP;
     const int n_groups = (int)((D + dgroup - 1) / dgroup);
     const size_t xw = (size_t)P * D * F, yw = e->conv_tc ? 0 : (size_t)D * P * RL_C * 4, pw = (size_t)n_groups * P * RL_C * 4;
     const size_t per_window = 2 * xw + (size_t)D + yw + pw;
@@ -1301,9 +1338,9 @@ int rl_run_group(mdk_rl_engine *e) {
             rl_lstm_tc_kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N), 2), LT_THREADS, LT_SMEM, s>>>(
                 d_gi, L.w_hi, (const uint8_t *)L.w_lo, layer_out[l], B, P);
         } else if (h384) {
-            rl_lstm_fp32<RL_H3><<<grid_fp32, RL_H3, 0, s>>>(d_gi, L.w_t, layer_out[l], B, P);
+            rl_lstm_fp32<RL_H3, false><<<grid_fp32, RL_H3, 0, s>>>(d_gi, L.w_t, layer_out[l], B, P, nullptr);
         } else {
-            rl_lstm_fp32<RL_H><<<grid_fp32, RL_H, 0, s>>>(d_gi, L.w_t, layer_out[l], B, P);
+            rl_lstm_fp32<RL_H, false><<<grid_fp32, RL_H, 0, s>>>(d_gi, L.w_t, layer_out[l], B, P, nullptr);
         }
         rl_mark(e, 3 + 2 * l);
         layer_in = layer_out[l];

@@ -4,7 +4,10 @@ medaka/torch_ext.py (run_epoch, ClipGrad, the learning-rate schedules).
 ``GRUTrainer`` drives an ``mdk_trainer`` (csrc/gru_train.cu): forward with saved activations, cross-entropy, BPTT,
 gradient reductions, norm / clip / skip and the optimizer step all run in the library's CUDA kernels in fp32; the weights,
 their gradient and the optimizer state stay on the device.  Mixed precision (``amp=True``) and the read-level
-LatentSpaceLSTM are not implemented.  The learning-rate schedule is a plain function of the step, computed on the host.
+LatentSpaceLSTM are not implemented here.  The learning-rate schedule is a plain function of the step, computed on the host.
+
+``RLTrainer`` does the same for the read-level LatentSpaceLSTM through an ``mdk_rl_trainer`` (csrc/rl_train.cu), with
+batch-statistics BatchNorm as in ``model.train()``.
 """
 import csv
 import functools
@@ -50,6 +53,21 @@ def optimizer_args(optimizer, optim_args=None):
             raise ValueError("optimizer argument {}={!r} is not implemented for {}".format(k, v, optimizer))
         args[k] = v
     return args
+
+
+def _optim_desc(optimizer, args):
+    od = _lm.ffi.new("mdk_optim_desc *")
+    od.kind = _KINDS[optimizer]
+    od.alpha = args.get("alpha", 0.0)
+    b1, b2 = args.get("betas", (0.0, 0.0))
+    od.beta1, od.beta2 = b1, b2
+    od.eps = args.get("eps", 0.0)
+    od.weight_decay = args.get("weight_decay", 0.0)
+    od.momentum = args.get("momentum", 0.0)
+    od.dampening = args.get("dampening", 0.0)
+    od.momentum_decay = args.get("momentum_decay", 0.0)
+    od.nesterov = 1 if args.get("nesterov", False) else 0
+    return od
 
 
 # ---------------------------------------------------------------------------------------------- schedules and clipping
@@ -210,18 +228,7 @@ class GRUTrainer(object):
         """One of 'rmsprop', 'adam', 'nadam', 'sgd' with torch.optim's arguments (the reference's defaults when
         ``optim_args`` is None); resets the optimizer state."""
         args = optimizer_args(optimizer, optim_args)
-        od = _lm.ffi.new("mdk_optim_desc *")
-        od.kind = _KINDS[optimizer]
-        od.alpha = args.get("alpha", 0.0)
-        b1, b2 = args.get("betas", (0.0, 0.0))
-        od.beta1, od.beta2 = b1, b2
-        od.eps = args.get("eps", 0.0)
-        od.weight_decay = args.get("weight_decay", 0.0)
-        od.momentum = args.get("momentum", 0.0)
-        od.dampening = args.get("dampening", 0.0)
-        od.momentum_decay = args.get("momentum_decay", 0.0)
-        od.nesterov = 1 if args.get("nesterov", False) else 0
-        _lm.check(_lm.lib.mdk_trainer_set_optimizer(self._tr, od))
+        _lm.check(_lm.lib.mdk_trainer_set_optimizer(self._tr, _optim_desc(optimizer, args)))
         self.optimizer, self.optim_args, self.lr = optimizer, args, float(args["lr"])
 
     def set_bptt_windows(self, nb):
@@ -358,6 +365,223 @@ def workspace_bytes(num_features, gru_size, B, T):
     return int(b[0]), int(budget[0])
 
 
+RL_BUFFERS = ("read_level_conv.convs.2.running_mean", "read_level_conv.convs.2.running_var",
+              "read_level_conv.convs.5.running_mean", "read_level_conv.convs.5.running_var")
+RL_NBT = ("read_level_conv.convs.2.num_batches_tracked", "read_level_conv.convs.5.num_batches_tracked")
+
+
+def rl_param_shapes(lstm_size=128, cnn_size=128, use_dwells=False):
+    """named_parameters() of the reference's LatentSpaceLSTM (bidirectional, kernel sizes 1 and 17): name -> shape."""
+    H, C, nin = lstm_size, cnn_size, 6 + 1 + (1 if use_dwells else 0)
+    out = {"base_embedder.weight": (6, 6), "strand_embedder.weight": (3, 6),
+           "read_level_conv.convs.0.weight": (C, nin, 1), "read_level_conv.convs.0.bias": (C,),
+           "read_level_conv.convs.2.weight": (C,), "read_level_conv.convs.2.bias": (C,),
+           "read_level_conv.convs.3.weight": (C, C, 17), "read_level_conv.convs.3.bias": (C,),
+           "read_level_conv.convs.5.weight": (C,), "read_level_conv.convs.5.bias": (C,),
+           "read_level_conv.expansion_layer.weight": (H, C), "read_level_conv.expansion_layer.bias": (H,),
+           "pre_pool_expansion_layer.weight": (H, C), "pre_pool_expansion_layer.bias": (H,)}
+    for layer in range(2):
+        for sfx in ("", "_reverse"):
+            n_in = H if layer == 0 else 2 * H
+            out["lstm.weight_ih_l%d%s" % (layer, sfx)] = (4 * H, n_in)
+            out["lstm.weight_hh_l%d%s" % (layer, sfx)] = (4 * H, H)
+            out["lstm.bias_ih_l%d%s" % (layer, sfx)] = (4 * H,)
+            out["lstm.bias_hh_l%d%s" % (layer, sfx)] = (4 * H,)
+    out["linear.weight"] = (5, 2 * H)
+    out["linear.bias"] = (5,)
+    return out
+
+
+def rl_state_dict_keys(lstm_size=128, use_dwells=False):
+    """state_dict() keys of the reference's LatentSpaceLSTM: parameters with each BatchNorm's buffers after its own."""
+    keys = []
+    for k in rl_param_shapes(lstm_size, use_dwells=use_dwells):
+        keys.append(k)
+        if k.endswith(("convs.2.bias", "convs.5.bias")):
+            base = k[:-len("bias")]
+            keys += [base + "running_mean", base + "running_var", base + "num_batches_tracked"]
+    return keys
+
+
+def _rl_features(x):
+    """int8 [B, P, D, F] features: collated batches are uint8 (torch_ext.Batch.collate), whose strand -1 reads back as
+    255; the unsafe cast restores it, as the read-level engine's wrapper does."""
+    if hasattr(x, "detach"):
+        x = x.detach().cpu().numpy()
+    x = np.asarray(x)
+    out = np.empty(x.shape, np.int8)
+    np.copyto(out, x, casting="unsafe")
+    if out.ndim != 4:
+        raise ValueError("read-level features must be [B, P, D, F]")
+    return out
+
+
+class RLTrainer(object):
+    """The read-level LatentSpaceLSTM (latent_space_lstm.py) under training on an H100, fp32 (the reference's
+    amp=False): lstm_size 128 or 384, cnn_size 128, with or without dwells."""
+
+    STAGES = ("stats", "forward", "lstm", "head", "bptt", "read_backward", "reductions", "optimizer")
+
+    def __init__(self, lstm_size=128, cnn_size=128, use_dwells=False, num_classes=5, kernel_sizes=(1, 17),
+                 pooler_type="mean", bidirectional=True, device=0, optimizer="rmsprop", optim_args=None, amp=False,
+                 **unused):
+        if amp:
+            raise NotImplementedError("mixed-precision training (amp=True) is not implemented: training runs in fp32")
+        if (num_classes != 5 or list(kernel_sizes) != [1, 17] or pooler_type != "mean" or not bidirectional
+                or cnn_size != 128 or lstm_size not in (128, 384)):
+            raise NotImplementedError("only the bidirectional, mean-pooled LatentSpaceLSTM with kernel sizes [1, 17], "
+                                      "cnn_size 128, lstm_size 128 or 384 and 5 classes is implemented")
+        self.lstm_size, self.cnn_size, self.use_dwells = lstm_size, cnn_size, bool(use_dwells)
+        self.shapes = rl_param_shapes(lstm_size, cnn_size, use_dwells)
+        self._device = int(device)
+        self._tr = None
+        lib = _lm.load()
+        _lm.require_gpu(self._device)
+        pt = _lm.ffi.new("mdk_rl_trainer **")
+        _lm.check(lib.mdk_rl_trainer_create(self._device, lstm_size, cnn_size, 1 if use_dwells else 0, 5, pt))
+        self._tr = pt[0]
+        n = _lm.ffi.new("int64_t *")
+        _lm.check(lib.mdk_rl_trainer_num_params(self._tr, n))
+        self.n_params = int(n[0])
+        self.set_optimizer(optimizer, optim_args)
+
+    def close(self):
+        if self._tr is not None and _lm.lib is not None:
+            _lm.lib.mdk_rl_trainer_destroy(self._tr)
+        self._tr = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def set_optimizer(self, optimizer="rmsprop", optim_args=None):
+        """As GRUTrainer.set_optimizer."""
+        args = optimizer_args(optimizer, optim_args)
+        _lm.check(_lm.lib.mdk_rl_trainer_set_optimizer(self._tr, _optim_desc(optimizer, args)))
+        self.optimizer, self.optim_args, self.lr = optimizer, args, float(args["lr"])
+
+    def load_state_dict(self, state_dict):
+        """The reference's state dict (parameters, BatchNorm buffers, the unused expansion_layer); resets the
+        optimizer state."""
+        keys = rl_state_dict_keys(self.lstm_size, self.use_dwells)
+        missing = [k for k in keys if k not in state_dict]
+        unexpected = [k for k in state_dict if k not in keys]
+        if missing or unexpected:
+            raise RuntimeError("Error(s) in loading state_dict: missing {}, unexpected {}".format(missing, unexpected))
+        for k in keys:
+            v = state_dict[k]
+            if hasattr(v, "detach"):
+                v = v.detach().cpu().numpy()
+            a = np.ascontiguousarray(np.asarray(v, dtype=np.float32).reshape(-1))
+            shape = self.shapes.get(k, (1,) if k in RL_NBT else (self.cnn_size,))
+            if a.size != int(np.prod(shape)):
+                raise RuntimeError("size mismatch for {}: expected {}, got {}".format(k, shape, np.shape(v)))
+            _lm.check(_lm.lib.mdk_rl_trainer_load(self._tr, k.encode(), _lm.ffi.cast("const float *", _lm.ffi.from_buffer(a)),
+                                                  a.size))
+        return self
+
+    def _unflatten(self, flat):
+        out, o = {}, 0
+        for k, shape in self.shapes.items():
+            n = int(np.prod(shape))
+            out[k] = flat[o:o + n].reshape(shape)
+            o += n
+        return out
+
+    def flat_params(self):
+        out = np.empty(self.n_params, np.float32)
+        _lm.check(_lm.lib.mdk_rl_trainer_read_params(self._tr, _lm.ffi.cast("float *", _lm.ffi.from_buffer(out)),
+                                                     self.n_params))
+        return out
+
+    def buffers(self):
+        """The BatchNorm buffers: running statistics (float32) and num_batches_tracked (int64 scalars)."""
+        out = np.empty(4 * self.cnn_size, np.float32)
+        nbt = _lm.ffi.new("int64_t[2]")
+        _lm.check(_lm.lib.mdk_rl_trainer_read_buffers(self._tr, _lm.ffi.cast("float *", _lm.ffi.from_buffer(out)),
+                                                      out.size, nbt))
+        res = {k: out[i * self.cnn_size:(i + 1) * self.cnn_size] for i, k in enumerate(RL_BUFFERS)}
+        res.update({k: np.array(int(nbt[i]), np.int64) for i, k in enumerate(RL_NBT)})
+        return res
+
+    def state_dict(self):
+        """Weights and buffers as numpy arrays in the reference's state-dict keys and order."""
+        sd = self._unflatten(self.flat_params())
+        sd.update(self.buffers())
+        return {k: sd[k] for k in rl_state_dict_keys(self.lstm_size, self.use_dwells)}
+
+    def grads(self):
+        """The gradients of the last train_step, before clipping; expansion_layer, which gets none, is left out."""
+        out = np.empty(self.n_params, np.float32)
+        _lm.check(_lm.lib.mdk_rl_trainer_read_grads(self._tr, _lm.ffi.cast("float *", _lm.ffi.from_buffer(out)),
+                                                    self.n_params))
+        return {k: v for k, v in self._unflatten(out).items() if not k.startswith("read_level_conv.expansion_layer")}
+
+    @staticmethod
+    def _batch_arrays(batch):
+        x = batch.read_level_features if hasattr(batch, "read_level_features") else batch[0]
+        labels = batch.labels if hasattr(batch, "labels") else batch[1]
+        x = _rl_features(x)
+        if hasattr(labels, "detach"):
+            labels = labels.detach().cpu().numpy()
+        labels = np.asarray(labels)
+        if labels.ndim == 3 and labels.shape[-1] == 1:
+            labels = labels[..., 0]
+        if labels.shape != x.shape[:2]:
+            raise ValueError("features must be [B, P, D, F] and labels [B, P]")
+        return x, np.ascontiguousarray(labels, dtype=np.int32)
+
+    def _call(self, fn, x, *args):
+        B, P, D, F = x.shape
+        return fn(self._tr, _lm.ffi.cast("const int8_t *", _lm.ffi.from_buffer(x)), *args[:1], B, P, D, F, *args[1:])
+
+    def train_step(self, batch, lr=None, max_norm=None):
+        """As GRUTrainer.train_step, on read-level batches (read_level_features int8 / uint8 [B, P, D, F])."""
+        x, labels = self._batch_arrays(batch)
+        st = _lm.ffi.new("mdk_train_stats *")
+        _lm.check(self._call(_lm.lib.mdk_rl_trainer_step, x, _lm.ffi.cast("const int32_t *", _lm.ffi.from_buffer(labels)),
+                             float(self.lr if lr is None else lr), float(max_norm) if max_norm is not None else 0.0, st))
+        return float(st.loss), GRUTrainer._metrics(st, batch), float(st.grad_norm), bool(st.skipped)
+
+    def process_batch(self, batch, want_probs=False):
+        """The reference's validation (model.eval(): running statistics) without a backward pass."""
+        x, labels = self._batch_arrays(batch)
+        B, P = labels.shape
+        st = _lm.ffi.new("mdk_train_stats *")
+        probs = np.empty((B, P, 5), np.float32) if want_probs else None
+        pp = _lm.ffi.cast("float *", _lm.ffi.from_buffer(probs)) if want_probs else _lm.ffi.NULL
+        _lm.check(self._call(_lm.lib.mdk_rl_trainer_eval, x, _lm.ffi.cast("const int32_t *", _lm.ffi.from_buffer(labels)),
+                             pp, _lm.ffi.NULL, st))
+        metrics = {"n_model_correct": int(st.n_correct), "n_positions": int(st.n_positions)}
+        return (float(st.loss), metrics) + ((probs,) if want_probs else ())
+
+    def forward_arrays(self, x):
+        """(probs, logits) float32 [B, P, 5] of the validation forward, without labels."""
+        x = _rl_features(x)
+        B, P = x.shape[:2]
+        probs, logits = np.empty((B, P, 5), np.float32), np.empty((B, P, 5), np.float32)
+        _lm.check(self._call(_lm.lib.mdk_rl_trainer_eval, x, _lm.ffi.NULL,
+                             _lm.ffi.cast("float *", _lm.ffi.from_buffer(probs)),
+                             _lm.ffi.cast("float *", _lm.ffi.from_buffer(logits)), _lm.ffi.NULL))
+        return probs, logits
+
+    def stage_ms(self):
+        """Device times of the last train_step by stage (STAGES)."""
+        ms = _lm.ffi.new("float[8]")
+        _lm.check(_lm.lib.mdk_rl_trainer_stage_ms(self._tr, ms))
+        return dict(zip(self.STAGES, [float(v) for v in ms]))
+
+
+def rl_workspace_bytes(lstm_size, B, P, D, F):
+    """(device bytes a read-level train_step of B x P x D x F needs, the budget beyond which it is refused)."""
+    lib = _lm.load()
+    b, budget = _lm.ffi.new("size_t *"), _lm.ffi.new("size_t *")
+    _lm.check(lib.mdk_rl_trainer_workspace_bytes(lstm_size, B, P, D, F, b, budget))
+    return int(b[0]), int(budget[0])
+
+
 # ---------------------------------------------------------------------------------------------------------- batching
 def encoded_labels_to_training_vectors(enc_labels):
     """HaploidLabelScheme.encoded_labels_to_training_vectors (labels.py): sparse one-hot [n, 1]; legacy labels with two
@@ -369,11 +593,24 @@ def encoded_labels_to_training_vectors(enc_labels):
 
 
 class TrainBatch(object):
-    """What a training step reads of torch_ext.Batch: counts_matrix [B, T, F], labels [B, T] and, when a caller has
-    them, majority_vote_probs [B, T, 5] (n_argmax_correct)."""
+    """What a training step reads of torch_ext.Batch: counts_matrix [B, T, F] or read_level_features int8
+    [B, P, D, F], labels [B, T] and, when a caller has them, majority_vote_probs [B, T, 5] (n_argmax_correct)."""
 
-    def __init__(self, counts_matrix, labels, majority_vote_probs=None):
+    def __init__(self, counts_matrix=None, labels=None, majority_vote_probs=None, read_level_features=None):
         self.counts_matrix, self.labels, self.majority_vote_probs = counts_matrix, labels, majority_vote_probs
+        if read_level_features is not None:
+            self.read_level_features = read_level_features
+
+
+def pad_to_max_depth(read_level_features):
+    """Batch.collate's padding of read-level samples [P, D_i, F] to the batch's maximum depth: int8 [B, P, Dmax, F],
+    zeros past each sample's reads."""
+    depths = [f.shape[1] for f in read_level_features]
+    B, (P, _, F) = len(read_level_features), read_level_features[0].shape
+    out = np.zeros((B, P, max(depths), F), np.int8)
+    for i, f in enumerate(read_level_features):
+        np.copyto(out[i, :, :depths[i], :], np.asarray(f), casting="unsafe")
+    return out
 
 
 class TrainBatcher(object):
@@ -388,8 +625,9 @@ class TrainBatcher(object):
             self.label_scheme = ds.get_meta("label_scheme")
             self.feature_encoder = ds.get_meta("feature_encoder")
             self.feature_shape = ds.load_sample(self.samples[0][0]).features.shape
-        if len(self.feature_shape) != 2:
-            raise NotImplementedError("training reads counts-matrix features only (the read-level model is not trained)")
+        if len(self.feature_shape) not in (2, 3):
+            raise NotImplementedError("training reads counts-matrix or read-level features only")
+        self.read_level = len(self.feature_shape) == 3
         generator = np.random.default_rng(self.seed)
         if isinstance(validation, float):
             generator.shuffle(self.samples)
@@ -429,9 +667,13 @@ class TrainBatcher(object):
             for key, fname in samples[i * self.batch_size:(i + 1) * self.batch_size]:
                 with datastore.DataStore(fname) as ds:
                     s = ds.load_sample(key)
-                feats.append(np.asarray(s.features, np.float32))
+                feats.append(np.asarray(s.features) if self.read_level else np.asarray(s.features, np.float32))
                 labels.append(encoded_labels_to_training_vectors(s.labels)[:, 0])
-            yield TrainBatch(np.stack(feats), np.stack(labels).astype(np.int64))
+            labels = np.stack(labels).astype(np.int64)
+            if self.read_level:
+                yield TrainBatch(labels=labels, read_level_features=pad_to_max_depth(feats))
+            else:
+                yield TrainBatch(np.stack(feats), labels)
 
 
 # ---------------------------------------------------------------------------------------------------------- the loop
@@ -480,6 +722,28 @@ def _init_state_dict(num_features, gru_size, seed):
     return sd
 
 
+def _init_rl_state_dict(kwargs, seed):
+    """A fresh LatentSpaceLSTM's state dict: torch's modules built in the reference's construction order under
+    torch.manual_seed(seed), so the weights equal model_from_dict's under the same seed."""
+    import torch
+    H, C = int(kwargs.get("lstm_size", 128)), int(kwargs.get("cnn_size", 128))
+    nin = 6 + 1 + (1 if kwargs.get("use_dwells", False) else 0)
+    torch.manual_seed(seed)
+    mods = [("base_embedder.", torch.nn.Embedding(6, 6)), ("strand_embedder.", torch.nn.Embedding(3, 6)),
+            ("read_level_conv.convs.0.", torch.nn.Conv1d(nin, C, kernel_size=1, padding=0)),
+            ("read_level_conv.convs.2.", torch.nn.BatchNorm1d(C)),
+            ("read_level_conv.convs.3.", torch.nn.Conv1d(C, C, kernel_size=17, padding=8)),
+            ("read_level_conv.convs.5.", torch.nn.BatchNorm1d(C)),
+            ("read_level_conv.expansion_layer.", torch.nn.Linear(C, H)),
+            ("pre_pool_expansion_layer.", torch.nn.Linear(C, H)),
+            ("lstm.", torch.nn.LSTM(H, H, num_layers=2, bidirectional=True, batch_first=True)),
+            ("linear.", torch.nn.Linear(2 * H, 5))]
+    sd = {}
+    for prefix, m in mods:
+        sd.update({prefix + k: v.detach().numpy() for k, v in m.state_dict().items()})
+    return sd
+
+
 def run_epoch(trainer, batches, clip_grad=None, lr_scheduler=None, loss_log=None, is_training_epoch=False):
     """torch_ext.run_epoch: (mean batch loss, metrics) with the reference's metric names.  As there, the learning-rate
     schedule advances once per batch of a validation epoch too, when one is given."""
@@ -487,7 +751,7 @@ def run_epoch(trainer, batches, clip_grad=None, lr_scheduler=None, loss_log=None
     total = {"n_model_correct": 0, "n_positions": 0}
     sum_loss, n_batches, n_samples, t0 = 0.0, 0, 0, perf_counter()
     for batch in batches:
-        n_samples += batch.labels.shape[0]
+        n_samples += np.shape(batch.labels)[0]
         if is_training_epoch:
             lr = lr_scheduler.get_last_lr()[0] if lr_scheduler is not None else trainer.lr
             max_norm = clip_grad.max_norm() if clip_grad is not None else None
@@ -531,13 +795,21 @@ def run_training(train_name, batcher, model_fp=None, epochs=10, optimizer="rmspr
             ", ".join(sorted(loss_args))))
     os.makedirs(train_name, exist_ok=True)
     model_dict, weights = _model_dict(model_fp)
-    if model_dict.get("type") != "GRUModel":
-        raise NotImplementedError("only the consensus GRUModel is trained")
-    kw = model_dict["kwargs"]
-    num_features, gru_size = int(kw.get("num_features", 10)), int(kw.get("gru_size", 128))
-    trainer = GRUTrainer(num_features=num_features, num_classes=int(kw.get("num_classes", 5)), gru_size=gru_size,
-                         device=device, optimizer=optimizer, optim_args=optim_args, amp=amp)
-    trainer.load_state_dict(weights if weights is not None else _init_state_dict(num_features, gru_size, seed))
+    kw = model_dict.get("kwargs", {})
+    if model_dict.get("type") == "LatentSpaceLSTM":
+        from medaka_b200 import read_level
+        import types
+        read_level.LatentSpaceLSTM.check_feature_encoder_compatibility(
+            types.SimpleNamespace(use_dwells=bool(kw.get("use_dwells", False))), batcher.feature_encoder)
+        trainer = RLTrainer(device=device, optimizer=optimizer, optim_args=optim_args, amp=amp, **kw)
+        trainer.load_state_dict(weights if weights is not None else _init_rl_state_dict(kw, seed))
+    elif model_dict.get("type") == "GRUModel":
+        num_features, gru_size = int(kw.get("num_features", 10)), int(kw.get("gru_size", 128))
+        trainer = GRUTrainer(num_features=num_features, num_classes=int(kw.get("num_classes", 5)), gru_size=gru_size,
+                             device=device, optimizer=optimizer, optim_args=optim_args, amp=amp)
+        trainer.load_state_dict(weights if weights is not None else _init_state_dict(num_features, gru_size, seed))
+    else:
+        raise NotImplementedError("only the consensus GRUModel and the read-level LatentSpaceLSTM are trained")
     meta = {"model_function": functools.partial(datastore._ref_model_from_dict, model_dict),
             "label_scheme": batcher.label_scheme, "feature_encoder": batcher.feature_encoder}
     clip_grad = ClipGrad() if quantile_grad_clip else FixedClip(2.0)
