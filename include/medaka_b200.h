@@ -642,6 +642,15 @@ int mdk_rl_trainer_workspace_bytes(int32_t lstm_size, int64_t B, int64_t P, int6
 /* device times of the last step in ms: stats pass, forward pass (with the copies), LSTM forward, loss and head
  * backward, BPTT, read backward pass, reductions, optimizer step */
 int mdk_rl_trainer_stage_ms(mdk_rl_trainer *tr, float *ms);
+/* windows per CTA of the LSTM BPTT kernel: 1, 2, 4 or 8, or 0 (default) to choose from B as mdk_trainer_set_bptt_windows
+ * does.  The gradients do not depend on it.  For tests and measurements. */
+int mdk_rl_trainer_set_bptt_windows(mdk_rl_trainer *tr, int nb);
+/* the (window, read) rows of one slice of the forward and read backward passes: rows >= 1 caps the slice at
+ * min(rows, the automatic length), 0 (default) takes the automatic length (the per-read scratch's capacity, at most
+ * 65535 rows).  The workspace is sized for the automatic length.  For tests and measurements. */
+int mdk_rl_trainer_set_slice_rows(mdk_rl_trainer *tr, int64_t rows);
+/* windows per CTA the BPTT kernel runs at for a batch of B windows, under the current setting */
+int mdk_rl_trainer_bptt_windows(mdk_rl_trainer *tr, int64_t B, int *nb);
 
 #ifdef __cplusplus
 }

@@ -671,6 +671,8 @@ struct mdk_rl_trainer {
     mdk_optim_desc opt{};
     int64_t opt_steps = 0;
     double mu_product = 1.0;
+    int bptt_windows = 0;                    // 0: from B
+    int64_t slice_rows = 0;                  // 0: rlt_slice_rows
     cudaEvent_t ev[16] = {};
     int ev_kind[16] = {};
     int n_ev = 0;
@@ -865,6 +867,7 @@ void accum(mdk_rl_trainer *tr, int64_t nparts, int n, bool reset) {
 }
 
 int bptt_nb(const mdk_rl_trainer *tr, int64_t B) {
+    if (tr->bptt_windows) return tr->bptt_windows;
     for (int nb : {1, 2, 4})
         if (((B + nb - 1) / nb) * 2 <= tr->sm_count) return nb;
     return 8;
@@ -888,6 +891,12 @@ cudaError_t launch_bptt_h(int nb, const float *save, const float *dh, const floa
     case 4: return launch_bptt_t<HS, 4>(save, dh, w0, w1, dgi, B, P, s);
     default: return launch_bptt_t<HS, 8>(save, dh, w0, w1, dgi, B, P, s);
     }
+}
+
+// the rows of one slice of the forward and read backward passes: the automatic length, capped by the setting
+int64_t step_slice_rows(const mdk_rl_trainer *tr, int64_t P, int64_t rows) {
+    const int64_t sl = rlt_slice_rows(P, rows);
+    return tr->slice_rows ? std::min(tr->slice_rows, sl) : sl;
 }
 
 RltIn rlt_in(mdk_rl_trainer *tr, int64_t P, int64_t D, int64_t F) {
@@ -961,7 +970,7 @@ int forward_train(mdk_rl_trainer *tr, const RlWs &v, int64_t B, int64_t P, int64
     rlt_bn_stats_kernel<<<1, RL_C, 0, s>>>(tr->tot, (double)N, mean1, invstd1, tr->run, tr->run + RL_C);
     MDK_CUDA(cudaGetLastError());
     mark(tr, RS_STATS);
-    const int64_t sl = rlt_slice_rows(P, rows), ptiles = (P + CV_PT - 1) / CV_PT;
+    const int64_t sl = step_slice_rows(tr, P, rows), ptiles = (P + CV_PT - 1) / CV_PT;
     float *y1 = tr->scr;
     MDK_CUDA(cudaMemsetAsync(v.pooled, 0, (size_t)B * P * RL_C * sizeof(float), s));
     MDK_CUDA(cudaMemsetAsync(tr->tot, 0, 2 * RL_C * sizeof(double), s));
@@ -1055,7 +1064,7 @@ int backward(mdk_rl_trainer *tr, const RlWs &v, int64_t B, int64_t P, int64_t D,
     MDK_CUDA(cudaGetLastError());
     // the read pass: totals [0, C) db17, [C, C + 56 C) BN1's sums
     const RltIn in = rlt_in(tr, P, D, F);
-    const int64_t sl = rlt_slice_rows(P, rows), ptiles = (P + CV_PT - 1) / CV_PT;
+    const int64_t sl = step_slice_rows(tr, P, rows), ptiles = (P + CV_PT - 1) / CV_PT;
     float *y1 = tr->scr, *dpre = tr->scr + sl * P * RL_C;
     double *tot17 = tr->tot + RLT_NQ * RL_C;
     MDK_CUDA(cudaMemsetAsync(tr->tot, 0, (RLT_NQ + 1) * RL_C * sizeof(double), s));
@@ -1380,6 +1389,28 @@ int mdk_rl_trainer_workspace_bytes(int32_t lstm_size, int64_t B, int64_t P, int6
 int mdk_rl_trainer_stage_ms(mdk_rl_trainer *tr, float *ms) {
     MDK_REQUIRE(tr && ms, MDK_ERR_ARG, "rl_trainer_stage_ms: NULL argument");
     for (int i = 0; i < RS_N; ++i) ms[i] = tr->stage_ms[i];
+    return MDK_OK;
+}
+
+int mdk_rl_trainer_set_bptt_windows(mdk_rl_trainer *tr, int nb) {
+    MDK_REQUIRE(tr, MDK_ERR_ARG, "rl_trainer_set_bptt_windows: NULL argument");
+    MDK_REQUIRE(nb == 0 || nb == 1 || nb == 2 || nb == 4 || nb == 8, MDK_ERR_ARG,
+                "rl_trainer_set_bptt_windows: 0, 1, 2, 4 or 8");
+    tr->bptt_windows = nb;
+    return MDK_OK;
+}
+
+int mdk_rl_trainer_set_slice_rows(mdk_rl_trainer *tr, int64_t rows) {
+    MDK_REQUIRE(tr, MDK_ERR_ARG, "rl_trainer_set_slice_rows: NULL argument");
+    MDK_REQUIRE(rows >= 0, MDK_ERR_ARG, "rl_trainer_set_slice_rows: rows >= 0 (0: automatic)");
+    tr->slice_rows = rows;
+    return MDK_OK;
+}
+
+int mdk_rl_trainer_bptt_windows(mdk_rl_trainer *tr, int64_t B, int *nb) {
+    MDK_REQUIRE(tr && nb, MDK_ERR_ARG, "rl_trainer_bptt_windows: NULL argument");
+    MDK_REQUIRE(B >= 1, MDK_ERR_ARG, "rl_trainer_bptt_windows: need B >= 1");
+    *nb = bptt_nb(tr, B);
     return MDK_OK;
 }
 

@@ -462,6 +462,23 @@ class RLTrainer(object):
         _lm.check(_lm.lib.mdk_rl_trainer_set_optimizer(self._tr, _optim_desc(optimizer, args)))
         self.optimizer, self.optim_args, self.lr = optimizer, args, float(args["lr"])
 
+    def set_bptt_windows(self, nb):
+        """Schedule hook for tests and benchmarks: windows per CTA of the LSTM BPTT kernel (1, 2, 4 or 8), or 0 to
+        choose from the batch size.  The gradients do not depend on it."""
+        _lm.check(_lm.lib.mdk_rl_trainer_set_bptt_windows(self._tr, int(nb)))
+
+    def bptt_windows(self, B):
+        """Windows per CTA the BPTT kernel runs at for a batch of B windows, under the current setting."""
+        nb = _lm.ffi.new("int *")
+        _lm.check(_lm.lib.mdk_rl_trainer_bptt_windows(self._tr, int(B), nb))
+        return int(nb[0])
+
+    def set_slice_rows(self, rows):
+        """Schedule hook for tests and benchmarks: cap the (window, read) rows of one slice of the forward and read
+        backward passes at ``rows``, or 0 for the automatic length (what the per-read scratch holds).  Only the fp32
+        order of the sums across slices depends on it."""
+        _lm.check(_lm.lib.mdk_rl_trainer_set_slice_rows(self._tr, int(rows)))
+
     def load_state_dict(self, state_dict):
         """The reference's state dict (parameters, BatchNorm buffers, the unused expansion_layer); resets the
         optimizer state."""

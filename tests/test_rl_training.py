@@ -1,11 +1,14 @@
 """Read-level training on the CPU: the float64 oracle (oracle/rl_train_oracle.py) against the unmodified reference's
-three training steps (tests/golden/rl_train_steps.npz, tests/golden/make_rl_train_golden.py), the trainer's state-dict
-layout, read-level batching and the argument errors raised before the library loads."""
+three training steps (tests/golden/rl_train_steps.npz, tests/golden/make_rl_train_golden.py), its restatement against
+torch's modules, the proof that the GPU file's gradient bar sees every ablated term of the backward pass (each moves some
+tensor by more than 3x the bar), the trainer's state-dict layout, read-level batching and the argument errors raised
+before the library loads."""
 import os
 import sys
 
 import numpy as np
 import pytest
+import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
@@ -60,6 +63,84 @@ def test_oracle_reproduces_the_reference_golden(case):
     assert dcorrect <= 1
     for k in ("read_level_conv.convs.2.num_batches_tracked", "read_level_conv.convs.5.num_batches_tracked"):
         assert int(w3[k]) == 7 + mk.STEPS
+
+
+@pytest.mark.parametrize("H", [128, 384])
+def test_restated_lstm_equals_torch(H):
+    """The per-step LSTM that carries the LSTM ablations is torch.nn.LSTM without one (float64, 1e-12)."""
+    torch.manual_seed(H)
+    mod = torch.nn.LSTM(H, H, num_layers=2, bidirectional=True, batch_first=True).double()
+    h = torch.randn(3, 17, H, dtype=torch.float64, requires_grad=True)
+    want = mod(h)[0]
+    got = rl_train_oracle.lstm(mod, h)
+    assert (got - want).abs().max() <= 1e-12 * want.abs().max()
+    gw = torch.autograd.grad((want * torch.cos(want)).sum(), [h] + list(mod.parameters()))
+    gg = torch.autograd.grad((got * torch.cos(got)).sum(), [h] + list(mod.parameters()))
+    for a, b in zip(gw, gg):
+        assert (a - b).abs().max() <= 1e-12 * a.abs().max()
+
+
+@pytest.mark.parametrize("H,dw", [(128, False), (384, True)])
+def test_restated_oracle_equals_the_modules(H, dw):
+    """The whole restatement (k = 17 convolution with its backward written out, BatchNorm, per-step LSTM) without an
+    ablation: loss, gradients and running statistics of torch's modules."""
+    from tests.test_rl_training_gpu import batch, sd_for
+    sd = sd_for(H, dw)
+    x, y = batch(2, 20, 4, dw)
+    m0, m1 = rl_train_oracle.build(sd, dw), rl_train_oracle.build(sd, dw)
+    l0, g0, c0 = rl_train_oracle.loss_and_grads(m0, x, y)
+    l1, g1, c1 = rl_train_oracle.loss_and_grads(m1, x, y, restated=True)
+    assert abs(l1 / l0 - 1) <= 1e-12 and c0 == c1
+    assert sorted(g0) == sorted(g1)
+    for k in g0:
+        assert np.abs(g1[k] - g0[k]).max() <= 1e-12 * np.abs(g0[k]).max(), k
+    b0, b1 = m0.state_dict(), m1.state_dict()
+    for k in training.RL_BUFFERS + training.RL_NBT:
+        assert torch.equal(b0[k], b1[k]), k
+
+
+def test_a_flipped_relu_keeps_the_values_and_moves_the_gradient_at_one_element():
+    """oracle flips (the side of an undecidable ReLU): the loss and running statistics stay, the gradient changes by
+    one element's dpre2, so db17 moves in the flipped channel only"""
+    from tests.test_rl_training_gpu import ablation_case
+    sd, dw, (x, y) = ablation_case(P=20)
+    m0, m1 = rl_train_oracle.build(sd, dw), rl_train_oracle.build(sd, dw)
+    l0, g0, _ = rl_train_oracle.loss_and_grads(m0, x, y, restated=True)
+    r = rl_train_oracle.relu_margins(rl_train_oracle.build(sd, dw), x)["conv17"]
+    flip = torch.zeros(r.shape, dtype=torch.bool)
+    flip[tuple(torch.nonzero(r == r.min())[0].tolist())] = True
+    l1, g1, _ = rl_train_oracle.loss_and_grads(m1, x, y, flip={"conv17": flip})
+    assert abs(l1 / l0 - 1) <= 1e-15
+    for k in training.RL_BUFFERS:
+        assert torch.equal(m0.state_dict()[k], m1.state_dict()[k]), k
+    c = int(torch.nonzero(flip)[0, 1])
+    d = np.abs(g1["read_level_conv.convs.3.bias"] - g0["read_level_conv.convs.3.bias"])
+    assert d[c] > 1e-6 * np.abs(g0["read_level_conv.convs.3.bias"]).max()
+    assert np.delete(d, c).max() <= 1e-12 * np.abs(g0["read_level_conv.convs.3.bias"]).max()
+
+
+def test_rl_ablations_change_the_oracle_and_are_named():
+    from tests.test_rl_training_gpu import ablation_case
+    sd, dw, (x, y) = ablation_case(P=20)
+    _, ref, _ = rl_train_oracle.loss_and_grads(rl_train_oracle.build(sd, dw), x, y)
+    for which in rl_train_oracle.ABLATIONS:
+        _, g, _ = rl_train_oracle.loss_and_grads(rl_train_oracle.build(sd, dw), x, y, ablation=which)
+        assert any(not np.allclose(g[k], ref[k], rtol=1e-6, atol=0) for k in ref), which
+    with pytest.raises(ValueError):
+        rl_train_oracle.loss_and_grads(rl_train_oracle.build(sd, dw), x, y, ablation="nope")
+
+
+def test_rl_ablations_exceed_the_bars():
+    """Every ablated term moves some gradient tensor by more than 3x the GPU file's bar, at its first parity case."""
+    from tests import test_rl_training_gpu as gpu
+    sd, dw, (x, y) = gpu.ablation_case()
+    _, ref, _ = rl_train_oracle.loss_and_grads(rl_train_oracle.build(sd, dw), x, y)
+    for which in rl_train_oracle.ABLATIONS:
+        _, g, _ = rl_train_oracle.loss_and_grads(rl_train_oracle.build(sd, dw), x, y, ablation=which)
+        worst, k = gpu.grad_error(g, ref)
+        print("rl-train-ablation %-20s max per-tensor effect %.3g (%.0fx the bar, %s)"
+              % (which, worst, worst / gpu.GRAD_BAR, k))
+        assert worst > 3 * gpu.GRAD_BAR, (which, worst)
 
 
 @pytest.mark.parametrize("case", mk.CASES, ids=[c[0] for c in mk.CASES])

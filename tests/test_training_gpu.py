@@ -311,6 +311,41 @@ def test_non_finite_gradient_skips_the_step():
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize("kind", ["adam", "nadam"])
+def test_a_skipped_step_does_not_count(kind):
+    """good step, a NaN feature (skipped), good step: the weights are the rule's at t = 1 and 2, so the skip advanced
+    neither Adam's bias correction nor NAdam's mu_product"""
+    from medaka_b200 import training
+    F, H = 10, 128
+    sd, _, _ = _case(H, F, 3, 50, seed=4)
+    keys = training.state_dict_keys()
+    args = training.optimizer_args(kind, None)
+    tr = _trainer(sd, F, H, optimizer=kind)
+    f32 = lambda v: tuple(f32(u) for u in v) if isinstance(v, tuple) else (   # noqa: E731
+        float(np.float32(v)) if isinstance(v, float) else v)
+    opt = train_oracle.Optimizer(kind, **{k: f32(v) for k, v in args.items()})
+    p0 = train_oracle.flatten(sd, keys)
+    p = p0
+    _, bad, yb = _case(H, F, 3, 50, seed=11)
+    bad = bad.copy()
+    bad[1, 7, 3] = np.nan
+    for x, y, skip in (_case(H, F, 3, 50, seed=10)[1:] + (False,), (bad, yb, True),
+                       _case(H, F, 3, 50, seed=12)[1:] + (False,)):
+        _, _, norm, skipped = tr.train_step((x, y), lr=1e-3, max_norm=2.0)
+        assert skipped == skip
+        if not skip:
+            gf = train_oracle.flatten(tr.grads(), keys)
+            p = opt.step(p, gf * train_oracle.clip_coef(norm, 2.0), lr=f32(1e-3))
+            p = p.astype(np.float32).astype(np.float64)
+    got = train_oracle.flatten(tr.state_dict(), keys)
+    tr.close()
+    ulp = np.spacing(np.abs(got).astype(np.float32)).astype(np.float64)
+    err = np.maximum(np.abs(got - p) - ulp, 0).max() / np.abs(p - p0).max()
+    print("train-skip %s: max (|w - w_ref| - ulp) / max |step| = %.3g" % (kind, err))
+    assert err < STEP_BAR
+
+
+@pytest.mark.gpu
 def test_bad_labels_and_budget_are_argument_errors():
     from medaka_b200 import libmedaka, training
     sd, x, y = _case(128, 10, 2, 20)
