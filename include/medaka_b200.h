@@ -602,8 +602,10 @@ int mdk_trainer_workspace_bytes(const mdk_model_desc *desc, int64_t B, int64_t T
  * backward, BPTT recurrences, gradient reductions (and layer 1's dX), optimizer step (norm, update, weight repack) */
 int mdk_trainer_stage_ms(mdk_trainer *tr, float *ms);
 /* windows per CTA of the BPTT kernel: 1, 2, 4 or 8, or 0 (default) to choose from B (the fewest whose CTAs still fill
- * no more than one wave).  For measurements. */
+ * no more than one wave).  The gradients do not depend on it.  For tests and measurements. */
 int mdk_trainer_set_bptt_windows(mdk_trainer *tr, int nb);
+/* windows per CTA the BPTT kernel runs at for a batch of B windows, under the current setting */
+int mdk_trainer_bptt_windows(mdk_trainer *tr, int64_t B, int *nb);
 
 /* ---- read-level training: medaka train for the LatentSpaceLSTM the read-level engine accepts (bidirectional, mean
  * pooling, kernel sizes 1 and 17, cnn_size 128, lstm_size 128 or 384, 5 classes, with or without dwells), fp32.  The

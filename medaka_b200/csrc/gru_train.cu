@@ -165,7 +165,7 @@ struct ParamLayout {
 // the features and the label
 static int64_t train_floats_per_pos(int F, int hs) { return (int64_t)28 * hs + 3 * NCLS + F + 1; }
 // Past this the step fails instead of taking the card: 100 windows x 10 000 columns at gru_size 256 (the reference's
-// default training shape) need 28.8 GB
+// default training shape) need 29.5 GB
 constexpr int64_t TRAIN_WS_BUDGET = (int64_t)64 << 30;
 
 }  // namespace mdk
@@ -640,6 +640,13 @@ int mdk_trainer_set_bptt_windows(mdk_trainer *tr, int nb) {
     MDK_REQUIRE(tr, MDK_ERR_ARG, "trainer is NULL");
     MDK_REQUIRE(nb == 0 || nb == 1 || nb == 2 || nb == 4 || nb == 8, MDK_ERR_ARG, "trainer_set_bptt_windows: 0, 1, 2, 4 or 8");
     tr->bptt_windows = nb;
+    return MDK_OK;
+}
+
+int mdk_trainer_bptt_windows(mdk_trainer *tr, int64_t B, int *nb) {
+    MDK_REQUIRE(tr && nb, MDK_ERR_ARG, "trainer_bptt_windows: NULL argument");
+    MDK_REQUIRE(B >= 1, MDK_ERR_ARG, "trainer_bptt_windows: need B >= 1");
+    *nb = bptt_nb(tr, B);
     return MDK_OK;
 }
 

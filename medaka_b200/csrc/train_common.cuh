@@ -283,14 +283,21 @@ __global__ void __launch_bounds__(256) transpose_kernel(const float *__restrict_
         if (c0 + i < C && r0 + tx < R) dst[(int64_t)(c0 + i) * R + r0 + tx] = tile[tx][i];
 }
 
-// Split-M geometry of one reduction over M rows: about two waves of output tiles x splits, chunks of whole slices
+// Split-M geometry of one reduction over M rows: about two waves of output tiles x splits, chunks of whole slices and
+// of at most CHAIN_ROWS rows.  Each partial is a sequential fp32 sum over its chunk, whose rounding error grows with the
+// square root of its length: at 100 x 10 000 positions two waves alone make chunks of up to 166 672 rows, which miss a
+// signal-bearing gradient by several times the error of torch's fp32 training.  Chunks of at most 4 096 rows keep every
+// chain near the lengths the gradient bars were calibrated on; the partials are still added in a fixed order.
 struct Split {
     int splits;
     int64_t chunk;
 };
+constexpr int64_t CHAIN_ROWS = 4096;
+static_assert(CHAIN_ROWS % RM == 0, "chunks of whole slices");
 static Split split_for(int64_t M, int64_t tiles) {
     int64_t s = std::max<int64_t>(1, (2 * 132 + tiles - 1) / tiles);
     s = std::min<int64_t>(s, std::max<int64_t>(1, M / 256));
+    s = std::max<int64_t>(s, (M + CHAIN_ROWS - 1) / CHAIN_ROWS);
     int64_t chunk = (M + s - 1) / s;
     chunk = (chunk + RM - 1) / RM * RM;
     if (chunk == 0) chunk = RM;

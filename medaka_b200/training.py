@@ -232,7 +232,15 @@ class GRUTrainer(object):
         self.optimizer, self.optim_args, self.lr = optimizer, args, float(args["lr"])
 
     def set_bptt_windows(self, nb):
+        """Schedule hook for tests and benchmarks: windows per CTA of the BPTT kernel (1, 2, 4 or 8), or 0 to choose
+        from the batch size.  The gradients do not depend on it."""
         _lm.check(_lm.lib.mdk_trainer_set_bptt_windows(self._tr, int(nb)))
+
+    def bptt_windows(self, B):
+        """Windows per CTA the BPTT kernel runs at for a batch of B windows, under the current setting."""
+        nb = _lm.ffi.new("int *")
+        _lm.check(_lm.lib.mdk_trainer_bptt_windows(self._tr, int(B), nb))
+        return int(nb[0])
 
     def load_state_dict(self, state_dict):
         """torch state-dict layout (GRUModel.state_dict()); resets the optimizer state."""

@@ -99,6 +99,27 @@ def loss_and_grads(state_dict, feats, labels, ablation=None):
     return float(loss), {k: grads[k].numpy() for k in state_dict}, logits.numpy()
 
 
+def loss_and_grads_chunked(state_dict, feats, labels, windows=10):
+    """loss_and_grads over slices of ``windows`` windows at a time, so that a training batch's activations never exist
+    at once (100 x 10 000 columns at gru_size 256 would hold over 100 GB of float64 activations).  The windows are
+    independent, and the loss is a mean over all B*T positions: each slice's loss and gradients are weighted by its
+    share of the positions and added up.  Returns (loss, grads, logits [B, T, 5]) as loss_and_grads does.
+
+    At 100 x 10 000 on 8 CPU cores it took 299 s at gru_size 256 and 177 s at gru_size 128 (349 s and 234 s on
+    another 8-core host), with a peak of 9.8 GB at the default 10 windows per slice."""
+    feats, labels = np.asarray(feats), np.asarray(labels)
+    B, T = labels.shape
+    loss, grads, logits = 0.0, {}, np.empty((B, T, 5))
+    for b0 in range(0, B, windows):
+        b1 = min(B, b0 + windows)
+        share = (b1 - b0) / B
+        l_, g, logits[b0:b1] = loss_and_grads(state_dict, feats[b0:b1], labels[b0:b1])
+        loss += share * l_
+        for k, v in g.items():
+            grads[k] = grads.get(k, 0.0) + share * v
+    return loss, grads, logits
+
+
 def autograd_loss_and_grads(state_dict, feats, labels):
     """The same loss and gradients from torch autograd on gru_oracle.GRUOracle in float64."""
     from oracle import gru_oracle

@@ -41,16 +41,37 @@ def test_ablations_change_the_oracle_and_are_named():
         train_oracle.loss_and_grads(sd, x, y, ablation="nope")
 
 
-def test_ablations_exceed_the_bars():
-    """Every dropped term moves some gradient tensor by more than 3x the GPU file's bar, at one of its shapes."""
-    sd, x, y = gpu.ablation_case()
+def _ablations_exceed_the_bars(H, sd, x, y):
     _, ref, _ = train_oracle.loss_and_grads(sd, x, y)
     for which in train_oracle.ABLATIONS:
         _, g, _ = train_oracle.loss_and_grads(sd, x, y, ablation=which)
         err = gpu.grad_errors(g, ref)
-        worst = max(err.values())
-        print("train-ablation %-14s max per-tensor effect %.3g (%.0fx the bar)" % (which, worst, worst / gpu.GRAD_BAR))
-        assert worst > 3 * gpu.GRAD_BAR, (which, worst)
+        worst = max(err, key=err.get)
+        print("train-ablation H=%d %-14s max per-tensor effect %.3g (%.0fx the bar, %s)"
+              % (H, which, err[worst], err[worst] / gpu.GRAD_BAR, worst))
+        assert err[worst] > 3 * gpu.GRAD_BAR, (which, err[worst])
+
+
+def test_ablations_exceed_the_bars():
+    """Every dropped term moves some gradient tensor by more than 3x the GPU file's bar, at one of its shapes."""
+    _ablations_exceed_the_bars(128, *gpu.ablation_case())
+
+
+def test_ablations_exceed_the_bars_at_gru_size_256():
+    """The same at the width medaka train builds by default, on a batch the CPU oracle runs in seconds"""
+    _ablations_exceed_the_bars(256, *gpu._case(256, 10, 2, 200))
+
+
+def test_chunked_oracle_equals_the_whole_batch():
+    """Slices of 3 windows out of 7 (the last one short), weighted by their share of the positions, give the
+    whole batch's loss, gradients and logits"""
+    sd, x, y = _case(H=16, F=10, B=7, T=9)
+    loss, g, logits = train_oracle.loss_and_grads(sd, x, y)
+    c_loss, c_g, c_logits = train_oracle.loss_and_grads_chunked(sd, x, y, windows=3)
+    assert abs(c_loss - loss) <= 1e-12 * abs(loss)
+    err = gpu.grad_errors(c_g, g)
+    assert max(err.values()) < 1e-12, err
+    np.testing.assert_allclose(c_logits, logits, rtol=1e-12, atol=0)
 
 
 OPTIMIZERS = [

@@ -9,7 +9,8 @@ limit, 1980 MHz max SM clock) over every case of test_gradients_match_the_oracle
   worst loss error       6.7e-8   (the same case); 3.9e-9 on 8 x 10 000
   smallest ablation      3.86e-2  (h_t in place of h_{t-1} in dW_hh; the other five terms move some tensor by 0.25 to
                          1.8), measured by tests/test_training.py::test_ablations_exceed_the_bars on the oracle at
-                         gru_size 128, 2 x 60
+                         gru_size 128, 2 x 60; 2.31e-2 at gru_size 256, 2 x 200
+The same bars hold at the default training batch, 100 x 10 000, in tests/test_training_production.py.
 GRAD_BAR = 1e-5 is 9.7x the worst error and 1/3860 of the smallest ablation effect; LOSS_BAR = 1e-6 is 15x the worst
 loss error.  A kernel that drops any term of the backward pass fails the bar by orders of magnitude; fp32 reordering
 of the sums does not come near it.  Three optimizer steps against the oracle's float64 rules move the weights within
