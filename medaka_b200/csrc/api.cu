@@ -377,6 +377,9 @@ struct GruCall {
         const HeadVariant hv{ln.d_ref, ln.d_calls, ln.d_pred_q, ln.d_ref_q};
         int rc;
         if (quals && (rc = ensure_quals(ln))) return rc;
+        // a group the workspace cannot take (the budget at gru_size 256) is refused before it claims a slot of the
+        // event ring: the timings then cover the groups that ran, and the next forward records into the same slots
+        if ((rc = prepare_weights(e)) || (rc = ensure_workspace(e, *ln.ws, pk.windows, pk.len))) return rc;
         cudaStream_t s = ln.ws->stream;
         e->ev = e->evr[e->fwd_count % mdk_engine::EV_RING];
         e->fwd_count++;

@@ -318,11 +318,17 @@ class GRUTrainer(object):
         metrics["n_positions"] = int(stats.n_positions)
         return metrics
 
+    def _checked(self, feats, labels=None):
+        """The kernels read B x T x num_features floats: features of another width are refused, not misread."""
+        if feats.ndim != 3 or feats.shape[2] != self.num_features:
+            raise ValueError("expected features of shape [B, T, {}], got {}".format(self.num_features, feats.shape))
+        return feats, labels
+
     def train_step(self, batch, lr=None, max_norm=None):
         """One step (forward, loss, backward, clip, update) at learning rate ``lr`` (the optimizer's when None),
         clipping at ``max_norm`` (none when None).  Returns (loss, metrics, grad_norm, skipped); a non-finite gradient
         skips the update."""
-        feats, labels = self._batch_arrays(batch)
+        feats, labels = self._checked(*self._batch_arrays(batch))
         B, T = labels.shape
         st = _lm.ffi.new("mdk_train_stats *")
         _lm.check(_lm.lib.mdk_trainer_step(
@@ -334,7 +340,7 @@ class GRUTrainer(object):
     def process_batch(self, batch, want_probs=False):
         """Loss and metrics of a batch without a backward pass (the reference's process_batch under no_grad):
         (loss, {'n_model_correct', ['n_argmax_correct',] 'n_positions'}), plus the probabilities with want_probs."""
-        feats, labels = self._batch_arrays(batch)
+        feats, labels = self._checked(*self._batch_arrays(batch))
         B, T = labels.shape
         st = _lm.ffi.new("mdk_train_stats *")
         probs = np.empty((B, T, 5), np.float32) if want_probs else None
@@ -347,7 +353,7 @@ class GRUTrainer(object):
 
     def forward_arrays(self, feats):
         """(probs, logits) float32 [B, T, 5] of the training forward, without labels."""
-        feats = np.ascontiguousarray(feats, dtype=np.float32)
+        feats, _ = self._checked(np.ascontiguousarray(feats, dtype=np.float32))
         B, T = feats.shape[:2]
         probs, logits = np.empty((B, T, 5), np.float32), np.empty((B, T, 5), np.float32)
         _lm.check(_lm.lib.mdk_trainer_eval(
@@ -723,10 +729,14 @@ class CSVLogger(object):
         self.fh.close()
 
 
-def _model_dict(model_fp):
+def _model_dict(model_fp, batcher=None):
     from medaka_b200 import datastore
     if model_fp is None:
-        return DEFAULT_MODEL_DICT, None
+        # the default consensus model at the width of the store's counts (one to four datatypes: F = 10 to 40)
+        if batcher is None or getattr(batcher, "read_level", False):
+            return DEFAULT_MODEL_DICT, None
+        kwargs = dict(DEFAULT_MODEL_DICT["kwargs"], num_features=int(batcher.feature_shape[-1]))
+        return dict(DEFAULT_MODEL_DICT, kwargs=kwargs), None
     if model_fp.endswith(".gz"):
         store = datastore.ModelStoreTGZ(model_fp)
         return store.model_kwargs(), store._unpack()._weights
@@ -819,7 +829,7 @@ def run_training(train_name, batcher, model_fp=None, epochs=10, optimizer="rmspr
         raise ValueError("loss argument(s) {} are not implemented: the loss is CrossEntropyLoss()".format(
             ", ".join(sorted(loss_args))))
     os.makedirs(train_name, exist_ok=True)
-    model_dict, weights = _model_dict(model_fp)
+    model_dict, weights = _model_dict(model_fp, batcher)
     kw = model_dict.get("kwargs", {})
     if model_dict.get("type") == "LatentSpaceLSTM":
         from medaka_b200 import read_level
