@@ -321,7 +321,16 @@ int mdk_rl_destroy(mdk_rl_engine *e);
 int mdk_rl_load(mdk_rl_engine *e, const char *name, const float *data, int64_t n);
 /* which parts run on wgmma with fp16 hi/lo operand pairs (bit set) or on the fp32 CUDA cores (validation twins):
  * bit 0 = the k = 17 convolution (99 % of the network's FLOPs at lstm_size 128), bit 1 = the LSTM recurrences (at
- * lstm_size 384 also the LSTM input projections).  Default 3. */
+ * lstm_size 384 also the LSTM input projections).  Default 3: three fp16 products per contraction
+ * (hi.hi + hi.lo + lo.hi), fp32-faithful.
+ * bit 2 = the fp16 mode, medaka's own GPU default (the model in half precision under autocast): every contraction that
+ * bits 0 and 1 put on the tensor cores takes the single product hi.hi, operands rounded to the nearest fp16 with fp32
+ * accumulation: the k = 17 convolution (weights and its input y1), at lstm_size 384 the LSTM input projections (W_ih and
+ * their input, z or h0), and the recurrences (W_hh and the h fed back).  Everything else is unchanged: embedding, k = 1
+ * convolution, BatchNorm, ReLU, pooling and pre_pool_expansion_layer, gate math, c and h, head and softmax; at lstm_size
+ * 128 the input projections stay fp32 (gemm_fp32_kernel).  The fp32 twins ignore bit 2.  So 7 = fp16, 3 = tc, 0 = fp32.
+ * The mode is read when a window is staged and when its group is launched: a call that changes it launches the open
+ * group first, so no group mixes modes and windows submitted before the change run in the old mode. */
 int mdk_rl_set_conv(mdk_rl_engine *e, int tensor_cores);
 int mdk_rl_forward(mdk_rl_engine *e, const int8_t *x_host, int64_t B, int64_t P, int64_t D, int64_t F,
                    float *probs_host);

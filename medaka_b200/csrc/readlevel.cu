@@ -12,7 +12,9 @@
 // other sizes are refused.  BatchNorm runs in inference mode (running statistics), in torch's operation order
 // ((x - mean) * invstd * weight + bias).
 //
-// Kernels (the tensor-core ones run by default; mdk_rl_set_conv selects the fp32 CUDA-core twins for validation):
+// Kernels (the tensor-core ones run by default; mdk_rl_set_conv selects the fp32 CUDA-core twins for validation, and the
+// fp16 mode: rl_conv17_fp16_kernel, rl_proj_fp16_kernel, rl_lstm_fp16_kernel and rl_lstm384_fp16_kernel, the FP16 = true
+// forms of the four tensor-core kernels' bodies, one fp16 product hi.hi per contraction):
 //   rl_mask_kernel        which (window, read) rows are non-empty (x.sum((1, -1)) != 0, :163-165)
 //   rl_conv17_tc_kernel   embedding + k = 1 convolution + ReLU + BN1 built in shared memory, the k = 17 convolution as
 //                         a wgmma implicit GEMM, ReLU + BN2 and the masked SUM over a group of reads (99 % of the FLOPs)
@@ -198,6 +200,8 @@ __global__ void __launch_bounds__(256) rl_conv17_pool_kernel(const float *__rest
 //       descriptor's start address moved down t rows (K-major, no swizzle: a row is 16 bytes inside its k-group block)
 //   D = registers, M64 N128 per warpgroup (warpgroup g: output channels 64g .. 64g + 63); three fp16 products per
 //       contraction like the GRU kernels (fp32-faithful)
+// FP16 (the fp16 mode): one product, W_hi . y1_hi.  The activation tile is one plane, and the ring streams only the 17 hi
+// planes of the same pre-tiled weights: 8 MMAs per tap.
 // A CTA owns (window b, 128 positions, a group of reads): for each read it builds the activation tile in shared memory
 // straight from the int8 features (embedding + k = 1 convolution + ReLU + BN1, never written to HBM), runs 17 x 24 MMAs
 // against one pass of the weights, folds the accumulators through ReLU + BN2 into per-thread sums, and writes the
@@ -208,20 +212,21 @@ constexpr int CT_BPLANE = (RL_C / 8) * CT_ROWS * 16;     // 36 864 B
 constexpr int CT_BTILE = 2 * CT_BPLANE;                  // hi + lo of one read's activation tile
 constexpr int CT_WPLANE = (RL_C / 8) * RL_C * 16;        // 32 768 B: one plane of one tap = one ring stage
 constexpr int CT_STAGES = 2;
-constexpr int CT_OFF_W = CT_BTILE;
-constexpr int CT_OFF_IN = CT_OFF_W + CT_STAGES * CT_WPLANE;
-constexpr int CT_OFF_BAR = CT_OFF_IN + CT_ROWS * 8 * 4;
-constexpr int CT_SMEM = CT_OFF_BAR + 64;
+template <bool FP16> constexpr int CT_OFF_W = FP16 ? CT_BPLANE : CT_BTILE;
+template <bool FP16> constexpr int CT_OFF_IN = CT_OFF_W<FP16> + CT_STAGES * CT_WPLANE;
+template <bool FP16> constexpr int CT_OFF_BAR = CT_OFF_IN<FP16> + CT_ROWS * 8 * 4;
+template <bool FP16> constexpr int CT_SMEM = CT_OFF_BAR<FP16> + 64;
 
-__global__ void __launch_bounds__(256, 1) rl_conv17_tc_kernel(const int8_t *__restrict__ x, const uint8_t *__restrict__ mask,
-                                                              RlConv1 c1, RlConv17 c17, const uint8_t *__restrict__ w_tc,
-                                                              int64_t P, int D, int F, int use_dwells, int dgroup,
-                                                              float *__restrict__ partial) {
+template <bool FP16>
+__device__ __forceinline__ void rl_conv17_body(const int8_t *__restrict__ x, const uint8_t *__restrict__ mask, RlConv1 c1,
+                                               RlConv17 c17, const uint8_t *__restrict__ w_tc, int64_t P, int D, int F,
+                                               int use_dwells, int dgroup, float *__restrict__ partial) {
     extern __shared__ __align__(128) uint8_t smem_ct[];
     uint8_t *sb = smem_ct;                                             // [hi | lo][k-group][144][8 halfs]
-    uint8_t *sw = smem_ct + CT_OFF_W;                                  // [stage][k-group][128][8 halfs]
-    float *sin = reinterpret_cast<float *>(smem_ct + CT_OFF_IN);       // [144][8]
-    uint64_t *full = reinterpret_cast<uint64_t *>(smem_ct + CT_OFF_BAR);
+    uint8_t *sw = smem_ct + CT_OFF_W<FP16>;                            // [stage][k-group][128][8 halfs]
+    float *sin = reinterpret_cast<float *>(smem_ct + CT_OFF_IN<FP16>); // [144][8]
+    uint64_t *full = reinterpret_cast<uint64_t *>(smem_ct + CT_OFF_BAR<FP16>);
+    constexpr int NPLANES = FP16 ? RL_TAPS : 2 * RL_TAPS;             // weight planes per read
     const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
     const int gq = lane >> 2, cq = lane & 3;
     const int64_t b = blockIdx.z;
@@ -252,9 +257,9 @@ __global__ void __launch_bounds__(256, 1) rl_conv17_tc_kernel(const int8_t *__re
     for (int i = 0; i < 64; ++i) pooled[i] = 0.f;
     const int d0 = g * dgroup, d1 = min(D, d0 + dgroup);
     uint32_t it = 0;             // weight-plane stages consumed so far
-    auto issue = [&](uint32_t k) {   // stage k of the running sequence = plane (k % 34) of the taps
+    auto issue = [&](uint32_t k) {   // stage k of the running sequence = plane (k % 34) of the taps (FP16: tap k % 17's hi)
         const uint32_t st = k % CT_STAGES;
-        const uint8_t *src = w_tc + (size_t)(k % (2 * RL_TAPS)) * CT_WPLANE;     // [tap][hi | lo] back to back
+        const uint8_t *src = w_tc + (size_t)(FP16 ? k % RL_TAPS * 2 : k % (2 * RL_TAPS)) * CT_WPLANE;   // [tap][hi | lo]
         mbar_arrive_expect_tx(&full[st], CT_WPLANE);
         bulk_g2s(sw + st * CT_WPLANE, src, CT_WPLANE, &full[st]);
     };
@@ -292,19 +297,20 @@ __global__ void __launch_bounds__(256, 1) rl_conv17_tc_kernel(const int8_t *__re
             split_f16(y, hi, lo);
             const int off = (bc >> 3) * (CT_ROWS * 16) + r * 16 + (bc & 7) * 2;
             *reinterpret_cast<__half *>(sb + off) = hi;
-            *reinterpret_cast<__half *>(sb + CT_BPLANE + off) = lo;
+            if (!FP16) *reinterpret_cast<__half *>(sb + CT_BPLANE + off) = lo;
         }
         fence_proxy_async_smem();
         __syncthreads();
         // ---- 17 taps x (hi plane, lo plane) of the weights.  Each plane starts a fresh wgmma accumulator (16 or 8 MMAs
         // deep) that is added into the fp32 sum on the CUDA cores: one accumulator chained over all 34 planes (400 MMAs,
         // K = 17 x 128 x 3) lost ~10x the fp32 path's accuracy on the pooled output in the tensor core's accumulation.
+        // FP16 keeps the per-tap accumulators: 17 hi planes, 8 MMAs each.
         float sum[64];
 #pragma unroll
         for (int k = 0; k < 64; ++k) sum[k] = 0.f;
-        for (int ps = 0; ps < 2 * RL_TAPS; ++ps, ++it) {
+        for (int ps = 0; ps < NPLANES; ++ps, ++it) {
             const uint32_t st = it % CT_STAGES;
-            const int t = ps >> 1, lo_plane = ps & 1;
+            const int t = FP16 ? ps : ps >> 1, lo_plane = FP16 ? 0 : ps & 1;
             mbar_wait(&full[st], (it / CT_STAGES) & 1);
             wg_fence();
             const uint32_t a0 = smem_u32(sw + st * CT_WPLANE) + wg * 64 * 16;
@@ -315,13 +321,13 @@ __global__ void __launch_bounds__(256, 1) rl_conv17_tc_kernel(const int8_t *__re
                 const uint64_t ad = make_smem_desc(a0 + ks * 2 * (RL_C * 16), RL_C * 16, 128);
                 const uint64_t bh = make_smem_desc(bb0 + ks * 2 * (CT_ROWS * 16), CT_ROWS * 16, 128);
                 Wgmma<128>::ss(acc, ad, bh, ks ? 1u : 0u);
-                if (!lo_plane) Wgmma<128>::ss(acc, ad, make_smem_desc(bb0 + CT_BPLANE + ks * 2 * (CT_ROWS * 16), CT_ROWS * 16, 128), 1u);
+                if (!FP16 && !lo_plane) Wgmma<128>::ss(acc, ad, make_smem_desc(bb0 + CT_BPLANE + ks * 2 * (CT_ROWS * 16), CT_ROWS * 16, 128), 1u);
             }
             wg_commit();
             wg_wait_all();
             wg_hold(acc);
             __syncthreads();                                       // both warpgroups have read stage st
-            if (tid == 0 && ps + 2 < 2 * RL_TAPS) issue(it + 2);
+            if (tid == 0 && ps + 2 < NPLANES) issue(it + 2);
 #pragma unroll
             for (int k = 0; k < 64; ++k) sum[k] += acc[k];
         }
@@ -339,6 +345,19 @@ __global__ void __launch_bounds__(256, 1) rl_conv17_tc_kernel(const int8_t *__re
         const int n = 8 * (k >> 2) + 2 * cq + (k & 1);
         if (p0 + n < P) dst[(int64_t)n * RL_C + 8 * ((k >> 1) & 1)] = pooled[k];
     }
+}
+
+__global__ void __launch_bounds__(256, 1) rl_conv17_tc_kernel(const int8_t *__restrict__ x, const uint8_t *__restrict__ mask,
+                                                              RlConv1 c1, RlConv17 c17, const uint8_t *__restrict__ w_tc,
+                                                              int64_t P, int D, int F, int use_dwells, int dgroup,
+                                                              float *__restrict__ partial) {
+    rl_conv17_body<false>(x, mask, c1, c17, w_tc, P, D, F, use_dwells, dgroup, partial);
+}
+__global__ void __launch_bounds__(256, 1) rl_conv17_fp16_kernel(const int8_t *__restrict__ x, const uint8_t *__restrict__ mask,
+                                                                RlConv1 c1, RlConv17 c17, const uint8_t *__restrict__ w_tc,
+                                                                int64_t P, int D, int F, int use_dwells, int dgroup,
+                                                                float *__restrict__ partial) {
+    rl_conv17_body<true>(x, mask, c1, c17, w_tc, P, D, F, use_dwells, dgroup, partial);
 }
 
 // ---------------------------------------------------------------------------------------------- mean + Linear(C -> H)
@@ -459,13 +478,14 @@ __global__ void __launch_bounds__(H) rl_lstm_fp32(const float *__restrict__ gi, 
 //   B = the h tile [16 windows][128] (fp16 hi | lo, K-major, double buffered: step t reads buffer t & 1)
 //   D = four M64 N16 accumulators per warpgroup, preloaded with the input pre-activations; three products per
 //       contraction: W_hi.h_hi, W_hi.h_lo, W_lo.h_hi
-// One CTA = 16 windows of one direction, two warpgroups; c and h stay in registers.
+// One CTA = 16 windows of one direction, two warpgroups; c and h stay in registers.  FP16 (the fp16 mode): one product,
+// W_hi.h_hi; no lo plane in shared memory, and the h tile holds h's hi plane only.
 constexpr int LT_N = 16;
 constexpr int LT_WLO_GATE = (RL_H / 8) * RL_H * 16;          // 32 768 B: one gate's lo plane as A operand tiles
 constexpr int LT_KG = LT_N * 16 + 16;                        // k-group stride of the h tile (+16 B spreads the stores)
 constexpr int LT_HPLANE = (RL_H / 8) * LT_KG;
-constexpr int LT_OFF_H = 4 * LT_WLO_GATE;
-constexpr int LT_SMEM = LT_OFF_H + 4 * LT_HPLANE;
+template <bool FP16> constexpr int LT_OFF_H = FP16 ? 0 : 4 * LT_WLO_GATE;
+template <bool FP16> constexpr int LT_SMEM = LT_OFF_H<FP16> + 4 * LT_HPLANE;
 constexpr int LT_THREADS = 256;
 // element (direction d, gate row r, column k) of W_hh's lo plane in the tiles above: [dir][gate][k-group][row][8 halfs]
 inline size_t lt_lo_index(int d, int r, int k) {
@@ -475,12 +495,13 @@ inline size_t lt_lo_index(int d, int r, int k) {
 __device__ __forceinline__ float lt_sigmoid(float x) { return rcp_approx(1.0f + ex2_approx(-1.4426950408889634f * x)); }
 __device__ __forceinline__ float lt_tanh(float x) { return fmaf(-2.0f, rcp_approx(1.0f + ex2_approx(2.8853900817779268f * x)), 1.0f); }
 
-__global__ void __launch_bounds__(LT_THREADS, 1) rl_lstm_tc_kernel(const float *__restrict__ gi, const __half *__restrict__ w_hi,
-                                                            const uint8_t *__restrict__ w_lo_tiles, float *__restrict__ out,
-                                                            int64_t B, int64_t P) {
+template <bool FP16>
+__device__ __forceinline__ void rl_lstm_body(const float *__restrict__ gi, const __half *__restrict__ w_hi,
+                                             const uint8_t *__restrict__ w_lo_tiles, float *__restrict__ out, int64_t B,
+                                             int64_t P) {
     extern __shared__ __align__(128) uint8_t smem_lt[];
     uint8_t *swlo = smem_lt;
-    uint8_t *sh = smem_lt + LT_OFF_H;                            // [buf 2][hi | lo] LT_HPLANE
+    uint8_t *sh = smem_lt + LT_OFF_H<FP16>;                      // [buf 2][hi | lo] LT_HPLANE
     const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
     const int gq = lane >> 2, cq = lane & 3;
     const int dir = blockIdx.y;
@@ -489,7 +510,8 @@ __global__ void __launch_bounds__(LT_THREADS, 1) rl_lstm_tc_kernel(const float *
     const int j0 = wg * 64 + warp * 16 + gq;                   // hidden units j0 and j0 + 8
     {
         const uint4 *src = reinterpret_cast<const uint4 *>(w_lo_tiles + (size_t)dir * 4 * LT_WLO_GATE);
-        for (int i = tid; i < 4 * LT_WLO_GATE / 16; i += LT_THREADS) reinterpret_cast<uint4 *>(swlo)[i] = src[i];
+        if (!FP16)
+            for (int i = tid; i < 4 * LT_WLO_GATE / 16; i += LT_THREADS) reinterpret_cast<uint4 *>(swlo)[i] = src[i];
         for (int i = tid; i < 4 * LT_HPLANE / 16; i += LT_THREADS) reinterpret_cast<uint4 *>(sh)[i] = make_uint4(0u, 0u, 0u, 0u);
     }
     uint32_t whi[4][RL_H / 16][4];
@@ -532,6 +554,7 @@ __global__ void __launch_bounds__(LT_THREADS, 1) rl_lstm_tc_kernel(const float *
             for (int ks = 0; ks < RL_H / 16; ++ks) {
                 const uint64_t bh = make_smem_desc(h_hi + ks * 2 * LT_KG, LT_KG, 128);
                 Wgmma<16>::rs(acc[g], whi[g][ks], bh, 1u);
+                if (FP16) continue;
                 Wgmma<16>::rs(acc[g], whi[g][ks], make_smem_desc(h_lo + ks * 2 * LT_KG, LT_KG, 128), 1u);
                 Wgmma<16>::ss(acc[g], make_smem_desc(wl + g * LT_WLO_GATE + ks * 2 * (RL_H * 16), RL_H * 16, 128), bh, 1u);
             }
@@ -554,12 +577,23 @@ __global__ void __launch_bounds__(LT_THREADS, 1) rl_lstm_tc_kernel(const float *
             __half hi, lo;
             split_f16(h, hi, lo);
             *reinterpret_cast<__half *>(hw + (j >> 3) * LT_KG + wdw * 16 + (j & 7) * 2) = hi;
-            *reinterpret_cast<__half *>(hw + LT_HPLANE + (j >> 3) * LT_KG + wdw * 16 + (j & 7) * 2) = lo;
+            if (!FP16) *reinterpret_cast<__half *>(hw + LT_HPLANE + (j >> 3) * LT_KG + wdw * 16 + (j & 7) * 2) = lo;
         }
         if (step + 1 < P) fetch(dir ? (t - 1) : (t + 1));
         fence_proxy_async_smem();
         __syncthreads();
     }
+}
+
+__global__ void __launch_bounds__(LT_THREADS, 1) rl_lstm_tc_kernel(const float *__restrict__ gi, const __half *__restrict__ w_hi,
+                                                                   const uint8_t *__restrict__ w_lo_tiles,
+                                                                   float *__restrict__ out, int64_t B, int64_t P) {
+    rl_lstm_body<false>(gi, w_hi, w_lo_tiles, out, B, P);
+}
+__global__ void __launch_bounds__(LT_THREADS, 1) rl_lstm_fp16_kernel(const float *__restrict__ gi, const __half *__restrict__ w_hi,
+                                                                     const uint8_t *__restrict__ w_lo_tiles,
+                                                                     float *__restrict__ out, int64_t B, int64_t P) {
+    rl_lstm_body<true>(gi, w_hi, w_lo_tiles, out, B, P);
 }
 
 // ============================================================================================== lstm_size = 384
@@ -576,7 +610,9 @@ constexpr int RL_G43 = 4 * RL_H3;                  // 1536 gate rows per directi
 //   A = W, pre-tiled per (128-row block, 64-wide K chunk) as [hi | lo][k-group 8][row 128][8 halfs] (32 KiB, one bulk copy)
 //   B = X, read as fp32 and split into fp16 hi / lo while it is staged ([hi | lo][k-group 8][position 128][8 halfs])
 // K runs in 64-wide chunks through two stages: while the 12 MMAs of chunk c run, the threads stage the activations of
-// chunk c + 1 and the bulk copy brings its weights.  Three products per contraction (DESIGN §3).
+// chunk c + 1 and the bulk copy brings its weights.  Three products per contraction (DESIGN §3); FP16 (the fp16 mode):
+// one, W_hi . X_hi: the bulk copy brings the hi half of each weight chunk and X is staged as its hi plane, 4 MMAs per
+// chunk.
 constexpr int PJ_M = 128;
 constexpr int PJ_N = 128;
 constexpr int PJ_KC = 64;
@@ -587,9 +623,9 @@ constexpr int PJ_STAGE = PJ_WCHUNK + 2 * PJ_XPLANE;         // 64 KiB
 constexpr int PJ_OFF_BAR = 2 * PJ_STAGE;
 constexpr int PJ_SMEM = PJ_OFF_BAR + 64;
 
-__global__ void __launch_bounds__(256, 1) rl_proj_tc_kernel(const float *__restrict__ X, const uint8_t *__restrict__ w_tc,
-                                                            const float *__restrict__ bias, float *__restrict__ C, int64_t M,
-                                                            int K, int N) {
+template <bool FP16>
+__device__ __forceinline__ void rl_proj_body(const float *__restrict__ X, const uint8_t *__restrict__ w_tc,
+                                             const float *__restrict__ bias, float *__restrict__ C, int64_t M, int K, int N) {
     extern __shared__ __align__(128) uint8_t smem_pj[];
     uint64_t *full = reinterpret_cast<uint64_t *>(smem_pj + PJ_OFF_BAR);
     const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
@@ -605,8 +641,9 @@ __global__ void __launch_bounds__(256, 1) rl_proj_tc_kernel(const float *__restr
     __syncthreads();
     auto issue_w = [&](int c) {
         const int st = c & 1;
-        mbar_arrive_expect_tx(&full[st], PJ_WCHUNK);
-        bulk_g2s(smem_pj + st * PJ_STAGE, w_tc + ((size_t)rb * nchunks + c) * PJ_WCHUNK, PJ_WCHUNK, &full[st]);
+        constexpr int bytes = FP16 ? PJ_WPLANE : PJ_WCHUNK;
+        mbar_arrive_expect_tx(&full[st], bytes);
+        bulk_g2s(smem_pj + st * PJ_STAGE, w_tc + ((size_t)rb * nchunks + c) * PJ_WCHUNK, bytes, &full[st]);
     };
     auto stage_x = [&](int c) {
         uint8_t *xs = smem_pj + (c & 1) * PJ_STAGE + PJ_WCHUNK;
@@ -623,7 +660,7 @@ __global__ void __launch_bounds__(256, 1) rl_proj_tc_kernel(const float *__restr
             __half2 hv[2] = {__halves2half2(h0, h1), __halves2half2(h2, h3)};
             __half2 lv[2] = {__halves2half2(l0, l1), __halves2half2(l2, l3)};
             *reinterpret_cast<uint2 *>(xs + off) = *reinterpret_cast<uint2 *>(hv);
-            *reinterpret_cast<uint2 *>(xs + PJ_XPLANE + off) = *reinterpret_cast<uint2 *>(lv);
+            if (!FP16) *reinterpret_cast<uint2 *>(xs + PJ_XPLANE + off) = *reinterpret_cast<uint2 *>(lv);
         }
     };
     // each 64-wide K chunk runs in a fresh accumulator (12 MMAs) that is added into the fp32 sum on the CUDA cores: one
@@ -649,8 +686,10 @@ __global__ void __launch_bounds__(256, 1) rl_proj_tc_kernel(const float *__restr
             const uint64_t bh = make_smem_desc(xbase + ks * 2 * (PJ_N * 16), PJ_N * 16, 128);
             const uint64_t bl = make_smem_desc(xbase + PJ_XPLANE + ks * 2 * (PJ_N * 16), PJ_N * 16, 128);
             Wgmma<128>::ss(acc, ah, bh, ks ? 1u : 0u);
-            Wgmma<128>::ss(acc, ah, bl, 1u);
-            Wgmma<128>::ss(acc, al, bh, 1u);
+            if (!FP16) {
+                Wgmma<128>::ss(acc, ah, bl, 1u);
+                Wgmma<128>::ss(acc, al, bh, 1u);
+            }
         }
         wg_commit();
         if (c + 1 < nchunks) {
@@ -673,6 +712,17 @@ __global__ void __launch_bounds__(256, 1) rl_proj_tc_kernel(const float *__restr
     }
 }
 
+__global__ void __launch_bounds__(256, 1) rl_proj_tc_kernel(const float *__restrict__ X, const uint8_t *__restrict__ w_tc,
+                                                            const float *__restrict__ bias, float *__restrict__ C, int64_t M,
+                                                            int K, int N) {
+    rl_proj_body<false>(X, w_tc, bias, C, M, K, N);
+}
+__global__ void __launch_bounds__(256, 1) rl_proj_fp16_kernel(const float *__restrict__ X, const uint8_t *__restrict__ w_tc,
+                                                              const float *__restrict__ bias, float *__restrict__ C, int64_t M,
+                                                              int K, int N) {
+    rl_proj_body<true>(X, w_tc, bias, C, M, K, N);
+}
+
 // ---------------------------------------------------------------------------------------------- recurrence on a cluster
 // Per time step G^T[4H = 1536][16 windows] = W_hh . h^T with h the 16 windows' previous output, split over a cluster of
 // 8 CTAs: CTA rank r owns hidden units 48r .. 48r + 47, i.e. 192 gate rows (4 gates x 48 units), in three warpgroups of
@@ -688,7 +738,8 @@ __global__ void __launch_bounds__(256, 1) rl_proj_tc_kernel(const float *__restr
 // thread waits (acquire, cluster scope, bounded) on its own CTA's barrier for all 8 arrivals before the next step's MMAs
 // read the buffer.  That wait after the last step is also the exit barrier: once a CTA has seen its 8 arrivals, no peer
 // writes into its shared memory any more.  The buffer a step writes was last read by the MMAs of the step before, which
-// every CTA completed (wgmma.wait_group) before it arrived.
+// every CTA completed (wgmma.wait_group) before it arrived.  FP16 (the fp16 mode): one product, W_hi.h_hi, 24 MMAs per
+// step in the same three chains; no lo plane in shared memory, and only h's hi plane goes to the peers.
 constexpr int L3_CL = 8;                                     // CTAs per cluster
 constexpr int L3_UNITS = RL_H3 / L3_CL;                      // 48 hidden units per CTA
 constexpr int L3_THREADS = 384;                              // 3 warpgroups
@@ -698,10 +749,10 @@ constexpr int L3_KG = LT_N * 16 + 16;                        // k-group stride o
 constexpr int L3_HPLANE = (RL_H3 / 8) * L3_KG;               // 13 056 B
 constexpr int L3_XS = 20;                                    // window stride of the gate exchange (floats): no bank conflicts
 constexpr int L3_XCH_WG = 4 * LT_N * L3_XS * 4;              // 5 KiB
-constexpr int L3_OFF_H = 3 * L3_WLO_WG;
-constexpr int L3_OFF_X = L3_OFF_H + 4 * L3_HPLANE;
-constexpr int L3_OFF_BAR = L3_OFF_X + 3 * L3_XCH_WG;
-constexpr int L3_SMEM = L3_OFF_BAR + 16;                     // 210 KiB
+template <bool FP16> constexpr int L3_OFF_H = FP16 ? 0 : 3 * L3_WLO_WG;
+template <bool FP16> constexpr int L3_OFF_X = L3_OFF_H<FP16> + 4 * L3_HPLANE;
+template <bool FP16> constexpr int L3_OFF_BAR = L3_OFF_X<FP16> + 3 * L3_XCH_WG;
+template <bool FP16> constexpr int L3_SMEM = L3_OFF_BAR<FP16> + 16;     // 210 KiB (FP16: 66 KiB)
 // element (direction d, gate row r, column k) of W_hh's lo plane in the tiles above: per (direction, cluster rank,
 // warpgroup) [k-group][row m = 16 gate + unit within the warpgroup][8 halfs]
 inline size_t l3_lo_index(int d, int r, int k) {
@@ -709,13 +760,14 @@ inline size_t l3_lo_index(int d, int r, int k) {
     return (((size_t)(d * L3_CL + rank) * 3 + wg) * (RL_H3 / 8) + k / 8) * (64 * 8) + m * 8 + k % 8;
 }
 
-__global__ void __cluster_dims__(L3_CL, 1, 1) __launch_bounds__(L3_THREADS, 1)
-    rl_lstm384_tc_kernel(const float *__restrict__ gi, const __half *__restrict__ w_hi, const uint8_t *__restrict__ w_lo_tiles,
-                         float *__restrict__ out, int64_t B, int64_t P) {
+template <bool FP16>
+__device__ __forceinline__ void rl_lstm384_body(const float *__restrict__ gi, const __half *__restrict__ w_hi,
+                                                const uint8_t *__restrict__ w_lo_tiles, float *__restrict__ out, int64_t B,
+                                                int64_t P) {
     extern __shared__ __align__(128) uint8_t smem_l3[];
     uint8_t *swlo = smem_l3;
-    uint8_t *sh = smem_l3 + L3_OFF_H;                            // [buf 2][hi | lo] L3_HPLANE
-    uint64_t *hbar = reinterpret_cast<uint64_t *>(smem_l3 + L3_OFF_BAR);
+    uint8_t *sh = smem_l3 + L3_OFF_H<FP16>;                      // [buf 2][hi | lo] L3_HPLANE
+    uint64_t *hbar = reinterpret_cast<uint64_t *>(smem_l3 + L3_OFF_BAR<FP16>);
     const int tid = threadIdx.x, wg = tid >> 7, wt = tid & 127, warp = (tid >> 5) & 3, lane = tid & 31;
     const int gq = lane >> 2, cq = lane & 3;
     const uint32_t rank = cluster_ctarank();
@@ -723,10 +775,11 @@ __global__ void __cluster_dims__(L3_CL, 1, 1) __launch_bounds__(L3_THREADS, 1)
     const int64_t b0 = (int64_t)(blockIdx.x / L3_CL) * LT_N;
     const int nb = (int)min((int64_t)LT_N, B - b0);
     const int u0 = (int)rank * L3_UNITS + wg * 16;                 // first hidden unit of this warpgroup
-    float *xw = reinterpret_cast<float *>(smem_l3 + L3_OFF_X + wg * L3_XCH_WG);     // [gate 4][window 16][L3_XS]
+    float *xw = reinterpret_cast<float *>(smem_l3 + L3_OFF_X<FP16> + wg * L3_XCH_WG);  // [gate 4][window 16][L3_XS]
     {
         const uint4 *src = reinterpret_cast<const uint4 *>(w_lo_tiles + ((size_t)dir * L3_CL + rank) * 3 * L3_WLO_WG);
-        for (int i = tid; i < 3 * L3_WLO_WG / 16; i += L3_THREADS) reinterpret_cast<uint4 *>(swlo)[i] = src[i];
+        if (!FP16)
+            for (int i = tid; i < 3 * L3_WLO_WG / 16; i += L3_THREADS) reinterpret_cast<uint4 *>(swlo)[i] = src[i];
         for (int i = tid; i < 4 * L3_HPLANE / 16; i += L3_THREADS) reinterpret_cast<uint4 *>(sh)[i] = make_uint4(0u, 0u, 0u, 0u);
     }
     if (tid == 0) {
@@ -781,6 +834,7 @@ __global__ void __cluster_dims__(L3_CL, 1, 1) __launch_bounds__(L3_THREADS, 1)
             float (&a)[8] = ks < L3_KS / 3 ? acc : ks < 2 * L3_KS / 3 ? acc2 : acc3;
             const uint64_t bh = make_smem_desc(h_hi + ks * 2 * L3_KG, L3_KG, 128);
             Wgmma<16>::rs(a, whi[ks], bh, (ks == L3_KS / 3 || ks == 2 * L3_KS / 3) ? 0u : 1u);
+            if (FP16) continue;
             Wgmma<16>::rs(a, whi[ks], make_smem_desc(h_lo + ks * 2 * L3_KG, L3_KG, 128), 1u);
             Wgmma<16>::ss(a, make_smem_desc(wl + ks * 2 * (64 * 16), 64 * 16, 128), bh, 1u);
         }
@@ -819,13 +873,24 @@ __global__ void __cluster_dims__(L3_CL, 1, 1) __launch_bounds__(L3_THREADS, 1)
 #pragma unroll
         for (int q = 0; q < L3_CL; ++q) {
             st_cluster_u32(peer_h[q] + nxt, hw);
-            st_cluster_u32(peer_h[q] + nxt + L3_HPLANE, lw);
+            if (!FP16) st_cluster_u32(peer_h[q] + nxt + L3_HPLANE, lw);
         }
         fence_proxy_async_cluster();
         __syncthreads();
         if (tid < L3_CL) mbar_arrive_cluster(bar_peer + (uint32_t)((buf ^ 1) * 8));
         mbar_wait_cluster(&hbar[buf ^ 1], (uint32_t)(step >> 1) & 1u);
     }
+}
+
+__global__ void __cluster_dims__(L3_CL, 1, 1) __launch_bounds__(L3_THREADS, 1)
+    rl_lstm384_tc_kernel(const float *__restrict__ gi, const __half *__restrict__ w_hi, const uint8_t *__restrict__ w_lo_tiles,
+                         float *__restrict__ out, int64_t B, int64_t P) {
+    rl_lstm384_body<false>(gi, w_hi, w_lo_tiles, out, B, P);
+}
+__global__ void __cluster_dims__(L3_CL, 1, 1) __launch_bounds__(L3_THREADS, 1)
+    rl_lstm384_fp16_kernel(const float *__restrict__ gi, const __half *__restrict__ w_hi, const uint8_t *__restrict__ w_lo_tiles,
+                           float *__restrict__ out, int64_t B, int64_t P) {
+    rl_lstm384_body<true>(gi, w_hi, w_lo_tiles, out, B, P);
 }
 
 // Linear(2H = 768 -> 5) + softmax + argmax: one warp per position, 24 inputs per lane, the weights in shared memory.
@@ -995,6 +1060,7 @@ struct mdk_rl_engine {
     __half *c17_tc = nullptr;      // [17 taps][hi | lo][k-group 16][co 128][8 halfs]: the tensor-core kernel's A operand tiles
     int conv_tc = 1;               // 1: k = 17 convolution on wgmma (default), 0: fp32 CUDA cores
     int lstm_tc = 1;               // 1: LSTM recurrence on wgmma (default), 0: fp32 CUDA cores
+    int fp16 = 0;                  // 1: the wgmma stages take one fp16 product per contraction (the fp16 mode)
     float *pool_w = nullptr, *pool_b = nullptr;
     RlLstmLayer lstm[2];
     float *lin_w = nullptr, *lin_b = nullptr;
@@ -1088,11 +1154,12 @@ int rl_wave_windows(mdk_rl_engine *e, int *out) {
     if (e->H == RL_H) {
         e->wave = LT_N * (e->sm_count / 2);
     } else {
-        MDK_CUDA(cudaFuncSetAttribute(rl_lstm384_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L3_SMEM));
+        // the three-product kernel: the fp16 one needs less shared memory and fits as many clusters
+        MDK_CUDA(cudaFuncSetAttribute(rl_lstm384_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L3_SMEM<false>));
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3(L3_CL, 2);
         cfg.blockDim = dim3(L3_THREADS);
-        cfg.dynamicSmemBytes = L3_SMEM;
+        cfg.dynamicSmemBytes = L3_SMEM<false>;
         cudaLaunchAttribute attr;
         attr.id = cudaLaunchAttributeClusterDimension;
         attr.val.clusterDim.x = L3_CL;
@@ -1266,7 +1333,10 @@ int rl_conv(mdk_rl_engine *e, const int8_t *x, int64_t n, int64_t P, int64_t D, 
     float *d_y1 = (float *)(e->conv + o_y1), *d_part = (float *)(e->conv + o_part);
     RlConv1 c1{e->emb_base, e->emb_strand, e->c1_w, e->c1_b, e->bn1[0], e->bn1[1], e->bn1[2], e->bn1[3]};
     RlConv17 c17{e->c17_wt, e->c17_b, e->bn2[0], e->bn2[1], e->bn2[2], e->bn2[3]};
-    if (e->conv_tc) MDK_CUDA(cudaFuncSetAttribute(rl_conv17_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CT_SMEM));
+    if (e->conv_tc && e->fp16)
+        MDK_CUDA(cudaFuncSetAttribute(rl_conv17_fp16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CT_SMEM<true>));
+    else if (e->conv_tc)
+        MDK_CUDA(cudaFuncSetAttribute(rl_conv17_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CT_SMEM<false>));
     else MDK_CUDA(cudaFuncSetAttribute(rl_conv17_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RL_CONV_SMEM));
     for (int64_t s0 = 0; s0 < n; s0 += slice) {
         const int64_t B = std::min(slice, n - s0);
@@ -1284,9 +1354,13 @@ int rl_conv(mdk_rl_engine *e, const int8_t *x, int64_t n, int64_t P, int64_t D, 
         if (woff + s0 == 0) rl_mark(e, 0);
         const int8_t *d_x = e->xbuf[k];
         rl_mask_kernel<<<(unsigned)(B * D), 256, 0, s>>>(d_x, P, (int)D, (int)F, d_mask);
-        if (e->conv_tc) {
-            rl_conv17_tc_kernel<<<dim3((unsigned)((P + CT_NPOS - 1) / CT_NPOS), (unsigned)n_groups, (unsigned)B), 256, CT_SMEM, s>>>(
-                d_x, d_mask, c1, c17, (const uint8_t *)e->c17_tc, P, (int)D, (int)F, e->use_dwells, dgroup, d_part);
+        const dim3 grid_tc((unsigned)((P + CT_NPOS - 1) / CT_NPOS), (unsigned)n_groups, (unsigned)B);
+        if (e->conv_tc && e->fp16) {
+            rl_conv17_fp16_kernel<<<grid_tc, 256, CT_SMEM<true>, s>>>(d_x, d_mask, c1, c17, (const uint8_t *)e->c17_tc, P,
+                                                                         (int)D, (int)F, e->use_dwells, dgroup, d_part);
+        } else if (e->conv_tc) {
+            rl_conv17_tc_kernel<<<grid_tc, 256, CT_SMEM<false>, s>>>(d_x, d_mask, c1, c17, (const uint8_t *)e->c17_tc, P,
+                                                                           (int)D, (int)F, e->use_dwells, dgroup, d_part);
         } else {
             rl_embed_conv1_kernel<<<dim3((unsigned)((P + 31) / 32), (unsigned)(B * D)), RL_C, 0, s>>>(d_x, d_mask, c1, P, (int)D, (int)F,
                                                                                                  e->use_dwells, d_y1);
@@ -1306,6 +1380,37 @@ int rl_conv(mdk_rl_engine *e, const int8_t *x, int64_t n, int64_t P, int64_t D, 
     return MDK_OK;
 }
 
+// The LSTM input projection at lstm_size 384 and the recurrence of one layer on the tensor cores, in the fp16 mode's
+// one-product form (FP16) or the three-product default
+template <bool FP16>
+cudaError_t rl_proj_tc(const float *in, const RlLstmLayer &L, float *gi, int64_t BP, int K, int N, cudaStream_t s) {
+    const auto kernel = FP16 ? rl_proj_fp16_kernel : rl_proj_tc_kernel;
+    const cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PJ_SMEM);
+    if (err != cudaSuccess) return err;
+    kernel<<<dim3((unsigned)((BP + PJ_N - 1) / PJ_N), N / PJ_M), 256, PJ_SMEM, s>>>(
+        in, (const uint8_t *)L.w_ih_tc, L.bias, gi, BP, K, N);
+    return cudaGetLastError();
+}
+
+template <bool FP16>
+cudaError_t rl_rec_tc(bool h384, const float *gi, const RlLstmLayer &L, float *out, int64_t B, int64_t P, cudaStream_t s) {
+    cudaError_t err;
+    if (h384) {
+        const auto kernel = FP16 ? rl_lstm384_fp16_kernel : rl_lstm384_tc_kernel;
+        err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L3_SMEM<FP16>);
+        if (err != cudaSuccess) return err;
+        kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N * L3_CL), 2), L3_THREADS, L3_SMEM<FP16>, s>>>(
+            gi, L.w_hi, (const uint8_t *)L.w_lo, out, B, P);
+    } else {
+        const auto kernel = FP16 ? rl_lstm_fp16_kernel : rl_lstm_tc_kernel;
+        err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LT_SMEM<FP16>);
+        if (err != cudaSuccess) return err;
+        kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N), 2), LT_THREADS, LT_SMEM<FP16>, s>>>(
+            gi, L.w_hi, (const uint8_t *)L.w_lo, out, B, P);
+    }
+    return cudaGetLastError();
+}
+
 // Run the sealed group: the projections, both recurrences and the head over all of its windows on the compute stream,
 // then each call's probabilities (and labels) from the group buffers to its own buffers on copy_out.
 int rl_run_group(mdk_rl_engine *e) {
@@ -1323,20 +1428,14 @@ int rl_run_group(mdk_rl_engine *e) {
         const RlLstmLayer &L = e->lstm[l];
         const int in = l == 0 ? e->H : 2 * e->H;
         if (h384 && e->lstm_tc) {
-            MDK_CUDA(cudaFuncSetAttribute(rl_proj_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PJ_SMEM));
-            rl_proj_tc_kernel<<<dim3((unsigned)((BP + PJ_N - 1) / PJ_N), G8 / PJ_M), 256, PJ_SMEM, s>>>(
-                layer_in, (const uint8_t *)L.w_ih_tc, L.bias, d_gi, BP, in, G8);
+            MDK_CUDA(e->fp16 ? rl_proj_tc<true>(layer_in, L, d_gi, BP, in, G8, s) : rl_proj_tc<false>(layer_in, L, d_gi, BP, in, G8, s));
         } else {
             MDK_CUDA(launch_gemm_fp32(layer_in, L.w_ih, L.bias, d_gi, BP, in, G8, s));
         }
         rl_mark(e, 2 + 2 * l);
-        if (h384 && e->lstm_tc) {
-            rl_lstm384_tc_kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N * L3_CL), 2), L3_THREADS, L3_SMEM, s>>>(
-                d_gi, L.w_hi, (const uint8_t *)L.w_lo, layer_out[l], B, P);
-        } else if (e->lstm_tc) {
-            MDK_CUDA(cudaFuncSetAttribute(rl_lstm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LT_SMEM));
-            rl_lstm_tc_kernel<<<dim3((unsigned)((B + LT_N - 1) / LT_N), 2), LT_THREADS, LT_SMEM, s>>>(
-                d_gi, L.w_hi, (const uint8_t *)L.w_lo, layer_out[l], B, P);
+        if (e->lstm_tc) {
+            MDK_CUDA(e->fp16 ? rl_rec_tc<true>(h384, d_gi, L, layer_out[l], B, P, s)
+                             : rl_rec_tc<false>(h384, d_gi, L, layer_out[l], B, P, s));
         } else if (h384) {
             rl_lstm_fp32<RL_H3, false><<<grid_fp32, RL_H3, 0, s>>>(d_gi, L.w_t, layer_out[l], B, P, nullptr);
         } else {
@@ -1480,8 +1579,16 @@ int mdk_rl_load(mdk_rl_engine *e, const char *name, const float *data, int64_t n
 
 int mdk_rl_set_conv(mdk_rl_engine *e, int tensor_cores) {
     MDK_REQUIRE(e, MDK_ERR_ARG, "rl_set_conv: engine is NULL");
-    e->conv_tc = (tensor_cores & 1) ? 1 : 0;
-    e->lstm_tc = (tensor_cores & 2) ? 1 : 0;
+    const int conv_tc = (tensor_cores & 1) ? 1 : 0, lstm_tc = (tensor_cores & 2) ? 1 : 0, fp16 = (tensor_cores & 4) ? 1 : 0;
+    if (conv_tc != e->conv_tc || lstm_tc != e->lstm_tc || fp16 != e->fp16) {
+        // the open group's convolutions ran in the old mode: its LSTM and head run in that mode too
+        MDK_CUDA(cudaSetDevice(e->device));
+        const int rc = rl_launch(e);
+        if (rc) return rc;
+    }
+    e->conv_tc = conv_tc;
+    e->lstm_tc = lstm_tc;
+    e->fp16 = fp16;
     return MDK_OK;
 }
 

@@ -52,11 +52,23 @@ class LatentSpaceLSTM(object):
         return self
 
     def set_conv(self, tensor_cores=True, lstm_tensor_cores=None):
-        """k = 17 convolution / LSTM recurrences on the tensor cores (default) or on the fp32 CUDA cores (validation)."""
+        """k = 17 convolution / LSTM recurrences on the tensor cores (default, three fp16 products per contraction) or on
+        the fp32 CUDA cores (validation)."""
         if lstm_tensor_cores is None:
             lstm_tensor_cores = tensor_cores
         _lm.check(_lm.lib.mdk_rl_set_conv(self._engine, (1 if tensor_cores else 0) | (2 if lstm_tensor_cores else 0)))
         self._fp32_conv = not tensor_cores
+
+    PRECISIONS = {"tc": 3, "fp16": 7, "fp32": 0}      # mdk_rl_set_conv's bits
+
+    def set_precision(self, mode):
+        """'tc' (default: wgmma, three fp16 products per contraction, fp32-faithful), 'fp16' (wgmma, one product hi.hi
+        per contraction: what medaka runs on a GPU without --full_precision) or 'fp32' (the CUDA-core twins).  The mode
+        travels with the model to every entry point; windows submitted before a change run in the old mode."""
+        if mode not in self.PRECISIONS:
+            raise ValueError("precision must be one of %s, got %r" % (", ".join(self.PRECISIONS), mode))
+        _lm.check(_lm.lib.mdk_rl_set_conv(self._engine, self.PRECISIONS[mode]))
+        self._fp32_conv = mode == "fp32"
 
     STAGES = ("convolution", "projection_0", "recurrence_0", "projection_1", "recurrence_1", "head")
 

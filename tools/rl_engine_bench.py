@@ -2,7 +2,7 @@
 """Read-level network on reference-shaped traffic: packed asynchronous calls against one synchronous call per batch.
 
     python tools/rl_engine_bench.py [--lstm-sizes 384,128] [--batches 8] [--batch-size 100] [--positions 10000]
-                                    [--reads 100] [--runs 2]
+                                    [--reads 100] [--runs 2] [--precision tc[,fp16]]
 
 Traffic: `batches` batches of `batch-size` windows of P positions x D featuriser-like reads with dwells (the reference's
 default batch of 100 chunks of 10 000 columns and 100 reads), the same seeded batch every time.  Two ways, alternating in
@@ -12,7 +12,9 @@ one process, `runs` times each after one warm-up batch of each:
   sync    forward_arrays: the call pattern of the earlier predict_on_batch (mdk_rl_forward calls of windows_per_call
           windows under the default max_cells / max_bytes, each running the recurrences on its own), on this engine, whose
           mdk_rl_forward is submit + wait with one group per call
-Prints one JSON line per lstm_size: positions/s of every run (host clock from the first submit to the last result in
+--precision names the engine modes (LatentSpaceLSTM.set_precision); with several, every mode is warmed up and each run
+goes through the modes in turn, both ways each.
+Prints one JSON line per lstm_size and mode: positions/s of every run (host clock from the first submit to the last result in
 host memory), the max |dprob| and the label mismatches between the two ways on the batch, and the card's name, power
 limit and max SM clock read in the same call.  Writes nothing.
 """
@@ -79,7 +81,11 @@ def main():
     ap.add_argument("--positions", type=int, default=10000)
     ap.add_argument("--reads", type=int, default=100)
     ap.add_argument("--runs", type=int, default=2)
+    ap.add_argument("--precision", default="tc", help="comma-separated modes: tc, fp16")
     args = ap.parse_args()
+    modes = args.precision.split(",")
+    if not set(modes) <= {"tc", "fp16"}:
+        raise SystemExit("--precision: tc and / or fp16")
     from medaka_b200 import libmedaka as lm
     from medaka_b200 import read_level
     from oracle import rl_oracle
@@ -89,29 +95,35 @@ def main():
     for H in (int(h) for h in args.lstm_sizes.split(",")):
         m = read_level.LatentSpaceLSTM(lstm_size=H, use_dwells=True)
         m.load_state_dict(rl_oracle.synth_rl_state_dict(0, lstm_size=H, use_dwells=True))
-        _packed(m, batch, 1, P)                          # warm-up: every kernel and buffer of both ways
-        _sync(m, batch, 1)
-        rates = {"packed": [], "sync": []}
-        firsts = {}
+        for mode in modes:                               # warm-up: every kernel and buffer of both ways
+            m.set_precision(mode)
+            _packed(m, batch, 1, P)
+            _sync(m, batch, 1)
+        rates = {mode: {"packed": [], "sync": []} for mode in modes}
+        firsts = {mode: {} for mode in modes}
         card = _card()
         for _ in range(args.runs):
-            dt, firsts["packed"] = _packed(m, batch, n, P)
-            rates["packed"].append(n * B * P / dt)
-            dt, firsts["sync"] = _sync(m, batch, n)
-            rates["sync"].append(n * B * P / dt)
+            for mode in modes:
+                m.set_precision(mode)
+                dt, firsts[mode]["packed"] = _packed(m, batch, n, P)
+                rates[mode]["packed"].append(n * B * P / dt)
+                dt, firsts[mode]["sync"] = _sync(m, batch, n)
+                rates[mode]["sync"].append(n * B * P / dt)
         card_after = _card()
-        pp, pl = firsts["packed"]
-        ps = firsts["sync"]
-        print(json.dumps({
-            "metric": "read_level_positions_per_s", "lstm_size": H, "batches": n, "batch_size": B, "positions": P,
-            "reads": D, "dwells": True, "group_windows": m.preferred_batch_size(),
-            "sync_windows_per_call": m.windows_per_call(P, D, 5),
-            "packed": [round(r) for r in rates["packed"]], "sync": [round(r) for r in rates["sync"]],
-            "speedup": round(min(rates["packed"]) / max(rates["sync"]), 3),
-            "max_abs_prob_diff": float(np.abs(pp - ps).max()),
-            "label_mismatches_packed_vs_sync_argmax": int((pl != np.argmax(ps, -1)).sum()),
-            "bit_identical": bool(np.array_equal(pp, ps)),
-            **card, "card_after": card_after}))
+        for mode in modes:
+            pp, pl = firsts[mode]["packed"]
+            ps = firsts[mode]["sync"]
+            r = rates[mode]
+            print(json.dumps({
+                "metric": "read_level_positions_per_s", "lstm_size": H, "precision": mode, "batches": n,
+                "batch_size": B, "positions": P, "reads": D, "dwells": True, "group_windows": m.preferred_batch_size(),
+                "sync_windows_per_call": m.windows_per_call(P, D, 5),
+                "packed": [round(v) for v in r["packed"]], "sync": [round(v) for v in r["sync"]],
+                "speedup": round(min(r["packed"]) / max(r["sync"]), 3),
+                "max_abs_prob_diff": float(np.abs(pp - ps).max()),
+                "label_mismatches_packed_vs_sync_argmax": int((pl != np.argmax(ps, -1)).sum()),
+                "bit_identical": bool(np.array_equal(pp, ps)),
+                **card, "card_after": card_after}))
         m.close()
 
 
