@@ -43,6 +43,13 @@ extern "C" {
 /* precision modes of the GRU gate matmuls */
 #define MDK_PREC_TC 0    /* wgmma tensor cores, fp16 hi/lo split operands (3 MMAs), fp32 accumulate */
 #define MDK_PREC_FP32 1  /* CUDA-core fp32 FFMA path: validation / --full_precision */
+#define MDK_PREC_FP16 2  /* wgmma tensor cores, one fp16 product per contraction (hi.hi), fp32 accumulate: the arithmetic
+                            medaka itself runs on a GPU without --full_precision (the model in half precision).  Rounded
+                            to fp16: W_hh and the h fed back at every step, the layer-1 projection's W_ih and its input h0,
+                            and at gru_size 128 with F <= 16 (fused layer-0 projection) W_ih0 and the features.  fp32 as
+                            on MDK_PREC_TC: the CUDA-core layer-0 projection (F > 16 at 128, every F at 256), the biases,
+                            the gate math and h state, the head.  Same kernels' bodies, tile choice and workspaces as
+                            MDK_PREC_TC; h0 keeps ~22 bits (read_activation(0) reads it as on MDK_PREC_TC). */
 
 /* how many 16-window tiles each CTA of the tensor-core recurrences runs (mdk_engine_set_rec_mode) */
 #define MDK_REC_AUTO 0      /* two whatever the batch size when F <= 16 (a group's layer-1 recurrence then runs on half the
@@ -116,7 +123,9 @@ int mdk_engine_destroy(mdk_engine *e);
 int mdk_engine_load_gru(mdk_engine *e, int layer, int direction, const float *w_ih,
                         const float *w_hh, const float *b_ih, const float *b_hh);
 int mdk_engine_load_linear(mdk_engine *e, const float *w, const float *b);
-/* TorchModel.half() / --full_precision (medaka/prediction.py:164-168): MDK_PREC_* */
+/* TorchModel.half() / --full_precision (medaka/prediction.py:164-168): MDK_PREC_*; any other value fails with
+ * MDK_ERR_ARG.  The mode is read when a group is launched: a call that changes it launches the open group first, so no
+ * group mixes modes and windows submitted before the change run in the mode they were submitted in. */
 int mdk_engine_set_precision(mdk_engine *e, int mode);
 int mdk_engine_get_precision(mdk_engine *e, int *mode);
 /* MDK_REC_*: tiles per CTA of the recurrent kernels (A/B measurements; AUTO is the default).  At gru_size 256 the

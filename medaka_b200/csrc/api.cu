@@ -204,7 +204,7 @@ static int run_forward256(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int
     if ((rc = ensure_h1(ws, H2_256))) return rc;
     const int64_t P = B * T;
     cudaStream_t s = ws.stream, s1 = ws.l1_stream;
-    const bool tc = e->precision == MDK_PREC_TC;
+    const bool tc = e->precision != MDK_PREC_FP32, fp16 = e->precision == MDK_PREC_FP16;
     const LayerWeights &l0 = e->layer[0], &l1 = e->layer[1];
     float *h0 = static_cast<float *>(ws.h0);
     MDK_CUDA(cudaStreamWaitEvent(s, ws.l1_done, 0));
@@ -212,14 +212,14 @@ static int run_forward256(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int
     MDK_CUDA(launch_inproj0(feats_dev, l0.w_in_packed, l0.bias_gi, ws.gi, P, e->desc.num_features,
                             T, tc ? 1 : 0, s, H256));
     MDK_CUDA(cudaEventRecord(e->ev[2], s));
-    if (tc) MDK_CUDA(launch_rec256_tc(ws.gi, l0.w_hh_tm, l0.b_hn_tc, h0, B, T, s));
+    if (tc) MDK_CUDA(launch_rec256_tc(ws.gi, l0.w_hh_tm, l0.b_hn_tc, h0, B, T, fp16, s));
     else MDK_CUDA(launch_rec_fp32(ws.gi, l0.w_hh_t, l0.b_hn, h0, B, T, s, H256));
     MDK_CUDA(cudaEventRecord(e->ev[3], s));
-    if (tc) MDK_CUDA(launch_gemm256_tc(h0, l1.w_in_tc, l1.bias_gi_tc, ws.gi, tiled_rows(B, T), s));
+    if (tc) MDK_CUDA(launch_gemm256_tc(h0, l1.w_in_tc, l1.bias_gi_tc, ws.gi, tiled_rows(B, T), fp16, s));
     else MDK_CUDA(launch_gemm_fp32(h0, l1.w_in_packed, l1.bias_gi, ws.gi, P, H2_256, GI256_COLS, s));
     MDK_CUDA(cudaEventRecord(e->ev[4], s));
     MDK_CUDA(cudaStreamWaitEvent(s1, e->ev[4], 0));
-    if (tc) MDK_CUDA(launch_rec256_tc(ws.gi, l1.w_hh_tm, l1.b_hn_tc, ws.h1, B, T, s1));
+    if (tc) MDK_CUDA(launch_rec256_tc(ws.gi, l1.w_hh_tm, l1.b_hn_tc, ws.h1, B, T, fp16, s1));
     else MDK_CUDA(launch_rec_fp32(ws.gi, l1.w_hh_t, l1.b_hn, ws.h1, B, T, s1, H256));
     MDK_CUDA(cudaEventRecord(e->ev[5], s1));
     MDK_CUDA(cudaEventRecord(ws.l1_done, s1));
@@ -247,7 +247,8 @@ static int run_forward(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int64_
         return run_forward256(e, ws, feats_dev, B, T, probs_dev, logits_dev, labels_dev, quals_dev, var);
     const int64_t P = B * T;
     cudaStream_t s = ws.stream, s1 = ws.l1_stream;
-    const bool tc = e->precision == MDK_PREC_TC;
+    // tc: the tensor-core kernels, in the fp16 mode's one-product form or the three-product default
+    const bool tc = e->precision != MDK_PREC_FP32, fp16 = e->precision == MDK_PREC_FP16;
     int launches = 0;
     const bool fuse_x = tc && e->layer[0].w_x_tm != nullptr;     // F <= 16
     // Recurrent kernels of the tensor-core path.  With the fused layer-0 projection AUTO runs two tiles per CTA (one
@@ -276,14 +277,16 @@ static int run_forward(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int64_
     if (tc) {
         const RecX fx{feats_dev, e->layer[0].w_x_tm, e->layer[0].bias_gi_tc, e->desc.num_features};
         MDK_CUDA(launch_rec_tc(ws.gi, fuse_x ? &fx : nullptr, e->layer[0].w_hh_tm, e->layer[0].b_hn_tc, tiles_per_cta,
-                               OUT_TILES, ws.h0, nullptr, B, T, s));
+                               OUT_TILES, ws.h0, nullptr, B, T, fp16, s));
     } else {
         MDK_CUDA(launch_rec_fp32(ws.gi, e->layer[0].w_hh_t, e->layer[0].b_hn, (float *)ws.h0, B, T, s));
     }
     launches++;
     if (fuse_x) MDK_CUDA(cudaStreamWaitEvent(s, ws.l1_done, 0));
     MDK_CUDA(cudaEventRecord(e->ev[3], s));
-    if (tc) MDK_CUDA(launch_gemm_tc(ws.h0, e->layer[1].w_in_tc, e->layer[1].bias_gi_tc, ws.gi, tiled_rows(B, T), e->sm_count, s));
+    if (tc)
+        MDK_CUDA(launch_gemm_tc(ws.h0, e->layer[1].w_in_tc, e->layer[1].bias_gi_tc, ws.gi, tiled_rows(B, T), e->sm_count,
+                                fp16, s));
     else MDK_CUDA(launch_gemm_fp32((const float *)ws.h0, e->layer[1].w_in_packed, e->layer[1].bias_gi, ws.gi, P, H2, GI_COLS, s));
     launches++;
     MDK_CUDA(cudaEventRecord(e->ev[4], s));
@@ -291,7 +294,8 @@ static int run_forward(mdk_engine *e, mdk_ws &ws, const float *feats_dev, int64_
     MDK_CUDA(cudaStreamWaitEvent(s1, e->ev[4], 0));
     if (tc) {
         MDK_CUDA(launch_rec_tc(ws.gi, nullptr, e->layer[1].w_hh_tm, e->layer[1].b_hn_tc, tiles_per_cta,
-                               fuse_head ? OUT_LOGITS : OUT_ROWS, fuse_head ? (void *)ws.plog : ws.h1, e->lin_w, B, T, s1));
+                               fuse_head ? OUT_LOGITS : OUT_ROWS, fuse_head ? (void *)ws.plog : ws.h1, e->lin_w, B, T, fp16,
+                               s1));
     } else {
         MDK_CUDA(launch_rec_fp32(ws.gi, e->layer[1].w_hh_t, e->layer[1].b_hn, ws.h1, B, T, s1));
     }
@@ -614,7 +618,14 @@ int mdk_engine_load_linear(mdk_engine *e, const float *w, const float *b) {
 
 int mdk_engine_set_precision(mdk_engine *e, int mode) {
     MDK_REQUIRE(e, MDK_ERR_ARG, "engine is NULL");
-    MDK_REQUIRE(mode == MDK_PREC_TC || mode == MDK_PREC_FP32, MDK_ERR_ARG, "set_precision: unknown mode");
+    MDK_REQUIRE(mode == MDK_PREC_TC || mode == MDK_PREC_FP32 || mode == MDK_PREC_FP16, MDK_ERR_ARG,
+                "set_precision: unknown mode");
+    if (mode != e->precision) {
+        // the open group's windows were submitted in the old mode: they run in it
+        MDK_CUDA(cudaSetDevice(e->device));
+        const int rc = launch_group(e);
+        if (rc) return rc;
+    }
     e->precision = mode;
     return MDK_OK;
 }

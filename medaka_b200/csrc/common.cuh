@@ -292,7 +292,7 @@ struct mdk_lane {
 struct mdk_engine {
     int device = 0;
     mdk_model_desc desc{};
-    int precision = MDK_PREC_TC;
+    int precision = MDK_PREC_TC;  // MDK_PREC_*: read when a group is launched (set_precision launches the open one first)
     int sm_count = 132;
     int rec_mode = MDK_REC_AUTO;  // tiles per CTA of the tensor-core recurrences (MDK_REC_*)
     int64_t wave256 = 0;          // gru_size 256: windows of one wave of the cluster recurrence (16 per 2 clusters)
@@ -362,8 +362,9 @@ struct RecX {               // fused layer-0 input projection (rec_tc_kernel FUS
 enum { OUT_TILES = 0, OUT_ROWS = 1, OUT_LOGITS = 2 };
 // one layer's recurrence, both directions, tiles_per_cta (1 or 2) 16-window tiles per CTA.  xin: the fused layer-0 input
 // projection (OUT_TILES only), or nullptr to read the pre-activations from gi.  out: h0 tiles, h1 rows or plog (out_kind).
+// fp16: the fp16 mode's kernels (one product per contraction, rec_fp16_kernel), else the three-product ones.
 cudaError_t launch_rec_tc(const float *gi, const RecX *xin, const __half *w_hh_tm, const float *b_hn, int tiles_per_cta,
-                          int out_kind, void *out, const float *lin_w, int64_t B, int64_t T, cudaStream_t s);
+                          int out_kind, void *out, const float *lin_w, int64_t B, int64_t T, bool fp16, cudaStream_t s);
 // head on the partial logits of the fused path: sum of the two directions + bias -> softmax / argmax (/ quals / var,
 // as launch_head)
 cudaError_t launch_head_plog(const float *plog, const float *lin_b, int64_t B, int64_t T, float *probs, float *logits,
@@ -371,16 +372,16 @@ cudaError_t launch_head_plog(const float *plog, const float *lin_b, int64_t B, i
                              const HeadVariant *var = nullptr);
 constexpr int PLOG_TS_FLOATS = NCLS * WT;     // 80 floats per (tile-step, direction)
 cudaError_t launch_gemm_tc(const void *x_tiles, const __half *w_in_tm, const float *bias, float *gi, int64_t P,
-                           int sm_count, cudaStream_t s);
+                           int sm_count, bool fp16, cudaStream_t s);
 int selftest_umma(int device, const float *A, const float *B, float *D, int N, int K, int variant);
 // gru256.cu: the tensor-core path at gru_size 256.  gi [tiled rows][1536] and h [tiled rows][512] fp32 (gru256.cu).
-// One layer's recurrence, both directions, one 4-CTA cluster per (16-window tile, direction):
+// One layer's recurrence, both directions, one 4-CTA cluster per (16-window tile, direction); fp16 as launch_rec_tc's:
 cudaError_t launch_rec256_tc(const float *gi, const __half *w_hh_tm, const float *b_hn, float *h_out, int64_t B,
-                             int64_t T, cudaStream_t s);
+                             int64_t T, bool fp16, cudaStream_t s);
 // clusters of the recurrence that are resident at once (one wave)
 cudaError_t rec256_max_clusters(int *clusters);
 // layer-1 input projection over M tiled rows (w_in_tm: LayerWeights::w_in_tc at 256)
-cudaError_t launch_gemm256_tc(const float *h0, const __half *w_in_tm, const float *bias, float *gi, int64_t M,
+cudaError_t launch_gemm256_tc(const float *h0, const __half *w_in_tm, const float *bias, float *gi, int64_t M, bool fp16,
                               cudaStream_t s);
 // pileup.cu
 // exclusive scan of n per-block counts, in place, by one block: counts[i] = sum of counts[0, i), counts[n] = the total

@@ -5,6 +5,8 @@
 //   gi [rows][1536]  columns dir * 768 + gate * 256 + j
 //   h  [rows][512]   columns dir * 256 + j (h0, read by the projection; h1, read by the head)
 // The layer-0 input projection and the head are the width-templated kernels of misc.cu.
+// MDK_PREC_FP16: rec256_fp16_kernel and gemm256_fp16_kernel, the FP16 = true forms of the same bodies, take one product
+// per contraction, hi.hi (operands rounded to the nearest fp16, fp32 accumulation).
 #include "common.cuh"
 #include "ptx.cuh"
 
@@ -40,6 +42,8 @@ __device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], uint32_t smem_addr
 // into the next h buffer of all 4 CTAs with st.shared::cluster, and as fp32 into the output rows.  One cluster barrier
 // (release / acquire) per step then publishes the buffer; it also orders the step's exchange reads before the next
 // step's writes, and the one after the last step keeps every CTA alive until no peer writes into its shared memory.
+// FP16 (rec256_fp16_kernel): one product, W_hi.h_hi, 32 MMAs per warp-step; no W lo block in shared memory, and only h's
+// hi half goes to the peers.  h still leaves the kernel as fp32 rows.
 constexpr int R2_CL = 4;                        // CTAs per cluster
 constexpr int R2_UNITS = H256 / R2_CL;          // 64 hidden units per CTA
 constexpr int R2_ROWS = 3 * R2_UNITS;           // 192 gate rows per CTA
@@ -50,15 +54,17 @@ constexpr int R2_XS = WT + 8;                   // row stride of the gate exchan
 constexpr int R2_WLO_BYTES = R2_ROWS * R2_KP * 2;           // 99 KiB
 constexpr int R2_HPLANE = WT * R2_KP;                       // halfs of one h plane (hi or lo)
 constexpr int R2_HBUF_BYTES = 2 * 2 * R2_HPLANE * 2;        // [buffer][hi | lo], 33 KiB
-constexpr int R2_SMEM = R2_WLO_BYTES + R2_HBUF_BYTES + R2_ROWS * R2_XS * 4;   // 150 KiB (18 KiB exchange)
+template <bool FP16> constexpr int R2_WLO = FP16 ? 0 : R2_WLO_BYTES;
+template <bool FP16>
+constexpr int R2_SMEM = R2_WLO<FP16> + R2_HBUF_BYTES + R2_ROWS * R2_XS * 4;   // 150 KiB (18 KiB exchange; FP16: 51 KiB)
 
-__global__ void __cluster_dims__(R2_CL, 1, 1) __launch_bounds__(R2_THREADS, 1)
-    rec256_tc_kernel(const float *__restrict__ gi, const __half *__restrict__ w_hh_tm, const float *__restrict__ b_hn,
-                     float *__restrict__ h_out, int64_t T) {
+template <bool FP16>
+__device__ __forceinline__ void rec256_body(const float *__restrict__ gi, const __half *__restrict__ w_hh_tm,
+                                            const float *__restrict__ b_hn, float *__restrict__ h_out, int64_t T) {
     extern __shared__ __align__(16) uint8_t smem[];
     __half *wlo = reinterpret_cast<__half *>(smem);
-    __half *hbuf = reinterpret_cast<__half *>(smem + R2_WLO_BYTES);     // [buf][part][window][R2_KP]
-    float *xch = reinterpret_cast<float *>(smem + R2_WLO_BYTES + R2_HBUF_BYTES);   // [gate row][R2_XS]
+    __half *hbuf = reinterpret_cast<__half *>(smem + R2_WLO<FP16>);     // [buf][part][window][R2_KP]
+    float *xch = reinterpret_cast<float *>(smem + R2_WLO<FP16> + R2_HBUF_BYTES);   // [gate row][R2_XS]
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t rank = cluster_ctarank();
     const int dir = blockIdx.y;
@@ -80,7 +86,7 @@ __global__ void __cluster_dims__(R2_CL, 1, 1) __launch_bounds__(R2_THREADS, 1)
             ahi[ks][3] = *reinterpret_cast<const uint32_t *>(p + 8 * H256 + 8);
         }
     }
-    for (int i = tid; i < R2_ROWS * (H256 / 8); i += R2_THREADS) {
+    for (int i = tid; i < (FP16 ? 0 : R2_ROWS * (H256 / 8)); i += R2_THREADS) {
         const int r = i / (H256 / 8), kc = (i % (H256 / 8)) * 8, g = r / R2_UNITS, u = r % R2_UNITS;
         const __half *src = w_hh_tm + (((size_t)(dir * 2 + 1) * 3 + g) * H256 + u0 + u) * H256 + kc;
         *reinterpret_cast<uint4 *>(wlo + r * R2_KP + kc) = *reinterpret_cast<const uint4 *>(src);
@@ -138,6 +144,11 @@ __global__ void __cluster_dims__(R2_CL, 1, 1) __launch_bounds__(R2_THREADS, 1)
         for (int ks = 0; ks < R2_KS; ++ks) {
             uint32_t bh[4], bl[4], alo[4];
             ldmatrix_x4(bh, hhi + ks * 32);
+            if constexpr (FP16) {
+#pragma unroll
+                for (int nt = 0; nt < 2; ++nt) mma16816(acc[nt], ahi[ks], bh[2 * nt], bh[2 * nt + 1]);
+                continue;
+            }
             ldmatrix_x4(bl, hlo + ks * 32);
             ldmatrix_x4(alo, a_lo_addr + ks * 32);
 #pragma unroll
@@ -180,7 +191,7 @@ __global__ void __cluster_dims__(R2_CL, 1, 1) __launch_bounds__(R2_THREADS, 1)
 #pragma unroll
                 for (int q = 0; q < R2_CL; ++q) {
                     st_cluster_u32(peer[q] + off, vhi);
-                    st_cluster_u32(peer[q] + off + R2_HPLANE * 2, vlo);
+                    if (!FP16) st_cluster_u32(peer[q] + off + R2_HPLANE * 2, vlo);
                 }
                 *reinterpret_cast<float2 *>(h_out + ((tile * T + t) * WT + w) * H2_256 + dir * H256 + uc) =
                     make_float2(hn[0], hn[1]);
@@ -190,13 +201,26 @@ __global__ void __cluster_dims__(R2_CL, 1, 1) __launch_bounds__(R2_THREADS, 1)
     }
 }
 
+__global__ void __cluster_dims__(R2_CL, 1, 1) __launch_bounds__(R2_THREADS, 1)
+    rec256_tc_kernel(const float *__restrict__ gi, const __half *__restrict__ w_hh_tm, const float *__restrict__ b_hn,
+                     float *__restrict__ h_out, int64_t T) {
+    rec256_body<false>(gi, w_hh_tm, b_hn, h_out, T);
+}
+__global__ void __cluster_dims__(R2_CL, 1, 1) __launch_bounds__(R2_THREADS, 1)
+    rec256_fp16_kernel(const float *__restrict__ gi, const __half *__restrict__ w_hh_tm, const float *__restrict__ b_hn,
+                       float *__restrict__ h_out, int64_t T) {
+    rec256_body<true>(gi, w_hh_tm, b_hn, h_out, T);
+}
+
+// (the three-product kernel: the fp16 one needs less shared memory and fits at least as many clusters, so one wave, and
+// with it the group size, does not depend on the precision)
 cudaError_t rec256_max_clusters(int *clusters) {
-    cudaError_t e = cudaFuncSetAttribute(rec256_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, R2_SMEM);
+    cudaError_t e = cudaFuncSetAttribute(rec256_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, R2_SMEM<false>);
     if (e != cudaSuccess) return e;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(R2_CL, NDIR);
     cfg.blockDim = dim3(R2_THREADS);
-    cfg.dynamicSmemBytes = R2_SMEM;
+    cfg.dynamicSmemBytes = R2_SMEM<false>;
     cudaLaunchAttribute attr;
     attr.id = cudaLaunchAttributeClusterDimension;
     attr.val.clusterDim.x = R2_CL;
@@ -207,14 +231,22 @@ cudaError_t rec256_max_clusters(int *clusters) {
     return cudaOccupancyMaxActiveClusters(clusters, (void *)rec256_tc_kernel, &cfg);
 }
 
-cudaError_t launch_rec256_tc(const float *gi, const __half *w_hh_tm, const float *b_hn, float *h_out, int64_t B,
-                             int64_t T, cudaStream_t s) {
-    if (B == 0 || T == 0) return cudaSuccess;
-    cudaError_t e = cudaFuncSetAttribute(rec256_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, R2_SMEM);
+template <bool FP16>
+static cudaError_t launch_rec256(const float *gi, const __half *w_hh_tm, const float *b_hn, float *h_out, int64_t B,
+                                 int64_t T, cudaStream_t s) {
+    const auto kernel = FP16 ? rec256_fp16_kernel : rec256_tc_kernel;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, R2_SMEM<FP16>);
     if (e != cudaSuccess) return e;
     const dim3 grid((unsigned)(((B + WT - 1) / WT) * R2_CL), NDIR);
-    rec256_tc_kernel<<<grid, R2_THREADS, R2_SMEM, s>>>(gi, w_hh_tm, b_hn, h_out, T);
+    kernel<<<grid, R2_THREADS, R2_SMEM<FP16>, s>>>(gi, w_hh_tm, b_hn, h_out, T);
     return cudaGetLastError();
+}
+
+cudaError_t launch_rec256_tc(const float *gi, const __half *w_hh_tm, const float *b_hn, float *h_out, int64_t B,
+                             int64_t T, bool fp16, cudaStream_t s) {
+    if (B == 0 || T == 0) return cudaSuccess;
+    return fp16 ? launch_rec256<true>(gi, w_hh_tm, b_hn, h_out, B, T, s)
+                : launch_rec256<false>(gi, w_hh_tm, b_hn, h_out, B, T, s);
 }
 
 // ---------------------------------------------------------------------------------------------- layer-1 projection
@@ -222,13 +254,14 @@ cudaError_t launch_rec256_tc(const float *gi, const __half *w_hh_tm, const float
 // At K = 512, N = 1536 the weights (3 MiB as hi / lo) do not fit the register operands of gemm_tc_kernel: 128 x 128
 // output blocks stream 32-wide K slices of both operands through shared memory.  The fp32 activations are split into hi /
 // lo as they are staged.  8 warps, 2 (M) x 4 (N), each a 64 x 32 block of 4 x 4 m16n8 tiles.
+// FP16 (gemm256_fp16_kernel): one product, x_hi.w_hi: only the hi planes are staged.
 constexpr int G2_BM = 128, G2_BN = 128, G2_BK = 32, G2_KP = G2_BK + 8;   // padded row: ldmatrix conflict-free
 
-__global__ void __launch_bounds__(256) gemm256_tc_kernel(const float *__restrict__ x, const __half *__restrict__ w_in_tm,
-                                                         const float *__restrict__ bias, float *__restrict__ gi,
-                                                         int64_t M) {
-    __shared__ __align__(16) __half sa[2][G2_BM * G2_KP];    // [hi | lo][row][k]
-    __shared__ __align__(16) __half sb[2][G2_BN * G2_KP];    // [hi | lo][col][k]
+template <bool FP16>
+__device__ __forceinline__ void gemm256_body(const float *__restrict__ x, const __half *__restrict__ w_in_tm,
+                                             const float *__restrict__ bias, float *__restrict__ gi, int64_t M) {
+    __shared__ __align__(16) __half sa[FP16 ? 1 : 2][G2_BM * G2_KP];    // [hi | lo][row][k]
+    __shared__ __align__(16) __half sb[FP16 ? 1 : 2][G2_BN * G2_KP];    // [hi | lo][col][k]
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int wm = warp >> 2, wn = warp & 3;
     const int64_t m0 = (int64_t)blockIdx.x * G2_BM;
@@ -252,7 +285,7 @@ __global__ void __launch_bounds__(256) gemm256_tc_kernel(const float *__restrict
             split_f16x2(v.x, v.y, h01, l01);
             split_f16x2(v.z, v.w, h23, l23);
             *reinterpret_cast<uint2 *>(&sa[0][r * G2_KP + kc]) = make_uint2(h01, h23);
-            *reinterpret_cast<uint2 *>(&sa[1][r * G2_KP + kc]) = make_uint2(l01, l23);
+            if constexpr (!FP16) *reinterpret_cast<uint2 *>(&sa[1][r * G2_KP + kc]) = make_uint2(l01, l23);
         }
         // weights: 128 rows x 32 k per plane = 512 uint4, 2 per thread per plane
 #pragma unroll
@@ -260,8 +293,9 @@ __global__ void __launch_bounds__(256) gemm256_tc_kernel(const float *__restrict
             const int idx = tid + 256 * i, r = idx >> 2, kc = (idx & 3) * 8;
             *reinterpret_cast<uint4 *>(&sb[0][r * G2_KP + kc]) =
                 *reinterpret_cast<const uint4 *>(whi + (size_t)r * H2_256 + k0 + kc);
-            *reinterpret_cast<uint4 *>(&sb[1][r * G2_KP + kc]) =
-                *reinterpret_cast<const uint4 *>(wlo + (size_t)r * H2_256 + k0 + kc);
+            if constexpr (!FP16)
+                *reinterpret_cast<uint4 *>(&sb[1][r * G2_KP + kc]) =
+                    *reinterpret_cast<const uint4 *>(wlo + (size_t)r * H2_256 + k0 + kc);
         }
         __syncthreads();
 #pragma unroll
@@ -270,12 +304,12 @@ __global__ void __launch_bounds__(256) gemm256_tc_kernel(const float *__restrict
 #pragma unroll
             for (int mt = 0; mt < 4; ++mt) {
                 ldmatrix_x4(ah[mt], a_addr + (uint32_t)((mt * 16 * G2_KP + ks * 16) * 2));
-                ldmatrix_x4(al[mt], a_addr + PLANE_A + (uint32_t)((mt * 16 * G2_KP + ks * 16) * 2));
+                if (!FP16) ldmatrix_x4(al[mt], a_addr + PLANE_A + (uint32_t)((mt * 16 * G2_KP + ks * 16) * 2));
             }
 #pragma unroll
             for (int np = 0; np < 2; ++np) {
                 ldmatrix_x4(bh[np], b_addr + (uint32_t)((np * 16 * G2_KP + ks * 16) * 2));
-                ldmatrix_x4(bl[np], b_addr + PLANE_B + (uint32_t)((np * 16 * G2_KP + ks * 16) * 2));
+                if (!FP16) ldmatrix_x4(bl[np], b_addr + PLANE_B + (uint32_t)((np * 16 * G2_KP + ks * 16) * 2));
             }
 #pragma unroll
             for (int mt = 0; mt < 4; ++mt)
@@ -283,6 +317,7 @@ __global__ void __launch_bounds__(256) gemm256_tc_kernel(const float *__restrict
                 for (int nt = 0; nt < 4; ++nt) {
                     const int np = nt >> 1, q = (nt & 1) * 2;
                     mma16816(acc[mt][nt], ah[mt], bh[np][q], bh[np][q + 1]);
+                    if (FP16) continue;
                     mma16816(acc[mt][nt], ah[mt], bl[np][q], bl[np][q + 1]);
                     mma16816(acc[mt][nt], al[mt], bh[np][q], bh[np][q + 1]);
                 }
@@ -306,11 +341,22 @@ __global__ void __launch_bounds__(256) gemm256_tc_kernel(const float *__restrict
     }
 }
 
-cudaError_t launch_gemm256_tc(const float *h0, const __half *w_in_tm, const float *bias, float *gi, int64_t M,
+__global__ void __launch_bounds__(256) gemm256_tc_kernel(const float *__restrict__ x, const __half *__restrict__ w_in_tm,
+                                                         const float *__restrict__ bias, float *__restrict__ gi,
+                                                         int64_t M) {
+    gemm256_body<false>(x, w_in_tm, bias, gi, M);
+}
+__global__ void __launch_bounds__(256) gemm256_fp16_kernel(const float *__restrict__ x, const __half *__restrict__ w_in_tm,
+                                                           const float *__restrict__ bias, float *__restrict__ gi,
+                                                           int64_t M) {
+    gemm256_body<true>(x, w_in_tm, bias, gi, M);
+}
+
+cudaError_t launch_gemm256_tc(const float *h0, const __half *w_in_tm, const float *bias, float *gi, int64_t M, bool fp16,
                               cudaStream_t s) {
     if (M == 0) return cudaSuccess;
     const dim3 grid((unsigned)((M + G2_BM - 1) / G2_BM), GI256_COLS / G2_BN);
-    gemm256_tc_kernel<<<grid, 256, 0, s>>>(h0, w_in_tm, bias, gi, M);
+    (fp16 ? gemm256_fp16_kernel : gemm256_tc_kernel)<<<grid, 256, 0, s>>>(h0, w_in_tm, bias, gi, M);
     return cudaGetLastError();
 }
 

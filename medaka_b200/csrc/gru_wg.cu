@@ -4,6 +4,9 @@
 // the fp32 CPU path (medaka/prediction.py:146-148).  To stay inside 1e-3 (scale-aware) of fp32 through a
 // 10 000-step recurrence, every operand is carried as an fp16 pair (hi + lo, ~22 significant bits) and each
 // product is three fp16 MMAs, hi*hi + hi*lo + lo*hi, accumulated in fp32.
+// MDK_PREC_FP16 (medaka's own GPU arithmetic, the model in half precision): rec_fp16_kernel and gemm_fp16_kernel, the
+// FP16 = true forms of the same kernel bodies, take one product per contraction, hi*hi: operands rounded to the nearest
+// fp16, fp32 accumulation.  The gate math, biases, h state and head stay fp32 as on the default path.
 //
 // Both kernels use the TRANSPOSED formulation  G^T[gate rows, N] = W[gate rows, K] . X^T[K, N]:
 //   A operand = weights (M = 64 gate rows per warpgroup, K-major = torch's native [out][in] layout)
@@ -37,6 +40,10 @@ namespace mdk {
 //           wide: 241-253 of 255).
 // At both tile counts r and z share one reciprocal (5 MUFU operations per value instead of 6), and the new h goes into
 // the tile as fp16 hi / lo pairs by stmatrix (.trans: the accumulator fragment transposed is the K-major tile's layout).
+// FP16 (rec_fp16_kernel): one product, W_hi.h_hi (and W_x,hi.x_hi); W_hh lo and W_x lo are not staged.  The h tile keeps
+// its hi and lo halves (lo rounded toward zero, split_f16x2_rz, so that h0 read back at ~22 bits rounds to the hi the
+// products used), and h0 leaves layer 0 at that precision as on the default path; at NT = 1 the RS MMA runs at N = 16 and
+// reads only the hi rows, at NT = 2 only the hi plane.  24 RS MMAs per warpgroup-step at either tile count.
 // FUSE_X (layer 0, F <= 16): the input projection W_ih . x_t is the same products per gate on an x tile laid out like
 // the h tile (K = 16), so layer 0 needs no gi buffer.  OUT: fp16 hi/lo operand tiles of the projection GEMM (layer 0:
 // copied under the next step's MMAs from the h tile buffer, which already holds them in that layout, see store_h0),
@@ -47,7 +54,7 @@ constexpr int RW_THREADS = 256;
 constexpr int RW_ABLK = (H / 8) * 64 * 16;          // W_hh lo of one (gate, warpgroup): [kg 16][row 64][8] = 16 KiB
 constexpr int RW_XBLK = 2 * 64 * 16;                // W_ih lo (K = 16) of one (gate, warpgroup): 2 KiB
 
-template <int NT, bool FUSE_X, int OUT>
+template <int NT, bool FUSE_X, int OUT, bool FP16 = false>
 struct RwCfg {
     static constexpr int N = NT * RT_N;
     static constexpr bool HL = NT == 1;             // hi and lo in one operand of 2N rows (see the kernel's header)
@@ -62,8 +69,8 @@ struct RwCfg {
     static constexpr int XLO = HL ? N * 16 : XPLANE;   // the same in the x tile
     static constexpr int RED = (RW_THREADS / 32) * NCLS * N;                     // head partials of one step (floats)
     static constexpr int wlo_off = 0;                                            // [gate 3][wg 2] RW_ABLK
-    static constexpr int wxlo_off = wlo_off + 6 * RW_ABLK;                       // [gate 3][wg 2] RW_XBLK
-    static constexpr int h_off = wxlo_off + (FUSE_X ? 6 * RW_XBLK : 0);          // [buf 2][plane PLANES] HPLANE
+    static constexpr int wxlo_off = wlo_off + (FP16 ? 0 : 6 * RW_ABLK);          // [gate 3][wg 2] RW_XBLK
+    static constexpr int h_off = wxlo_off + (FUSE_X && !FP16 ? 6 * RW_XBLK : 0); // [buf 2][plane PLANES] HPLANE
     static constexpr int x_off = h_off + 2 * PLANES * HPLANE;                    // [buf 2][plane PLANES] XPLANE
     static constexpr int red_off = x_off + (FUSE_X ? 2 * PLANES * XPLANE : 0);   // [buf 2][warp 8][class 5][N] fp32
     static constexpr int total = red_off + (OUT == OUT_LOGITS ? 2 * RED * 4 : 0);
@@ -72,16 +79,16 @@ struct RwCfg {
 
 __device__ __forceinline__ uint32_t ld_u32(const __half *p) { return *reinterpret_cast<const uint32_t *>(p); }
 
-template <int NT, bool FUSE_X, int OUT>
-__global__ void __launch_bounds__(RW_THREADS, 1)
-rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__ w_hh, const float *__restrict__ b_hn,
-              void *__restrict__ h_out, int64_t B, int64_t T, const float *__restrict__ lin_w,
-              float *__restrict__ plog) {
-    using L = RwCfg<NT, FUSE_X, OUT>;
+template <int NT, bool FUSE_X, int OUT, bool FP16>
+__device__ __forceinline__ void rec_body(const float *__restrict__ gi, RecX xin, const __half *__restrict__ w_hh,
+                                         const float *__restrict__ b_hn, void *__restrict__ h_out, int64_t B, int64_t T,
+                                         const float *__restrict__ lin_w, float *__restrict__ plog) {
+    using L = RwCfg<NT, FUSE_X, OUT, FP16>;
     constexpr int N = L::N, NA = N / 2;             // values per thread and gate (hidden unit x window)
-    constexpr int NACC = L::ROWS / 2;               // accumulator registers per gate (HL: NA more for the W_hi.h_lo columns)
+    constexpr bool HL2 = L::HL && !FP16;            // the accumulators hold the W_hi.h_lo columns too
+    constexpr int NACC = HL2 ? L::ROWS / 2 : NA;    // accumulator registers per gate (HL: NA more for the W_hi.h_lo columns)
     constexpr int NX = FUSE_X ? NACC : NA;          // axn: an accumulator only when the x projection is fused
-    using MMA = Wgmma<N>;                           // SS: W_lo . h_hi (x_hi)
+    using MMA = Wgmma<N>;                           // SS: W_lo . h_hi (x_hi); FP16: RS W_hi . h_hi (x_hi)
     using MMA_H = Wgmma<L::ROWS>;                   // RS: W_hi . the whole h (x) operand
     constexpr bool LOGITS = OUT == OUT_LOGITS;
     extern __shared__ __align__(128) uint8_t smem[];
@@ -96,12 +103,12 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
     // ---- prologue: zero the activation tiles, weights into shared memory and registers ----
     for (int i = tid; i < (L::total - L::h_off) / 16; i += RW_THREADS)
         reinterpret_cast<int4 *>(smem + L::h_off)[i] = make_int4(0, 0, 0, 0);
-    for (int i = tid; i < 3 * H * (H / 8); i += RW_THREADS) {
+    for (int i = tid; i < (FP16 ? 0 : 3 * H * (H / 8)); i += RW_THREADS) {
         const int kg = i & 15, r = (i >> 4) & (H - 1), gate = i >> 11;
         const uint4 v = *reinterpret_cast<const uint4 *>(w_hh + ((((size_t)dir * 2 + 1) * 3 + gate) * H + r) * H + kg * 8);
         *reinterpret_cast<uint4 *>(smem + L::wlo_off + (gate * 2 + (r >> 6)) * RW_ABLK + kg * 1024 + (r & 63) * 16) = v;
     }
-    if (FUSE_X) {
+    if (FUSE_X && !FP16) {
         for (int i = tid; i < 3 * H * 2; i += RW_THREADS) {
             const int kg = i & 1, r = (i >> 1) & (H - 1), gate = i >> 8;
             const uint4 v = *reinterpret_cast<const uint4 *>(xin.w_x + ((((size_t)dir * 2 + 1) * 3 + gate) * H + r) * 16 + kg * 8);
@@ -176,7 +183,7 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
                 axn[k] = v[2].x; axn[k + 1] = v[2].y;
                 an[k] = bhn[hb]; an[k + 1] = bhn[hb];
             }
-        if constexpr (L::HL) {
+        if constexpr (HL2) {
 #pragma unroll
             for (int k = NA; k < NACC; ++k) {
                 ar[k] = 0.f; az[k] = 0.f; an[k] = 0.f;
@@ -202,7 +209,7 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
         __half hi, lo;
         split_f16(v, hi, lo);
         *reinterpret_cast<__half *>(smem + L::x_off + buf * L::PLANES * L::XPLANE + xoff[m]) = hi;
-        *reinterpret_cast<__half *>(smem + L::x_off + buf * L::PLANES * L::XPLANE + L::XLO + xoff[m]) = lo;
+        if (!FP16) *reinterpret_cast<__half *>(smem + L::x_off + buf * L::PLANES * L::XPLANE + L::XLO + xoff[m]) = lo;
     };
     const int64_t t_first = dir ? T - 1 : 0;
     if (FUSE_X) {
@@ -300,7 +307,14 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
         wg_fence();
         // k-step outer, gate inner: consecutive MMAs go to different accumulators, so none waits for the one before it
         // (each accumulator still sums its products in the order k-step, then hi.hi, hi.lo, lo.hi)
-        if constexpr (L::HL) {
+        if constexpr (FP16) {
+#pragma unroll
+            for (int ks = 0; ks < H / 16; ++ks) {
+                const uint64_t bh = make_smem_desc(hb_addr + ks * 2 * L::KG, L::KG, 128);
+#pragma unroll
+                for (int gate = 0; gate < 3; ++gate) MMA::rs(gate == 0 ? ar : (gate == 1 ? az : an), whi[gate][ks], bh, 1u);
+            }
+        } else if constexpr (L::HL) {
 #pragma unroll
             for (int ks = 0; ks < H / 16; ++ks) {
                 const uint64_t bh = make_smem_desc(hb_addr + ks * 2 * L::KG, L::KG, 128);
@@ -329,7 +343,10 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
         if constexpr (FUSE_X) {
             const uint32_t xa = sbase + L::x_off + buf * L::PLANES * L::XPLANE;
             const uint64_t bh = make_smem_desc(xa, L::KG, 128);
-            if constexpr (L::HL) {
+            if constexpr (FP16) {
+#pragma unroll
+                for (int gate = 0; gate < 3; ++gate) MMA::rs(gate == 0 ? ar : (gate == 1 ? az : axn), wxhi[gate], bh, 1u);
+            } else if constexpr (L::HL) {
 #pragma unroll
                 for (int gate = 0; gate < 3; ++gate) MMA_H::rs(gate == 0 ? ar : (gate == 1 ? az : axn), wxhi[gate], bh, 1u);
 #pragma unroll
@@ -383,7 +400,7 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
 #pragma unroll
         for (int k = 0; k < NA; ++k) {
             float pr = ar[k], pz = az[k], pn = an[k], px = axn[k];
-            if constexpr (L::HL) {
+            if constexpr (HL2) {
                 pr += ar[k + NA]; pz += az[k + NA]; pn += an[k + NA];
                 if constexpr (FUSE_X) px += axn[k + NA];
             }
@@ -403,7 +420,10 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
         for (int i = 0; i < N / 8; ++i) {
             uint32_t hi[2], lo[2];
 #pragma unroll
-            for (int hb = 0; hb < 2; ++hb) split_f16x2(hp[4 * i + 2 * hb], hp[4 * i + 2 * hb + 1], hi[hb], lo[hb]);
+            for (int hb = 0; hb < 2; ++hb) {
+                if constexpr (FP16) split_f16x2_rz(hp[4 * i + 2 * hb], hp[4 * i + 2 * hb + 1], hi[hb], lo[hb]);
+                else split_f16x2(hp[4 * i + 2 * hb], hp[4 * i + 2 * hb + 1], hi[hb], lo[hb]);
+            }
             stmatrix_x4_trans(hst_addr + (buf ^ 1) * L::PLANES * L::HPLANE + i * 128, hi[0], hi[1], lo[0], lo[1]);
         }
         if (FUSE_X && step + 1 < T) {
@@ -438,11 +458,26 @@ rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__
     }
 }
 
-template <int NT, bool FX, int OUT>
+template <int NT, bool FUSE_X, int OUT>
+__global__ void __launch_bounds__(RW_THREADS, 1)
+rec_tc_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__ w_hh, const float *__restrict__ b_hn,
+              void *__restrict__ h_out, int64_t B, int64_t T, const float *__restrict__ lin_w,
+              float *__restrict__ plog) {
+    rec_body<NT, FUSE_X, OUT, false>(gi, xin, w_hh, b_hn, h_out, B, T, lin_w, plog);
+}
+template <int NT, bool FUSE_X, int OUT>
+__global__ void __launch_bounds__(RW_THREADS, 1)
+rec_fp16_kernel(const float *__restrict__ gi, RecX xin, const __half *__restrict__ w_hh, const float *__restrict__ b_hn,
+                void *__restrict__ h_out, int64_t B, int64_t T, const float *__restrict__ lin_w,
+                float *__restrict__ plog) {
+    rec_body<NT, FUSE_X, OUT, true>(gi, xin, w_hh, b_hn, h_out, B, T, lin_w, plog);
+}
+
+template <int NT, bool FX, int OUT, bool FP16>
 static cudaError_t launch_rec(const float *gi, const RecX &xin, const __half *w_hh_tm, const float *b_hn, void *out,
                               const float *lin_w, int64_t B, int64_t T, cudaStream_t s) {
-    auto kern = rec_tc_kernel<NT, FX, OUT>;
-    constexpr int smem_bytes = RwCfg<NT, FX, OUT>::total;
+    auto kern = FP16 ? rec_fp16_kernel<NT, FX, OUT> : rec_tc_kernel<NT, FX, OUT>;
+    constexpr int smem_bytes = RwCfg<NT, FX, OUT, FP16>::total;
     // (the attribute is per device: set it on every launch, a process may drive several GPUs)
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
     if (e != cudaSuccess) return e;
@@ -454,28 +489,31 @@ static cudaError_t launch_rec(const float *gi, const RecX &xin, const __half *w_
     return cudaGetLastError();
 }
 
-template <int NT>
+template <int NT, bool FP16>
 static cudaError_t launch_rec_nt(const float *gi, const RecX *xin, const __half *w_hh_tm, const float *b_hn, int out_kind,
                                  void *out, const float *lin_w, int64_t B, int64_t T, cudaStream_t s) {
     if (xin)    // the fused projection is layer 0, which feeds the GEMM
-        return out_kind == OUT_TILES ? launch_rec<NT, true, OUT_TILES>(gi, *xin, w_hh_tm, b_hn, out, nullptr, B, T, s)
+        return out_kind == OUT_TILES ? launch_rec<NT, true, OUT_TILES, FP16>(gi, *xin, w_hh_tm, b_hn, out, nullptr, B, T, s)
                                      : cudaErrorInvalidValue;
     const RecX none{nullptr, nullptr, nullptr, 0};
     switch (out_kind) {
-    case OUT_TILES: return launch_rec<NT, false, OUT_TILES>(gi, none, w_hh_tm, b_hn, out, nullptr, B, T, s);
-    case OUT_ROWS: return launch_rec<NT, false, OUT_ROWS>(gi, none, w_hh_tm, b_hn, out, nullptr, B, T, s);
+    case OUT_TILES: return launch_rec<NT, false, OUT_TILES, FP16>(gi, none, w_hh_tm, b_hn, out, nullptr, B, T, s);
+    case OUT_ROWS: return launch_rec<NT, false, OUT_ROWS, FP16>(gi, none, w_hh_tm, b_hn, out, nullptr, B, T, s);
     case OUT_LOGITS:
-        return lin_w ? launch_rec<NT, false, OUT_LOGITS>(gi, none, w_hh_tm, b_hn, out, lin_w, B, T, s) : cudaErrorInvalidValue;
+        return lin_w ? launch_rec<NT, false, OUT_LOGITS, FP16>(gi, none, w_hh_tm, b_hn, out, lin_w, B, T, s)
+                     : cudaErrorInvalidValue;
     }
     return cudaErrorInvalidValue;
 }
 
 cudaError_t launch_rec_tc(const float *gi, const RecX *xin, const __half *w_hh_tm, const float *b_hn, int tiles_per_cta,
-                          int out_kind, void *out, const float *lin_w, int64_t B, int64_t T, cudaStream_t s) {
+                          int out_kind, void *out, const float *lin_w, int64_t B, int64_t T, bool fp16, cudaStream_t s) {
     if (B == 0 || T == 0) return cudaSuccess;
-    switch (tiles_per_cta) {
-    case 1: return launch_rec_nt<1>(gi, xin, w_hh_tm, b_hn, out_kind, out, lin_w, B, T, s);
-    case 2: return launch_rec_nt<2>(gi, xin, w_hh_tm, b_hn, out_kind, out, lin_w, B, T, s);
+    switch (tiles_per_cta * 2 + (fp16 ? 1 : 0)) {
+    case 2: return launch_rec_nt<1, false>(gi, xin, w_hh_tm, b_hn, out_kind, out, lin_w, B, T, s);
+    case 3: return launch_rec_nt<1, true>(gi, xin, w_hh_tm, b_hn, out_kind, out, lin_w, B, T, s);
+    case 4: return launch_rec_nt<2, false>(gi, xin, w_hh_tm, b_hn, out_kind, out, lin_w, B, T, s);
+    case 5: return launch_rec_nt<2, true>(gi, xin, w_hh_tm, b_hn, out_kind, out, lin_w, B, T, s);
     }
     return cudaErrorInvalidValue;
 }
@@ -495,6 +533,8 @@ cudaError_t launch_rec_tc(const float *gi, const RecX *xin, const __half *w_hh_t
 // it out with one bulk store per lane (one window quad of one tile-step, 2 KiB contiguous in gi) while the next tile's
 // MMAs run.
 // Per element the sum runs in the order slice q, product (hi.hi, hi.lo, lo.hi), k-step.
+// FP16 (gemm_fp16_kernel): one product, W_in,hi . h0_hi: only the W hi fragments go to registers and the ring brings only
+// the hi plane of each slice (the h0 tiles keep both planes, read_activation(0) unpacks them).
 // =====================================================================================================
 constexpr int GW_THREADS = 256;
 constexpr int GW_QK = 8;                                        // k-groups per stage (K = 64)
@@ -513,9 +553,11 @@ constexpr int GW_SMEM = GW_BAR_OFF + 2 * GW_NQ * 8;
 static_assert(GW_SMEM <= 227 * 1024, "smem budget");
 static_assert(GW_TS * 4 == 32, "one bulk store per lane of warp 0");
 
-__global__ void __launch_bounds__(GW_THREADS, 1)
-gemm_tc_kernel(const uint8_t *__restrict__ x_tiles, const __half *__restrict__ w_in_tm, const float *__restrict__ bias,
-               float *__restrict__ gi, int64_t P, int64_t ntiles) {
+template <bool FP16>
+__device__ __forceinline__ void gemm_body(const uint8_t *__restrict__ x_tiles, const __half *__restrict__ w_in_tm,
+                                          const float *__restrict__ bias, float *__restrict__ gi, int64_t P,
+                                          int64_t ntiles) {
+    constexpr int WPLANES = FP16 ? 1 : 2, NPROD = FP16 ? 1 : 3;
     extern __shared__ __align__(128) uint8_t smem[];
     uint64_t *full = reinterpret_cast<uint64_t *>(smem + GW_BAR_OFF), *empty = full + GW_NQ;
     float *stg = reinterpret_cast<float *>(smem + GW_OUT_OFF);
@@ -527,9 +569,9 @@ gemm_tc_kernel(const uint8_t *__restrict__ x_tiles, const __half *__restrict__ w
     const int64_t my_tiles = blockIdx.y < ntiles ? (ntiles - 1 - blockIdx.y) / gridDim.y + 1 : 0;
     auto issue = [&](int64_t n, int q) {        // slice q of this CTA's n-th tile -> stage q
         const uint8_t *src = x_tiles + (blockIdx.y + n * gridDim.y) * (int64_t)XT_TILE_BYTES + q * GW_STAGE_PLANE;
-        mbar_arrive_expect_tx(&full[q], GW_STAGE);
+        mbar_arrive_expect_tx(&full[q], WPLANES * GW_STAGE_PLANE);
         bulk_g2s(smem + q * GW_STAGE, src, GW_STAGE_PLANE, &full[q]);
-        bulk_g2s(smem + q * GW_STAGE + GW_STAGE_PLANE, src + XT_PLANE_BYTES, GW_STAGE_PLANE, &full[q]);
+        if (!FP16) bulk_g2s(smem + q * GW_STAGE + GW_STAGE_PLANE, src + XT_PLANE_BYTES, GW_STAGE_PLANE, &full[q]);
     };
     if (tid == 0) {
         for (int q = 0; q < GW_NQ; ++q) {
@@ -541,9 +583,9 @@ gemm_tc_kernel(const uint8_t *__restrict__ x_tiles, const __half *__restrict__ w
             for (int q = 0; q < GW_NQ; ++q) issue(0, q);
     }
     // W (row-major fp16 [blk][plane][row j][k 256]) hi and lo A fragments of rows j0, j0 + 8 (layout: ptx.cuh Wgmma)
-    uint32_t wa[2][GW_KS][4];
+    uint32_t wa[WPLANES][GW_KS][4];
 #pragma unroll
-    for (int p = 0; p < 2; ++p)
+    for (int p = 0; p < WPLANES; ++p)
 #pragma unroll
         for (int ks = 0; ks < GW_KS; ++ks) {
             const __half *w = w_in_tm + (((size_t)blk * 2 + p) * H + j0) * H2 + ks * 16 + 2 * cq;
@@ -572,7 +614,7 @@ gemm_tc_kernel(const uint8_t *__restrict__ x_tiles, const __half *__restrict__ w
             mbar_wait(&full[q], (uint32_t)(n & 1));
             wg_fence();
 #pragma unroll
-            for (int prod = 0; prod < 3; ++prod) {
+            for (int prod = 0; prod < NPROD; ++prod) {
                 const int pa = prod == 2, pb = prod == 1;   // W part hi, hi, lo ; x part hi, lo, hi
 #pragma unroll
                 for (int kk = 0; kk < GW_QK / 2; ++kk) {
@@ -616,17 +658,29 @@ gemm_tc_kernel(const uint8_t *__restrict__ x_tiles, const __half *__restrict__ w
     if (tid < 32) bulk_wait_all();
 }
 
+__global__ void __launch_bounds__(GW_THREADS, 1)
+gemm_tc_kernel(const uint8_t *__restrict__ x_tiles, const __half *__restrict__ w_in_tm, const float *__restrict__ bias,
+               float *__restrict__ gi, int64_t P, int64_t ntiles) {
+    gemm_body<false>(x_tiles, w_in_tm, bias, gi, P, ntiles);
+}
+__global__ void __launch_bounds__(GW_THREADS, 1)
+gemm_fp16_kernel(const uint8_t *__restrict__ x_tiles, const __half *__restrict__ w_in_tm, const float *__restrict__ bias,
+                 float *__restrict__ gi, int64_t P, int64_t ntiles) {
+    gemm_body<true>(x_tiles, w_in_tm, bias, gi, P, ntiles);
+}
+
 cudaError_t launch_gemm_tc(const void *x_tiles, const __half *w_in_tm, const float *bias, float *gi, int64_t P,
-                           int sm_count, cudaStream_t s) {
+                           int sm_count, bool fp16, cudaStream_t s) {
     if (P == 0) return cudaSuccess;
     const int64_t ntiles = (P + XT_ROWS - 1) / XT_ROWS;
-    cudaError_t ea = cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GW_SMEM);
+    const auto kernel = fp16 ? gemm_fp16_kernel : gemm_tc_kernel;
+    cudaError_t ea = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GW_SMEM);
     if (ea != cudaSuccess) return ea;
     int64_t ct = sm_count / 6;
     if (ct < 1) ct = 1;
     if (ct > ntiles) ct = ntiles;
     dim3 grid(6, (unsigned)ct);
-    gemm_tc_kernel<<<grid, GW_THREADS, GW_SMEM, s>>>(reinterpret_cast<const uint8_t *>(x_tiles), w_in_tm, bias, gi, P, ntiles);
+    kernel<<<grid, GW_THREADS, GW_SMEM, s>>>(reinterpret_cast<const uint8_t *>(x_tiles), w_in_tm, bias, gi, P, ntiles);
     return cudaGetLastError();
 }
 

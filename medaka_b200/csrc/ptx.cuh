@@ -270,6 +270,15 @@ __device__ __forceinline__ void split_f16x2(float v0, float v1, uint32_t &hi, ui
     hi = *reinterpret_cast<const uint32_t *>(&h);
     lo = *reinterpret_cast<const uint32_t *>(&l);
 }
+// split_f16x2's hi with lo rounded toward zero: |lo| < half an fp16 unit of hi unless v lies exactly halfway, where
+// round-to-nearest-even picks hi again, so fp16(hi + lo) == hi for every v.  The fp16 mode's h0 tiles: the products read
+// hi only, and h0 read back as hi + lo (~22 bits) rounds to the very hi they used.
+__device__ __forceinline__ void split_f16x2_rz(float v0, float v1, uint32_t &hi, uint32_t &lo) {
+    const __half2 h = __floats2half2_rn(v0, v1);
+    const __half2 l = __halves2half2(__float2half_rz(v0 - __low2float(h)), __float2half_rz(v1 - __high2float(h)));
+    hi = *reinterpret_cast<const uint32_t *>(&h);
+    lo = *reinterpret_cast<const uint32_t *>(&l);
+}
 
 // ---------------------------------------------------------------- streaming global access
 __device__ __forceinline__ float ldg_stream(const float *p) {

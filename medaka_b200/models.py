@@ -18,7 +18,8 @@ from medaka_b200 import libmedaka as _lm
 
 ForwardOutput = collections.namedtuple("ForwardOutput", ["probs", "logits", "labels"])
 
-_PRECISIONS = {"tc": 0, "half": 0, "fp32": 1, "full": 1}
+# mdk_engine_set_precision's modes (MDK_PREC_*); "half" and "full" are the names half() and float() stand for
+_PRECISIONS = {"tc": 0, "half": 0, "fp32": 1, "full": 1, "fp16": 2}
 
 
 def _as_f32(x):
@@ -142,7 +143,12 @@ class GRUModel(object):
         return self
 
     def set_precision(self, mode):
-        """'tc' (wgmma, default) or 'fp32' (CUDA-core FFMA, the --full_precision path)."""
+        """'tc' (wgmma, default: three fp16 products per contraction, fp32-faithful), 'fp16' (wgmma, one product hi.hi
+        per contraction: what medaka runs on a GPU without --full_precision) or 'fp32' (CUDA-core FFMA, the
+        --full_precision path).  half() keeps selecting 'tc'.  The mode travels with the model to every entry point;
+        windows submitted before a change run in the old mode."""
+        if mode not in _PRECISIONS:
+            raise ValueError("precision must be one of %s, got %r" % (", ".join(_PRECISIONS), mode))
         _lm.check(_lm.lib.mdk_engine_set_precision(self._engine, _PRECISIONS[mode]))
 
     def parameters(self):

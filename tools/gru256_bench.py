@@ -1,13 +1,14 @@
 #!/usr/bin/env python
 """Consensus GRU at gru_size 256 (the width `medaka train` builds by default) against 128, in one process.
 
-    python tools/gru256_bench.py [--cols 10000] [--groups 3] [--warmup 1]
+    python tools/gru256_bench.py [--cols 10000] [--groups 3] [--warmup 1] [--precision tc,fp16] [--rounds 1]
 
 For each width: a model with seeded synthetic weights (F = 10), one engine group of preferred_batch_size() windows (one
 wave of that width's recurrence) x --cols featuriser-like columns, resident on the device, run --warmup times and then
 --groups times through mdk_engine_forward_dev.  The timed region spans the groups (mdk_engine_timer_start / _stop,
 device events).  Prints one JSON line per width: positions / s, the per-stage means of mdk_engine_mean_timings over the
-timed groups, the GRU multiply-accumulates per position, and the card's name and power limit.  Writes nothing.
+timed groups, the GRU multiply-accumulates per position, and the card's name and power limit.  With several --precision
+modes (GRUModel.set_precision: tc, fp16, fp32) each width runs in each mode in turn, --rounds times over.  Writes nothing.
 """
 import argparse
 import json
@@ -31,7 +32,7 @@ def gru_macs_per_position(H, F=10):
     return 2 * (3 * H * F + 3 * H * H) + 2 * (3 * H * 2 * H + 3 * H * H)
 
 
-def run(H, feats_all, cols, groups, warmup):
+def run(H, feats_all, cols, groups, warmup, precision="tc"):
     import torch
     from medaka_b200 import libmedaka as lm, models
     from oracle import synth
@@ -39,6 +40,7 @@ def run(H, feats_all, cols, groups, warmup):
     m = models.GRUModel(num_features=10, gru_size=H)
     try:
         m.load_state_dict(synth.synth_state_dict(0, gru_size=H))
+        m.set_precision(precision)
         B = m.preferred_batch_size()
         x = torch.from_numpy(feats_all[:B]).cuda()
         probs = torch.empty((B, cols, 5), dtype=torch.float32, device="cuda")
@@ -64,7 +66,7 @@ def run(H, feats_all, cols, groups, warmup):
         stages = {k: round(float(getattr(t, k)), 3) for k in ("inproj0_ms", "rec0_ms", "inproj1_ms", "rec1_ms",
                                                                 "head_ms", "total_ms")}
         pos = groups * B * cols
-        return {"gru_size": H, "windows_per_group": B, "cols": cols, "groups": groups,
+        return {"gru_size": H, "precision": precision, "windows_per_group": B, "cols": cols, "groups": groups,
                 "positions_per_s": pos / (ms[0] / 1e3), "elapsed_ms": float(ms[0]), "stage_ms_mean": stages,
                 "gru_macs_per_position": gru_macs_per_position(H)}
     finally:
@@ -76,6 +78,8 @@ def main():
     ap.add_argument("--cols", type=int, default=10000)
     ap.add_argument("--groups", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=1)
+    ap.add_argument("--precision", default="tc", help="comma-separated engine modes, run alternately")
+    ap.add_argument("--rounds", type=int, default=1)
     args = ap.parse_args()
     import numpy as np
     from medaka_b200 import libmedaka as lm, models
@@ -86,10 +90,12 @@ def main():
     m.close()
     feats = np.ascontiguousarray(gru_oracle.featuriser_like_features(most, args.cols, 10, seed=3))
     info = card()
-    for H in (256, 128):
-        r = run(H, feats, args.cols, args.groups, args.warmup)
-        r.update(card=info["name"], power_limit_w=info["power_limit_w"], timing="device events")
-        print(json.dumps(r), flush=True)
+    for _ in range(args.rounds):
+        for H in (256, 128):
+            for mode in args.precision.split(","):
+                r = run(H, feats, args.cols, args.groups, args.warmup, mode)
+                r.update(card=info["name"], power_limit_w=info["power_limit_w"], timing="device events")
+                print(json.dumps(r), flush=True)
 
 
 if __name__ == "__main__":

@@ -1,16 +1,17 @@
 #!/usr/bin/env python
 """Recurrent kernels of the tensor-core path at one and two 16-window tiles per CTA, on a full and on a half GPU.
 
-    python tools/rec_wave_bench.py [--cols 10000] [--repeats 4]
+    python tools/rec_wave_bench.py [--cols 10000] [--repeats 4] [--precision tc,fp16]
 
 Three device-resident forwards of the same 2112 x cols / 2 positions, run alternately `--repeats` times after one
 warm-up each (seeded synthetic weights and features, F = 10):
   one  1056 windows x cols      one tile per CTA, 132 CTAs (the engine's default group)
   two  2112 windows x cols / 2  two tiles per CTA, 132 CTAs (every SM busy with the two-tile kernel)
   half 1056 windows x cols      two tiles per CTA, 66 CTAs (half of the SMs idle)
-Per forward: the layer-0 / layer-1 recurrence and projection times from the engine's stage events
-(mdk_engine_mean_timings) and the median SM clock sampled through NVML while it ran.  Prints one JSON line with the
-card, its power limit, every run and the medians.  Writes nothing.
+With several --precision modes (GRUModel.set_precision: tc, fp16, fp32) every case runs in each, alternating within a
+repeat.  Per forward: positions / s and the per-stage times from the engine's stage events (mdk_engine_mean_timings),
+and the median SM clock sampled through NVML while it ran.  Prints one JSON line with the card, its power limit, every
+run and the medians.  Writes nothing.
 """
 import argparse
 import json
@@ -69,7 +70,9 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--cols", type=int, default=10000)
     ap.add_argument("--repeats", type=int, default=4)
+    ap.add_argument("--precision", default="tc", help="comma-separated engine modes, run alternately")
     args = ap.parse_args()
+    modes = args.precision.split(",")
     from medaka_b200 import libmedaka as lm
     from medaka_b200 import models
     from oracle import synth
@@ -78,7 +81,8 @@ def main():
     sms = int(info["sm_count"])
     T = args.cols - args.cols % 2
     B1 = 8 * sms                                  # one CTA per (tile, direction) at one tile per CTA
-    cases = {"one": ("one", B1, T), "two": ("pp", 2 * B1, T // 2), "half": ("pp", B1, T)}
+    shapes = {"one": ("one", B1, T), "two": ("pp", 2 * B1, T // 2), "half": ("pp", B1, T)}
+    cases = {(k if len(modes) == 1 else "%s/%s" % (p, k)): (p,) + c for p in modes for k, c in shapes.items()}
     m = models.GRUModel(num_features=10)
     m.load_state_dict(synth.synth_state_dict(0))
     m.reserve(B1, T)
@@ -94,7 +98,10 @@ def main():
     tm = ffi.new("mdk_timings *")
     clock = Clock()
 
-    def forward(mode, B, cols):
+    STAGES = ("inproj0_ms", "rec0_ms", "inproj1_ms", "rec1_ms", "head_ms", "total_ms")
+
+    def forward(precision, mode, B, cols):
+        m.set_precision(precision)
         m.set_rec_mode(mode)
 
         def run():
@@ -103,8 +110,9 @@ def main():
             lm.check(lib.mdk_engine_sync(m.engine))
         mhz = clock.during(run)
         lm.check(lib.mdk_engine_mean_timings(m.engine, 1, tm))
-        return {"rec0_ms": float(tm.rec0_ms), "rec1_ms": float(tm.rec1_ms), "inproj1_ms": float(tm.inproj1_ms),
-                "sm_mhz": mhz}
+        r = {k: float(getattr(tm, k)) for k in STAGES}
+        r.update(positions_per_s=B * cols / (r["total_ms"] / 1e3), sm_mhz=mhz)
+        return r
 
     for c in cases.values():
         forward(*c)
@@ -113,12 +121,11 @@ def main():
         for k, c in cases.items():
             runs[k].append(forward(*c))
     med = {k: {f: statistics.median(r[f] for r in v) if v[0][f] is not None else None
-               for f in ("rec0_ms", "rec1_ms", "inproj1_ms", "sm_mhz")} for k, v in runs.items()}
+               for f in STAGES + ("positions_per_s", "sm_mhz")} for k, v in runs.items()}
     print(json.dumps({
         "card": clock.card(), "sm_count": sms, "positions": P, "repeats": args.repeats,
-        "cases": {k: {"rec_mode": c[0], "windows": c[1], "cols": c[2]} for k, c in cases.items()},
-        "median": med, "runs": runs,
-        "two_vs_one": {f: med["two"][f] / med["one"][f] - 1.0 for f in ("rec0_ms", "rec1_ms")}}))
+        "cases": {k: {"precision": c[0], "rec_mode": c[1], "windows": c[2], "cols": c[3]} for k, c in cases.items()},
+        "median": med, "runs": runs}))
     m.close()
 
 
